@@ -2,7 +2,7 @@
 
 ``import paddle_b200 as paddle`` gives the reference's public namespace (python/paddle/__init__.py): Tensor, ops,
 nn, optimizer, amp, io, jit, distributed (+fleet), vision, ... backed by PyTorch tensors/autograd for the plumbing
-and hand-written sm_100a CUDA kernels (``paddle_b200/csrc``) for the hot paths.
+and hand-written sm_90a CUDA kernels (``paddle_b200/csrc``) for the hot paths.
 """
 from __future__ import annotations
 

@@ -1,6 +1,6 @@
 """In-tree build + load of the native extension (``paddle_b200/_C*.so``).
 
-* ``build()`` compiles every ``csrc/**/*.cu|cpp`` for sm_100a with ninja (cross-compiles without a GPU) into
+* ``build()`` compiles every ``csrc/**/*.cu|cpp`` for sm_90a with ninja (cross-compiles without a GPU) into
   ``paddle_b200/_build_cache/`` and copies the module next to this file.
 * ``load()`` imports the prebuilt module; on a GPU box a missing module is a hard error (no silent fallback).
 """
@@ -19,7 +19,7 @@ _NAME = "_C"
 _module = None
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--expt-relaxed-constexpr", "-Xptxas", "-v", "--threads", "4",
 ]
 
@@ -39,6 +39,9 @@ def build(verbose: bool = False):
     """Compile the extension in-tree. Returns the path of the built shared object."""
     from torch.utils import cpp_extension
 
+    from . import _wgmma_gen
+
+    _wgmma_gen.main()
     build_dir = os.path.join(_HERE, "_build_cache")
     os.makedirs(build_dir, exist_ok=True)
     os.environ.setdefault("MAX_JOBS", str(os.cpu_count() or 8))

@@ -188,7 +188,7 @@ _reexport(_FLEET + ".runtime", "paddle.distributed.fleet.runtime", [_FLEET + ".p
 @alias("device.xpu")
 def _xpu_module():
     def _none(*a, **k):
-        raise RuntimeError("XPU devices are not supported by paddle_b200 (sm_100a only)")
+        raise RuntimeError("XPU devices are not supported by paddle_b200 (sm_90a only)")
 
     return _mod(_PKG + ".device.xpu", "paddle.device.xpu: not available on this target", synchronize=_none, device_count=lambda: 0, set_debug_level=lambda level=1: None,
                 empty_cache=lambda: None, max_memory_allocated=lambda device=None: 0, memory_allocated=lambda device=None: 0)

@@ -1,5 +1,5 @@
 """CINN-role tensor compiler: fuses chains of elementwise / broadcast / last-axis-reduction ops of a recorded program into generated
-CUDA kernels for sm_100a.
+CUDA kernels for sm_90a.
 
     fn = paddle.jit.to_static(f, backend="CINN")          # no-grad calls run the fused program
     prog2, report = paddle_b200.cinn.compile_program(program, fetch_list)      # static.Program -> static.Program
@@ -7,9 +7,9 @@ CUDA kernels for sm_100a.
 Pipeline (reference: paddle/cinn - decompose, op fusion, group schedule, CodeGenCUDA_Dev, runtime module):
   recorded static.Program --translate_to_pir--> SSA IR --pir passes / DRR patterns--> `fusion.fuse` (groups; composite ops such as softmax,
   gelu, silu, mean are decomposed to primitives on the way in: `expr.Frontend`) --`codegen`--> CUDA C++ (flat 4-wide elementwise kernels;
-  warp-per-row / CTA-per-row reduction kernels) --`runtime`--> nvcc -gencode arch=compute_100a,code=sm_100a, cached in-tree, launched on
+  warp-per-row / CTA-per-row reduction kernels) --`runtime`--> nvcc -gencode arch=compute_90a,code=sm_90a, cached in-tree, launched on
   the current stream through ctypes.  The same bodies are emitted as plain C++ for the host, which is how tests/test_cinn_cpu.py runs the
-  compiler end to end without a GPU.  GEMM-shaped and attention ops are NOT generated: they stay on the hand-written tcgen05 kernels.
+  compiler end to end without a GPU.  GEMM-shaped and attention ops are NOT generated: they stay on the hand-written wgmma kernels.
 """
 from __future__ import annotations
 

@@ -1,9 +1,9 @@
-"""Code generation for a fusion group: CUDA C++ for sm_100a (the product) and plain C++ for the host (how the compiler is exercised on a
+"""Code generation for a fusion group: CUDA C++ for sm_90a (the product) and plain C++ for the host (how the compiler is exercised on a
 machine without a GPU; same expression bodies).
 
 Schedules
   * elementwise group  -> one grid-stride kernel over the flat domain; a second variant moves 4 elements per thread (8 when a 16-bit tensor is
-    streamed, so that its accesses are 16 bytes wide; picked at launch when every pointer is 16-byte aligned); the grid is capped at 148 SMs x 8 CTAs.
+    streamed, so that its accesses are 16 bytes wide; picked at launch when every pointer is 16-byte aligned); the grid is capped at 132 SMs x 8 CTAs.
   * group with reductions over the last axis -> a row kernel: one warp per row for rows of <= 256 columns (shuffle reductions, 8 rows per
     CTA), one 256-thread CTA per row up to 2048 columns, one 1024-thread CTA per row beyond (shuffle + one shared-memory exchange).
     Reductions that feed later elementwise work become successive passes over the row (pass s computes every reduction whose input depends
@@ -605,7 +605,7 @@ def host_source(spec):
 
 
 # ---- CUDA ------------------------------------------------------------------------------------------------------------------------------
-SM_COUNT = 148
+SM_COUNT = 132
 
 
 def _vec_width(spec):

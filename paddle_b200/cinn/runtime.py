@@ -1,6 +1,6 @@
 """Compile, cache and launch generated kernels.
 
-A kernel is compiled once per (source, target): `nvcc -gencode arch=compute_100a,code=sm_100a` into a small shared object whose `extern "C"`
+A kernel is compiled once per (source, target): `nvcc -gencode arch=compute_90a,code=sm_90a` into a small shared object whose `extern "C"`
 launcher is called through ctypes with raw device pointers and the current CUDA stream; the host target is `g++ -O2`.  Objects are cached
 in-tree under `paddle_b200/_build_cache/cinn/` (keyed by the hash of the source), so a warm cache travels with the package.
 Role parity: CINN's runtime module / NVRTC compile cache (paddle/cinn/runtime, paddle/cinn/backends/nvrtc)."""
@@ -55,7 +55,7 @@ def compile_source(src, target, keep_source=True):
         nvcc = _nvcc()
         if nvcc is None:
             raise CompileError("nvcc not found: generated CUDA kernels cannot be built")
-        cmd = [nvcc, "-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "--cudart", "shared", "-shared", "-Xcompiler", "-fPIC", "-o", tmp, path]
+        cmd = [nvcc, "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "--cudart", "shared", "-shared", "-Xcompiler", "-fPIC", "-o", tmp, path]
     else:
         cmd = ["g++", "-O2", "-std=c++17", "-shared", "-fPIC", "-fno-math-errno", "-o", tmp, path]
     r = subprocess.run(cmd, capture_output=True, text=True)

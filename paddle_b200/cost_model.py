@@ -1,6 +1,4 @@
 """paddle.cost_model: analytic step-time model used by distributed.auto_tuner. Parity: python/paddle/cost_model/cost_model.py."""
-import json
-import os
 
 
 class CostModel:
@@ -9,19 +7,15 @@ class CostModel:
 
     @staticmethod
     def _load_peaks():
-        p = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")
-        try:
-            return json.load(open(p))
-        except Exception:
-            return {"hbm_gbs": 6650.0, "bf16_tflops_sustained": 1400.0}
+        return {"hbm_gbs": 3350.0, "bf16_tflops_sustained": 989.0}   # NVIDIA's data sheet for the H100 SXM (HBM3, dense bf16); pass measured ones
 
-    def gemm_ms(self, m, n, k, eff=0.85):
-        return 2.0 * m * n * k / (self.peaks.get("bf16_tflops_sustained", 1400.0) * 1e9 * eff)
+    def gemm_ms(self, m, n, k, eff=0.30):
+        return 2.0 * m * n * k / (self.peaks.get("bf16_tflops_sustained", 989.0) * 1e9 * eff)
 
     def mem_ms(self, nbytes, eff=0.8):
-        return nbytes / (self.peaks.get("hbm_gbs", 6650.0) * 1e6 * eff)
+        return nbytes / (self.peaks.get("hbm_gbs", 3350.0) * 1e6 * eff)
 
-    def allreduce_ms(self, nbytes, world, bus_gbs=725.0):
+    def allreduce_ms(self, nbytes, world, bus_gbs=450.0):   # NVLink 4 data sheet, one direction; not measured
         return 0.0 if world <= 1 else 2.0 * (world - 1) / world * nbytes / (bus_gbs * 1e6)
 
     def profile_measure(self, main_program=None, startup_program=None, device="gpu", fetch_cost_list=("time",), feed=None, fetch_list=None, repeat=5):

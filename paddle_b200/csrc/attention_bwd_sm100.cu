@@ -1,22 +1,21 @@
-// Flash-attention backward for sm_100a (head_dim 128, bf16/fp16), tcgen05 + TMA.
+// Flash-attention backward for sm_90a (head_dim 128, bf16/fp16), wgmma + TMA, in two kernels that share no atomics:
 //
-// One CTA owns a 128-key K/V tile of one (batch, kv head) and walks the query tiles that can see it (and, under GQA, every
-// query head of the group).  Per query tile five 128x128x128 tensor-core GEMMs:
-//   S   = Q K^T          dP  = dO V^T                      (TMEM, lane = query row)
-//   dV += P^T dO         dK += dS^T Q                      (TMEM accumulators, lane = key row, live across the whole loop)
-//   dQ^T = K^T dS^T                                        (TMEM, lane = head dim; reduced into fp32 dQ with coalesced atomics)
-// P and dS are produced by the 128 softmax threads (thread = query row) from S, dP, the forward's logsumexp and
-// delta = rowsum(dO * O), and are written ONCE to shared memory in the 128B-swizzled [key-half][query row] layout that
-// serves both as MN-major A operand (P^T, dS^T) and as K-major B operand (dS^T of the dQ GEMM) by choice of descriptor
-// strides; the K tile is likewise consumed K-major (S) and MN-major (dQ^T) from one copy.
+//   dkv_kernel: one CTA owns a 128-key K/V tile of one (batch, kv head) - 64 keys per MMA warpgroup - and walks the 64-row query tiles
+//     that can see it (and, under GQA, every query head of the group).  It computes the TRANSPOSED tiles S^T = K Q^T and dP^T = V dO^T
+//     (accumulator row = key), so that P^T and dS^T, packed to 16 bits, are already the register A fragments of dV += P^T dO and
+//     dK += dS^T Q: nothing is staged in shared memory and the dV / dK accumulators stay in registers across the whole loop.
+//   dq_kernel: one CTA owns 128 query rows of one (batch, head) - 64 per warpgroup - and walks the 64-key tiles it can see: S = Q K^T,
+//     dP = dO V^T (accumulator row = query), dS packed in registers is the A fragment of dQ += dS K.  Every dQ element is written once,
+//     by one thread, in a fixed order: the result is bitwise reproducible without turn-taking and dQ needs no fp32 atomics.
+//   Recomputing S and dP in the second kernel costs 2 of 7 GEMMs; in exchange no tile is transposed through shared memory and the
+//     register budget of each kernel holds its accumulators without spilling.
+// The K and Q tiles are consumed K-major (S) and MN-major (dQ, dK) from one copy by choice of descriptor.
 //
 // Parity (behaviour): flash_attn_grad (paddle/phi/kernels/gpu/flash_attn_grad_kernel.cu -> flash-attention library).
-// Warps 0-7: softmax / dQ reduction / epilogue (two warpgroups, one 64-column half each), warp 8: TMA producer,
-// warp 9: TMEM alloc + MMA issuer.
-// TMEM columns: [0,128) S then dQ^T, [128,256) dP, [256,384) dV, [384,512) dK.
 #include <cuda.h>
 #include <cstdio>
 #include <string>
+#include <type_traits>
 
 #include "include/b200_common.cuh"
 #include "include/b200_ops.h"
@@ -26,20 +25,14 @@ namespace b200 {
 namespace attn_bwd {
 using namespace ptx;
 
-constexpr int BM = 128, BN = 128, HD = 128;
-constexpr int kThreads = 320;   // warps 0-7: softmax / dQ / epilogue (2 warpgroups), warp 8: TMA producer, warp 9: TMEM alloc + MMA issuer
-constexpr uint32_t TILE_BYTES = 128 * 128 * 2;
-constexpr uint32_t HALF_BYTES = TILE_BYTES / 2;
-constexpr uint32_t SMEM_BYTES = 6 * TILE_BYTES + 1024 + 256;
-constexpr uint32_t TMEM_COLS = 512;
-constexpr uint32_t S_COL = 0, DP_COL = 128, DV_COL = 256, DK_COL = 384;
-
-
-// Operand descriptors for one 128x128 bf16 tile stored as two 64-wide halves [half][row 0..127][128 B swizzled]:
-//   K-major use   (rows = M or N index, inner = K):   K step k (16 elems) inside half kb -> +kb*HALF + k*32,  LBO 16, SBO 1024
-//   MN-major use  (rows = K index, inner = M or N):   K step k (16 rows)                 -> +k*2048,         LBO HALF (next 64 M/N), SBO 1024
-__device__ __forceinline__ uint64_t desc_kmajor(uint32_t tile, int kb, int k) { return make_smem_desc(tile + kb * HALF_BYTES + k * 32, 16, 1024); }
-__device__ __forceinline__ uint64_t desc_mnmajor(uint32_t tile, int kk) { return make_smem_desc(tile + kk * 2048, HALF_BYTES, 1024); }
+constexpr int HD = 128;
+constexpr int kThreads = 288;      // dq_kernel: warps 0-7 two MMA warpgroups, warp 8 TMA producer
+constexpr int kThreadsDkv = 384;   // dkv_kernel: warpgroup 0 = producer (warp 0) giving its registers to the MMA warpgroups 1 and 2
+constexpr uint32_t BIG_BYTES = 128 * 128 * 2;     // a 128-row tile: two 64-wide d halves [half][row][128 B swizzled]
+constexpr uint32_t BIG_HALF = BIG_BYTES / 2;
+constexpr uint32_t SMALL_BYTES = 64 * 128 * 2;    // a 64-row tile, same structure
+constexpr uint32_t SMALL_HALF = SMALL_BYTES / 2;
+constexpr uint32_t SMEM_BYTES = 2 * BIG_BYTES + 4 * SMALL_BYTES + 1024 + 256;   // two resident 128-row tiles + two double-buffered 64-row tiles
 
 template <typename T> __device__ __forceinline__ uint32_t pack2(float a, float b);
 template <> __device__ __forceinline__ uint32_t pack2<__nv_bfloat16>(float a, float b) {
@@ -50,6 +43,12 @@ template <> __device__ __forceinline__ uint32_t pack2<__half>(float a, float b) 
   const __half2 v = __floats2half2_rn(a, b);
   return *reinterpret_cast<const uint32_t*>(&v);
 }
+__device__ __forceinline__ void keep_regs(uint32_t (&a)[4][4]) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) asm volatile("" : "+r"(a[i][j])::"memory");
+}
 
 struct Params {
   int b, sq, sk, h, hk;
@@ -57,272 +56,326 @@ struct Params {
   int causal, causal_off;
   const float* lse;      // [B,H,Sq] natural log
   const float* delta;    // [B,H,Sq]
-  float* dq;             // fp32 [B,Sq,H,D] (zero-initialised; reduced with atomics)
+  float* dq;             // fp32 [B,Sq,H,D]: every element is written
   void* dk;              // [B,Sk,Hk,D] with element strides (dkv_sb, dkv_ss, dkv_sh): may be slices of a packed dQKV tensor
   void* dv;
   int64_t dkv_sb, dkv_ss, dkv_sh;
-  int64_t dq_sb, dq_ss, dq_sh;   // element strides of the fp32 dQ accumulator [B,Sq,H,D] (may be laid out seq-major)
-  uint32_t idesc_kk;     // A K-major, B K-major   (S, dP)
-  uint32_t idesc_mm;     // A MN-major, B MN-major (dV, dK)
-  uint32_t idesc_mk;     // A MN-major, B K-major  (dQ^T)
+  int64_t dq_sb, dq_ss, dq_sh;   // element strides of the fp32 dQ [B,Sq,H,D] (may be laid out seq-major)
   const int4* colmask;   // [b, mask_heads, sk] hidden row ranges per key column (see AttnArgs::colmask); nullptr: none
   int mask_heads;
-  int* dq_sem;           // deterministic dQ: turn counter per (batch, head, query tile); nullptr = reduce in arrival order
+};
+
+// resident tile (128 rows) in slot 0 / 1, streamed tiles (64 rows): operand a in slots [0, 2), operand b in slots [2, 4)
+struct Smem {
+  uint32_t base;
+  __device__ uint32_t big(int i) const { return base + i * BIG_BYTES; }
+  __device__ uint32_t small(int i) const { return base + 2 * BIG_BYTES + i * SMALL_BYTES; }
+  __device__ uint32_t bar(int i) const { return base + 2 * BIG_BYTES + 4 * SMALL_BYTES + 8u * i; }
 };
 
 template <typename T, bool MASKED>
-__global__ void __launch_bounds__(kThreads, 1)
-bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
+__global__ void __launch_bounds__(kThreadsDkv, 1)
+dkv_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
            const __grid_constant__ CUtensorMap map_do, const Params p) {
+  constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
+  constexpr int BN = 128, BQ = 64;
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* gen = smem_raw + (base - smem_u32(smem_raw));
-  const uint32_t sK = base, sV = base + TILE_BYTES, sQ = base + 2 * TILE_BYTES, sDO = base + 3 * TILE_BYTES, sP = base + 4 * TILE_BYTES,
-                 sDS = base + 5 * TILE_BYTES;
-  const uint32_t bars = base + 6 * TILE_BYTES;
-  const uint32_t kv_full = bars, qdo_full = bars + 8, qdo_empty = bars + 16, s_full = bars + 24, s_free = bars + 32, pds_full = bars + 40,
-                 dq_full = bars + 48, acc_done = bars + 56;
-  volatile uint32_t* tmem_ptr = reinterpret_cast<volatile uint32_t*>(gen + 6 * TILE_BYTES + 8 * 8);
+  const Smem sm{(smem_u32(smem_raw) + 1023u) & ~1023u};
+  const uint32_t sK = sm.big(0), sV = sm.big(1);
+  auto sQ = [&](int s) { return sm.small(s); };
+  auto sDO = [&](int s) { return sm.small(2 + s); };
+  const uint32_t kv_full = sm.bar(0);
+  auto qdo_full = [&](int s) { return sm.bar(1 + s); };
+  auto qdo_empty = [&](int s) { return sm.bar(3 + s); };     // 8 warp arrivals
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_tile = blockIdx.x, kv_head = blockIdx.y, batch = blockIdx.z;
   const int n0 = n_tile * BN;
   const int group = p.h / p.hk;
-  const int num_m = (p.sq + BM - 1) / BM;
+  const int num_m = (p.sq + BQ - 1) / BQ;
   int m_first = 0;
-  if (p.causal) {                       // first query row that can see key n0: i >= n0 - causal_off
+  if (p.causal) {                       // first query row that can see key n0 + BN - 1 or an earlier one of the tile: i >= n0 - causal_off
     const int r0 = max(0, n0 - p.causal_off);
-    m_first = min(num_m, r0 / BM);
+    m_first = min(num_m, r0 / BQ);
   }
   const int tiles_per_head = num_m - m_first;
   const int total = tiles_per_head * group;    // iteration it -> (query head = kv_head*group + it / tiles_per_head, m tile = m_first + it % tiles_per_head)
 
-  if (warp == 8 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_k) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_v) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_do) : "memory");
-    mbar_init(kv_full, 1); mbar_init(qdo_full, 1); mbar_init(qdo_empty, 1); mbar_init(s_full, 1); mbar_init(s_free, 8);
-    mbar_init(pds_full, 8); mbar_init(dq_full, 1); mbar_init(acc_done, 1);
+  if (warp == 0 && lane == 0) {
+    tma_prefetch_desc(&map_q); tma_prefetch_desc(&map_k); tma_prefetch_desc(&map_v); tma_prefetch_desc(&map_do);
+    mbar_init(kv_full, 1);
+    for (int s = 0; s < 2; ++s) { mbar_init(qdo_full(s), 1); mbar_init(qdo_empty(s), 8); }
     fence_barrier_init();
     fence_proxy_async();
-  } else if (warp == 9) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32((const void*)tmem_ptr)), "r"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 8) {
-    if (lane == 0 && total > 0) {
+  if (warp < 4) {
+    reg_dealloc<40>();
+    if (warp == 0 && lane == 0 && total > 0) {
       // ================= TMA producer =================
-      mbar_expect_tx(kv_full, 2 * TILE_BYTES);
+      mbar_expect_tx(kv_full, 2 * BIG_BYTES);
       tma_load_4d(sK, &map_k, kv_full, 0, n0, kv_head, batch);
-      tma_load_4d(sK + HALF_BYTES, &map_k, kv_full, 64, n0, kv_head, batch);
+      tma_load_4d(sK + BIG_HALF, &map_k, kv_full, 64, n0, kv_head, batch);
       tma_load_4d(sV, &map_v, kv_full, 0, n0, kv_head, batch);
-      tma_load_4d(sV + HALF_BYTES, &map_v, kv_full, 64, n0, kv_head, batch);
+      tma_load_4d(sV + BIG_HALF, &map_v, kv_full, 64, n0, kv_head, batch);
       for (int it = 0; it < total; ++it) {
+        const int s = it & 1;
         const int head = kv_head * group + it / tiles_per_head;
-        const int m0 = (m_first + it % tiles_per_head) * BM;
-        mbar_wait(qdo_empty, (it & 1) ^ 1);
-        mbar_expect_tx(qdo_full, 2 * TILE_BYTES);
-        tma_load_4d(sQ, &map_q, qdo_full, 0, m0, head, batch);
-        tma_load_4d(sQ + HALF_BYTES, &map_q, qdo_full, 64, m0, head, batch);
-        tma_load_4d(sDO, &map_do, qdo_full, 0, m0, head, batch);
-        tma_load_4d(sDO + HALF_BYTES, &map_do, qdo_full, 64, m0, head, batch);
+        const int m0 = (m_first + it % tiles_per_head) * BQ;
+        mbar_wait(qdo_empty(s), ((it >> 1) & 1) ^ 1);
+        mbar_expect_tx(qdo_full(s), 2 * SMALL_BYTES);
+        tma_load_4d(sQ(s), &map_q, qdo_full(s), 0, m0, head, batch);
+        tma_load_4d(sQ(s) + SMALL_HALF, &map_q, qdo_full(s), 64, m0, head, batch);
+        tma_load_4d(sDO(s), &map_do, qdo_full(s), 0, m0, head, batch);
+        tma_load_4d(sDO(s) + SMALL_HALF, &map_do, qdo_full(s), 64, m0, head, batch);
       }
-    }
-  } else if (warp == 9) {
-    if (lane == 0 && total > 0) {
-      // ================= MMA issuer =================
-      mbar_wait(kv_full, 0);
-      for (int it = 0; it < total; ++it) {
-        const uint32_t ph = it & 1;
-        mbar_wait(qdo_full, ph);
-        mbar_wait(s_free, ph ^ 1);        // S / dQ^T columns drained by the softmax warps (previous iteration)
-        tc_fence_after();
-#pragma unroll
-        for (int kb = 0; kb < 2; ++kb)
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            umma_f16(tmem_base + S_COL, desc_kmajor(sQ, kb, k), desc_kmajor(sK, kb, k), p.idesc_kk, (kb | k) != 0);    // S = Q K^T
-            umma_f16(tmem_base + DP_COL, desc_kmajor(sDO, kb, k), desc_kmajor(sV, kb, k), p.idesc_kk, (kb | k) != 0);  // dP = dO V^T
-          }
-        umma_commit(s_full);
-        mbar_wait(pds_full, ph);
-        tc_fence_after();
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {     // K dimension = 128 query rows, 16 per MMA
-          umma_f16(tmem_base + DV_COL, desc_mnmajor(sP, kk), desc_mnmajor(sDO, kk), p.idesc_mm, (it | kk) != 0);   // dV += P^T dO
-          umma_f16(tmem_base + DK_COL, desc_mnmajor(sDS, kk), desc_mnmajor(sQ, kk), p.idesc_mm, (it | kk) != 0);   // dK += dS^T Q
-        }
-        umma_commit(qdo_empty);              // Q / dO tiles may be overwritten by the next loads
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk)       // K dimension = 128 keys; A = K tile read MN-major (M = head dim), B = dS read K-major (N = query)
-          umma_f16(tmem_base + S_COL, desc_mnmajor(sK, kk), desc_kmajor(sDS, kk >> 2, kk & 3), p.idesc_mk, kk != 0);  // dQ^T = K^T dS^T
-        umma_commit(dq_full);
-      }
-      umma_commit(acc_done);
     }
   } else {
-    // ================= softmax / dQ reduction / epilogue: 2 warpgroups, each owns one 64-column half =================
-    const int half = warp >> 2;                      // key half for S/dP, query half for dQ^T, head-dim half for dV/dK
-    const int rl = (warp & 3) * 32 + lane;           // TMEM lane
-    const uint32_t lane_off = (uint32_t)((warp & 3) * 32) << 16;
+    // ================= MMA warpgroups: wg owns keys [64 wg, 64 wg + 64) of the tile; accumulator row = key, column = query =================
+    reg_alloc<232>();
+    const int wg = (warp >> 2) - 1, q = lane & 3;
+    const int rl = wg * 64 + (warp & 3) * 16 + (lane >> 2);      // tile-relative key rows rl and rl + 8
     constexpr float kLog2e = 1.4426950408889634f;
+    float dv_acc[HD / 2], dk_acc[HD / 2];
+#pragma unroll
+    for (int i = 0; i < HD / 2; ++i) { dv_acc[i] = 0.f; dk_acc[i] = 0.f; }
+    if (total > 0) mbar_wait(kv_full, 0);
     for (int it = 0; it < total; ++it) {
-      const uint32_t ph = it & 1;
+      const int s = it & 1;
       const int head = kv_head * group + it / tiles_per_head;
-      const int m0 = (m_first + it % tiles_per_head) * BM;
-      const int row = m0 + rl;
-      const bool row_ok = row < p.sq;
-      const int64_t stat = ((int64_t)batch * p.h + head) * p.sq + row;
-      const float lse2 = row_ok ? p.lse[stat] * kLog2e : 0.f;
-      const float dl = row_ok ? p.delta[stat] : 0.f;
-      const int lim = p.causal ? min(p.sk - 1, row + p.causal_off) : p.sk - 1;   // last visible key of this query row
-      const int4* cm = MASKED ? p.colmask + ((int64_t)batch * p.mask_heads + (p.mask_heads > 1 ? head : 0)) * p.sk : nullptr;
-      (void)cm;
-      mbar_wait(s_full, ph);
-      tc_fence_after();
-      // previous iteration's dV/dK/dQ MMAs have retired (we waited dq_full below), so the P / dS tiles are free
+      const int m0 = (m_first + it % tiles_per_head) * BQ;
+      const int64_t stat0 = ((int64_t)batch * p.h + head) * p.sq;
+      mbar_wait(qdo_full(s), (it >> 1) & 1);
+      float st[BQ / 2], dpt[BQ / 2];
+      wgmma_fence_regs(st);
+      wgmma_fence_regs(dpt);
+      wgmma_fence();
 #pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t rs[32], rp[32];
-        tmem_ld_32x32(tmem_base + lane_off + S_COL + half * 64 + c * 32, rs);
-        tmem_ld_32x32(tmem_base + lane_off + DP_COL + half * 64 + c * 32, rp);
+      for (int kb = 0; kb < 2; ++kb)
 #pragma unroll
-        for (int q8 = 0; q8 < 4; ++q8) {
-          uint32_t up[4], ud[4];
+        for (int k = 0; k < 4; ++k) {
+          wgmma_ss_n64<BF16, 0, 0>(st, make_smem_desc(sK + kb * BIG_HALF + wg * 8192 + k * 32, 16, 1024),
+                                   make_smem_desc(sQ(s) + kb * SMALL_HALF + k * 32, 16, 1024), (kb | k) != 0);      // S^T = K Q^T
+          wgmma_ss_n64<BF16, 0, 0>(dpt, make_smem_desc(sV + kb * BIG_HALF + wg * 8192 + k * 32, 16, 1024),
+                                   make_smem_desc(sDO(s) + kb * SMALL_HALF + k * 32, 16, 1024), (kb | k) != 0);     // dP^T = V dO^T
+        }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(st);
+      wgmma_fence_regs(dpt);
+      int4 cm[2];
+      if constexpr (MASKED) {
+        const int4* cmp = p.colmask + ((int64_t)batch * p.mask_heads + (p.mask_heads > 1 ? head : 0)) * p.sk;
 #pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            float pv[2], ds[2];
-#pragma unroll
-            for (int t2 = 0; t2 < 2; ++t2) {
-              const int i = q8 * 8 + 2 * e + t2;
-              const int key = n0 + half * 64 + c * 32 + i;
-              float x = ex2(fmaf(__uint_as_float(rs[i]), p.scale_log2, -lse2));
-              if (!row_ok || key > lim) x = 0.f;
-              if constexpr (MASKED) {
-                if (key < p.sk) {
-                  const int4 m = __ldg(cm + key);
-                  if ((row >= m.x && row < m.y) || (row >= m.z && row < m.w)) x = 0.f;
-                }
-              }
-              pv[t2] = x;
-              ds[t2] = x * (__uint_as_float(rp[i]) - dl) * p.scale;
-            }
-            up[e] = pack2<T>(pv[0], pv[1]);
-            ud[e] = pack2<T>(ds[0], ds[1]);
-          }
-          const int col = c * 32 + q8 * 8;              // key index inside this 64-key half
-          const uint32_t off = half * HALF_BYTES + rl * 128 + (((col >> 3) ^ (rl & 7)) << 4);
-          asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sP + off), "r"(up[0]), "r"(up[1]), "r"(up[2]), "r"(up[3]) : "memory");
-          asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sDS + off), "r"(ud[0]), "r"(ud[1]), "r"(ud[2]), "r"(ud[3]) : "memory");
+        for (int h = 0; h < 2; ++h) {
+          const int key = n0 + rl + h * 8;
+          cm[h] = key < p.sk ? __ldg(cmp + key) : make_int4(0, 0, 0, 0);
         }
       }
-      fence_proxy_async();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(pds_full);          // 8 warp arrivals
-      // dQ^T tile: TMEM lane = head-dim index (d = rl), columns = query rows; this warpgroup handles query columns [half*64, +64)
-      mbar_wait(dq_full, ph);
-      tc_fence_after();
-      // Transpose through shared memory (the P + dS tiles are free: every MMA of this iteration has retired) into a row-major
-      // fp32 [query][d] tile, then let the TMA engine reduce each 512-byte row into dQ (cp.reduce.async.bulk ... add.f32).
-      const uint32_t sDQ = sP;   // 64 KB: sP and sDS are adjacent
-#pragma unroll 1
-      for (int c = 0; c < 2; ++c) {
-        uint32_t r[32];
-        tmem_ld_32x32(tmem_base + lane_off + S_COL + half * 64 + c * 32, r);
+      // P^T = exp2(S^T scale - lse[query]), dS^T = P^T (dP^T - delta[query]) scale, packed as A fragments (16-query step ks = column groups 2 ks, 2 ks + 1)
+      uint32_t pa[BQ / 16][4], dsa[BQ / 16][4];
 #pragma unroll
-        for (int i = 0; i < 32; ++i)
-          asm volatile("st.shared.b32 [%0], %1;" ::"r"(sDQ + (uint32_t)(half * 64 + c * 32 + i) * 512u + (uint32_t)rl * 4u), "r"(r[i]) : "memory");
-      }
-      tc_fence_before();
-      fence_proxy_async();
-      // Deterministic mode (FLAGS_cudnn_deterministic): the fp32 adds of the bulk reduce are order dependent, so the key tiles take turns on
-      // a query tile in ascending order (tile n waits for the counter to reach n; every key tile from 0 on contributes to every query tile
-      // it visits, masked or not).  CTAs with a lower blockIdx.x are dispatched first, so the tile waited for is resident or done.
-      int* sem = nullptr;
-      if (p.dq_sem) {
-        sem = p.dq_sem + ((int64_t)batch * p.h + head) * num_m + (m0 / BM);
-        if (threadIdx.x == 0) {
-          uint64_t t0 = 0;
-          uint32_t spins = 0;
-          while (true) {
-            int v;
-            asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(sem) : "memory");
-            if (v >= n_tile) break;
-            if (++spins == 4096) t0 = globaltimer_ns();
-            if (spins > 4096 && (spins & 1023) == 0 && globaltimer_ns() - t0 > 10000000000ull) {
-              printf("b200 attention bwd: deterministic dQ turn timeout (block %d,%d,%d)\n", blockIdx.x, blockIdx.y, blockIdx.z);
-              __trap();
+      for (int jn = 0; jn < BQ / 8; ++jn) {
+        float pv[4], ds[4];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int row = m0 + jn * 8 + 2 * q + e;      // query
+          const bool row_ok = row < p.sq;
+          const float lse2 = row_ok ? __ldg(p.lse + stat0 + row) * kLog2e : 0.f;
+          const float dl = row_ok ? __ldg(p.delta + stat0 + row) : 0.f;
+          const int lim = p.causal ? min(p.sk - 1, row + p.causal_off) : p.sk - 1;   // last visible key of this query row
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int key = n0 + rl + h * 8;
+            float x = ex2(fmaf(st[jn * 4 + h * 2 + e], p.scale_log2, -lse2));
+            if (!row_ok || key > lim) x = 0.f;
+            if constexpr (MASKED) {
+              if ((row >= cm[h].x && row < cm[h].y) || (row >= cm[h].z && row < cm[h].w)) x = 0.f;
             }
+            pv[h * 2 + e] = x;
+            ds[h * 2 + e] = x * (dpt[jn * 4 + h * 2 + e] - dl) * p.scale;
           }
         }
+        pa[jn >> 1][(jn & 1) * 2 + 0] = pack2<T>(pv[0], pv[1]);
+        pa[jn >> 1][(jn & 1) * 2 + 1] = pack2<T>(pv[2], pv[3]);
+        dsa[jn >> 1][(jn & 1) * 2 + 0] = pack2<T>(ds[0], ds[1]);
+        dsa[jn >> 1][(jn & 1) * 2 + 1] = pack2<T>(ds[2], ds[3]);
       }
-      asm volatile("bar.sync 1, 256;" ::: "memory");      // both softmax warpgroups: the whole [128][128] fp32 tile is in smem (and it is our turn)
-      if (half == 0 && m0 + rl < p.sq) {
-        float* dst = p.dq + (int64_t)batch * p.dq_sb + (int64_t)(m0 + rl) * p.dq_ss + (int64_t)head * p.dq_sh;
-        asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f32 [%0], [%1], 512;" ::"l"(dst), "r"(sDQ + (uint32_t)rl * 512u) : "memory");
+      wgmma_fence_regs(dv_acc);
+      wgmma_fence_regs(dk_acc);
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < BQ / 16; ++ks) {   // B = dO / Q tile read MN-major (N = head dim): 16 query rows = 2048 B per step, d halves SMALL_HALF apart
+        wgmma_rs_n128<BF16, 1>(dv_acc, pa[ks], make_smem_desc(sDO(s) + ks * 2048, SMALL_HALF, 1024), 1);   // dV += P^T dO
+        wgmma_rs_n128<BF16, 1>(dk_acc, dsa[ks], make_smem_desc(sQ(s) + ks * 2048, SMALL_HALF, 1024), 1);   // dK += dS^T Q
       }
-      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-      if (sem) {
-        asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");      // the adds have been performed, not just read from smem
-        __threadfence();
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        if (threadIdx.x == 0) asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(sem), "r"(n_tile + 1) : "memory");
-      } else {
-        asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // the tile in shared memory may be overwritten
-      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(dv_acc);
+      wgmma_fence_regs(dk_acc);
+      keep_regs(pa);
+      keep_regs(dsa);
       __syncwarp();
-      if (lane == 0) mbar_arrive(s_free);            // 8 warp arrivals
+      if (lane == 0) mbar_arrive(qdo_empty(s));
     }
-    // epilogue: dV, dK rows (lane = key row); this warpgroup writes head-dim columns [half*64, +64)
-    if (total > 0) {
-      mbar_wait(acc_done, 0);
-      tc_fence_after();
-    }
-    const int key = n0 + rl;
-    const int64_t kv_off = (int64_t)batch * p.dkv_sb + (int64_t)key * p.dkv_ss + (int64_t)kv_head * p.dkv_sh + half * 64;
-    T* dv_row = reinterpret_cast<T*>(p.dv) + kv_off;
-    T* dk_row = reinterpret_cast<T*>(p.dk) + kv_off;
-#pragma unroll 1
-    for (int c = 0; c < 2; ++c) {
-      uint32_t rv[32], rk[32];
-      if (total > 0) {
-        tmem_ld_32x32(tmem_base + lane_off + DV_COL + half * 64 + c * 32, rv);
-        tmem_ld_32x32(tmem_base + lane_off + DK_COL + half * 64 + c * 32, rk);
-      } else {
+    // epilogue: dV, dK rows (accumulator row = key)
 #pragma unroll
-        for (int i = 0; i < 32; ++i) { rv[i] = 0u; rk[i] = 0u; }
-      }
-      if (key < p.sk) {
+    for (int h = 0; h < 2; ++h) {
+      const int key = n0 + rl + h * 8;
+      if (key >= p.sk) continue;
+      const int64_t kv_off = (int64_t)batch * p.dkv_sb + (int64_t)key * p.dkv_ss + (int64_t)kv_head * p.dkv_sh;
+      T* dv_row = reinterpret_cast<T*>(p.dv) + kv_off;
+      T* dk_row = reinterpret_cast<T*>(p.dk) + kv_off;
 #pragma unroll
-        for (int q8 = 0; q8 < 4; ++q8) {
-          uint4 ov, ok;
-          ov.x = pack2<T>(__uint_as_float(rv[q8 * 8 + 0]), __uint_as_float(rv[q8 * 8 + 1]));
-          ov.y = pack2<T>(__uint_as_float(rv[q8 * 8 + 2]), __uint_as_float(rv[q8 * 8 + 3]));
-          ov.z = pack2<T>(__uint_as_float(rv[q8 * 8 + 4]), __uint_as_float(rv[q8 * 8 + 5]));
-          ov.w = pack2<T>(__uint_as_float(rv[q8 * 8 + 6]), __uint_as_float(rv[q8 * 8 + 7]));
-          ok.x = pack2<T>(__uint_as_float(rk[q8 * 8 + 0]), __uint_as_float(rk[q8 * 8 + 1]));
-          ok.y = pack2<T>(__uint_as_float(rk[q8 * 8 + 2]), __uint_as_float(rk[q8 * 8 + 3]));
-          ok.z = pack2<T>(__uint_as_float(rk[q8 * 8 + 4]), __uint_as_float(rk[q8 * 8 + 5]));
-          ok.w = pack2<T>(__uint_as_float(rk[q8 * 8 + 6]), __uint_as_float(rk[q8 * 8 + 7]));
-          *reinterpret_cast<uint4*>(dv_row + c * 32 + q8 * 8) = ov;
-          *reinterpret_cast<uint4*>(dk_row + c * 32 + q8 * 8) = ok;
-        }
+      for (int jn = 0; jn < HD / 8; ++jn) {
+        *reinterpret_cast<uint32_t*>(dv_row + jn * 8 + 2 * q) = pack2<T>(dv_acc[jn * 4 + h * 2], dv_acc[jn * 4 + h * 2 + 1]);
+        *reinterpret_cast<uint32_t*>(dk_row + jn * 8 + 2 * q) = pack2<T>(dk_acc[jn * 4 + h * 2], dk_acc[jn * 4 + h * 2 + 1]);
       }
     }
-    tc_fence_before();
+  }
+}
+
+template <typename T, bool MASKED>
+__global__ void __launch_bounds__(kThreads, 1)
+dq_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
+          const __grid_constant__ CUtensorMap map_do, const Params p) {
+  constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
+  constexpr int BM = 128, BK = 64;
+  extern __shared__ uint8_t smem_raw[];
+  const Smem sm{(smem_u32(smem_raw) + 1023u) & ~1023u};
+  const uint32_t sQ = sm.big(0), sDO = sm.big(1);
+  auto sK = [&](int s) { return sm.small(s); };
+  auto sV = [&](int s) { return sm.small(2 + s); };
+  const uint32_t qdo_full = sm.bar(0);
+  auto kv_full = [&](int s) { return sm.bar(1 + s); };
+  auto kv_empty = [&](int s) { return sm.bar(3 + s); };     // 8 warp arrivals
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int m_tile = (int)gridDim.x - 1 - (int)blockIdx.x;   // long (late) rows first under the causal mask
+  const int head = blockIdx.y, batch = blockIdx.z;
+  const int kv_head = head / (p.h / p.hk);
+  const int m0 = m_tile * BM;
+  int n_tiles = (p.sk + BK - 1) / BK;
+  if (p.causal) {
+    const int last_key = min(p.sk - 1, m0 + BM - 1 + p.causal_off);
+    n_tiles = last_key < 0 ? 0 : min(n_tiles, last_key / BK + 1);
   }
 
+  if (warp == 8 && lane == 0) {
+    tma_prefetch_desc(&map_q); tma_prefetch_desc(&map_k); tma_prefetch_desc(&map_v); tma_prefetch_desc(&map_do);
+    mbar_init(qdo_full, 1);
+    for (int s = 0; s < 2; ++s) { mbar_init(kv_full(s), 1); mbar_init(kv_empty(s), 8); }
+    fence_barrier_init();
+    fence_proxy_async();
+  }
   __syncthreads();
-  if (warp == 9) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
+
+  if (warp == 8) {
+    if (lane == 0 && n_tiles > 0) {
+      // ================= TMA producer =================
+      mbar_expect_tx(qdo_full, 2 * BIG_BYTES);
+      tma_load_4d(sQ, &map_q, qdo_full, 0, m0, head, batch);
+      tma_load_4d(sQ + BIG_HALF, &map_q, qdo_full, 64, m0, head, batch);
+      tma_load_4d(sDO, &map_do, qdo_full, 0, m0, head, batch);
+      tma_load_4d(sDO + BIG_HALF, &map_do, qdo_full, 64, m0, head, batch);
+      for (int j = 0; j < n_tiles; ++j) {
+        const int s = j & 1, n0 = j * BK;
+        mbar_wait(kv_empty(s), ((j >> 1) & 1) ^ 1);
+        mbar_expect_tx(kv_full(s), 2 * SMALL_BYTES);
+        tma_load_4d(sK(s), &map_k, kv_full(s), 0, n0, kv_head, batch);
+        tma_load_4d(sK(s) + SMALL_HALF, &map_k, kv_full(s), 64, n0, kv_head, batch);
+        tma_load_4d(sV(s), &map_v, kv_full(s), 0, n0, kv_head, batch);
+        tma_load_4d(sV(s) + SMALL_HALF, &map_v, kv_full(s), 64, n0, kv_head, batch);
+      }
+    }
+  } else {
+    // ================= MMA warpgroups: wg owns query rows [64 wg, 64 wg + 64); accumulator row = query, column = key / head dim =================
+    const int wg = warp >> 2, q = lane & 3;
+    const int rl = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    constexpr float kLog2e = 1.4426950408889634f;
+    float dq_acc[HD / 2];
+#pragma unroll
+    for (int i = 0; i < HD / 2; ++i) dq_acc[i] = 0.f;
+    float lse2[2], dl[2];
+    int lim[2];
+    bool row_ok[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = m0 + rl + h * 8;
+      row_ok[h] = row < p.sq;
+      const int64_t stat = ((int64_t)batch * p.h + head) * p.sq + row;
+      lse2[h] = row_ok[h] ? p.lse[stat] * kLog2e : 0.f;
+      dl[h] = row_ok[h] ? p.delta[stat] : 0.f;
+      lim[h] = p.causal ? min(p.sk - 1, row + p.causal_off) : p.sk - 1;
+    }
+    const int4* cmp = MASKED ? p.colmask + ((int64_t)batch * p.mask_heads + (p.mask_heads > 1 ? head : 0)) * p.sk : nullptr;
+    (void)cmp;
+    if (n_tiles > 0) mbar_wait(qdo_full, 0);
+    for (int j = 0; j < n_tiles; ++j) {
+      const int s = j & 1, n0 = j * BK;
+      mbar_wait(kv_full(s), (j >> 1) & 1);
+      float sv[BK / 2], dpv[BK / 2];
+      wgmma_fence_regs(sv);
+      wgmma_fence_regs(dpv);
+      wgmma_fence();
+#pragma unroll
+      for (int kb = 0; kb < 2; ++kb)
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          wgmma_ss_n64<BF16, 0, 0>(sv, make_smem_desc(sQ + kb * BIG_HALF + wg * 8192 + k * 32, 16, 1024),
+                                   make_smem_desc(sK(s) + kb * SMALL_HALF + k * 32, 16, 1024), (kb | k) != 0);      // S = Q K^T
+          wgmma_ss_n64<BF16, 0, 0>(dpv, make_smem_desc(sDO + kb * BIG_HALF + wg * 8192 + k * 32, 16, 1024),
+                                   make_smem_desc(sV(s) + kb * SMALL_HALF + k * 32, 16, 1024), (kb | k) != 0);      // dP = dO V^T
+        }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(sv);
+      wgmma_fence_regs(dpv);
+      uint32_t dsa[BK / 16][4];
+#pragma unroll
+      for (int jn = 0; jn < BK / 8; ++jn) {
+        float ds[4];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int key = n0 + jn * 8 + 2 * q + e;
+          int4 m = make_int4(0, 0, 0, 0);
+          if constexpr (MASKED) { if (key < p.sk) m = __ldg(cmp + key); }
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = m0 + rl + h * 8;
+            float x = ex2(fmaf(sv[jn * 4 + h * 2 + e], p.scale_log2, -lse2[h]));
+            if (!row_ok[h] || key > lim[h]) x = 0.f;
+            if constexpr (MASKED) {
+              if ((row >= m.x && row < m.y) || (row >= m.z && row < m.w)) x = 0.f;
+            }
+            ds[h * 2 + e] = x * (dpv[jn * 4 + h * 2 + e] - dl[h]) * p.scale;
+          }
+        }
+        dsa[jn >> 1][(jn & 1) * 2 + 0] = pack2<T>(ds[0], ds[1]);
+        dsa[jn >> 1][(jn & 1) * 2 + 1] = pack2<T>(ds[2], ds[3]);
+      }
+      wgmma_fence_regs(dq_acc);
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < BK / 16; ++ks)     // B = K tile read MN-major (N = head dim): 16 key rows = 2048 B per step
+        wgmma_rs_n128<BF16, 1>(dq_acc, dsa[ks], make_smem_desc(sK(s) + ks * 2048, SMALL_HALF, 1024), 1);   // dQ += dS K
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(dq_acc);
+      keep_regs(dsa);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(kv_empty(s));
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = m0 + rl + h * 8;
+      if (!row_ok[h]) continue;
+      float* dst = p.dq + (int64_t)batch * p.dq_sb + (int64_t)row * p.dq_ss + (int64_t)head * p.dq_sh;
+#pragma unroll
+      for (int jn = 0; jn < HD / 8; ++jn)
+        *reinterpret_cast<float2*>(dst + jn * 8 + 2 * q) = make_float2(dq_acc[jn * 4 + h * 2], dq_acc[jn * 4 + h * 2 + 1]);
+    }
   }
 }
 
@@ -363,13 +416,13 @@ static EncodeTiledFn get_encode() {
   }
   return fn;
 }
-static bool make_map4(CUtensorMap* out, const void* ptr, int d, int s, int h, int b, int64_t ss, int64_t sh, int64_t sb, int dtype) {
+static bool make_map4(CUtensorMap* out, const void* ptr, int d, int s, int h, int b, int64_t ss, int64_t sh, int64_t sb, uint32_t box_rows, int dtype) {
   bind_primary_context();
   EncodeTiledFn enc = get_encode();
   if (!enc) { set_last_error(__FILE__, __LINE__, "cuTensorMapEncodeTiled unavailable"); return false; }
   cuuint64_t dims[4] = {(cuuint64_t)d, (cuuint64_t)s, (cuuint64_t)h, (cuuint64_t)b};
   cuuint64_t strides[3] = {(cuuint64_t)ss * 2, (cuuint64_t)sh * 2, (cuuint64_t)sb * 2};
-  cuuint32_t box[4] = {64, 128, 1, 1};
+  cuuint32_t box[4] = {64, box_rows, 1, 1};
   cuuint32_t estr[4] = {1, 1, 1, 1};
   CUresult r = enc(out, dtype == kBF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(ptr),
                    dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -380,30 +433,23 @@ static bool make_map4(CUtensorMap* out, const void* ptr, int d, int s, int h, in
   }
   return true;
 }
-static uint32_t make_idesc(int dtype, bool a_mn, bool b_mn) {
-  uint32_t d = 0;
-  d |= 1u << 4;
-  const uint32_t f = dtype == kBF16 ? 1u : 0u;
-  d |= f << 7;
-  d |= f << 10;
-  d |= (a_mn ? 1u : 0u) << 15;
-  d |= (b_mn ? 1u : 0u) << 16;
-  d |= (uint32_t)(128 >> 3) << 17;
-  d |= (uint32_t)(128 >> 4) << 24;
-  return d;
-}
-
 }  // namespace attn_bwd
 
 int attention_bwd(const AttnBwdArgs& a, cudaStream_t s) {
   using namespace attn_bwd;
   if (!attention_fwd_supported(a.fwd)) return 1;
   const AttnArgs& f = a.fwd;
-  CUtensorMap mq, mk, mv, mdo;
-  if (!make_map4(&mq, f.q, f.d, f.sq, f.h, f.b, f.q_strides[1], f.q_strides[2], f.q_strides[0], f.dtype)) return 2;
-  if (!make_map4(&mk, f.k, f.d, f.sk, f.hk, f.b, f.k_strides[1], f.k_strides[2], f.k_strides[0], f.dtype)) return 2;
-  if (!make_map4(&mv, f.v, f.d, f.sk, f.hk, f.b, f.v_strides[1], f.v_strides[2], f.v_strides[0], f.dtype)) return 2;
-  if (!make_map4(&mdo, a.d_o, f.d, f.sq, f.h, f.b, a.o_strides[1], a.o_strides[2], a.o_strides[0], f.dtype)) return 2;
+  if (a.dq_strides[0] % 2 || a.dq_strides[1] % 2 || a.dq_strides[2] % 2 || (reinterpret_cast<uintptr_t>(a.dq) & 7)) return 1;   // float2 stores
+  if (a.dkv_strides[0] % 2 || a.dkv_strides[1] % 2 || a.dkv_strides[2] % 2) return 1;
+  // every operand as a 128-row box map (the resident tile of a kernel) and as a 64-row box map (the streamed tile of the other kernel)
+  CUtensorMap mq[2], mk[2], mv[2], mdo[2];
+  for (int i = 0; i < 2; ++i) {
+    const uint32_t rows = i ? 64 : 128;
+    if (!make_map4(&mq[i], f.q, f.d, f.sq, f.h, f.b, f.q_strides[1], f.q_strides[2], f.q_strides[0], rows, f.dtype)) return 2;
+    if (!make_map4(&mk[i], f.k, f.d, f.sk, f.hk, f.b, f.k_strides[1], f.k_strides[2], f.k_strides[0], rows, f.dtype)) return 2;
+    if (!make_map4(&mv[i], f.v, f.d, f.sk, f.hk, f.b, f.v_strides[1], f.v_strides[2], f.v_strides[0], rows, f.dtype)) return 2;
+    if (!make_map4(&mdo[i], a.d_o, f.d, f.sq, f.h, f.b, a.o_strides[1], a.o_strides[2], a.o_strides[0], rows, f.dtype)) return 2;
+  }
   const int64_t rows = (int64_t)f.b * f.sq * f.h;
   const int wpb = 8;
   if (f.dtype == kBF16)
@@ -417,21 +463,22 @@ int attention_bwd(const AttnBwdArgs& a, cudaStream_t s) {
   p.causal = f.causal; p.causal_off = f.sk - f.sq;
   p.colmask = reinterpret_cast<const int4*>(f.colmask);
   p.mask_heads = f.mask_heads > 0 ? f.mask_heads : 1;
-  p.dq_sem = a.dq_sem;
   p.lse = f.lse; p.delta = a.delta; p.dq = a.dq; p.dk = a.dk; p.dv = a.dv;
   p.dkv_sb = a.dkv_strides[0]; p.dkv_ss = a.dkv_strides[1]; p.dkv_sh = a.dkv_strides[2];
   p.dq_sb = a.dq_strides[0]; p.dq_ss = a.dq_strides[1]; p.dq_sh = a.dq_strides[2];
-  p.idesc_kk = make_idesc(f.dtype, false, false);
-  p.idesc_mm = make_idesc(f.dtype, true, true);
-  p.idesc_mk = make_idesc(f.dtype, true, false);
-  dim3 grid((f.sk + BN - 1) / BN, f.hk, f.b);
-  static bool attr_set[4] = {false, false, false, false};
-  auto go = [&](auto kern, int slot) {
+  const dim3 grid_kv((f.sk + 127) / 128, f.hk, f.b), grid_q((f.sq + 127) / 128, f.h, f.b);
+  static bool attr_set[8] = {false, false, false, false, false, false, false, false};
+  auto go = [&](auto kern, int slot, dim3 grid, int threads, const CUtensorMap& q, const CUtensorMap& k, const CUtensorMap& v, const CUtensorMap& d_o) {
     if (!attr_set[slot]) { B200_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES)); attr_set[slot] = true; }
-    kern<<<grid, kThreads, SMEM_BYTES, s>>>(mq, mk, mv, mdo, p);
+    kern<<<grid, threads, SMEM_BYTES, s>>>(q, k, v, d_o, p);
   };
-  if (f.dtype == kBF16) { if (p.colmask) go(bwd_kernel<__nv_bfloat16, true>, 0); else go(bwd_kernel<__nv_bfloat16, false>, 1); }
-  else { if (p.colmask) go(bwd_kernel<__half, true>, 2); else go(bwd_kernel<__half, false>, 3); }
+  if (f.dtype == kBF16) {
+    if (p.colmask) { go(dkv_kernel<__nv_bfloat16, true>, 0, grid_kv, kThreadsDkv, mq[1], mk[0], mv[0], mdo[1]); go(dq_kernel<__nv_bfloat16, true>, 1, grid_q, kThreads, mq[0], mk[1], mv[1], mdo[0]); }
+    else { go(dkv_kernel<__nv_bfloat16, false>, 2, grid_kv, kThreadsDkv, mq[1], mk[0], mv[0], mdo[1]); go(dq_kernel<__nv_bfloat16, false>, 3, grid_q, kThreads, mq[0], mk[1], mv[1], mdo[0]); }
+  } else {
+    if (p.colmask) { go(dkv_kernel<__half, true>, 4, grid_kv, kThreadsDkv, mq[1], mk[0], mv[0], mdo[1]); go(dq_kernel<__half, true>, 5, grid_q, kThreads, mq[0], mk[1], mv[1], mdo[0]); }
+    else { go(dkv_kernel<__half, false>, 6, grid_kv, kThreadsDkv, mq[1], mk[0], mv[0], mdo[1]); go(dq_kernel<__half, false>, 7, grid_q, kThreads, mq[0], mk[1], mv[1], mdo[0]); }
+  }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }
   return 0;

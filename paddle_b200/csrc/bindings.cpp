@@ -485,7 +485,7 @@ Tensor gemm_grouped(const Tensor& a, const Tensor& b, const Tensor& tile_expert,
   g.a_is_km = 0; g.b_is_nk = b_is_nk; g.epilogue = 0; g.dtype = dt_code(a); g.out_dtype = dt_code(d);
   g.stride_a = 0; g.stride_b = b.stride(0); g.stride_d = 0;
   g.grouped = 1; g.groups = (int)b.size(0); g.tile_expert = tile_expert.data_ptr<int>();
-  int rc = b200::gemm_tcgen05_2cta(g, cur_stream());
+  int rc = b200::gemm_tcgen05(g, cur_stream());
   g_launches += 1;
   check_err();
   TORCH_CHECK(rc == 0, "paddle_b200.gemm_grouped launch failed rc=", rc);
@@ -509,7 +509,7 @@ void gemm_grouped_wgrad(const Tensor& x, const Tensor& dy, const Tensor& expert_
   g.a_is_km = 1; g.b_is_nk = 0; g.epilogue = 4; g.dtype = dt_code(x); g.out_dtype = dt_code(out);
   g.stride_a = 0; g.stride_b = 0; g.stride_d = out.stride(0);
   g.grouped = 2; g.groups = (int)out.size(0); g.expert_k0 = expert_k0.data_ptr<int>(); g.expert_kb = expert_kb.data_ptr<int>();
-  int rc = b200::gemm_tcgen05_2cta(g, cur_stream());
+  int rc = b200::gemm_tcgen05(g, cur_stream());
   g_launches += 1;
   check_err();
   TORCH_CHECK(rc == 0, "paddle_b200.gemm_grouped_wgrad launch failed rc=", rc);
@@ -814,7 +814,7 @@ std::vector<Tensor> attention_fwd(const Tensor& q, const Tensor& k, const Tensor
   return {out, lse};
 }
 
-static bool g_deterministic = false;     // FLAGS_cudnn_deterministic: order-dependent reductions take a fixed order
+static bool g_deterministic = false;     // FLAGS_cudnn_deterministic (the attention backward is order-independent as it is)
 
 // backward of attention_fwd: returns (dq [B,Sq,H,D], dk, dv [B,Sk,Hk,D]) in the input dtype
 std::vector<Tensor> attention_bwd(const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& out, const Tensor& lse, const Tensor& d_out,
@@ -825,14 +825,12 @@ std::vector<Tensor> attention_bwd(const Tensor& q, const Tensor& k, const Tensor
   set_colmask(a.fwd, colmask);
   TORCH_CHECK(out.is_contiguous() && d_out.is_contiguous() && lse.is_contiguous() && lse.scalar_type() == at::kFloat, "attention_bwd: out / d_out / lse layout");
   a.fwd.o = out.data_ptr(); a.fwd.lse = lse.data_ptr<float>();
-  Tensor dq32 = torch::zeros({a.fwd.b, a.fwd.sq, a.fwd.h, a.fwd.d}, q.options().dtype(at::kFloat));
+  Tensor dq32 = torch::empty({a.fwd.b, a.fwd.sq, a.fwd.h, a.fwd.d}, q.options().dtype(at::kFloat));
   Tensor dk = torch::empty({a.fwd.b, a.fwd.sk, a.fwd.hk, a.fwd.d}, q.options());
   Tensor dv = torch::empty_like(dk);
   Tensor delta = torch::empty({a.fwd.b, a.fwd.h, a.fwd.sq}, q.options().dtype(at::kFloat));
   a.d_o = d_out.data_ptr(); a.delta = delta.data_ptr<float>(); a.dq = dq32.data_ptr<float>(); a.dk = dk.data_ptr(); a.dv = dv.data_ptr();
   for (int i = 0; i < 3; ++i) { a.dkv_strides[i] = dk.stride(i); a.o_strides[i] = out.stride(i); a.dq_strides[i] = dq32.stride(i); }
-  Tensor sem;
-  if (g_deterministic) { sem = torch::zeros({a.fwd.b, a.fwd.h, (a.fwd.sq + 127) / 128}, q.options().dtype(at::kInt)); a.dq_sem = sem.data_ptr<int>(); }
   int rc = b200::attention_bwd(a, cur_stream());
   g_launches += 2;
   check_err();
@@ -856,13 +854,11 @@ Tensor attention_bwd_packed(const Tensor& qkv, int64_t nh, int64_t nkv, const Te
   a.fwd.o = out.data_ptr(); a.fwd.lse = lse.data_ptr<float>();
   Tensor dqkv = torch::empty_like(qkv);
   Tensor dk = bs(dqkv.narrow(2, nh, nkv)), dv = bs(dqkv.narrow(2, nh + nkv, nkv));
-  Tensor dq32_mem = torch::zeros(out.sizes(), qkv.options().dtype(at::kFloat));     // same memory order as `out`
+  Tensor dq32_mem = torch::empty(out.sizes(), qkv.options().dtype(at::kFloat));     // same memory order as `out`
   Tensor dq32 = bs(dq32_mem);
   Tensor delta = torch::empty({a.fwd.b, a.fwd.h, a.fwd.sq}, qkv.options().dtype(at::kFloat));
   a.d_o = d_out.data_ptr(); a.delta = delta.data_ptr<float>(); a.dq = dq32_mem.data_ptr<float>(); a.dk = dk.data_ptr(); a.dv = dv.data_ptr();
   for (int i = 0; i < 3; ++i) { a.dkv_strides[i] = dk.stride(i); a.o_strides[i] = ov.stride(i); a.dq_strides[i] = dq32.stride(i); }
-  Tensor sem;
-  if (g_deterministic) { sem = torch::zeros({a.fwd.b, a.fwd.h, (a.fwd.sq + 127) / 128}, qkv.options().dtype(at::kInt)); a.dq_sem = sem.data_ptr<int>(); }
   int rc = b200::attention_bwd(a, cur_stream());
   g_launches += 2;
   check_err();

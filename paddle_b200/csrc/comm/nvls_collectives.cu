@@ -11,7 +11,7 @@
 // pointer, the local replica pointer and every rank's signal pad.  Cross-rank barriers are the epoch protocol of p2p_collectives.cu on
 // two words at the END of the signal pads (the front belongs to torch's own barrier channels).
 //
-// Status: compiled for sm_100a (SASS holds the multimem instructions); NOT yet run on hardware - opt-in behind FLAGS_b200_nvls.
+// Status: compiled for sm_90a (SASS holds the multimem instructions); NOT yet run on hardware - opt-in behind FLAGS_b200_nvls.
 // Parity (role): NCCL's NVLS algorithm under ProcessGroupNCCL::AllReduce (paddle/fluid/distributed/collective/process_group_nccl.cc).
 #include <cstdio>
 

@@ -414,8 +414,7 @@ void p2p_allreduce(const int64_t* bases, int64_t off, int64_t n, int dtype, int 
   Peers P = make_peers(bases, world);
   B200_DISPATCH_DTYPE(dtype, T, {
     constexpr int N = Vec16<T>::N;
-    // measured on 2 x B200 (6.5 GB slab): more peer loads in flight per thread (U = 4) was SLOWER (53.6 vs 29.3 ms) - the loop is bound by
-    // the posted remote stores, not by load latency - so every world size keeps one vector per thread and iteration
+    // one vector per thread and iteration at every world size: the loop is bound by the posted remote stores, not by load latency
     allreduce_kernel<T, 1><<<comm_grid(n / N / world + 1), kThreads, 0, s>>>(P, off, n, rank, world, epoch, counter);
   });
   B200_CUDA_CHECK(cudaGetLastError());

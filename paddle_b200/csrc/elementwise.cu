@@ -1,4 +1,4 @@
-// SwiGLU, rotary embedding, residual add for sm_100a (HBM-bound: 16-byte vector access, streaming hints).
+// SwiGLU, rotary embedding, residual add for sm_90a (HBM-bound: 16-byte vector access, streaming hints).
 // Parity (behaviour): python/paddle/incubate/nn/functional/swiglu.py, fused_rotary_position_embedding.py
 // (paddle/phi/kernels/fusion/gpu/fused_rope_kernel.cu).
 #include "include/b200_common.cuh"

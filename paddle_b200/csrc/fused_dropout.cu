@@ -1,4 +1,4 @@
-// Fused bias + dropout + residual-add and bias + activation for sm_100a (HBM-bound: one pass, 16-byte vectors, Philox per vector).
+// Fused bias + dropout + residual-add and bias + activation for sm_90a (HBM-bound: one pass, 16-byte vectors, Philox per vector).
 //
 // Parity (behaviour): python/paddle/incubate/nn/functional/fused_dropout_add.py (paddle/phi/kernels/fusion/gpu/fused_dropout_add_kernel.cu),
 // fused_bias_dropout_residual_layer_norm (the elementwise half; the LayerNorm half is csrc/norm.cu), fused_bias_act

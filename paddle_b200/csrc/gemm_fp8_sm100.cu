@@ -1,13 +1,13 @@
-// FP8 (E4M3 / E5M2) GEMM for sm_100a: same persistent warp-specialised structure as gemm_sm100.cu (TMA -> 128B-swizzled smem
-// ring -> tcgen05.mma -> TMEM double-buffered accumulators -> tcgen05.ld epilogue), with `kind::f8f6f4` MMAs (K = 32 per
-// instruction, 2x the bf16 rate), fp32 accumulation and a per-tensor dequantisation scale (+ bias / activation) fused in the
-// epilogue.  Both operands are K-major ("TN" GEMM): A [M,K], B [N,K], 1 byte per element.
+// FP8 (E4M3 / E5M2) GEMM for sm_90a: same persistent warp-specialised structure as gemm_sm100.cu (TMA -> 128B-swizzled smem ring ->
+// wgmma.mma_async from two consumer warpgroups -> register epilogue), with fp8 MMAs (K = 32 per instruction, 2x the bf16 rate), fp32
+// accumulation and a per-tensor dequantisation scale (+ bias / activation) fused in the epilogue.  Both operands are K-major ("TN"
+// GEMM): A [M,K], B [N,K], 1 byte per element.
 //
 // MX variant (`MX = true`, BN = 128): OCP microscaling - one E8M0 (power-of-two) scale per 32 consecutive K elements of every A row
-// and B row.  The scale bytes travel as 512-byte blocks (128 rows x 4 k-blocks, byte = (row % 32) * 16 + (row / 32) * 4 + k-block: the
-// layout tcgen05.cp.32x128b.warpx4 scatters into 4 TMEM columns of every lane quadrant), one bulk copy per operand and stage; the issuer
-// copies them smem -> TMEM in front of the stage's four `tcgen05.mma.kind::mxf8f6f4.block_scale` (the k-block is selected by the
-// a_sf_id / b_sf_id fields of the instruction descriptor), so dequantisation costs no epilogue work and no extra pass.
+// and B row.  The scale bytes travel as 512-byte blocks (128 rows x 4 k-blocks, byte = (row % 32) * 16 + (row / 32) * 4 + k-block), one
+// bulk copy per operand and stage.  Hopper's MMA has no block-scale input, so every 32-wide k-block is multiplied into a scratch
+// accumulator and added to the running one as acc += scratch * 2^sfa[row] * 2^sfb[col] in registers: exact (powers of two), one pass,
+// and the other warpgroup's MMAs run under this warpgroup's scaling.
 //
 // Parity (behaviour): fp8_fp8_half_gemm_fused (paddle/phi/kernels/fusion/fp8_gemm/fp8_gemm_with_cublasLt/*) which calls cuBLASLt.
 #include <cuda.h>
@@ -25,92 +25,70 @@ using namespace ptx;
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 128;  // 128 x 1B = 128B = one swizzle atom row
-constexpr int UMMA_K = 32;    // kind::f8f6f4: 32 elements (32 bytes) per MMA along K
+constexpr int MMA_K = 32;     // 32 fp8 elements (32 bytes) per MMA along K
 constexpr int kStages = 4;
-constexpr int kThreads = 256;
-constexpr int kAccStages = 2;
+constexpr int kThreads = 384; // producer warpgroup + two MMA warpgroups (64 rows each)
+constexpr int kConsumerWarps = 8;
 constexpr uint32_t A_STAGE_BYTES = BLOCK_M * BLOCK_K;      // 16 KB
 
 constexpr uint32_t SF_BLOCK_BYTES = 512;   // scale bytes of 128 rows x 128 k (4 blocks of 32)
 
 template <int BN, bool MX = false> struct Cfg {
   static constexpr uint32_t B_STAGE_BYTES = BN * BLOCK_K;
-  static constexpr uint32_t SF_BYTES = MX ? 2048u : 0u;          // [SFA 512 | SFB 512 per 128 columns] behind the operand tiles
-  static constexpr uint32_t SF_TX = MX ? SF_BLOCK_BYTES * (1 + BN / 128) : 0u;
+  static constexpr uint32_t SF_BYTES = MX ? 1024u : 0u;          // [SFA 512 | SFB 512] behind the operand tiles
+  static constexpr uint32_t SF_TX = MX ? 2 * SF_BLOCK_BYTES : 0u;
   static constexpr uint32_t STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES + SF_BYTES;
   static constexpr uint32_t TX_BYTES = A_STAGE_BYTES + B_STAGE_BYTES + SF_TX;
-  // MX at BN = 256 keeps ONE accumulator (256 columns) so that the scale columns fit: a 128-wide tile reads A and B from shared memory
-  // at 128 B/clk for full-rate fp8 MMAs - all the pipe has, before the TMA writes - and tops out at ~1.5 PFLOP/s; the 256-wide tile
-  // needs 96 B/clk and wins even without the epilogue overlap.
-  static constexpr int ACC = (MX && BN == 256) ? 1 : kAccStages;
-  static constexpr uint32_t SF_COL0 = ACC * BN;                  // MX: per smem stage 4 columns SFA + BN / 32 columns SFB after the accumulators
-  static constexpr uint32_t SF_STAGE_COLS = BN == 256 ? 16 : 8;
-  static constexpr uint32_t TMEM_COLS = MX ? 512u : kAccStages * BN;  // powers of two >= 32
   static constexpr uint32_t SMEM_BYTES = kStages * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
-  static_assert(!MX || ACC * BN + kStages * SF_STAGE_COLS <= 512, "MX: TMEM budget");
+  static_assert(BN == 128, "one 128-column scale block per stage; scratch + running accumulators of a wider tile would not fit in registers");
   static_assert(SMEM_BYTES <= 232448, "fp8 gemm: shared memory budget");
 };
-
-
-
-
-
-
 
 struct Params {
   int m, n, k, batch;
   void* d;
   const void* bias;
   int64_t ldd, stride_d;
-  int in_dtype, out_dtype;
-  int has_bias, act, accumulate;
+  int out_dtype;
+  int has_bias, act;
   float scale;
   const float* scale_a;   // optional device scalars (per-tensor dequantisation factors produced by quantize_fp8): no host round trip
   const float* scale_b;
   const uint8_t* sfa;     // MX: E8M0 scale blocks [m / 128][k / 128][512] of A, same for B over n
   const uint8_t* sfb;
-  uint32_t idesc;
 };
 
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
+__device__ __forceinline__ float e8m0(uint32_t byte) { return __uint_as_float(byte << 23); }   // 2^(byte - 127)
+__device__ __forceinline__ uint32_t ld_shared_u8(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(addr));
+  return v;
+}
 
 template <typename TO>
-__device__ __forceinline__ void store_row_chunk(TO* __restrict__ dst, const float (&v)[32], int valid, bool accumulate) {
-  if (valid >= 32 && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
-    constexpr int N = Vec16<TO>::N;
-#pragma unroll
-    for (int q = 0; q < 32 / N; ++q) {
-      Vec16<TO> o;
-      if (accumulate) {
-        Vec16<TO> old = ld16(dst + q * N);
-#pragma unroll
-        for (int j = 0; j < N; ++j) o.v[j] = from_f<TO>(v[q * N + j] + to_f(old.v[j]));
-      } else {
-#pragma unroll
-        for (int j = 0; j < N; ++j) o.v[j] = from_f<TO>(v[q * N + j]);
-      }
-      st16(dst + q * N, o);
-    }
+__device__ __forceinline__ void store_pair(TO* __restrict__ dst, float v0, float v1, int valid) {
+  if (valid >= 2 && (reinterpret_cast<uintptr_t>(dst) & (2 * sizeof(TO) - 1)) == 0) {
+    struct alignas(2 * sizeof(TO)) Pair { TO a, b; };
+    Pair o;
+    o.a = from_f<TO>(v0);
+    o.b = from_f<TO>(v1);
+    *reinterpret_cast<Pair*>(dst) = o;
   } else {
-#pragma unroll
-    for (int j = 0; j < 32; ++j)
-      if (j < valid) dst[j] = from_f<TO>(accumulate ? v[j] + to_f(dst[j]) : v[j]);
+    if (valid >= 1) dst[0] = from_f<TO>(v0);
+    if (valid >= 2) dst[1] = from_f<TO>(v1);
   }
 }
 
-template <int BN, bool MX>
+template <int BN, bool A5, bool B5, bool MX>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const Params p) {
   using C = Cfg<BN, MX>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;  // SWIZZLE_128B needs 1024B alignment
-  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
   const uint32_t bar_base = smem_base + kStages * C::STAGE_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (kStages + s); };
-  auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * kStages + s); };
-  auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * kStages + kAccStages + s); };
-  volatile uint32_t* tmem_ptr_smem = reinterpret_cast<volatile uint32_t*>(smem_gen + kStages * C::STAGE_BYTES + 8 * (2 * kStages + 2 * kAccStages));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_m = (p.m + BLOCK_M - 1) / BLOCK_M, num_n = (p.n + BN - 1) / BN;
@@ -121,18 +99,11 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&map_a);
     tma_prefetch_desc(&map_b);
-    for (int s = 0; s < kStages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-    for (int s = 0; s < kAccStages; ++s) { mbar_init(tfull_bar(s), 1); mbar_init(tempty_bar(s), 4); }
+    for (int s = 0; s < kStages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kConsumerWarps); }
     fence_barrier_init();
     fence_proxy_async();
-  } else if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32((const void*)tmem_ptr_smem)), "r"(C::TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
   // tile order: groups of 8 M-tiles sweep N (operand panels stay L2-resident across the wave)
   auto tile_coords = [&](int tile, int& bz, int& mb, int& nb) {
@@ -148,8 +119,9 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant
     nb = r / gsz;
   };
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    reg_dealloc<56>();
+    if (warp == 0 && lane == 0) {
       // ================= TMA producer =================
       int stage = 0;
       uint32_t phase = 0;
@@ -168,122 +140,119 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant
           tma_load_3d(sb, &map_b, full_bar(stage), k0, n0, bz, hint);  // box {128 k bytes, BN n}
           if constexpr (MX) {
             bulk_load(sb + C::B_STAGE_BYTES, p.sfa + ((int64_t)mb * num_kb + kb) * SF_BLOCK_BYTES, SF_BLOCK_BYTES, full_bar(stage));
-#pragma unroll
-            for (int h = 0; h < BN / 128; ++h)
-              bulk_load(sb + C::B_STAGE_BYTES + (1 + h) * SF_BLOCK_BYTES, p.sfb + ((int64_t)(nb * (BN / 128) + h) * num_kb + kb) * SF_BLOCK_BYTES, SF_BLOCK_BYTES, full_bar(stage));
+            bulk_load(sb + C::B_STAGE_BYTES + SF_BLOCK_BYTES, p.sfb + ((int64_t)nb * num_kb + kb) * SF_BLOCK_BYTES, SF_BLOCK_BYTES, full_bar(stage));
           }
           if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ================= MMA issuer =================
-      int stage = 0;
-      uint32_t phase = 0;
-      int local = 0;
-      const uint64_t desc_a0 = make_smem_desc(smem_base, 16, 1024), desc_b0 = make_smem_desc(smem_base + A_STAGE_BYTES, 16, 1024);
-      const uint64_t desc_sf0 = make_sf_desc(smem_base + A_STAGE_BYTES + C::B_STAGE_BYTES);
-      (void)desc_sf0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++local) {
-        const int as = local % C::ACC;
-        const uint32_t aphase = (local / C::ACC) & 1;
-        mbar_wait(tempty_bar(as), aphase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + as * BN;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
-          // descriptors are built once (desc_a0 / desc_b0 / desc_sf0 below the loop head) and advanced by adding to the address field
-          const uint64_t soff = (uint64_t)((stage * C::STAGE_BYTES) >> 4);
-          uint32_t tsfa = 0, tsfb = 0;
-          if constexpr (MX) {      // scale bytes smem -> TMEM; tcgen05.cp and tcgen05.mma execute in issue order
-            tsfa = tmem_base + C::SF_COL0 + stage * C::SF_STAGE_COLS;
-            tsfb = tsfa + 4;
-            tmem_cp_sf(tsfa, desc_sf0 + soff);
-#pragma unroll
-            for (int h = 0; h < BN / 128; ++h) tmem_cp_sf(tsfb + 4 * h, desc_sf0 + soff + (uint64_t)(((1 + h) * SF_BLOCK_BYTES) >> 4));
-          }
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-            const uint64_t adesc = desc_a0 + soff + 2 * k, bdesc = desc_b0 + soff + 2 * k;   // K-major: 32 fp8 elements = 32 B per step
-            if constexpr (MX) umma_mxf8(tmem_d, adesc, bdesc, p.idesc | ((uint32_t)k << 29) | ((uint32_t)k << 4), tsfa, tsfb, (kb | k) != 0);   // a_sf_id, b_sf_id = k-block
-            else umma_f8(tmem_d, adesc, bdesc, p.idesc, (kb | k) != 0);
-          }
-          umma_commit(empty_bar(stage));  // frees the smem slot once these MMAs retire
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(tfull_bar(as));      // accumulator complete -> epilogue
-      }
-    }
-  } else if (warp >= 4) {
-    // ================= epilogue =================
-    const int ew = warp - 4;  // TMEM lane quadrant (warp id % 4)
-    int local = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++local) {
+  } else {
+    // ================= MMA + epilogue: warpgroup wg owns rows [64 wg, 64 wg + 64) of the tile =================
+    reg_alloc<224>();
+    const int wg = (warp >> 2) - 1, ww = warp & 3;
+    const int rl = wg * 64 + ww * 16 + (lane >> 2);     // first of this thread's two tile rows (the other is rl + 8)
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[BN / 2];
+    const float dq = p.scale * (p.scale_a ? *p.scale_a : 1.f) * (p.scale_b ? *p.scale_b : 1.f);
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       int bz, mb, nb;
       tile_coords(tile, bz, mb, nb);
-      const int as = local % C::ACC;
-      const uint32_t aphase = (local / C::ACC) & 1;
-      mbar_wait(tfull_bar(as), aphase);
-      tc_fence_after();
-      const int row = mb * BLOCK_M + ew * 32 + lane;
-      const bool row_ok = row < p.m;
-      const float dq = p.scale * (p.scale_a ? *p.scale_a : 1.f) * (p.scale_b ? *p.scale_b : 1.f);
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      if constexpr (!MX) {
+        // The tensor core keeps fewer mantissa bits than fp32 while it accumulates fp8 products, which shows after a few thousand k:
+        // every 128-wide k-block is summed by the MMA into a scratch fragment and added to the running sum in fp32 registers.
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(full_bar(stage), phase);
+          const uint32_t sa = smem_base + stage * C::STAGE_BYTES + wg * 8192, sb = smem_base + stage * C::STAGE_BYTES + A_STAGE_BYTES;
+          float t[BN / 2];
+          wgmma_fence_regs(t);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < BLOCK_K / MMA_K; ++k)      // K-major: 32 fp8 elements = 32 B per step inside the swizzle row
+            wgmma_f8_n128<A5, B5>(t, make_smem_desc(sa + k * 32, 16, 1024), make_smem_desc(sb + k * 32, 16, 1024), k != 0);
+          wgmma_commit();
+          wgmma_wait<0>();
+          wgmma_fence_regs(t);
+          __syncwarp();
+          if (lane == 0) mbar_arrive(empty_bar(stage));
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) acc[i] += t[i];
+          if (++stage == kStages) { stage = 0; phase ^= 1; }
+        }
+      } else {
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(full_bar(stage), phase);
+          const uint32_t sa = smem_base + stage * C::STAGE_BYTES + wg * 8192, sb = smem_base + stage * C::STAGE_BYTES + A_STAGE_BYTES;
+          const uint32_t sfa = sb + C::B_STAGE_BYTES, sfb = sfa + SF_BLOCK_BYTES;
 #pragma unroll 1
-      for (int c = 0; c < BN / 32; ++c) {
-        const int col0 = nb * BN + c * 32;
-        if (col0 >= p.n) break;  // warp-uniform
-        uint32_t r[32];
-        tmem_ld_32x32(tmem_base + ((uint32_t)(ew * 32) << 16) + as * BN + c * 32, r);
-        tmem_ld_wait();
-        float v[32];
+          for (int k = 0; k < BLOCK_K / MMA_K; ++k) {
+            float t[BN / 2];
+            wgmma_fence_regs(t);
+            wgmma_fence();
+            wgmma_f8_n128<A5, B5>(t, make_smem_desc(sa + k * 32, 16, 1024), make_smem_desc(sb + k * 32, 16, 1024), 0);
+            wgmma_commit();
+            // this thread's two row scales and, per 8-column group, two column scales of k-block k
+            const float ra0 = e8m0(ld_shared_u8(sfa + (rl & 31) * 16 + (rl >> 5) * 4 + k));
+            const float ra1 = e8m0(ld_shared_u8(sfa + ((rl + 8) & 31) * 16 + ((rl + 8) >> 5) * 4 + k));
+            wgmma_wait<0>();
+            wgmma_fence_regs(t);
 #pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-        const int valid = min(32, p.n - col0);
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] *= dq;           // per-tensor dequantisation scale (scale_a * scale_b)
-        if (p.has_bias) {
-          if (p.out_dtype == kBF16) {
-            const __nv_bfloat16* b = (const __nv_bfloat16*)p.bias + col0;
-#pragma unroll
-            for (int j = 0; j < 32; ++j) if (j < valid) v[j] += __bfloat162float(b[j]);
-          } else if (p.out_dtype == kF16) {
-            const __half* b = (const __half*)p.bias + col0;
-#pragma unroll
-            for (int j = 0; j < 32; ++j) if (j < valid) v[j] += __half2float(b[j]);
-          } else {
-            const float* b = (const float*)p.bias + col0;
-#pragma unroll
-            for (int j = 0; j < 32; ++j) if (j < valid) v[j] += b[j];
+            for (int j = 0; j < BN / 8; ++j) {
+              const int c = j * 8 + (lane & 3) * 2;
+              const float cb0 = e8m0(ld_shared_u8(sfb + (c & 31) * 16 + (c >> 5) * 4 + k));
+              const float cb1 = e8m0(ld_shared_u8(sfb + ((c + 1) & 31) * 16 + ((c + 1) >> 5) * 4 + k));
+              acc[j * 4 + 0] = fmaf(t[j * 4 + 0], ra0 * cb0, acc[j * 4 + 0]);
+              acc[j * 4 + 1] = fmaf(t[j * 4 + 1], ra0 * cb1, acc[j * 4 + 1]);
+              acc[j * 4 + 2] = fmaf(t[j * 4 + 2], ra1 * cb0, acc[j * 4 + 2]);
+              acc[j * 4 + 3] = fmaf(t[j * 4 + 3], ra1 * cb1, acc[j * 4 + 3]);
+            }
           }
-        }
-        if (p.act == 1) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = gelu_erf(v[j]);
-        } else if (p.act == 2) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-        }
-        if (row_ok) {
-          void* dptr = p.d;
-          int64_t off = (int64_t)bz * p.stride_d + (int64_t)row * p.ldd + col0;
-          if (p.out_dtype == kBF16) store_row_chunk((__nv_bfloat16*)dptr + off, v, valid, p.accumulate);
-          else if (p.out_dtype == kF16) store_row_chunk((__half*)dptr + off, v, valid, p.accumulate);
-          else store_row_chunk((float*)dptr + off, v, valid, p.accumulate);
+          __syncwarp();
+          if (lane == 0) mbar_arrive(empty_bar(stage));
+          if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(as));
-    }
-  }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(C::TMEM_COLS) : "memory");
+      // ---- epilogue from the accumulator fragment ----
+      const int r0 = mb * BLOCK_M + rl;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = nb * BN + j * 8 + (lane & 3) * 2;
+        const int valid = p.n - col;
+        if (valid <= 0) continue;
+        float b0 = 0.f, b1 = 0.f;
+        if (p.has_bias) {
+          if (p.out_dtype == kBF16) {
+            const __nv_bfloat16* b = (const __nv_bfloat16*)p.bias + col;
+            b0 = __bfloat162float(b[0]);
+            if (valid > 1) b1 = __bfloat162float(b[1]);
+          } else if (p.out_dtype == kF16) {
+            const __half* b = (const __half*)p.bias + col;
+            b0 = __half2float(b[0]);
+            if (valid > 1) b1 = __half2float(b[1]);
+          } else {
+            const float* b = (const float*)p.bias + col;
+            b0 = b[0];
+            if (valid > 1) b1 = b[1];
+          }
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = r0 + h * 8;
+          float v0 = acc[j * 4 + h * 2] * dq + b0, v1 = acc[j * 4 + h * 2 + 1] * dq + b1;   // per-tensor dequantisation scale (scale_a * scale_b)
+          if (p.act == 1) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
+          else if (p.act == 2) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+          if (row < p.m) {
+            const int64_t off = (int64_t)bz * p.stride_d + (int64_t)row * p.ldd + col;
+            if (p.out_dtype == kBF16) store_pair((__nv_bfloat16*)p.d + off, v0, v1, valid);
+            else if (p.out_dtype == kF16) store_pair((__half*)p.d + off, v0, v1, valid);
+            else store_pair((float*)p.d + off, v0, v1, valid);
+          }
+        }
+      }
+    }
   }
 }
 
@@ -318,29 +287,7 @@ static bool make_map8(CUtensorMap* out, const void* ptr, uint64_t k, uint64_t ro
   }
   return true;
 }
-static uint32_t make_idesc(int a_e5m2, int b_e5m2, int bn) {
-  uint32_t d = 0;
-  d |= 1u << 4;                                   // c_format = F32
-  d |= (a_e5m2 ? 1u : 0u) << 7;                   // a_format: E4M3 = 0, E5M2 = 1
-  d |= (b_e5m2 ? 1u : 0u) << 10;                  // b_format
-  d |= (uint32_t)(bn >> 3) << 17;                 // n_dim
-  d |= (uint32_t)(BLOCK_M >> 4) << 24;            // m_dim
-  return d;
-}
-
-// block-scaled descriptor (cute::UMMA::InstrDescriptorBlockScaled): no c_format (always fp32); bits [4,6) b_sf_id, 23 scale format
-// (1 = E8M0), [29,31) a_sf_id - the two ids are OR-ed in per MMA
-static uint32_t make_idesc_mx(int a_e5m2, int b_e5m2, int bn) {
-  uint32_t d = 0;
-  d |= (a_e5m2 ? 1u : 0u) << 7;
-  d |= (b_e5m2 ? 1u : 0u) << 10;
-  d |= (uint32_t)(bn >> 3) << 17;
-  d |= 1u << 23;
-  d |= (uint32_t)(BLOCK_M >> 4) << 24;
-  return d;
-}
-
-template <int BN, bool MX>
+template <int BN, bool A5, bool B5, bool MX>
 static int launch(const GemmFp8Args& g, cudaStream_t s) {
   using C = Cfg<BN, MX>;
   CUtensorMap ma, mb;
@@ -350,16 +297,14 @@ static int launch(const GemmFp8Args& g, cudaStream_t s) {
   Params p;
   p.m = g.m; p.n = g.n; p.k = g.k; p.batch = (int)batch;
   p.d = g.d; p.bias = g.bias; p.ldd = g.ldd; p.stride_d = g.stride_d;
-  p.in_dtype = 0; p.out_dtype = g.out_dtype;
+  p.out_dtype = g.out_dtype;
   p.has_bias = g.bias ? 1 : 0;
   p.act = g.act;
-  p.accumulate = 0;
   p.scale = g.scale;
   p.scale_a = g.scale_a_dev; p.scale_b = g.scale_b_dev;
   p.sfa = g.sfa; p.sfb = g.sfb;
-  p.idesc = MX ? make_idesc_mx(g.a_e5m2, g.b_e5m2, BN) : make_idesc(g.a_e5m2, g.b_e5m2, BN);
   static bool attr_set = false;
-  auto kern = gemm_fp8_kernel<BN, MX>;
+  auto kern = gemm_fp8_kernel<BN, A5, B5, MX>;
   if (!attr_set) {
     B200_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
     attr_set = true;
@@ -372,6 +317,12 @@ static int launch(const GemmFp8Args& g, cudaStream_t s) {
   return 0;
 }
 
+template <int BN, bool MX>
+static int launch_types(const GemmFp8Args& g, cudaStream_t s) {
+  if (g.a_e5m2) return g.b_e5m2 ? launch<BN, true, true, MX>(g, s) : launch<BN, true, false, MX>(g, s);
+  return g.b_e5m2 ? launch<BN, false, true, MX>(g, s) : launch<BN, false, false, MX>(g, s);
+}
+
 }  // namespace gemm8
 
 int gemm_fp8_tcgen05(const GemmFp8Args& g, cudaStream_t s) {
@@ -381,10 +332,9 @@ int gemm_fp8_tcgen05(const GemmFp8Args& g, cudaStream_t s) {
     // MX: whole 128 x 128 x 128 scale blocks only
     if (!g.sfa || !g.sfb || g.m % 128 || g.n % 128 || g.k % 128 || g.batch > 1) return 1;
     if ((reinterpret_cast<uintptr_t>(g.sfa) | reinterpret_cast<uintptr_t>(g.sfb)) & 15) return 1;
-    return g.n % 256 == 0 ? gemm8::launch<256, true>(g, s) : gemm8::launch<128, true>(g, s);
+    return gemm8::launch_types<128, true>(g, s);
   }
-  if (g.n <= 128) return gemm8::launch<128, false>(g, s);
-  return gemm8::launch<256, false>(g, s);
+  return gemm8::launch_types<128, false>(g, s);
 }
 
 }  // namespace b200

@@ -1,14 +1,12 @@
-// Weight-only quantised GEMM for sm_100a: out[M,N] = x[M,K] (bf16 / fp16) @ dequant(Wq[N,K] int8 | int4) * scale[N] (+ bias), M <= 64.
+// Weight-only quantised GEMM for sm_90a: out[M,N] = x[M,K] (bf16 / fp16) @ dequant(Wq[N,K] int8 | int4) * scale[N] (+ bias), M <= 64.
 //
 // The int8 / int4 weights never exist as 16-bit values in HBM or in shared memory: TMA streams raw [128 channels x 128 B] boxes into a
-// deep ring, sixteen dequantise warps expand them IN REGISTERS with packed 16-bit magic-number arithmetic and store them straight into
-// TMEM (tcgen05.st), and tcgen05.mma reads its A operand from there.  The problem is computed transposed (D^T[N, M] = W[N, K] x^T) so
-// that the weight tile is the 128-row A operand at full UMMA height even when M is a handful of decode tokens, the per-channel scale is
-// a per-thread scalar in the epilogue (TMEM lane = output channel), and the token tile (UMMA N = 16 / 64) only costs what the batch
-// needs.  Narrow layers are split along K over a thread-block CLUSTER whose CTAs reduce their partial tiles through DSMEM - no
-// workspace, no atomics, no second kernel.  What each design step bought (k = 5120, n = 15360, m = 1, B200, profiles/
-// bench_weight_only_r2.json and ncu_weight_only_r2.md): 64-byte boxes + one issuer + smem operand 43 us; four issuers 30 us; weight
-// producer no longer throttled by the activation ring 23 us (cuBLAS bf16 on the 2x larger weight: 25 us).
+// ring, the two MMA warpgroups expand them IN REGISTERS straight into the A-operand fragment layout of wgmma (A from registers, B =
+// the activation tile in shared memory).  The problem is computed transposed (D^T[N, M] = W[N, K] x^T) so that the weight tile is the
+// 64-row A operand of each warpgroup even when M is a handful of decode tokens, the per-channel scale is a per-thread scalar in the
+// epilogue (accumulator row = output channel), and the token tile (MMA N = 16 / 64) only costs what the batch needs.  Narrow layers
+// are split along K over a thread-block CLUSTER whose CTAs reduce their partial tiles through DSMEM - no workspace, no atomics, no
+// second kernel.
 //
 // Parity: paddle/phi/kernels/gpu/weight_only_linear_kernel.cu:27, python/paddle/nn/quant/quantized_linear.py:183.
 #include <cuda.h>
@@ -27,11 +25,10 @@ bool make_map(CUtensorMap* out, const void* ptr, uint64_t inner, uint64_t rows, 
 namespace wo {
 using namespace ptx;
 
-constexpr int BLOCK_N = 128;     // output channels per CTA = UMMA M (TMEM lanes)
+constexpr int BLOCK_N = 128;     // output channels per CTA: 64 per MMA warpgroup
 constexpr int BLOCK_K = 64;
-__host__ __device__ constexpr int wo_threads(int G) { return 32 * (4 + 4 * G + (G > 3 ? G - 3 : 0)); }   // producer, 3 issuers, 4G dequantise, issuers 3 ..
-__host__ __device__ constexpr uint32_t pow2_at_least(uint32_t v) { uint32_t r = 32; while (r < v) r *= 2; return r; }
-
+constexpr int kThreads = 288;    // warps 0-7: two MMA warpgroups (dequantise + wgmma + epilogue), warp 8: TMA producer
+constexpr uint32_t W_BYTES = BLOCK_N * 128;   // 16 KB raw box
 
 struct Params {
   int m, n, k;                 // tokens, output channels, reduction
@@ -40,64 +37,55 @@ struct Params {
   const void* bias;            // [n] in the activation dtype or nullptr
   void* out;                   // [m, n] activation dtype (splits == 1)
   int splits;                  // blockIdx.y extent = cluster size: the CTAs of one output tile
-  int bf16;                    // activation dtype: 1 bf16, 0 fp16
-  uint32_t idesc;
 };
 
-// PTX prmt in its default mode: selector nibble bit 3 replicates the sign bit of the selected byte (the __byte_perm intrinsic only documents 3 bits)
-__device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t b, uint32_t sel) {
-  uint32_t d;
-  asm("prmt.b32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(sel));
-  return d;
+template <bool BF16> __device__ __forceinline__ uint32_t pack2(float a, float b) {
+  if constexpr (BF16) {
+    const __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
+    return *reinterpret_cast<const uint32_t*>(&v);
+  } else {
+    const __half2 v = __floats2half2_rn(a, b);
+    return *reinterpret_cast<const uint32_t*>(&v);
+  }
 }
-__device__ __forceinline__ __half2 u32_as_half2(uint32_t v) { return *reinterpret_cast<__half2*>(&v); }
-__device__ __forceinline__ uint32_t half2_as_u32(__half2 v) { return *reinterpret_cast<uint32_t*>(&v); }
-__device__ __forceinline__ __nv_bfloat162 u32_as_bf162(uint32_t v) { return *reinterpret_cast<__nv_bfloat162*>(&v); }
-__device__ __forceinline__ uint32_t bf162_as_u32(__nv_bfloat162 v) { return *reinterpret_cast<uint32_t*>(&v); }
+__device__ __forceinline__ uint32_t ld_shared_u16(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.u16 %0, [%1];" : "=r"(v) : "r"(addr));
+  return v;
+}
+__device__ __forceinline__ uint32_t ld_shared_u8(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(addr));
+  return v;
+}
+// two consecutive k of one channel -> one packed 16-bit pair in the activation dtype (|value| <= 128: exact in bf16 and fp16)
+template <bool INT4, bool BF16> __device__ __forceinline__ uint32_t dequant_pair(uint32_t raw) {
+  if constexpr (INT4) return pack2<BF16>((float)((int)((raw & 0xFu) ^ 8u) - 8), (float)((int)(((raw >> 4) & 0xFu) ^ 8u) - 8));   // low nibble = even k
+  else return pack2<BF16>((float)(int8_t)(raw & 0xFFu), (float)(int8_t)((raw >> 8) & 0xFFu));
+}
+__device__ __forceinline__ void keep_regs(uint32_t (&a)[4]) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(a[i])::"memory");
+}
 
-// NTOK: token tile (UMMA N).  INT4: two weights per byte (low nibble = even k).
+// NTOK: token tile (MMA N).  INT4: two weights per byte (low nibble = even k).
 //
-// Data path of one 64-wide k-block:  TMA raw box (128 channels x 128 B, shared by 2 int8 / 4 int4 k-blocks) -> one thread per channel
-// row reads its 64 (32) bytes, expands them to 64 bf16 / fp16 in registers and stores them with tcgen05.st into the TMEM rows the tensor
-// core reads its A operand from (tcgen05.mma with A in TMEM) -> D^T[128 channels, NTOK tokens] += A x_tile^T.  The dequantised weights
-// never touch shared memory: the first version wrote them to a swizzled smem tile and the MMA read them back, and that round trip
-// (16 KB written + 16 KB read per k-block on top of the raw bytes) saturated the 128 B/clk shared-memory pipe at ~600 cycles per k-block.
-//
-// Warp roles for G ring slots: warp 0 TMA producer; warps 1-3 and 4+4G .. issuers 0 .. G-1 (warp 1 also owns the TMEM allocation);
-// warps 4 .. 4+4G-1 dequantise, four per group = one per TMEM lane quadrant (a warp may only touch lanes 32 (warp % 4) ..).  Group g
-// converts k-blocks g, g + G, ... into TMEM slot g and issuer g multiplies them: the MMAs are tiny (NTOK columns), a k-block costs what
-// its ISSUE sequence costs (~800 cycles for one thread), so every slot has its own issuer and the chains of G k-blocks overlap.
-template <int NTOK, int G, int WST, int XPER, bool INT4, bool BF16>
-__global__ void __launch_bounds__(wo_threads(G), 1)
+// Data path of one 64-wide k-block:  TMA raw box (128 channels x 128 B, shared by 2 int8 / 4 int4 k-blocks) + the activation tiles of
+// those k-blocks in one ring stage -> every MMA thread reads exactly the bytes of its own A-fragment elements (rows lane / 4 and + 8 of
+// its warp's 16 channels, k = 2 (lane % 4) .. + 1 and + 8 of each 16-wide step), converts them and issues wgmma with A in registers ->
+// D^T[64 channels, NTOK tokens] += A x_tile^T.  The dequantised weights never touch shared memory.
+template <int NTOK, int WST, bool INT4, bool BF16>
+__global__ void __launch_bounds__(kThreads, 1)
 wo_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_x, const Params p) {
   constexpr int KB_PER_W = INT4 ? 4 : 2;                        // k-blocks covered by one raw box
-  constexpr uint32_t W_BYTES = BLOCK_N * 128;                   // 16 KB raw box
   constexpr uint32_t X_BYTES = NTOK * BLOCK_K * 2;
-  constexpr int ACC_PER = NTOK <= 16 ? 2 : 1;                   // independent TMEM accumulators per issuer (summed in the epilogue)
-  constexpr int NACC = G * ACC_PER;
-  constexpr uint32_t A_COLS = BLOCK_K / 2;                      // one slot: 128 lanes x 32 columns, two 16-bit k values per column
-  constexpr uint32_t A_COL0 = NACC * NTOK;                      // accumulators first, then the G operand slots
-  constexpr uint32_t TMEM_COLS = pow2_at_least(A_COL0 + G * A_COLS);
-  static_assert(TMEM_COLS <= 512, "weight-only gemm: TMEM budget");
-  static_assert(NTOK * 512 <= WST * W_BYTES, "weight-only gemm: the split-K partial tile is staged in the raw weight ring");
-  // Activation tiles: XPER private stages per issuer (k-block i -> stage (i % G) * XPER + (i / G) % XPER), so every x_full barrier has ONE
-  // waiter that sees its phases in order.  (A ring shared by all issuers lets one issuer run a whole phase ahead of another and read
-  // the parity of the previous phase as "done".)
-  constexpr int XST = G * XPER;
+  constexpr uint32_t STAGE_BYTES = W_BYTES + KB_PER_W * X_BYTES;
+  static_assert(NTOK * 512 <= WST * STAGE_BYTES, "weight-only gemm: the split-K partial tile is staged in the ring");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* gen = smem_raw + (base - smem_u32(smem_raw));
-  const uint32_t wring = base;                                  // [WST] raw weight boxes
-  const uint32_t xring = wring + WST * W_BYTES;                 // [XST] activation tiles
-  const uint32_t bars = xring + XST * X_BYTES;
-  auto w_full = [&](int s) { return bars + 8u * s; };
-  auto w_empty = [&](int s) { return bars + 8u * (WST + s); };
-  auto x_full = [&](int s) { return bars + 8u * (2 * WST + s); };
-  auto x_empty = [&](int s) { return bars + 8u * (2 * WST + XST + s); };
-  auto a_ready = [&](int s) { return bars + 8u * (2 * WST + 2 * XST + s); };
-  auto a_empty = [&](int s) { return bars + 8u * (2 * WST + 2 * XST + G + s); };
-  const uint32_t tfull = bars + 8u * (2 * WST + 2 * XST + 2 * G);
-  volatile uint32_t* tmem_ptr = reinterpret_cast<volatile uint32_t*>(gen + WST * W_BYTES + XST * X_BYTES + 8 * (2 * WST + 2 * XST + 2 * G + 1));
+  const uint32_t bars = base + WST * STAGE_BYTES;
+  auto full = [&](int s) { return bars + 8u * s; };
+  auto empty = [&](int s) { return bars + 8u * (WST + s); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n0 = blockIdx.x * BLOCK_N;
@@ -105,199 +93,115 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
   const int num_kb_total = (p.k + BLOCK_K - 1) / BLOCK_K;
   const int kb0 = blockIdx.y * p.kb_per_split;
   const int num_kb = max(0, min(p.kb_per_split, num_kb_total - kb0));
+  const int num_box = (num_kb + KB_PER_W - 1) / KB_PER_W;    // kb0 is a multiple of KB_PER_W (launcher), so boxes start on 128-byte columns
 
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_x) : "memory");
-    for (int s = 0; s < WST; ++s) { mbar_init(w_full(s), 1); mbar_init(w_empty(s), KB_PER_W * 4); }
-    for (int s = 0; s < XST; ++s) { mbar_init(x_full(s), 1); mbar_init(x_empty(s), 1); }
-    for (int s = 0; s < G; ++s) { mbar_init(a_ready(s), 4); mbar_init(a_empty(s), 1); }
-    mbar_init(tfull, G);
+  if (warp == 8 && lane == 0) {
+    tma_prefetch_desc(&map_w);
+    tma_prefetch_desc(&map_x);
+    for (int s = 0; s < WST; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 8); }
     fence_barrier_init();
     fence_proxy_async();
-  } else if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32((const void*)tmem_ptr)), "r"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  const bool is_dq = warp >= 4 && warp < 4 + 4 * G;
-  const int ew = warp & 3;                                  // TMEM lane quadrant this warp may access (hardware: warp id % 4)
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
-      // ================= TMA producer: raw quantised weights, one box per KB_PER_W k-blocks, throttled only by the box ring.  (The
-      // activation tiles are loaded by the issuers: on this thread their small ring capped the weight bytes in flight.) =================
-      const int num_box = (num_kb + KB_PER_W - 1) / KB_PER_W;
-      for (int j = 0; j < num_box; ++j) {                   // kb0 is a multiple of KB_PER_W (launcher), so boxes start on 128-byte columns
-        const int ws = j % WST;
-        mbar_wait(w_empty(ws), ((j / WST) & 1) ^ 1);
-        mbar_expect_tx(w_full(ws), W_BYTES);
-        tma_load_2d(wring + ws * W_BYTES, &map_w, w_full(ws), (kb0 + j * KB_PER_W) * (INT4 ? BLOCK_K / 2 : BLOCK_K), n0);
-      }
-    }
-  } else if (!is_dq) {
-    if (lane == 0) {
-      // ================= MMA issuers: D^T[128 channels, NTOK tokens] += A(TMEM slot g)[128, 64] x_tile[NTOK, 64]^T =================
-      const int g = warp < 4 ? warp - 1 : warp - (4 + 4 * G) + 3;
-      if (g < G) {
-        const uint64_t bdesc0 = make_smem_desc(xring, 16, 1024);
-        const uint32_t tacc = tmem_base + (uint32_t)(g * ACC_PER * NTOK), ta = tmem_base + A_COL0 + (uint32_t)g * A_COLS;
-        int aph = 0;
-        // issuer g also streams its own activation tiles: the tile of local iteration jj goes to private stage jj % XPER, XPER - 1 ahead
-        auto load_x = [&](int jj) {
-          const int i2 = g + jj * G;
-          if (i2 >= num_kb) return;
-          const int st = g * XPER + jj % XPER;
-          mbar_wait(x_empty(st), ((jj / XPER) & 1) ^ 1);     // the MMAs of iteration jj - XPER (committed XPER - 1 iterations ago) are done
-          mbar_expect_tx(x_full(st), X_BYTES);
-          tma_load_3d(xring + st * X_BYTES, &map_x, x_full(st), (kb0 + i2) * BLOCK_K, tok0, 0);
-        };
-        for (int jj = 0; jj < XPER - 1; ++jj) load_x(jj);
-        for (int i = g, j = 0; i < num_kb; i += G, ++j) {
-          load_x(j + XPER - 1);
-          const int s = g * XPER + j % XPER;
-          mbar_wait(x_full(s), (j / XPER) & 1);              // the activation tile of this k-block has landed
-          mbar_wait(a_ready(g), aph);                        // dequantise group g has stored the weight rows (tcgen05.st, waited, fenced)
-          aph ^= 1;
-          tc_fence_after();
-          const uint64_t bd = bdesc0 + (uint64_t)((s * X_BYTES) >> 4);
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / 16; ++k)
-            umma_f16_ts(tacc + (uint32_t)((k % ACC_PER) * NTOK), ta + 8u * k, bd + 2 * k, p.idesc, (i != g || k >= ACC_PER) ? 1u : 0u);
-          umma_commit(x_empty(s));
-          umma_commit(a_empty(g));
-        }
-        umma_commit(tfull);
+      // ================= TMA producer: one raw weight box and the activation tiles of its k-blocks per stage =================
+      for (int j = 0; j < num_box; ++j) {
+        const int st = j % WST;
+        const int nvalid = min(KB_PER_W, num_kb - j * KB_PER_W);
+        mbar_wait(empty(st), ((j / WST) & 1) ^ 1);
+        mbar_expect_tx(full(st), W_BYTES + nvalid * X_BYTES);
+        const uint32_t sw = base + st * STAGE_BYTES;
+        tma_load_2d(sw, &map_w, full(st), (kb0 + j * KB_PER_W) * (INT4 ? BLOCK_K / 2 : BLOCK_K), n0);
+        for (int sub = 0; sub < nvalid; ++sub)
+          tma_load_3d(sw + W_BYTES + sub * X_BYTES, &map_x, full(st), (kb0 + j * KB_PER_W + sub) * BLOCK_K, tok0, 0);
       }
     }
   } else {
-    // ================= dequantise warps (warps 4-7 also run the epilogue): thread = one channel row of the box =================
-    const int grp = (warp - 4) >> 2;
-    const int r = ew * 32 + lane;                            // channel row inside the tile = TMEM lane
-    const uint32_t ta = tmem_base + ((uint32_t)(ew * 32) << 16) + A_COL0 + (uint32_t)grp * A_COLS;
-    for (int i = grp; i < num_kb; i += G) {
-      const int j = i / KB_PER_W, ws = j % WST, sub = i % KB_PER_W;
-      mbar_wait(w_full(ws), (j / WST) & 1);
-      const uint32_t rowp = wring + ws * W_BYTES + r * 128;  // 128 rows x 128 B, SWIZZLE_128B: 16-byte piece c of row r sits at piece c ^ (r & 7)
-      // 64 dequantised values, two per register, k ascending, in the activation dtype (tcgen05 kind::f16 rejects mixed f16 x bf16
-      // operands).  The conversion rate is what bounds this kernel once the loads are deep enough, so it is done with packed 16-bit
-      // arithmetic and magic numbers instead of int -> fp32 -> 16-bit:
-      //   fp16: 0x6400 | u = 1024 + u exactly (10-bit mantissa holds a whole byte); one HSUB2 / HFMA2 removes the offset.
-      //   bf16: only 7 mantissa bits: 0x4300 | (b & 0x7F) = 128 + low7 and 0x4300 | (b & 0x80) = 128 + 128 sign, whose difference is the
-      //         two's-complement byte; int4 nibbles (value + 8 < 128) fit directly.
-      uint32_t o[32];
-      if constexpr (!INT4) {
-        uint4 v[4];
+    // ================= MMA warpgroups: dequantise into the A fragment, D^T[64 channels, NTOK tokens] += A x_tile^T =================
+    const int wg = warp >> 2, q = lane & 3;
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // channel rows r0 and r0 + 8 of the tile ((r0 + 8) & 7 == r0 & 7)
+    float acc[NTOK / 2];
 #pragma unroll
-        for (int q = 0; q < 4; ++q)
-          asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v[q].x), "=r"(v[q].y), "=r"(v[q].z), "=r"(v[q].w) : "r"(rowp + (((sub * 4 + q) ^ (r & 7)) << 4)));
+    for (int i = 0; i < NTOK / 2; ++i) acc[i] = 0.f;
+    for (int j = 0; j < num_box; ++j) {
+      const int st = j % WST;
+      const int nvalid = min(KB_PER_W, num_kb - j * KB_PER_W);
+      mbar_wait(full(st), (j / WST) & 1);
+      const uint32_t sw = base + st * STAGE_BYTES;
+      const uint32_t row0 = sw + r0 * 128, row1 = row0 + 8 * 128;   // 128 rows x 128 B, SWIZZLE_128B: 16-byte piece c of row r sits at piece c ^ (r & 7)
+      const uint32_t sx = r0 & 7;
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const uint32_t w4[4] = {v[q].x, v[q].y, v[q].z, v[q].w};
+      for (int sub = 0; sub < KB_PER_W; ++sub) {
+        if (sub < nvalid) {
+          uint32_t a[4][4];
 #pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            if constexpr (BF16) {
-#pragma unroll
-              for (int hh = 0; hh < 2; ++hh) {
-                const uint32_t t = __byte_perm(w4[e], 0x43434343u, hh ? 0x5342 : 0x5140);      // [0x43 b1 0x43 b0]
-                o[q * 8 + e * 2 + hh] = bf162_as_u32(__hsub2(u32_as_bf162(t & 0xFF7FFF7Fu), u32_as_bf162(t & 0xFF80FF80u)));
-              }
-            } else {
-              const uint32_t u = w4[e] ^ 0x80808080u;        // byte + 128 in 0..255
-              const __half2 bias8 = u32_as_half2(0x64806480u);   // 1024 + 128
-              o[q * 8 + e * 2] = half2_as_u32(__hsub2(u32_as_half2(__byte_perm(u, 0x64646464u, 0x5140)), bias8));
-              o[q * 8 + e * 2 + 1] = half2_as_u32(__hsub2(u32_as_half2(__byte_perm(u, 0x64646464u, 0x5342)), bias8));
+          for (int s = 0; s < 4; ++s) {       // 16-wide k-step s of this k-block
+            if constexpr (!INT4) {            // piece = 16 k = 16 bytes
+              const uint32_t off = (((uint32_t)(sub * 4 + s) ^ sx) << 4) + 2 * q;
+              a[s][0] = dequant_pair<false, BF16>(ld_shared_u16(row0 + off));
+              a[s][1] = dequant_pair<false, BF16>(ld_shared_u16(row1 + off));
+              a[s][2] = dequant_pair<false, BF16>(ld_shared_u16(row0 + off + 8));
+              a[s][3] = dequant_pair<false, BF16>(ld_shared_u16(row1 + off + 8));
+            } else {                          // piece = 32 k = 16 bytes: step s is its half s & 1, byte c = (k = 2c, k = 2c + 1)
+              const uint32_t off = (((uint32_t)(sub * 2 + (s >> 1)) ^ sx) << 4) + (s & 1) * 8 + q;
+              a[s][0] = dequant_pair<true, BF16>(ld_shared_u8(row0 + off));
+              a[s][1] = dequant_pair<true, BF16>(ld_shared_u8(row1 + off));
+              a[s][2] = dequant_pair<true, BF16>(ld_shared_u8(row0 + off + 4));
+              a[s][3] = dequant_pair<true, BF16>(ld_shared_u8(row1 + off + 4));
             }
           }
-        }
-      } else {
-        uint4 v[2];
+          const uint32_t xs = sw + W_BYTES + sub * X_BYTES;
+          wgmma_fence_regs(acc);
+          wgmma_fence();
 #pragma unroll
-        for (int q = 0; q < 2; ++q)
-          asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v[q].x), "=r"(v[q].y), "=r"(v[q].z), "=r"(v[q].w) : "r"(rowp + (((sub * 2 + q) ^ (r & 7)) << 4)));
-        // byte c = (k = 2c low nibble, k = 2c + 1 high nibble), nibble ^ 8 = value + 8
-#pragma unroll
-        for (int q = 0; q < 2; ++q) {
-          const uint32_t w4[4] = {v[q].x, v[q].y, v[q].z, v[q].w};
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            if constexpr (BF16) {
-              // low / high nibbles as separate byte vectors; PRMT picks byte c of each and zero-fills the upper bytes (selector | 8
-              // replicates the sign bit of a byte < 16): [0 hi 0 lo] | 0x43004300 = (128 + lo, 128 + hi), minus 136
-              const uint32_t lo = (w4[e] ^ 0x88888888u) & 0x0F0F0F0Fu, hi = ((w4[e] >> 4) ^ 0x88888888u) & 0x0F0F0F0Fu;
-              const __nv_bfloat162 off = u32_as_bf162(0x43084308u);   // 136
-#pragma unroll
-              for (int b = 0; b < 4; ++b) {
-                const uint32_t t = prmt(lo, hi, 0x8080 + b * 0x0001 + (4 + b) * 0x0100) | 0x43004300u;
-                o[q * 16 + e * 4 + b] = bf162_as_u32(__hsub2(u32_as_bf162(t), off));
-              }
-            } else {
-              // [0x64 byte 0x64 byte] & 0x64F0640F = (1024 + lo, 1024 + 16 hi); HFMA2 with (1, 1/16) and (-1032, -72) leaves (lo - 8, hi - 8)
-              const __half2 mul4 = u32_as_half2(0x2C003C00u), add4 = u32_as_half2(0xD480E408u);
-              const uint32_t u = w4[e] ^ 0x88888888u;
-#pragma unroll
-              for (int b = 0; b < 4; ++b) {
-                const uint32_t t = __byte_perm(u, 0x64646464u, 0x4040 + b * 0x0101) & 0x64F0640Fu;
-                o[q * 16 + e * 4 + b] = half2_as_u32(__hfma2(u32_as_half2(t), mul4, add4));
-              }
-            }
+          for (int s = 0; s < 4; ++s) {
+            const uint64_t bdesc = make_smem_desc(xs + s * 32, 16, 1024);
+            if constexpr (NTOK == 16) wgmma_rs_n16<BF16, 0>(acc, a[s], bdesc, 1);
+            else wgmma_rs_n64<BF16, 0>(acc, a[s], bdesc, 1);
           }
+          wgmma_commit();
+          wgmma_wait<0>();                    // the fragment registers are read asynchronously: they stay untouched until the MMAs retire
+          wgmma_fence_regs(acc);
+#pragma unroll
+          for (int s = 0; s < 4; ++s) keep_regs(a[s]);
         }
       }
       __syncwarp();
-      if (lane == 0) mbar_arrive(w_empty(ws));               // the raw bytes are in registers: the box slot may be refilled
-      mbar_wait(a_empty(grp), ((i / G) & 1) ^ 1);            // the MMAs that read this slot's previous contents have completed
-      tc_fence_after();
-      tmem_st32(ta, o);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(a_ready(grp));
+      if (lane == 0) mbar_arrive(empty(st));
     }
-    // ---- epilogue (warps 4-7: one per TMEM lane quadrant): TMEM lane = output channel, column = token ----
-    if (warp < 8) {
-      if (num_kb > 0) {
-        mbar_wait(tfull, 0);
-        tc_fence_after();
+    // ---- epilogue: accumulator row = output channel, column = token ----
+    if (p.splits > 1) {
+      // split-K inside a cluster: park the partial tile [token][channel] in this CTA's shared memory (the ring is idle once BOTH
+      // warpgroups have consumed their last box); the cluster reduces it below through DSMEM
+      named_bar_sync(1, 256);
+#pragma unroll
+      for (int jn = 0; jn < NTOK / 8; ++jn)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int tok = jn * 8 + 2 * q + (e & 1), chl = r0 + (e >> 1) * 8;
+          asm volatile("st.shared.f32 [%0], %1;" ::"r"(base + (uint32_t)((tok * BLOCK_N + chl) * 4)), "f"(acc[jn * 4 + e]) : "memory");
+        }
+    } else {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int ch = n0 + r0 + h * 8;
+        if (ch >= p.n) continue;
+        const float sc = p.scale[ch];
+        float bv = 0.f;
+        if (p.bias) bv = BF16 ? __bfloat162float(((const __nv_bfloat16*)p.bias)[ch]) : __half2float(((const __half*)p.bias)[ch]);
+#pragma unroll
+        for (int jn = 0; jn < NTOK / 8; ++jn)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int tok = tok0 + jn * 8 + 2 * q + e;
+            if (tok >= p.m) continue;
+            const float y = acc[jn * 4 + h * 2 + e] * sc + bv;
+            if constexpr (BF16) ((__nv_bfloat16*)p.out)[(int64_t)tok * p.n + ch] = __float2bfloat16_rn(y);
+            else ((__half*)p.out)[(int64_t)tok * p.n + ch] = __float2half_rn(y);
+          }
       }
-      const int chl = ew * 32 + lane, ch = n0 + chl;
-      const bool ch_ok = ch < p.n;
-      const float sc = ch_ok ? p.scale[ch] : 0.f;
-      float bv = 0.f;
-      if (ch_ok && p.bias && p.splits == 1) bv = BF16 ? __bfloat162float(((const __nv_bfloat16*)p.bias)[ch]) : __half2float(((const __half*)p.bias)[ch]);
-      const int nacc = min(G, num_kb) * ACC_PER;           // accumulators that received at least one MMA (issuer g has work iff num_kb > g)
-#pragma unroll 1
-      for (int c = 0; c < NTOK / 16; ++c) {
-        uint32_t acc[16];
-#pragma unroll
-        for (int j = 0; j < 16; ++j) acc[j] = 0u;
-        for (int a = 0; a < nacc; ++a) {
-          uint32_t r2[16];
-          tmem_ld16(tmem_base + ((uint32_t)(ew * 32) << 16) + a * NTOK + c * 16, r2);
-#pragma unroll
-          for (int j = 0; j < 16; ++j) acc[j] = __float_as_uint(__uint_as_float(acc[j]) + __uint_as_float(r2[j]));
-        }
-        if (p.splits > 1) {
-          // split-K inside a cluster: park the partial tile [token][channel] in this CTA's shared memory (the raw weight ring is idle
-          // now: every box was consumed before the last MMA could be issued); the cluster reduces it below through DSMEM
-#pragma unroll
-          for (int j = 0; j < 16; ++j)
-            asm volatile("st.shared.b32 [%0], %1;" ::"r"(wring + (uint32_t)(((c * 16 + j) * BLOCK_N + chl) * 4)), "r"(acc[j]) : "memory");
-          continue;
-        }
-        if (!ch_ok) continue;
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const int tok = tok0 + c * 16 + j;
-          if (tok >= p.m) break;
-          const float y = __uint_as_float(acc[j]) * sc + bv;
-          if constexpr (BF16) ((__nv_bfloat16*)p.out)[(int64_t)tok * p.n + ch] = __float2bfloat16_rn(y);
-          else ((__half*)p.out)[(int64_t)tok * p.n + ch] = __float2half_rn(y);
-        }
-      }
-      tc_fence_before();
     }
   }
   if (p.splits > 1) {
@@ -311,11 +215,11 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
       for (int c = (int)rank * 4 + (warp - 4); c < tok_n * 4; c += p.splits * 4) {
         const int tok = c >> 2, chl = (c & 3) * 32 + lane, ch = n0 + chl;
         float acc = 0.f;
-        const uint32_t local = wring + (uint32_t)((tok * BLOCK_N + chl) * 4);
-        for (int q = 0; q < p.splits; ++q) {
+        const uint32_t local = base + (uint32_t)((tok * BLOCK_N + chl) * 4);
+        for (int qq = 0; qq < p.splits; ++qq) {
           uint32_t remote;
           float v;
-          asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(local), "r"(q));
+          asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(local), "r"(qq));
           asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(remote) : "memory");
           acc += v;
         }
@@ -328,11 +232,6 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
       }
     }
     cluster_sync();                                        // nobody leaves while a peer may still read its partial tile
-  }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
   }
 }
 
@@ -364,33 +263,23 @@ static bool make_w_map(CUtensorMap* out, const void* w, int n, int row_bytes) {
   return true;
 }
 
-static uint32_t make_idesc(bool bf16, int ntok) {
-  uint32_t d = 0;
-  d |= 1u << 4;                                  // fp32 accumulate
-  d |= (bf16 ? 1u : 0u) << 7;                    // A (dequantised weights, TMEM) in the activation dtype: mixed f16 x bf16 traps
-  d |= (bf16 ? 1u : 0u) << 10;                   // B (activations)
-  d |= (uint32_t)(ntok >> 3) << 17;              // UMMA N = tokens
-  d |= (uint32_t)(BLOCK_N >> 4) << 24;           // UMMA M = 128 channels
-  return d;
-}
-
-template <int NTOK, int G, int WST, int XPER, bool INT4, bool BF16>
+template <int NTOK, int WST, bool INT4, bool BF16>
 static int launch(const WoGemmArgs& g, const CUtensorMap& mw, cudaStream_t s) {
-  constexpr int XST = G * XPER;
-  constexpr uint32_t SMEM = WST * BLOCK_N * 128 + XST * NTOK * BLOCK_K * 2 + 1024 + 512;
+  constexpr int KB_PER_W = INT4 ? 4 : 2;
+  constexpr uint32_t SMEM = WST * (W_BYTES + KB_PER_W * NTOK * BLOCK_K * 2) + 1024 + 256;
   static_assert(SMEM <= 232448, "weight-only gemm: shared memory budget");
-  static_assert(8 * (2 * WST + 2 * XST + 2 * G + 1) + 8 <= 512, "weight-only gemm: barrier area");
+  static_assert(8 * 2 * WST <= 256, "weight-only gemm: barrier area");
   constexpr int kMaxSplits = 8;                 // portable cluster size
   CUtensorMap mx;
   if (!gemm::make_map(&mx, g.x, g.k, g.m, 1, g.k, 0, BLOCK_K, NTOK, g.bf16 ? kBF16 : kF16)) return 2;
-  auto kern = wo_gemm_kernel<NTOK, G, WST, XPER, INT4, BF16>;
+  auto kern = wo_gemm_kernel<NTOK, WST, INT4, BF16>;
   static bool attr_set = false;
   static int wave_ctas[kMaxSplits + 1];         // CTAs the device holds at once when they come in clusters of `splits`
   if (!attr_set) {
     B200_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
     for (int c = 1; c <= kMaxSplits; ++c) {
       cudaLaunchConfig_t cfg = {};
-      cfg.gridDim = dim3(1, c, 1); cfg.blockDim = dim3(wo_threads(G)); cfg.dynamicSmemBytes = SMEM;
+      cfg.gridDim = dim3(1, c, 1); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = SMEM;
       cudaLaunchAttribute at[1];
       at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = 1; at[0].val.clusterDim.y = c; at[0].val.clusterDim.z = 1;
       cfg.attrs = at; cfg.numAttrs = 1;
@@ -420,10 +309,9 @@ static int launch(const WoGemmArgs& g, const CUtensorMap& mw, cudaStream_t s) {
   }
   p.splits = splits;
   p.kb_per_split = kb_per;
-  p.scale = g.scale; p.bias = g.bias; p.out = g.out; p.bf16 = g.bf16;
-  p.idesc = make_idesc(g.bf16, NTOK);
+  p.scale = g.scale; p.bias = g.bias; p.out = g.out;
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(n_tiles, splits, t_tiles); cfg.blockDim = dim3(wo_threads(G)); cfg.dynamicSmemBytes = SMEM; cfg.stream = s;
+  cfg.gridDim = dim3(n_tiles, splits, t_tiles); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = SMEM; cfg.stream = s;
   cudaLaunchAttribute at[1];
   at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = 1; at[0].val.clusterDim.y = splits; at[0].val.clusterDim.z = 1;
   cfg.attrs = at; cfg.numAttrs = 1;
@@ -434,8 +322,8 @@ static int launch(const WoGemmArgs& g, const CUtensorMap& mw, cudaStream_t s) {
 
 template <bool INT4, bool BF16>
 static int dispatch_tok(const WoGemmArgs& g, const CUtensorMap& mw, cudaStream_t s) {
-  if (g.m <= 16) return launch<16, 4, 10, 4, INT4, BF16>(g, mw, s);      // decode: 160 KB of raw weights in flight
-  return launch<64, 4, 8, 3, INT4, BF16>(g, mw, s);
+  if (g.m <= 16) return launch<16, 8, INT4, BF16>(g, mw, s);      // decode: 128 KB of raw weights in flight
+  return launch<64, 4, INT4, BF16>(g, mw, s);
 }
 
 }  // namespace wo

@@ -1,4 +1,4 @@
-// Common device helpers for the sm_100a kernels (no torch headers in .cu files: keeps nvcc fast).
+// Common device helpers for the sm_90a kernels (no torch headers in .cu files: keeps nvcc fast).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -123,7 +123,7 @@ inline int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }

@@ -1,4 +1,4 @@
-// Host launch API of the sm_100a kernels. Plain C types only: bindings.cpp adapts at::Tensor to these.
+// Host launch API of the sm_90a kernels (entry points and file names keep the names they were introduced with). Plain C types only: bindings.cpp adapts at::Tensor to these.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -128,7 +128,7 @@ struct GemmArgs {
   void* ag_pad[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   void* ag_flags = nullptr;
   uint32_t ag_epoch = 0;
-  // Grouped GEMM over stacked expert weights (MoE), CTA-pair kernel only.  groups = number of experts E.
+  // Grouped GEMM over stacked expert weights (MoE).  groups = number of experts E.
   //   grouped == 1: A = [m, k] rows grouped by expert, every 256-row block belongs to ONE expert (segments padded to 256 rows);
   //                 tile_expert[m / 256] (device int32) = expert of the block or -1 (padding past the last expert);
   //                 B = stacked weights ([E, k, n] or [E, n, k] with b_is_nk, stride_b), D = [m, n].
@@ -139,10 +139,8 @@ struct GemmArgs {
   const int* expert_k0 = nullptr;
   const int* expert_kb = nullptr;
 };
-// returns 0 on success, nonzero if the shape is unsupported by the tcgen05 path (caller falls back)
+// returns 0 on success, nonzero if the shape is unsupported (the binding raises)
 int gemm_tcgen05(const GemmArgs& g, cudaStream_t s);
-// CTA-pair variant (cta_group::2, UMMA M=256): gemm_sm100_2cta.cu
-int gemm_tcgen05_2cta(const GemmArgs& g, cudaStream_t s);
 int gemm_tcgen05_supported(int m, int n, int k, int64_t lda, int64_t ldb, int64_t ldd, int a_is_km, int b_is_nk);
 
 // ---- gemm_fp8_sm100.cu ----------------------------------------------------------------------------------------
@@ -209,7 +207,7 @@ struct AttnArgs {
 int attention_fwd_supported(const AttnArgs& a);
 int attention_fwd(const AttnArgs& a, cudaStream_t s);
 // Backward (attention_bwd_sm100.cu). fwd: the forward's arguments with o (contiguous [B,Sq,H,D]) and lse filled in.
-// d_o: contiguous [B,Sq,H,D]; delta: fp32 scratch [B,H,Sq]; dq: fp32 [B,Sq,H,D] ZEROED by the caller; dk/dv: [B,Sk,Hk,D] views (dkv_strides).
+// d_o: contiguous [B,Sq,H,D]; delta: fp32 scratch [B,H,Sq]; dq: fp32 [B,Sq,H,D], every element written; dk/dv: [B,Sk,Hk,D] views (dkv_strides).
 struct AttnBwdArgs {
   AttnArgs fwd;
   const void* d_o;
@@ -220,7 +218,6 @@ struct AttnBwdArgs {
   int64_t dkv_strides[3];   // element strides (batch, seq, head) of dk and dv (16-byte aligned rows)
   int64_t o_strides[3];     // element strides (batch, seq, head) shared by the forward output `fwd.o` and d_o
   int64_t dq_strides[3];    // element strides (batch, seq, head) of the fp32 dq accumulator
-  int* dq_sem = nullptr;    // deterministic mode: zeroed int32 [B, H, ceil(Sq / 128)] turn counters - key tiles add into a dQ tile in ascending order
 };
 int attention_bwd(const AttnBwdArgs& a, cudaStream_t s);
 

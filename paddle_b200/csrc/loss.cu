@@ -1,4 +1,4 @@
-// Fused softmax + cross-entropy (single device and vocab-parallel pieces) for sm_100a.
+// Fused softmax + cross-entropy (single device and vocab-parallel pieces) for sm_90a.
 // Parity (behaviour): paddle/phi/kernels/gpu/cross_entropy_kernel.cu, c_softmax_with_cross_entropy_kernel.cu.
 // One CTA per row, one streaming pass (online softmax), fp32 math; backward is one read + one write and may run
 // in place over the logits buffer.

@@ -2,7 +2,7 @@
 // (paddle/phi/kernels/gpu/number_count_kernel.cu, assign_pos_kernel.cu, limit_by_capacity_kernel.cu,
 // prune_gate_by_capacity_kernel.cu:33) plus the planning / gather / combine kernels of the grouped-GEMM expert path
 // (csrc/gemm_sm100_2cta.cu, GemmArgs::grouped): token slots are laid out grouped by expert in 256-row aligned segments, so every
-// CTA-pair tile of the grouped GEMM belongs to exactly one expert and the tile scheduler only reads a small device table.
+// 256-row block of the grouped GEMM belongs to exactly one expert and the tile scheduler only reads a small device table.
 #include "include/b200_common.cuh"
 #include "include/b200_ops.h"
 

@@ -1,4 +1,4 @@
-// Fused RMSNorm / LayerNorm forward+backward for sm_100a.
+// Fused RMSNorm / LayerNorm forward+backward for sm_90a.
 // Parity (behaviour): paddle/phi/kernels/fusion/gpu/fused_layernorm_kernel.cu, fused_rms_norm (reference).
 // Design: one CTA per row, row cached in registers (16-byte vectors, block size sized to the row so no lane idles),
 // fp32 statistics; the backward is a persistent grid that keeps per-CTA dW/dB partial sums in registers across rows,

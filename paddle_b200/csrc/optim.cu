@@ -1,4 +1,4 @@
-// Fused optimizer kernels for sm_100a: AdamW (multi-precision), SGD-momentum, LAMB, grad-norm, unscale.
+// Fused optimizer kernels for sm_90a: AdamW (multi-precision), SGD-momentum, LAMB, grad-norm, unscale.
 // Parity (behaviour): paddle/phi/kernels/gpu/adamw_kernel.cu, fused_adam_kernel.cu, lamb_kernel.cu, amp_kernel.cu
 // (check_finite_and_unscale / update_loss_scaling), clip_by_global_norm.
 // Design: parameters live in flat arenas, so one launch covers one (dtype, hyper-parameter) group; clip coefficient,
@@ -13,7 +13,7 @@ namespace b200 {
 // ---- split master weights ------------------------------------------------------------------------------------------
 // fp32 master = bf16 parameter (round-to-nearest of the master, the value the forward uses) + a signed 16-bit residual of the
 // low mantissa bits: bits(master) = (bits(bf16) << 16) + residual.  4 bytes per parameter instead of 6 (bf16 copy + fp32 master):
-// on one B200 that is 26 GB of the 180 GB for a 13B model, which buys larger micro-batches instead of activation recompute.
+// 26 GB less for a 13B model, which buys larger micro-batches instead of activation recompute.
 // The only inexact case is a round-to-even tie whose residual is +0x8000 (stored as 0x7fff: one fp32 ulp).
 __device__ __forceinline__ float split_master_join(__nv_bfloat16 w, int16_t lo) {
   const uint32_t hi = (uint32_t)__bfloat16_as_ushort(w) << 16;

@@ -75,7 +75,7 @@ def estimate_memory_gb(m, c, optimizer_bytes=6.0, hbm_reserve_gb=4.0):
     mbs, seq, h = c["micro_batch"], m.seq, m.hidden
     sp = mp if c.get("sequence_parallel", mp > 1) else 1
     # saved activations of one layer with the lean fused blocks (kernels/fused_blocks.py): ~6.5 hidden-sized bf16 tensors per token at mp1
-    # (measured: 157.6 GB peak for 13B at micro-batch 2 = 130 GB of state + ~0.55 GB per layer); 4 live on the residual stream (sharded by
+    # (~0.55 GB per 13B layer at micro-batch 2); 4 live on the residual stream (sharded by
     # sequence parallel), the rest are mp-sharded
     full_layer = mbs * seq * h * 2 * (4.0 / sp + 2.5 / mp)
     ckpt_layer = mbs * seq * h * 2 / sp
@@ -91,15 +91,16 @@ def estimate_memory_gb(m, c, optimizer_bytes=6.0, hbm_reserve_gb=4.0):
     return (w + g + o + act + logits) / GB + hbm_reserve_gb
 
 
-def estimate_step_ms(m, c, cm=None, gemm_eff=0.80, attn_eff=0.45, global_batch=None):
-    """Analytic step time of candidate `c`; the constants are the efficiencies measured on B200 for the own kernels (DESIGN.md §4)."""
+def estimate_step_ms(m, c, cm=None, gemm_eff=0.30, attn_eff=0.19, global_batch=None):
+    """Analytic step time of candidate `c`; the efficiencies are shares of the data-sheet bf16 rate that the own kernels reached on an
+    H100 80GB HBM3 at 700 W (DESIGN.md §4): GEMMs of 8192 rows ~300 TFLOP/s, attention forward + backward ~190 TFLOP/s."""
     cm = cm or CostModel()
-    peak = cm.peaks.get("bf16_tflops_sustained", 1400.0) * 1e9         # FLOP per ms
+    peak = cm.peaks.get("bf16_tflops_sustained", 989.0) * 1e9         # FLOP per ms
     mp, pp, sh, dp = c["mp"], c["pp"], c["sharding"], c["dp"]
     tok = c["micro_batch"] * m.seq
     dense = 2.0 * tok * (m.attn_params + (3 if m.gated_ffn else 2) * m.hidden * m.ffn * (m.moe_topk if m.moe_experts else 1)) / mp
     attn = 2.0 * tok * m.seq * m.hidden / mp
-    fill = min(1.0, 0.88 + 0.12 * tok / 8192.0)                             # small micro-batches under-fill the 148-SM GEMM waves
+    fill = min(1.0, 0.80 + 0.20 * tok / 8192.0)                             # measured: 2048 / 4096 rows reach 0.84 / 0.88 of the 8192-row rate
     t_fwd = dense / (peak * gemm_eff * fill) + attn / (peak * attn_eff)
     rc = {"none": 0.0, "selective": 0.15, "full": 1.0}[c.get("recompute", "none")]
     t_layer = t_fwd * (3.0 + rc)
@@ -185,7 +186,7 @@ def prune_by_recompute(t, c):
 @register_prune
 def prune_by_memory(t, c):
     c["mem_gb"] = round(estimate_memory_gb(t["model"], c, t.get("optimizer_bytes", 6.0)), 1)
-    return c["mem_gb"] > t.get("hbm_gb", 180.0) * t.get("hbm_fraction", 0.94)
+    return c["mem_gb"] > t.get("hbm_gb", 80.0) * t.get("hbm_fraction", 0.94)
 
 
 def _dominates(a, b):
@@ -267,7 +268,7 @@ def rank(tuner_cfg, history=(), cm=None):
     return cands, space.pruned
 
 
-def search(num_gpus, hidden, layers, ffn, vocab, seq, global_batch, heads=None, hbm_gb=180.0, bytes_per_param=12, measure=None, top_k=5, **extra):
+def search(num_gpus, hidden, layers, ffn, vocab, seq, global_batch, heads=None, hbm_gb=80.0, bytes_per_param=12, measure=None, top_k=5, **extra):
     """Round-1 entry point: the `top_k` fastest candidates under the analytic model (or under `measure(cfg) -> ms`)."""
     cfg = dict(num_gpus=num_gpus, hidden=hidden, layers=layers, ffn=ffn, vocab=vocab, seq=seq, global_batch=global_batch, heads=heads, hbm_gb=hbm_gb,
                optimizer_bytes=bytes_per_param - 4, **extra)

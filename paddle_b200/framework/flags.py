@@ -6,22 +6,22 @@ import os
 _FLAGS = {
     "FLAGS_check_nan_inf": False,
     "FLAGS_cudnn_deterministic": False,
-    "FLAGS_use_fused_kernels": True,       # route nn/functional hot ops to the sm_100a kernels
+    "FLAGS_use_fused_kernels": True,       # route nn/functional hot ops to the sm_90a kernels
     "FLAGS_b200_sync_debug": False,        # serialise side streams (race triage)
     "FLAGS_b200_p2p_collectives": True,    # fused compute+collective kernels over peer memory
     "FLAGS_b200_gemm_backend": "tcgen05",  # "tcgen05" | "cublas"
     "FLAGS_b200_nvls": False,              # all-reduce through NVSwitch multicast (parallel/nvls.py, multimem.ld_reduce / st); not yet run on hardware
     "FLAGS_b200_decode_kernel": False,     # models.generation: decode steps attend through csrc/decode_attention.cu (CUDA, head_dim 128, fp16 / bf16)
-    "FLAGS_use_cinn": False,               # pir.optimize: fuse elementwise / reduction chains into generated sm_100a kernels (paddle_b200.cinn)
+    "FLAGS_use_cinn": False,               # pir.optimize: fuse elementwise / reduction chains into generated sm_90a kernels (paddle_b200.cinn)
     "FLAGS_enable_pir_api": False,         # static Executor: run programs through the native IR pass pipeline (paddle_b200.pir) before replay
-    "FLAGS_b200_fp8_block_scaled": False,  # with FLAGS_b200_fp8_linear: OCP MX scaling (one E8M0 scale per 32 k, applied by tcgen05 block_scale MMAs) instead of per-tensor
-    "FLAGS_b200_fp8_linear": False,        # nn.Linear / F.linear run as fp8 tcgen05 GEMMs (per-tensor scaling, e4m3 fwd / e5m2 grads)
+    "FLAGS_b200_fp8_block_scaled": False,  # with FLAGS_b200_fp8_linear: OCP MX scaling (one E8M0 scale per 32 k, applied per k-block in the fp8 GEMM) instead of per-tensor
+    "FLAGS_b200_fp8_linear": False,        # nn.Linear / F.linear run as fp8 wgmma GEMMs (per-tensor scaling, e4m3 fwd / e5m2 grads)
     "FLAGS_b200_pp_mailbox": True,         # pipeline p2p through the peer-memory mailbox (copy engine + flag) instead of NCCL send/recv
     "FLAGS_b200_fused_wgrad": True,        # weight-gradient GEMMs accumulate straight into the flat gradient arena (kernels/wgrad.py)
     "FLAGS_b200_split_master_weights": True,   # bf16 arenas keep fp32 master weights as bf16 parameter + int16 residual (4 B instead of 6 B per parameter)
     "FLAGS_b200_to_static_train_graph": True,  # to_static captures training calls (forward + backward CUDA graphs) after two eager warm-ups
-    "FLAGS_b200_moe_grouped_gemm": True,       # MoE experts run as grouped tcgen05 GEMMs with device-side routing
-    "FLAGS_b200_flash_attention": True,    # tcgen05 flash-attention forward (csrc/attention_sm100.cu)
+    "FLAGS_b200_moe_grouped_gemm": True,       # MoE experts run as grouped wgmma GEMMs with device-side routing
+    "FLAGS_b200_flash_attention": True,    # wgmma flash-attention forward (csrc/attention_sm100.cu)
     "FLAGS_embedding_deterministic": 0,
     "FLAGS_eager_delete_tensor_gb": 0.0,
     "FLAGS_fraction_of_gpu_memory_to_use": 0.92,

@@ -2,7 +2,7 @@
 (Config, create_predictor, Predictor, Tensor handles, PrecisionType, PlaceType, get_version...).
 
 The predictor loads ``jit.save`` artifacts (prefix.pdmodel + prefix.pdiparams) and serves them with CUDA-graph replay
-per input signature (jit.StaticFunction) - the sm_100a answer to the reference's IR-pass + TensorRT pipeline."""
+per input signature (jit.StaticFunction) - the sm_90a answer to the reference's IR-pass + TensorRT pipeline."""
 from __future__ import annotations
 
 import enum
@@ -317,10 +317,10 @@ class Config:
         return False
 
     def enable_xpu(self, *a, **k):
-        raise RuntimeError("XPU is not supported by paddle_b200 (sm_100a only)")
+        raise RuntimeError("XPU is not supported by paddle_b200 (sm_90a only)")
 
     def enable_custom_device(self, device_type, device_id=0, precision_mode=PrecisionType.Float32):
-        raise RuntimeError(f"custom device '{device_type}' is not supported by paddle_b200 (sm_100a only)")
+        raise RuntimeError(f"custom device '{device_type}' is not supported by paddle_b200 (sm_90a only)")
 
     def enable_onnxruntime(self):
         raise RuntimeError("onnxruntime is not part of this build; export with paddle.onnx.export and serve it externally")
@@ -528,7 +528,7 @@ class PredictorPool:
 def get_version():
     from .. import __version__
 
-    return f"paddle_b200 {__version__} (sm_100a)"
+    return f"paddle_b200 {__version__} (sm_90a)"
 
 
 def get_trt_compile_version():

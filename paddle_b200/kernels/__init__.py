@@ -1,4 +1,4 @@
-"""Python face of the sm_100a kernels (csrc/).  Each op is a torch.autograd.Function around the native launchers;
+"""Python face of the sm_90a kernels (csrc/).  Each op is a torch.autograd.Function around the native launchers;
 CPU tensors take a plain-PyTorch reference path (used by the CPU test-suite), CUDA tensors REQUIRE the extension."""
 from __future__ import annotations
 

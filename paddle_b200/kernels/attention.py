@@ -1,7 +1,7 @@
 """Attention entry point ([B,S,H,D] layout). Parity: paddle flash_attention / scaled_dot_product_attention
 (python/paddle/nn/functional/flash_attention.py).
 
-Dispatch: the sm_100a tcgen05 flash kernel (csrc/attention_sm100.cu) for fp16/bf16, head_dim 128, no explicit mask and no
+Dispatch: the sm_90a wgmma flash kernel (csrc/attention_sm100.cu) for fp16/bf16, head_dim 128, no explicit mask and no
 dropout — it reads q/k/v in place as strided views of a packed QKV projection; everything else takes the PyTorch SDPA
 (library) path.  Backward: csrc/attention_bwd_sm100.cu (B200_ATTN_BWD=own, default) or, for comparison, a library backward
 fed with our forward's (out, logsumexp) (B200_ATTN_BWD=cudnn|flash).
@@ -47,11 +47,11 @@ class _FlashAttn(torch.autograd.Function):
     def backward(ctx, do):
         q, k, v, out, lse = ctx.saved_tensors
         do = do.contiguous()
-        if _bwd_backend[0] == "own":   # csrc/attention_bwd_sm100.cu: tcgen05 S/dP/dV/dK/dQ GEMMs, fp32 dQ reduction
+        if _bwd_backend[0] == "own":   # csrc/attention_bwd_sm100.cu: wgmma dK/dV kernel + dQ kernel, no atomics
             dq, dk, dv = ext().attention_bwd(q, k, v, out, lse, do, ctx.scale, ctx.causal)
             return dq, dk, dv, None, None
         if _bwd_backend[0] == "cudnn" and q.shape[2] == k.shape[2]:
-            # Blackwell-tuned library backward fed with OUR forward's (out, logsumexp); [B,S,H,D] tensors enter as [B,H,S,D] views
+            # Hopper-tuned library backward fed with OUR forward's (out, logsumexp); [B,S,H,D] tensors enter as [B,H,S,D] views
             try:
                 z = torch.zeros((), dtype=torch.int64, device=q.device)
                 dq, dk, dv = torch.ops.aten._scaled_dot_product_cudnn_attention_backward(
@@ -68,7 +68,7 @@ class _FlashAttn(torch.autograd.Function):
 
 
 class _FlashAttnColMask(torch.autograd.Function):
-    """tcgen05 flash attention with a column-wise row-range mask (flashmask / packed variable-length sequences / sliding windows):
+    """wgmma flash attention with a column-wise row-range mask (flashmask / packed variable-length sequences / sliding windows):
     colmask int32 [B, 1|H, Sk, 4] = (lt_start, lt_end, ut_start, ut_end): key j hides query rows [lt_start, lt_end) and
     [ut_start, ut_end).  Forward and backward are the same kernels as the dense path (csrc/attention_sm100.cu,
     attention_bwd_sm100.cu) with the mask test added to their score-tile loops."""
@@ -134,7 +134,7 @@ def colmask_from_window(sq, sk, left, right, causal, device):
 
 
 def attention_colmask(q, k, v, colmask, causal=False, scale=None):
-    """[B,S,H,D] attention under a column-wise row-range mask on the own tcgen05 kernels; None if the operands do not qualify."""
+    """[B,S,H,D] attention under a column-wise row-range mask on the own wgmma kernels; None if the operands do not qualify."""
     q, k, v = raw(q), raw(k), raw(v)
     if not fused_ok(q, k, v, None, 0.0, causal):
         return None

@@ -1,7 +1,7 @@
-"""GEMM dispatch: tcgen05 kernel (csrc/gemm_sm100.cu) for bf16/fp16 CUDA operands, torch.matmul otherwise.
+"""GEMM dispatch: wgmma kernel (csrc/gemm_sm100.cu) for bf16/fp16 CUDA operands, torch.matmul otherwise.
 
 ``linear(x, W[in,out], b)`` is the framework's Linear primitive with a custom backward that runs all three GEMMs
-(y = xW, dx = dy W^T, dW = x^T dy) on the tcgen05 path without materialising any transpose: the operand "major"
+(y = xW, dx = dy W^T, dW = x^T dy) on the wgmma path without materialising any transpose: the operand "major"
 bits of the UMMA descriptors select K-major or MN-major smem tiles.
 """
 from __future__ import annotations
@@ -93,7 +93,7 @@ class _Linear(torch.autograd.Function):
 
 class _DeferLinear(torch.autograd.Function):
     """Device-agnostic linear whose weight gradient goes through a wgrad sink (used while a zero-bubble pipeline schedule is
-    deferring W passes and the tcgen05 fast path does not apply, e.g. the CPU/gloo tests or fp32 parameters)."""
+    deferring W passes and the wgmma fast path does not apply, e.g. the CPU/gloo tests or fp32 parameters)."""
 
     @staticmethod
     def forward(ctx, x, w, b, sink):

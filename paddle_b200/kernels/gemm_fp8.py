@@ -1,7 +1,7 @@
 """fp8 GEMM (per-tensor scaled e4m3 / e5m2 -> half, and OCP MX block-scaled e4m3) and fp8 Linears for O2-fp8 training.
 Parity: paddle.linalg.fp8_fp8_half_gemm_fused (python/paddle/tensor/linalg.py) -> phi fp8_gemm fusion kernels (cuBLASLt).
 
-CUDA path: csrc/gemm_fp8_sm100.cu — tcgen05 `kind::f8f6f4` MMAs, fp32 accumulation in TMEM, dequantisation scale + bias +
+CUDA path: csrc/gemm_fp8_sm100.cu — fp8 wgmma MMAs, fp32 accumulation in registers, dequantisation scale + bias +
 activation fused in the epilogue.  Both operands must be K-major (x [M,K], y [N,K], i.e. transpose_x=False, transpose_y=True);
 other layouts are brought into that form with one transposed copy.  CPU / unsupported shapes: fp32 reference."""
 from __future__ import annotations
@@ -85,7 +85,7 @@ def _scaled_gemm(a, b, sa, sb, bias, out_dtype):
 
 class _Fp8Linear(torch.autograd.Function):
     """y = x @ W (W: [in, out]) with e4m3 activations / weights in the forward and e5m2 output gradients in the backward (the fp8 recipe of
-    the reference's O2-fp8 AMP): three tcgen05 fp8 GEMMs, all TN.  Every operand is quantised ONCE by the fused kernels, which emit the
+    the reference's O2-fp8 AMP): three wgmma fp8 GEMMs, all TN.  Every operand is quantised ONCE by the fused kernels, which emit the
     transposed copy in the same pass; the dequantisation factors never leave the device."""
 
     @staticmethod
@@ -151,8 +151,8 @@ def dequantize_mx(q, sf):
 
 
 def mx_gemm(a, sfa, b, sfb, bias=None, out_dtype=torch.bfloat16):
-    """a [M,K], b [N,K] e4m3 with MX scale blocks -> (a * 2^sfa) @ (b * 2^sfb)^T: tcgen05.mma.kind::mxf8f6f4.block_scale, the scales
-    are applied by the tensor core (csrc/gemm_fp8_sm100.cu, MX variant)."""
+    """a [M,K], b [N,K] e4m3 with MX scale blocks -> (a * 2^sfa) @ (b * 2^sfb)^T: fp8 wgmma, the scales
+    are applied per 32-wide k-block in registers (csrc/gemm_fp8_sm100.cu, MX variant)."""
     a, sfa, b, sfb, bias = raw(a), raw(sfa), raw(b), raw(sfb), raw(bias)
     if use_fused(a) and a.shape[0] % 128 == 0 and b.shape[0] % 128 == 0 and a.shape[1] % 128 == 0:
         bb = bias.to(out_dtype).contiguous() if bias is not None else None

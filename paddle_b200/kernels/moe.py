@@ -1,8 +1,8 @@
-"""Device-side MoE routing and the grouped-GEMM expert FFN (csrc/moe.cu, csrc/gemm_sm100_2cta.cu grouped modes).
+"""Device-side MoE routing and the grouped-GEMM expert FFN (csrc/moe.cu, csrc/gemm_sm100.cu grouped modes).
 
 Token slots are laid out grouped by expert in 256-row aligned segments (`moe_route`: counts -> segment starts -> destination row of
 every slot, plus the tile -> expert table and the per-expert reduction ranges, all on the device); the expert FFN is then TWO launches
-of the persistent CTA-pair tcgen05 kernel over the stacked expert weights, whatever the number of experts, with no host
+of the persistent wgmma kernel over the stacked expert weights, whatever the number of experts, with no host
 synchronisation anywhere (the reference's fused_moe: paddle/phi/kernels/fusion/cutlass/fused_moe_kernel.cu:46, and its gate utility
 kernels number_count / assign_pos / limit_by_capacity / prune_gate_by_capacity_kernel.cu:33).
 """
@@ -15,7 +15,7 @@ from . import wgrad as WG
 
 
 def grouped_ok(x, w1, w2):
-    """The grouped tcgen05 path needs CUDA bf16 / fp16 operands and GEMM dims the CTA-pair kernel accepts."""
+    """The grouped wgmma path needs CUDA bf16 / fp16 operands and GEMM dims the kernel accepts."""
     from ..framework.flags import flag
     from . import use_fused
 
@@ -75,7 +75,7 @@ class _Combine(torch.autograd.Function):
 
 
 class _GroupedLinear(torch.autograd.Function):
-    """y[rows of expert e] = xp[rows of expert e] @ w[e]; ONE grouped tcgen05 launch for all experts."""
+    """y[rows of expert e] = xp[rows of expert e] @ w[e]; ONE grouped wgmma launch for all experts."""
 
     @staticmethod
     def forward(ctx, xp, w, plan_te, plan_k0, plan_kb, sink):

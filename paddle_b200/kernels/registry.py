@@ -166,14 +166,14 @@ def _register_builtin(f):
     G, A = "GPU", "ANY"
     r = f.register
     # GEMM family
-    r("matmul", G, HALF, "kernels.gemm:matmul", native="csrc/gemm_sm100_2cta.cu::gemm2_kernel, csrc/gemm_sm100.cu", priority=10)
+    r("matmul", G, HALF, "kernels.gemm:matmul", native="csrc/gemm_sm100.cu::gemm_kernel, csrc/gemm_sm100.cu", priority=10)
     r("matmul", A, ("*",), "ops.linalg:matmul")
-    r("linear", G, HALF, "kernels.gemm:linear", native="csrc/gemm_sm100_2cta.cu::gemm2_kernel (bias / activation epilogues)", priority=10)
+    r("linear", G, HALF, "kernels.gemm:linear", native="csrc/gemm_sm100.cu::gemm_kernel (bias / activation epilogues)", priority=10)
     r("linear", A, ("*",), "nn.functional:linear")
-    r("fp8_gemm", G, ("float8_e4m3fn", "float8_e5m2"), "kernels.gemm_fp8:fp8_gemm", native="csrc/gemm_fp8_sm100.cu (kind::f8f6f4)")
+    r("fp8_gemm", G, ("float8_e4m3fn", "float8_e5m2"), "kernels.gemm_fp8:fp8_gemm", native="csrc/gemm_fp8_sm100.cu")
     r("fp8_quantize", G, FLOAT, "kernels.gemm_fp8:quantize_fp8", native="csrc/quant_fp8.cu")
     r("mx_quantize", G, FLOAT, "kernels.gemm_fp8:quantize_mx", native="csrc/quant_fp8.cu::mx_quantize_kernel")
-    r("mx_gemm", G, ("float8_e4m3fn",), "kernels.gemm_fp8:mx_gemm", native="csrc/gemm_fp8_sm100.cu (kind::mxf8f6f4.block_scale)")
+    r("mx_gemm", G, ("float8_e4m3fn",), "kernels.gemm_fp8:mx_gemm", native="csrc/gemm_fp8_sm100.cu (MX scales applied in registers)")
     r("weight_only_linear", G, HALF, "nn.quant:weight_only_linear", native="csrc/gemm_wo_sm100.cu::wo_gemm_kernel", priority=10)
     r("weight_only_linear", A, ("*",), "nn.quant:weight_only_linear")
     # attention
@@ -196,7 +196,7 @@ def _register_builtin(f):
     r("cross_entropy_with_softmax", A, ALL_FLOAT, "kernels.loss:softmax_cross_entropy")
     r("fused_bias_dropout_residual", G, FLOAT, "incubate.nn.functional:fused_dropout_add", native="csrc/fused_dropout.cu::bias_dropout_add_fwd")
     # MoE
-    r("moe_expert_ffn", G, HALF, "kernels.moe:expert_ffn_grouped", native="csrc/moe.cu (routing), csrc/gemm_sm100_2cta.cu (grouped GEMM)")
+    r("moe_expert_ffn", G, HALF, "kernels.moe:expert_ffn_grouped", native="csrc/moe.cu (routing), csrc/gemm_sm100.cu (grouped GEMM)")
     # fused blocks
-    r("fused_rms_norm_linear", G, HALF, "kernels.fused_blocks:norm_linear", native="csrc/norm.cu + csrc/gemm_sm100_2cta.cu")
-    r("fused_swiglu_linear", G, HALF, "kernels.fused_blocks:swiglu_linear", native="csrc/elementwise.cu + csrc/gemm_sm100_2cta.cu")
+    r("fused_rms_norm_linear", G, HALF, "kernels.fused_blocks:norm_linear", native="csrc/norm.cu + csrc/gemm_sm100.cu")
+    r("fused_swiglu_linear", G, HALF, "kernels.fused_blocks:swiglu_linear", native="csrc/elementwise.cu + csrc/gemm_sm100.cu")

@@ -4,7 +4,7 @@ Two things the reference gets from separate mechanisms live here:
 
 * **fused accumulation** (role of ``fused_linear_param_grad_add``, /root/reference/paddle/phi/kernels/fusion/gpu/
   fused_linear_param_grad_add_kernel.cu): when a parameter's gradient is a view of a flat arena slab
-  (``parallel/arena.py``) the wgrad GEMM adds straight into it through the accumulate epilogue of the tcgen05 kernel,
+  (``parallel/arena.py``) the wgrad GEMM adds straight into it through the accumulate epilogue of the wgmma kernel,
   so no per-micro-batch ``dW`` tensor is allocated and autograd's in-place ``grad += dW`` kernel disappears.
 * **deferral** (zero-bubble pipeline schedules, /root/reference/python/paddle/distributed/passes/
   pipeline_scheduler_pass/pipeline_zero_bubble.py:62): inside ``deferring(queue)`` the backward of every linear only

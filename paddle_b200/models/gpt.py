@@ -1,6 +1,6 @@
 """GPT-3 family (pre-LN decoder, learned positions, GELU MLP, biases). Parity (role): the GPT used by the reference's
 GroupSharded / auto-parallel benchmarks (test/auto_parallel/get_gpt_model.py, PaddleNLP gpt modeling).
-Hot ops: fused-QKV tcgen05 GEMM with bias epilogue, tcgen05 flash attention, fused LayerNorm, bias+GELU GEMM epilogue."""
+Hot ops: fused-QKV wgmma GEMM with bias epilogue, wgmma flash attention, fused LayerNorm, bias+GELU GEMM epilogue."""
 from __future__ import annotations
 
 from dataclasses import dataclass

@@ -2,7 +2,7 @@
 
 Parity (role): the Llama used by the reference's hybrid-parallel benchmarks (test/auto_parallel/hybrid_strategy/
 semi_auto_llama.py; PaddleNLP llama modeling on fleet mpu layers + incubate fused ops).  Every hot op is one of this
-repo's sm_100a kernels: fused QKV / gate-up GEMMs (tcgen05), in-place packed rotary, fused residual-add+RMSNorm,
+repo's sm_90a kernels: fused QKV / gate-up GEMMs (wgmma), in-place packed rotary, fused residual-add+RMSNorm,
 SwiGLU, fused softmax-CE; row-parallel GEMMs go through parallel.fused_mp (GEMM + collective over peer memory).
 """
 from __future__ import annotations

@@ -1,6 +1,6 @@
 """Mixtral-style sparse MoE decoder (Llama attention + top-2 routed SwiGLU experts, expert parallel over a group).
 Parity (role): PaddleNLP mixtral / the reference's MoELayer benchmarks (python/paddle/incubate/distributed/models/moe/).
-Experts are stored stacked ([E_local, ...]) so the per-expert FFNs run as grouped tcgen05 GEMMs; tokens travel through the
+Experts are stored stacked ([E_local, ...]) so the per-expert FFNs run as grouped wgmma GEMMs; tokens travel through the
 expert-parallel all-to-all (incubate.moe.global_scatter / global_gather; peer-memory all-to-all kernel when available)."""
 from __future__ import annotations
 

@@ -8,7 +8,7 @@ preempted (its blocks go back to the pool; it is re-prefilled later from prompt 
 Every step packs the tokens of all scheduled sequences into ONE [tokens, hidden] batch: whole prompts for the sequences being prefilled,
 one token for the sequences being decoded.  The decoder layers run on the packed batch with the model's own sublayers; attention is
 `incubate.nn.paged_attention.block_attention` - on CUDA (head_dim 128, fp16 / bf16) one indexed scatter of the new K / V rows into the
-block pool, `decode_attention_paged` for the decode rows and one packed variable-length tcgen05 attention for the prefill rows.
+block pool, `decode_attention_paged` for the decode rows and one packed variable-length wgmma attention for the prefill rows.
 """
 from __future__ import annotations
 

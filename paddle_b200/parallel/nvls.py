@@ -4,7 +4,7 @@ Plumbing is torch.distributed._symmetric_memory (multicast object creation, bind
 the device code is ours (csrc/comm/nvls_collectives.cu).  A context owns ONE symmetric staging buffer per group; tensors are copied in and
 out of it (the gradient arenas of parallel/arena.py can be placed inside it to skip the copies: `NvlsContext.tensor`).
 
-Opt-in: FLAGS_b200_nvls (default off).  STATUS: the kernels are compiled for sm_100a (SASS shows LDGMC / multicast stores) but this path has
+Opt-in: FLAGS_b200_nvls (default off).  STATUS: the kernels are compiled for sm_90a (SASS shows LDGMC / multicast stores) but this path has
 NOT run on hardware yet; tests/test_distributed_gpu.py::test_nvls_* is the 2-GPU check.  Without multicast support (no NVSwitch, driver
 without fabric manager) `context_for` returns None and callers keep the peer-memory two-shot (parallel/symm.py) or NCCL.
 Parity (role): NCCL's NVLS algorithm behind ProcessGroupNCCL all-reduce / reduce-scatter / all-gather."""

@@ -64,7 +64,7 @@ def run_check():
     if torch.cuda.is_available():
         from .._build import load
 
-        print("native sm_100a extension:", "loaded" if load() is not None else "NOT BUILT")
+        print("native sm_90a extension:", "loaded" if load() is not None else "NOT BUILT")
     print("PaddlePaddle-compatible paddle_b200 is installed successfully!")
 
 

@@ -1,13 +1,13 @@
-"""paddle.utils.cpp_extension: build custom C++/CUDA ops for sm_100a.
+"""paddle.utils.cpp_extension: build custom C++/CUDA ops for sm_90a.
 Parity: python/paddle/utils/cpp_extension/{cpp_extension,extension_utils}.py (load, setup, CppExtension, CUDAExtension).
 
-Custom ops are pybind/torch extensions compiled with ``-gencode arch=compute_100a,code=sm_100a``; functions exported
+Custom ops are pybind/torch extensions compiled with ``-gencode arch=compute_90a,code=sm_90a``; functions exported
 from the module operate on paddle_b200 Tensors (they are torch tensors underneath)."""
 from __future__ import annotations
 
 import os
 
-SM100_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "--expt-relaxed-constexpr"]
+SM100_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--expt-relaxed-constexpr"]
 
 
 def _wrap_module(mod):

@@ -4,14 +4,14 @@ full_version = "3.0.0"
 major, minor, patch, rc = "3", "0", "0", "0"
 b200_version = "0.1.0"
 cuda_version = "12.9"
-cudnn_version = "none (hand-written sm_100a kernels)"
+cudnn_version = "none (hand-written sm_90a kernels)"
 istaged = True
 commit = "paddle_b200"
 with_pip_cuda_libraries = "OFF"
 
 
 def show():
-    print(f"full_version: {full_version}\ncuda: {cuda_version}\ncudnn: {cudnn_version}\ntarget: sm_100a")
+    print(f"full_version: {full_version}\ncuda: {cuda_version}\ncudnn: {cudnn_version}\ntarget: sm_90a")
 
 
 def cuda():

@@ -45,7 +45,7 @@ def probe(name, fn, mode="global"):
 probe("torch.mm", lambda: a @ b)
 probe("rms_norm_fwd", lambda: C.rms_norm_fwd(a, None, w, None, 1e-5))
 probe("gemm 1cta (M=64)", lambda: C.gemm(a[:64].contiguous(), b))
-probe("gemm (M=512, 2cta)", lambda: C.gemm(a, b))
+probe("gemm (M=512)", lambda: C.gemm(a, b))
 probe("gemm thread_local", lambda: C.gemm(a, b), "thread_local")
 probe("gemm relaxed", lambda: C.gemm(a, b), "relaxed")
 probe("swiglu_fwd", lambda: C.swiglu_fwd(a, a.clone()))

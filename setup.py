@@ -1,4 +1,4 @@
-"""Packaging entry: `python setup.py build_ext --inplace` (or `pip install -e .`) compiles every csrc/**/*.cu|cpp for sm_100a into
+"""Packaging entry: `python setup.py build_ext --inplace` (or `pip install -e .`) compiles every csrc/**/*.cu|cpp for sm_90a into
 paddle_b200/_C*.so with the same ninja build `__graft_entry__.build()` uses; `bdist_wheel` ships the prebuilt module.
 Parity (role): the reference's setup.py / CMake super-build (L0 of SURVEY.md) - one extension instead of ~60 external deps."""
 import os
@@ -11,7 +11,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 
 class BuildNative(Command):
-    description = "compile the sm_100a extension in-tree (nvcc cross-compiles without a GPU)"
+    description = "compile the sm_90a extension in-tree (nvcc cross-compiles without a GPU)"
     user_options = [("inplace", "i", "ignored: the module is always placed next to the package")]
 
     def initialize_options(self):

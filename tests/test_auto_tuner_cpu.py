@@ -20,7 +20,7 @@ def test_memory_model_matches_the_measured_single_gpu_footprint():
     m = AT.ModelSpec(5120, 40, 13824, 32000, 4096, heads=40)
     c = dict(dp=1, mp=1, pp=1, sharding=1, sharding_stage=1, micro_batch=2, accumulate=2, recompute="none", pp_schedule="1F1B", vpp=1, sequence_parallel=False)
     gb = AT.estimate_memory_gb(m, c, optimizer_bytes=6.0)
-    assert 150 < gb < 166, gb                                    # measured: 157.6 GB (profiles/scaling_r2.md)
+    assert 150 < gb < 166, gb                                    # 130 GB of state + activations: far beyond one 80 GB GPU
     c12 = dict(c)
     assert AT.estimate_memory_gb(m, c12, optimizer_bytes=12.0) > 180          # classic fp32 master + fp32 moments does not fit one GPU
     assert AT.estimate_memory_gb(m, dict(c, recompute="full")) < gb
@@ -44,13 +44,13 @@ def test_prune_rules_by_name():
 def test_rank_prefers_sensible_layouts_and_reports_pruning():
     cands, pruned = AT.rank(LLAMA13B)
     assert cands and pruned.get("prune_by_memory", 0) > 0 and pruned.get("prune_by_pp", 0) > 0
-    assert all(c["dp"] * c["mp"] * c["pp"] * c["sharding"] == 8 and c["mem_gb"] <= 180 * 0.94 for c in cands)
+    assert all(c["dp"] * c["mp"] * c["pp"] * c["sharding"] == 8 and c["mem_gb"] <= 80 * 0.94 for c in cands)
     assert cands[0]["est_ms"] <= cands[-1]["est_ms"]
     best = cands[0]
-    assert best["mp"] <= 4 and best["recompute"] != "full"                       # no needless recompute / tensor parallel at 8 GPUs with 180 GB
+    assert best["mp"] <= 4 and best["recompute"] != "full"                       # no needless recompute / tensor parallel at 8 GPUs with 80 GB
     same = [c for c in cands if (c["dp"], c["mp"], c["pp"], c["sharding"], c["micro_batch"], c["recompute"]) == (2, 2, 2, 1, 2, "none")]
     by = {c["pp_schedule"]: c["est_ms"] for c in same if c["vpp"] in (1, 2)}
-    assert by["ZBH1"] < by["1F1B"]                                                # zero-bubble beats 1F1B at equal layout (measured: 20.6 k vs 18.7 k tokens/s)
+    assert by["ZBH1"] < by["1F1B"]                                                # zero-bubble beats 1F1B at equal layout
     res = AT.search(**{k: v for k, v in LLAMA13B.items() if k != "optimizer_bytes"}, bytes_per_param=12, top_k=3)
     assert len(res) == 3 and res[0]["est_ms"] <= res[2]["est_ms"]
 

@@ -1,4 +1,4 @@
-"""Numerics of every sm_100a kernel vs a plain PyTorch fp32 reference (run on the B200 box: pytest -m gpu)."""
+"""Numerics of every sm_90a kernel vs a plain PyTorch fp32 reference (needs a GPU: pytest -m gpu)."""
 import pytest
 import torch
 
@@ -35,7 +35,7 @@ def test_gemm_layouts(a_km, b_nk, m, n, k, dtype):
     a_in = A.t().contiguous() if a_km else A
     b_in = B.t().contiguous() if b_nk else B
     if not _ext().gemm_supported(a_in, b_in, a_km, b_nk):
-        pytest.skip("shape not supported by tcgen05 path")
+        pytest.skip("shape not supported by wgmma path")
     out = _ext().gemm(a_in, b_in, None, a_km, b_nk, 0, None, None)
     ref = A.float() @ B.float()
     assert out.shape == (m, n)
@@ -275,7 +275,7 @@ def test_flash_attention_packed_views_and_backward():
 
 @pytest.mark.parametrize("b,s,h,hk,causal", [(1, 256, 2, 2, True), (2, 512, 4, 4, True), (1, 384, 4, 2, True), (1, 300, 2, 1, False), (1, 1024, 2, 2, True)])
 def test_flash_attention_bwd_kernel(b, s, h, hk, causal):
-    """tcgen05 backward kernel vs autograd of the fp32 reference."""
+    """wgmma backward kernel vs autograd of the fp32 reference."""
     torch.manual_seed(2)
     q = (torch.randn(b, s, h, 128, device="cuda") * 0.8).to(torch.bfloat16)
     k = (torch.randn(b, s, hk, 128, device="cuda") * 0.8).to(torch.bfloat16)
@@ -312,7 +312,7 @@ def test_flash_attention_packed_api():
 @pytest.mark.parametrize("m,n,k", [(256, 512, 1024), (300, 136, 256), (4096, 5120, 5120)])
 @pytest.mark.parametrize("a_dt,b_dt", [(torch.float8_e4m3fn, torch.float8_e4m3fn), (torch.float8_e5m2, torch.float8_e4m3fn)])
 def test_gemm_fp8(m, n, k, a_dt, b_dt):
-    """tcgen05 kind::f8f6f4 GEMM vs fp32 matmul of the same fp8 values."""
+    """fp8 wgmma GEMM vs fp32 matmul of the same fp8 values."""
     from paddle_b200.kernels import gemm_fp8 as K8
 
     torch.manual_seed(0)
@@ -518,7 +518,7 @@ def test_moe_gate_utility_kernels_match_cpu():
 
 @pytest.mark.parametrize("act", ["swiglu", "gelu"])
 def test_grouped_moe_ffn_matches_per_expert_loop(act):
-    """Grouped tcgen05 expert FFN (device routing + 2 grouped GEMM launches) == a per-expert fp32 loop, forward and all gradients."""
+    """Grouped wgmma expert FFN (device routing + 2 grouped GEMM launches) == a per-expert fp32 loop, forward and all gradients."""
     from paddle_b200.kernels import moe as KM
 
     torch.manual_seed(1)
@@ -585,7 +585,7 @@ def _dense_masked_attention(q, k, v, vis, causal):
 
 @pytest.mark.parametrize("kind", ["flashmask_causal_doc", "flashmask_4", "varlen", "window"])
 def test_attention_variants_run_on_own_kernels(kind):
-    """flashmask / flash_attn_unpadded / sliding-window attention launch attn::fwd_kernel + the tcgen05 backward (launch counter) and
+    """flashmask / flash_attn_unpadded / sliding-window attention launch attn::fwd_kernel + the wgmma backward (launch counter) and
     match a dense fp32 masked softmax, forward and gradients (reference python/paddle/nn/functional/flash_attention.py:593,1098)."""
     import paddle_b200.nn.functional as F
     from paddle_b200.kernels import attention as KAT
@@ -641,7 +641,7 @@ def test_attention_variants_run_on_own_kernels(kind):
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
 @pytest.mark.parametrize("k", [1344, 5120])      # 1344 = 21 k-blocks: ragged raw boxes and uneven cluster split-K ranks; 5120: many ring phases
 def test_weight_only_linear_dequant_in_sm(wdt, m, dtype, k):
-    """csrc/gemm_wo_sm100.cu (raw int8 / int4 weights by TMA, dequantised inside the SM, tcgen05, split-K for decode) vs dequantise + fp32
+    """csrc/gemm_wo_sm100.cu (raw int8 / int4 weights by TMA, dequantised inside the SM, wgmma, split-K for decode) vs dequantise + fp32
     matmul; the kernel must be the one that runs (launch counter)."""
     from paddle_b200.nn import quant as Q
 
@@ -681,7 +681,7 @@ def test_mx_quantize_matches_reference():
 @pytest.mark.parametrize("shape", [(128, 128, 128), (256, 384, 512), (384, 1024, 256), (256, 512, 1024)])
 @pytest.mark.parametrize("out_dtype", [torch.bfloat16, torch.float32])
 def test_mx_block_scaled_gemm(shape, out_dtype):
-    """tcgen05.mma.kind::mxf8f6f4.block_scale (csrc/gemm_fp8_sm100.cu, MX): the result equals the fp32 matmul of the DEQUANTISED operands,
+    """fp8 wgmma with the MX scales applied per 32-wide k-block in registers (csrc/gemm_fp8_sm100.cu, MX): the result equals the fp32 matmul of the DEQUANTISED operands,
     with scales that differ per row and per k-block (a wrong scale slot or byte shows up as an O(1) error)."""
     from paddle_b200.kernels import gemm_fp8 as G
 
@@ -696,7 +696,9 @@ def test_mx_block_scaled_gemm(shape, out_dtype):
     y = G.mx_gemm(aq, sa, bq, sb, bias, out_dtype)
     assert kernels.launch_count() == 1
     ref = G.dequantize_mx(aq, sa) @ G.dequantize_mx(bq, sb).t() + bias.float()
-    tol = 1e-2 if out_dtype == torch.bfloat16 else 1e-5
+    # fp32 output: Hopper's fp8 MMA sums the 32 products of a k-block with about 13 bits below the largest one (measured 4.6e-5 on
+    # H100 for every shape here); across k-blocks the kernel accumulates in fp32
+    tol = 1e-2 if out_dtype == torch.bfloat16 else 1e-4
     assert rel_err(y, ref) < tol, rel_err(y, ref)
 
 
@@ -786,7 +788,7 @@ def test_fused_bias_act_kernel(act, dtype):
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
 def test_paged_block_attention_decode_and_prefill(dtype):
     """incubate/nn/paged_attention.block_attention on CUDA: vectorised cache scatter, decode rows through decode_attention_paged (block-table
-    lookups in csrc/decode_attention.cu), prefill rows through the packed varlen tcgen05 attention - against the per-token reference."""
+    lookups in csrc/decode_attention.cu), prefill rows through the packed varlen wgmma attention - against the per-token reference."""
     from paddle_b200.incubate.nn import paged_attention as PA
 
     torch.manual_seed(0)
