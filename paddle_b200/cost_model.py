@@ -9,7 +9,7 @@ class CostModel:
     def _load_peaks():
         return {"hbm_gbs": 3350.0, "bf16_tflops_sustained": 989.0}   # NVIDIA's data sheet for the H100 SXM (HBM3, dense bf16); pass measured ones
 
-    def gemm_ms(self, m, n, k, eff=0.30):
+    def gemm_ms(self, m, n, k, eff=0.68):   # median share of 989 TFLOP/s of the own GEMM on Llama-2-7B's shapes (DESIGN.md §4)
         return 2.0 * m * n * k / (self.peaks.get("bf16_tflops_sustained", 989.0) * 1e9 * eff)
 
     def mem_ms(self, nbytes, eff=0.8):

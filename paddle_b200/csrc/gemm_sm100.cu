@@ -1,6 +1,6 @@
 // Persistent warp-specialised GEMM for sm_90a: TMA (cp.async.bulk.tensor) -> 128B-swizzled smem ring -> wgmma.mma_async
-// (bf16 / fp16 operands from shared memory, fp32 accumulators in registers) -> register epilogue with fused bias / activation /
-// accumulate.  Hand-written PTX; no CUTLASS.
+// (bf16 / fp16 operands from shared memory, fp32 accumulators in registers) -> epilogue with fused bias / activation / accumulate,
+// staged through swizzled shared memory and written by asynchronous TMA stores.  Hand-written PTX; no CUTLASS.
 //
 // Parity (behaviour): phi MatmulKernel / fused_gemm_epilogue (paddle/phi/kernels/fusion/gpu/fused_gemm_epilogue_kernel.cu)
 // which call cuBLASLt in the reference.
@@ -10,7 +10,8 @@
 //   B: [N,K] row-major (K-major, "b_is_nk")  or  [K,N] row-major (MN-major)  -> paddle Linear weight is [in,out]
 // Roles (384 threads = 3 warpgroups): warpgroup 0 = producer (warp 0 TMA, warp 1 the copy role of the fused all-gather) and gives its
 // registers away; warpgroups 1 and 2 each own 64 rows of the 128 x BN tile, issue the MMAs of a k-block as one commit group, keep one
-// group in flight, and write their accumulators out while the producer is already filling the ring for the next tile.
+// group in flight, and hand their accumulators to TMA stores while the producer is already filling the ring for the next tile.
+// No kernel here may contain a function call (printf, a __noinline__ function): ptxas then serializes every wgmma of the kernel (C7510).
 // Also in this kernel: strided batches, the grouped (MoE expert) modes, the reduce-scatter push epilogue and the fused all-gather.
 #include <cuda.h>
 #include <cstdio>
@@ -49,6 +50,7 @@ struct Params {
   int64_t ldd, stride_d;
   int in_dtype, out_dtype;
   int has_bias, act, accumulate;
+  int tma_store;           // D goes out through the shared staging buffer and TMA stores (map_d); 0 = per-thread global stores
   // grouped GEMM (MoE experts, see GemmArgs::grouped): 1 = rows grouped by expert (256-row block -> expert table), 2 = per-expert weight gradient
   int grouped;
   const int* tile_expert;
@@ -81,23 +83,23 @@ __device__ __forceinline__ uint32_t ld_acquire_gpu_u32(const uint32_t* p) {
   asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
   return v;
 }
-// bounded spins: a dead peer / protocol bug traps instead of hanging the GPU
-__device__ __forceinline__ void spin_sys_ge(const uint32_t* p, uint32_t target, const char* what) {
+// bounded spins: a dead peer / protocol bug traps instead of hanging the GPU (no printf: any call in this kernel serializes its wgmma)
+__device__ __forceinline__ void spin_sys_ge(const uint32_t* p, uint32_t target) {
   const uint64_t t0 = globaltimer_ns();
   while ((int32_t)(ld_acquire_sys_u32(p) - target) < 0) {
-    if (globaltimer_ns() - t0 > 10000000000ull) { printf("b200 gemm all-gather: timeout waiting for %s\n", what); __trap(); }
+    if (globaltimer_ns() - t0 > 10000000000ull) __trap();
   }
 }
 __device__ __forceinline__ void spin_gpu_ge(const uint32_t* p, uint32_t target) {
   const uint64_t t0 = globaltimer_ns();
   while (ld_acquire_gpu_u32(p) < target) {
-    if (globaltimer_ns() - t0 > 10000000000ull) { printf("b200 gemm all-gather: timeout waiting for a gathered row block\n"); __trap(); }
+    if (globaltimer_ns() - t0 > 10000000000ull) __trap();
   }
 }
 
 // Copy role of the fused all-gather: chunk g of the remote data is handled by warp (g % #CTAs); finished chunks bump the
 // counter of their 128-row block, which the TMA producers poll before loading A rows of that block.
-__device__ __noinline__ void ag_copy_role(const Params& p, int lane) {
+__device__ __forceinline__ void ag_copy_role(const Params& p, int lane) {
   const int nwarps = gridDim.x, wid = blockIdx.x;
   const int blocks_per_rank = p.ag_rows / BLOCK_M;
   const int64_t block_bytes = (int64_t)BLOCK_M * p.k * 2;
@@ -113,7 +115,7 @@ __device__ __noinline__ void ag_copy_role(const Params& p, int lane) {
     const int64_t rem = g - (int64_t)(pr - 1) * per_src;
     const int blk_in = (int)(rem / p.ag_chunks), ch = (int)(rem % p.ag_chunks);
     if (src != cur_src) {
-      if (lane == 0) spin_sys_ge(my_pad + kAgReadySlot * kPadRanks + src, p.ag_epoch, "a peer shard");
+      if (lane == 0) spin_sys_ge(my_pad + kAgReadySlot * kPadRanks + src, p.ag_epoch);
       __syncwarp();
       cur_src = src;
     }
@@ -143,7 +145,7 @@ __device__ __noinline__ void ag_copy_role(const Params& p, int lane) {
     }
   }
   if (wid == 0 && lane < p.ag_world && lane != p.ag_rank)        // peers finished reading my shard: it may be reused after exit
-    spin_sys_ge(my_pad + kAgDoneSlot * kPadRanks + lane, p.ag_epoch, "a peer to finish reading");
+    spin_sys_ge(my_pad + kAgDoneSlot * kPadRanks + lane, p.ag_epoch);
 }
 
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
@@ -168,16 +170,93 @@ __device__ __forceinline__ void store_pair(TO* __restrict__ dst, float v0, float
   }
 }
 
+// Staged epilogue: the consumer warpgroup's 64 x BN half-tile leaves as boxes of 64 rows x 128 bytes (64 16-bit or 32 fp32 columns),
+// written 128B-swizzled into one of two 8 KB slots of the warpgroup's staging buffer and stored by TMA. Box c (counted over the
+// warpgroup's whole run in `cnt`) uses slot c & 1, so it is written while the store of box c - 1 still reads the other slot.
+// Invariant: once the warpgroup has passed the named barrier of box c, slot (c + 1) & 1 is free (the elected thread waited for the
+// store of box c - 1 to finish reading it just before that barrier). In accumulate mode the old D box is TMA-loaded into its slot
+// first (box 0 of a tile during the mainloop, box c + 1 right after box c is stored) and added in fp32, rounded once, as in
+// store_pair. TMA clips the boxes at the tensor bounds, so partial tiles need no per-element tests.
+constexpr uint32_t kStageSlotBytes = 8192;
+
+template <typename TO, int BN>
+__device__ __forceinline__ void epilogue_tma(const float (&acc)[BN / 2], const Params& p, const CUtensorMap* map_d, uint8_t* stg,
+                                             uint32_t ld_bar, uint32_t& cnt, int m0, int n0, int zd, int ww, int lane, int bar_id) {
+  constexpr int CB = 128 / sizeof(TO);                    // columns per box
+  constexpr int NB = BN / CB;                             // boxes per half-tile (BN >= 64)
+  struct alignas(2 * sizeof(TO)) Pair { TO a, b; };
+  const int nbox = min(NB, (p.n - n0 + CB - 1) / CB);     // boxes that start right of column n are skipped
+  const bool elected = ww == 0 && lane == 0;
+  const int rq = lane >> 2;                               // row within the 8-row swizzle atom
+#pragma unroll
+  for (int b = 0; b < NB; ++b) {
+    if (b >= nbox) break;
+    uint8_t* slot = stg + (cnt & 1) * kStageSlotBytes;
+    if (p.accumulate) mbar_wait(ld_bar + 8 * (cnt & 1), (cnt >> 1) & 1);
+#pragma unroll
+    for (int jj = 0; jj < CB / 8; ++jj) {
+      const int j = b * (CB / 8) + jj;
+      const int col = n0 + j * 8 + (lane & 3) * 2;
+      const int valid = p.n - col;
+      float b0 = 0.f, b1 = 0.f;
+      if (p.has_bias && valid > 0) {
+        if (p.in_dtype == kBF16) {
+          const __nv_bfloat16* bp = (const __nv_bfloat16*)p.bias + col;
+          b0 = __bfloat162float(bp[0]);
+          if (valid > 1) b1 = __bfloat162float(bp[1]);
+        } else {
+          const __half* bp = (const __half*)p.bias + col;
+          b0 = __half2float(bp[0]);
+          if (valid > 1) b1 = __half2float(bp[1]);
+        }
+      }
+      const uint32_t byte = (jj * 8 + (lane & 3) * 2) * sizeof(TO);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        Pair* dst = reinterpret_cast<Pair*>(slot + (ww * 16 + h * 8 + rq) * 128 + (((byte >> 4) ^ rq) << 4) + (byte & 15));
+        float v0 = acc[j * 4 + h * 2] + b0, v1 = acc[j * 4 + h * 2 + 1] + b1;
+        if (p.act == 1) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
+        else if (p.act == 2) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+        if (p.accumulate) {
+          const Pair old = *dst;
+          v0 += to_f(old.a);
+          v1 += to_f(old.b);
+        }
+        Pair o;
+        o.a = from_f<TO>(v0);
+        o.b = from_f<TO>(v1);
+        *dst = o;
+      }
+    }
+    fence_proxy_async();                                  // generic-proxy writes -> the TMA store (async proxy) reads them
+    if (elected) bulk_wait_group_read<0>();               // the store of box cnt - 1 is done with the other slot
+    named_bar_sync(bar_id, 128);
+    if (elected) {
+      tma_store_3d(map_d, smem_u32(slot), n0 + b * CB, m0, zd);
+      bulk_commit_group();
+      if (p.accumulate && b + 1 < nbox) {
+        const uint32_t next = (cnt + 1) & 1;
+        mbar_expect_tx(ld_bar + 8 * next, kStageSlotBytes);
+        tma_load_3d(smem_u32(stg + next * kStageSlotBytes), map_d, ld_bar + 8 * next, n0 + (b + 1) * CB, m0, zd);
+      }
+    }
+    ++cnt;
+  }
+}
+
 template <int BN, bool BF16, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(kThreads, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const Params p) {
+gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
+            const __grid_constant__ CUtensorMap map_d, const Params p) {
   using C = Cfg<BN>;
   constexpr int kStages = C::kStages;
   extern __shared__ uint8_t smem_raw[];
+  __shared__ __align__(1024) uint8_t staging[2][2 * kStageSlotBytes];   // per consumer warpgroup (epilogue_tma)
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;  // SWIZZLE_128B needs 1024B alignment
   const uint32_t bar_base = smem_base + kStages * C::STAGE_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (kStages + s); };
+  auto load_bar = [&](int wg) { return bar_base + 8u * (2 * kStages + 2 * wg); };   // two slots per warpgroup (accumulate mode)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_m = (p.m + BLOCK_M - 1) / BLOCK_M, num_n = (p.n + BN - 1) / BN;
@@ -188,7 +267,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&map_a);
     tma_prefetch_desc(&map_b);
+    if (p.tma_store) tma_prefetch_desc(&map_d);
     for (int s = 0; s < kStages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kConsumerWarps); }
+    for (int s = 0; s < 4; ++s) mbar_init(load_bar(0) + 8u * s, 1);
     fence_barrier_init();
     fence_proxy_async();
   }
@@ -276,12 +357,19 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
     const int wg = (warp >> 2) - 1, ww = warp & 3;
     int stage = 0;
     uint32_t phase = 0;
+    uint32_t boxes = 0;                        // staged epilogue boxes issued by this warpgroup (epilogue_tma)
+    const bool elected = ww == 0 && lane == 0;
     float acc[BN / 2];
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       int bz, mb, nb;
       tile_coords(tile, bz, mb, nb);
       int za, zb, zd, kbeg, nkb;
       if (!tile_group(bz, mb, za, zb, zd, kbeg, nkb)) continue;
+      if (p.tma_store && p.accumulate && elected) {   // old D of the first epilogue box lands during the mainloop
+        const uint32_t s = boxes & 1;
+        mbar_expect_tx(load_bar(wg) + 8 * s, kStageSlotBytes);
+        tma_load_3d(smem_u32(staging[wg] + s * kStageSlotBytes), &map_d, load_bar(wg) + 8 * s, nb * BN, mb * BLOCK_M + wg * 64, zd);
+      }
       int prev = -1;
       for (int kb = 0; kb < nkb; ++kb) {
         mbar_wait(full_bar(stage), phase);
@@ -310,7 +398,15 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
       wgmma_fence_regs(acc);
       if (lane == 0) mbar_arrive(empty_bar(prev));
 
-      // ---- epilogue from the accumulator fragment: rows r0 and r0 + 8, per 8-column group the columns 2 (lane % 4), + 1 ----
+      if (p.tma_store) {
+        const int m0 = mb * BLOCK_M + wg * 64, n0 = nb * BN;
+        if (p.out_dtype == kBF16) epilogue_tma<__nv_bfloat16, BN>(acc, p, &map_d, staging[wg], load_bar(wg), boxes, m0, n0, zd, ww, lane, 1 + wg);
+        else if (p.out_dtype == kF16) epilogue_tma<__half, BN>(acc, p, &map_d, staging[wg], load_bar(wg), boxes, m0, n0, zd, ww, lane, 1 + wg);
+        else epilogue_tma<float, BN>(acc, p, &map_d, staging[wg], load_bar(wg), boxes, m0, n0, zd, ww, lane, 1 + wg);
+        continue;
+      }
+      // ---- register epilogue (reduce-scatter push, or D not 16-byte aligned for a tensor map) from the accumulator fragment:
+      // rows r0 and r0 + 8, per 8-column group the columns 2 (lane % 4), + 1 ----
       const int r0 = mb * BLOCK_M + wg * 64 + ww * 16 + (lane >> 2);
 #pragma unroll
       for (int j = 0; j < BN / 8; ++j) {
@@ -350,6 +446,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
         }
       }
     }
+    if (p.tma_store && elected) bulk_wait_group<0>();   // the staging buffer must outlive the last store's reads
   }
 }
 
@@ -444,6 +541,12 @@ static int launch(const GemmArgs& g, cudaStream_t s) {
   p.rs_rows = g.rs_rows;
   for (int i = 0; i < 8; ++i) p.rs_dst[i] = g.rs_dst[i];
   if (p.rs_world) p.ldd = g.n;
+  // TMA-store epilogue wherever D can be described by a tensor map: local memory, 16-byte aligned base and strides
+  CUtensorMap md{};
+  const uint64_t es = g.out_dtype == kF32 ? 4 : 2;
+  p.tma_store = !p.rs_world && (reinterpret_cast<uintptr_t>(g.d) & 15) == 0 && ((uint64_t)g.ldd * es) % 16 == 0 &&
+                (batch == 1 || ((uint64_t)g.stride_d * es) % 16 == 0);
+  if (p.tma_store && !make_map(&md, g.d, g.n, g.m, batch, g.ldd, g.stride_d, 128 / es, 64, g.out_dtype)) return 2;
   p.ag_world = 0;
   if (g.ag_world > 1) {
     // preconditions of the fused all-gather (checked by the caller as well): A is K-major with lda == k, whole 256-row blocks per rank
@@ -471,7 +574,7 @@ static int launch(const GemmArgs& g, cudaStream_t s) {
   static const int reserve = [] { const char* e = getenv("B200_GEMM_RESERVE_SMS"); const int v = e ? atoi(e) : 0; return v < 0 ? 0 : v; }();
   const int usable = sm_count() - reserve > 0 ? sm_count() - reserve : 1;
   const int grid = num_tiles < usable ? num_tiles : usable;
-  kern<<<grid, kThreads, C::SMEM_BYTES, s>>>(ma, mb, p);
+  kern<<<grid, kThreads, C::SMEM_BYTES, s>>>(ma, mb, md, p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }
   return 0;

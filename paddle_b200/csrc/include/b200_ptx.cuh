@@ -29,6 +29,7 @@ __device__ __forceinline__ uint64_t globaltimer_ns() {
   return t;
 }
 // Bounded wait: a protocol bug must trap (visible error, cudaErrorLaunchFailure) instead of hanging the GPU.
+// No printf here: a call inside a kernel that issues wgmma makes ptxas serialize every wgmma.mma_async of that kernel (C7510).
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   uint32_t done = 0, spins = 0;
   uint64_t t0 = 0;
@@ -42,10 +43,7 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         : "memory");
     if (done) break;
     if (++spins == 2048) t0 = globaltimer_ns();
-    if (spins > 2048 && (spins & 1023) == 0 && globaltimer_ns() - t0 > 4000000000ull) {
-      printf("b200: mbarrier wait timeout (block %d,%d,%d thread %d bar %u parity %u)\n", blockIdx.x, blockIdx.y, blockIdx.z, threadIdx.x, bar, parity);
-      __trap();
-    }
+    if (spins > 2048 && (spins & 1023) == 0 && globaltimer_ns() - t0 > 4000000000ull) __trap();
   }
 }
 
@@ -81,6 +79,16 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map
       ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+// tile shared -> global (async proxy; out-of-bounds parts of the box are not written), tracked per thread in bulk groups
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
+               ::"l"(map), "r"(src), "r"(c0), "r"(c1), "r"(c2) : "memory");
+}
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's committed bulk groups still read their shared-memory source
+template <int N> __device__ __forceinline__ void bulk_wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// at most N of this thread's committed bulk groups are still incomplete (their global writes not yet performed)
+template <int N> __device__ __forceinline__ void bulk_wait_group() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
 // contiguous bytes global -> shared, completion on an mbarrier
 __device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");

@@ -91,9 +91,10 @@ def estimate_memory_gb(m, c, optimizer_bytes=6.0, hbm_reserve_gb=4.0):
     return (w + g + o + act + logits) / GB + hbm_reserve_gb
 
 
-def estimate_step_ms(m, c, cm=None, gemm_eff=0.30, attn_eff=0.19, global_batch=None):
+def estimate_step_ms(m, c, cm=None, gemm_eff=0.68, attn_eff=0.18, global_batch=None):
     """Analytic step time of candidate `c`; the efficiencies are shares of the data-sheet bf16 rate that the own kernels reached on an
-    H100 80GB HBM3 at 700 W (DESIGN.md §4): GEMMs of 8192 rows ~300 TFLOP/s, attention forward + backward ~190 TFLOP/s."""
+    H100 80GB HBM3 at 700 W (DESIGN.md §4): GEMMs of Llama-2-7B's 4096-row shapes 580 - 790 TFLOP/s (median ~680), causal attention
+    forward + backward ~175 TFLOP/s."""
     cm = cm or CostModel()
     peak = cm.peaks.get("bf16_tflops_sustained", 989.0) * 1e9         # FLOP per ms
     mp, pp, sh, dp = c["mp"], c["pp"], c["sharding"], c["dp"]
