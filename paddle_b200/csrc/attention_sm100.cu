@@ -9,7 +9,14 @@
 // CTA = 128 query rows of one (batch, head): two MMA warpgroups of 64 rows each (warps 0-7) walk the key tiles with their own running
 // (max, sum) and O accumulator; nothing is exchanged between them, so one warpgroup's softmax runs under the other's MMAs.  Warp 8 is
 // the TMA producer (Q once, K and V double-buffered with separate barriers so that S of a tile can start before its V has landed).
+//
+// PAGED instantiation (prefill / chunked prefill for serving): the queries are the new tokens of each sequence, read in place from the
+// packed qkv rows, and K / V come straight from the block-table KV cache [num_blocks, Hkv, block_size, D].  A CTA takes one (sequence,
+// 128-row query tile) from a work list built on the device (heaviest tiles first) and walks only its own sequence's key tiles up to the
+// bottom-right causal limit.  A 128-key tile is assembled from {64 d, min(block_size, 64) rows} boxes, each at a 1024-byte multiple of
+// the tile, so the 128B-swizzled shared tile is byte-for-byte what one dense box would have written and the MMA code is unchanged.
 #include <cuda.h>
+#include <algorithm>
 #include <cstdio>
 #include <string>
 #include <type_traits>
@@ -48,12 +55,27 @@ struct Params {
   const int4* colmask;        // [b, mask_heads, sk] row ranges hidden from every key column (nullptr: none)
   int mask_heads;
 };
+// The paged instantiation's parameters (the dense ones keep the smaller Params: a different kernel-parameter block changes their code).
+// sq is the number of packed token rows, b the number of sequences.
+struct PagedParams : Params {
+  const int2* work;           // [gridDim.y] {sequence, query tile}; sequence < 0: spare CTA
+  const int* cu_q;            // [b] first packed row of each sequence's new tokens
+  const int* n_q;             // [b] new tokens (0: not a prefill sequence)
+  const int* past;            // [b] tokens already cached before them
+  const int* block_tables;    // [b, max_blocks]
+  int max_blocks, block_size;
+};
+
+__device__ __forceinline__ void st_shared_zero16(uint32_t addr) {
+  asm volatile("st.shared.v4.u32 [%0], {%1, %1, %1, %1};" ::"r"(addr), "r"(0) : "memory");
+}
 
 // MASKED: column-wise row-range mask (flashmask / varlen) compiled in; the dense instantiation carries none of its code or registers
-template <typename T, bool MASKED>
+// PAGED: queries = new tokens of each sequence, K / V read through the block table (see the file header); always causal, never MASKED
+template <typename T, bool MASKED, bool PAGED = false>
 __global__ void __launch_bounds__(kThreads, 1)
 fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
-           const __grid_constant__ CUtensorMap map_v, const Params p) {
+           const __grid_constant__ CUtensorMap map_v, const std::conditional_t<PAGED, PagedParams, Params> p) {
   constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -68,13 +90,25 @@ fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CU
   auto v_empty = [&](int s) { return bars + 8u * (7 + s); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m_tile = (int)gridDim.x - 1 - (int)blockIdx.x;   // long (late) rows first under the causal mask
-  const int head = blockIdx.y, batch = blockIdx.z;
+  int m_tile, head, batch, sk, causal_off, nrows, q0 = 0;
+  if constexpr (PAGED) {
+    const int2 w = p.work[blockIdx.y];
+    if (w.x < 0) return;                                      // spare CTA: the grid is an upper bound on the work list
+    batch = w.x; m_tile = w.y; head = blockIdx.x;
+    q0 = __ldg(p.cu_q + batch);
+    nrows = __ldg(p.n_q + batch);
+    causal_off = __ldg(p.past + batch);
+    sk = causal_off + nrows;
+  } else {
+    m_tile = (int)gridDim.x - 1 - (int)blockIdx.x;          // long (late) rows first under the causal mask
+    head = blockIdx.y; batch = blockIdx.z;
+    sk = p.sk; causal_off = p.causal_off; nrows = p.sq;
+  }
   const int kv_head = head / (p.h / p.hk);
   const int m0 = m_tile * BM;
-  int n_tiles = (p.sk + BN - 1) / BN;
-  if (p.causal) {
-    const int last_key = min(p.sk - 1, m0 + BM - 1 + p.causal_off);
+  int n_tiles = (sk + BN - 1) / BN;
+  if (p.causal) {                                            // always set for PAGED
+    const int last_key = min(sk - 1, m0 + BM - 1 + causal_off);
     n_tiles = last_key < 0 ? 0 : min(n_tiles, last_key / BN + 1);
   }
 
@@ -90,7 +124,36 @@ fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CU
   __syncthreads();
 
   if (warp == 8) {
-    if (lane == 0 && n_tiles > 0) {
+    if constexpr (PAGED) {
+      if (n_tiles > 0) {
+        // ================= TMA producer, paged: lane l loads box l % C of K half / V d-half l / C =================
+        const int bsz = p.block_size, R = min(bsz, 64), C = BN / R;   // C boxes of R key rows per 128-key K half and per 64-d V half
+        const int* bt = p.block_tables + (int64_t)batch * p.max_blocks;
+        const int last_blk = __ldg(bt + (sk - 1) / bsz);            // table entries past the sequence are never read
+        const int c = lane % C, half = lane / C;
+        if (lane == 0) {
+          mbar_expect_tx(q_full, TILE_BYTES);
+          tma_load_4d(sQ, &map_q, q_full, 0, q0 + m0, head, 0);
+          tma_load_4d(sQ + HALF_BYTES, &map_q, q_full, 64, q0 + m0, head, 0);
+        }
+        for (int j = 0; j < n_tiles; ++j) {
+          const int s = j & 1, key = j * BN + c * R;
+          const uint32_t ph = ((j >> 1) & 1) ^ 1;
+          // keys past the sequence come from a valid block (masked in S, zeroed in V) so every tile carries the same bytes
+          const int blk = lane < 2 * C ? (key < sk ? __ldg(bt + key / bsz) : last_blk) : 0;
+          const int row = key % bsz;
+          mbar_wait(k_empty(s), ph);
+          if (lane == 0) mbar_expect_tx(k_full(s), TILE_BYTES);
+          __syncwarp();
+          if (lane < 2 * C) tma_load_4d(sK(s) + half * HALF_BYTES + c * R * 128, &map_k, k_full(s), half * 64, row, kv_head, blk);
+          mbar_wait(v_empty(s), ph);
+          if (lane == 0) mbar_expect_tx(v_full(s), TILE_BYTES);
+          __syncwarp();
+          if (lane < 2 * C)
+            tma_load_4d(sV(s) + (c * R / 64) * HALF_BYTES + half * 8192 + (c * R % 64) * 128, &map_v, v_full(s), half * 64, row, kv_head, blk);
+        }
+      }
+    } else if (lane == 0 && n_tiles > 0) {
       // ================= TMA producer =================
       mbar_expect_tx(q_full, TILE_BYTES);
       tma_load_4d(sQ, &map_q, q_full, 0, m0, head, batch);
@@ -138,12 +201,13 @@ fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CU
       __syncwarp();
       if (lane == 0) mbar_arrive(k_empty(s));
       // ---- masks (raw logits; the softmax scale is folded into the exp2 FFMA) ----
-      const bool edge = (j * BN + BN > p.sk) || (p.causal && j * BN + BN - 1 > m0 + p.causal_off);
+      const bool edge = PAGED ? (j * BN + BN > sk) || (j * BN + BN - 1 > m0 + causal_off)
+                              : (j * BN + BN > p.sk) || (p.causal && j * BN + BN - 1 > m0 + p.causal_off);
       if (edge) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int row = m0 + rl + h * 8;
-          const int lim = (p.causal ? min(p.sk - 1, row + p.causal_off) : p.sk - 1) - j * BN;   // last visible key, tile-relative
+          const int lim = (p.causal ? min(sk - 1, row + causal_off) : sk - 1) - j * BN;   // last visible key, tile-relative
 #pragma unroll
           for (int jn = 0; jn < BN / 8; ++jn)
 #pragma unroll
@@ -203,6 +267,17 @@ fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CU
         pa[ks][3] = pack2<T>(sv[ks * 8 + 6], sv[ks * 8 + 7]);
       }
       mbar_wait(v_full(s), ph);
+      if constexpr (PAGED) {
+        if (j * BN + BN > sk) {   // V rows past the sequence hold stale cache contents (possibly NaN) and P = 0 does not cancel NaN: zero them
+          const int tid = threadIdx.x & 127;
+          for (int e = (sk - j * BN) * 16 + tid; e < BN * 16; e += 128) {   // 16-byte chunks: key row e / 16, d-half (e / 8) & 1
+            const int r = e >> 4;
+            st_shared_zero16(sV(s) + (r >> 6) * HALF_BYTES + ((e >> 3) & 1) * 8192 + (r & 63) * 128 + (e & 7) * 16);
+          }
+          fence_proxy_async();                    // generic-proxy stores before this warpgroup's wgmma reads them
+          named_bar_sync(1 + wg, 128);
+        }
+      }
       wgmma_fence_regs(o_acc);
       wgmma_fence();
 #pragma unroll
@@ -226,12 +301,12 @@ fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CU
       l += __shfl_xor_sync(0xffffffffu, l, 2);
       const float inv = l > 0.f ? 1.f / l : 0.f;
       const int row = m0 + rl + h * 8;
-      if (row < p.sq) {
-        T* orow = reinterpret_cast<T*>(p.o) + (int64_t)batch * p.o_sb + (int64_t)row * p.o_ss + (int64_t)head * p.o_sh;
+      if (row < nrows) {
+        T* orow = reinterpret_cast<T*>(p.o) + (PAGED ? 0 : (int64_t)batch * p.o_sb) + (int64_t)(q0 + row) * p.o_ss + (int64_t)head * p.o_sh;
 #pragma unroll
         for (int jn = 0; jn < HD / 8; ++jn)
           *reinterpret_cast<uint32_t*>(orow + jn * 8 + 2 * q) = pack2<T>(o_acc[jn * 4 + h * 2] * inv, o_acc[jn * 4 + h * 2 + 1] * inv);
-        if (q == 0 && p.lse) p.lse[((int64_t)batch * p.h + head) * p.sq + row] = l > 0.f ? (m_i[h] + log2f(l)) * 0.69314718055994531f : -INFINITY;
+        if (q == 0 && p.lse) p.lse[((int64_t)(PAGED ? 0 : batch) * p.h + head) * p.sq + q0 + row] = l > 0.f ? (m_i[h] + log2f(l)) * 0.69314718055994531f : -INFINITY;
       }
     }
   }
@@ -269,6 +344,50 @@ static bool make_map4(CUtensorMap* out, const void* ptr, int d, int s, int h, in
     return false;
   }
   return true;
+}
+
+// Work list of the paged kernel: one (sequence, 128-row query tile) per slot, sorted by key tiles (heaviest first, ties in sequence
+// order) so a long prefix starts early instead of running alone at the end; slots past the list get sequence -1.  One CTA; the
+// O(tiles^2) ranking is a few hundred thousand compares at the largest batches, well under the attention it schedules.
+// scratch: int32 [slots] key-tile counts followed by [b + 1] tile offsets.
+__global__ void __launch_bounds__(1024) paged_work_kernel(const int* __restrict__ n_q, const int* __restrict__ past, int b, int slots,
+                                                          int* scratch, int2* work) {
+  int* keys = scratch;
+  int* start = scratch + slots;
+  if (threadIdx.x == 0) {
+    int acc = 0;
+    for (int i = 0; i < b; ++i) { start[i] = acc; acc += (max(n_q[i], 0) + BM - 1) / BM; }
+    start[b] = acc;
+  }
+  __syncthreads();
+  const int n = min(start[b], slots);
+  auto seq_of = [&](int w) {   // last sequence whose first tile is <= w (sequences without tiles share their successor's offset)
+    int lo = 0, hi = b - 1;
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (start[mid] <= w) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+  };
+  for (int w = threadIdx.x; w < n; w += blockDim.x) {
+    const int sq = seq_of(w), m0 = (w - start[sq]) * BM;
+    keys[w] = (past[sq] + min(n_q[sq] - 1, m0 + BM - 1)) / BN + 1;   // key tiles up to the causal limit of the tile's last row
+  }
+  __syncthreads();
+  for (int w = threadIdx.x; w < slots; w += blockDim.x) {
+    if (w < n) {
+      const int kw = keys[w];
+      int rank = 0;
+      for (int u = 0; u < n; ++u) {
+        const int ku = keys[u];
+        rank += (ku > kw) || (ku == kw && u < w);
+      }
+      const int sq = seq_of(w);
+      work[rank] = make_int2(sq, w - start[sq]);
+    } else {
+      work[w] = make_int2(-1, -1);
+    }
+  }
 }
 
 }  // namespace attn
@@ -319,6 +438,58 @@ int attention_fwd(const AttnArgs& a, cudaStream_t s) {
   } else {
     auto kern = fwd_kernel<__half, true>;
     if (!attr_h_m) { B200_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES)); attr_h_m = true; }
+    kern<<<grid, kThreads, SMEM_BYTES, s>>>(mq, mk, mv, p);
+  }
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) { set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }
+  return 0;
+}
+
+int attention_paged_prefill_slots(int t, int b) { return (t + attn::BM - 1) / attn::BM + b; }
+int attention_paged_prefill_scratch_ints(int t, int b) { return 3 * attention_paged_prefill_slots(t, b) + b + 1; }
+
+int attention_paged_prefill_supported(const PagedAttnArgs& a) {
+  if (a.d != 128 || (a.dtype != kBF16 && a.dtype != kF16)) return 0;
+  if (a.hk <= 0 || a.h % a.hk) return 0;
+  if (a.block_size != 16 && a.block_size != 32 && a.block_size != 64 && a.block_size != 128 && a.block_size != 256) return 0;
+  if (a.q_strides[0] % 8 || a.q_strides[1] % 8 || a.o_strides[0] % 8 || a.o_strides[1] % 8) return 0;   // 16-byte rows
+  if ((reinterpret_cast<uintptr_t>(a.q) | reinterpret_cast<uintptr_t>(a.k_cache) | reinterpret_cast<uintptr_t>(a.v_cache) |
+       reinterpret_cast<uintptr_t>(a.o)) & 15) return 0;
+  return 1;
+}
+
+int attention_paged_prefill(const PagedAttnArgs& a, cudaStream_t s) {
+  using namespace attn;
+  if (!attention_paged_prefill_supported(a)) return 1;
+  if (a.t == 0 || a.b == 0) return 0;
+  const int slots = attention_paged_prefill_slots(a.t, a.b);
+  const int64_t blk = (int64_t)a.block_size * a.d;
+  const uint32_t rows = (uint32_t)std::min(a.block_size, 64);
+  CUtensorMap mq, mk, mv;
+  // q: {d, token, head, 1} over the strided [T, H, D] view; caches: {d, row in block, kv head, block}
+  if (!make_map4(&mq, a.q, a.d, a.t, a.h, 1, a.q_strides[0], a.q_strides[1], a.q_strides[0] * a.t, BM, a.dtype)) return 2;
+  if (!make_map4(&mk, a.k_cache, a.d, a.block_size, a.hk, a.num_blocks, a.d, blk, blk * a.hk, rows, a.dtype)) return 2;
+  if (!make_map4(&mv, a.v_cache, a.d, a.block_size, a.hk, a.num_blocks, a.d, blk, blk * a.hk, rows, a.dtype)) return 2;
+  int2* work = reinterpret_cast<int2*>(a.scratch);
+  paged_work_kernel<<<1, 1024, 0, s>>>(a.n_q, a.past, a.b, slots, a.scratch + 2 * slots, work);
+  PagedParams p = {};
+  p.b = a.b; p.sq = a.t; p.sk = 0; p.h = a.h; p.hk = a.hk;
+  p.scale_log2 = a.scale * 1.4426950408889634f;
+  p.causal = 1; p.causal_off = 0;
+  p.o = a.o; p.lse = a.lse;
+  p.o_sb = 0; p.o_ss = a.o_strides[0]; p.o_sh = a.o_strides[1];
+  p.colmask = nullptr; p.mask_heads = 1;
+  p.work = work; p.cu_q = a.cu_q; p.n_q = a.n_q; p.past = a.past;
+  p.block_tables = a.block_tables; p.max_blocks = a.max_blocks; p.block_size = a.block_size;
+  dim3 grid(a.h, slots);   // every head of the heaviest tile is dispatched first
+  static bool attr_bf = false, attr_h = false;
+  if (a.dtype == kBF16) {
+    auto kern = fwd_kernel<__nv_bfloat16, false, true>;
+    if (!attr_bf) { B200_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES)); attr_bf = true; }
+    kern<<<grid, kThreads, SMEM_BYTES, s>>>(mq, mk, mv, p);
+  } else {
+    auto kern = fwd_kernel<__half, false, true>;
+    if (!attr_h) { B200_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES)); attr_h = true; }
     kern<<<grid, kThreads, SMEM_BYTES, s>>>(mq, mk, mv, p);
   }
   cudaError_t e = cudaGetLastError();

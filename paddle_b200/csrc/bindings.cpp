@@ -814,6 +814,50 @@ std::vector<Tensor> attention_fwd(const Tensor& q, const Tensor& k, const Tensor
   return {out, lse};
 }
 
+// Causal prefill over the paged KV cache (new K / V already written to the caches): q [T,H,D] view of the packed qkv rows, caches
+// [num_blocks,Hkv,block_size,D], block_tables int32 [B,max_blocks], cu_q / n_q / past int32 [B] (n_q = 0: sequence skipped); writes
+// out [T,H*D] at the new tokens' rows only, and lse fp32 [H,T] at the same rows when given.  No host read of the lengths.
+void attention_fwd_paged(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& block_tables, const Tensor& cu_q,
+                         const Tensor& n_q, const Tensor& past, double scale, const Tensor& out, const OptT& lse) {
+  TORCH_CHECK(q.is_cuda() && q.dim() == 3 && q.stride(2) == 1, "attention_fwd_paged: q must be a CUDA [T,H,D] view with unit head_dim stride");
+  TORCH_CHECK(k_cache.dim() == 4 && v_cache.dim() == 4 && k_cache.is_contiguous() && v_cache.is_contiguous() && k_cache.sizes() == v_cache.sizes(),
+              "attention_fwd_paged: caches must be contiguous [num_blocks,Hkv,block_size,D] of one shape");
+  TORCH_CHECK(k_cache.scalar_type() == q.scalar_type() && v_cache.scalar_type() == q.scalar_type(), "attention_fwd_paged: q and caches must share a dtype");
+  TORCH_CHECK(k_cache.device() == q.device() && v_cache.device() == q.device(), "attention_fwd_paged: q and caches must be on one device");
+  TORCH_CHECK(block_tables.device() == q.device() && block_tables.scalar_type() == at::kInt && block_tables.is_contiguous() && block_tables.dim() == 2,
+              "attention_fwd_paged: block_tables must be int32 [B, max_blocks] on the device");
+  const int64_t b = block_tables.size(0);
+  for (const Tensor* t : {&cu_q, &n_q, &past})
+    TORCH_CHECK(t->device() == q.device() && t->scalar_type() == at::kInt && t->is_contiguous() && t->numel() == b,
+                "attention_fwd_paged: cu_q / n_q / past must be int32 [B] on the device");
+  TORCH_CHECK(out.device() == q.device() && out.scalar_type() == q.scalar_type() && out.dim() == 2 && out.size(0) == q.size(0) &&
+              out.size(1) == q.size(1) * q.size(2) && out.stride(1) == 1, "attention_fwd_paged: out must be [T, H*D] with unit inner stride");
+  b200::PagedAttnArgs a;
+  a.q = q.data_ptr(); a.k_cache = k_cache.data_ptr(); a.v_cache = v_cache.data_ptr(); a.o = out.data_ptr(); a.lse = nullptr;
+  a.t = (int)q.size(0); a.h = (int)q.size(1); a.d = (int)q.size(2);
+  a.num_blocks = (int)k_cache.size(0); a.hk = (int)k_cache.size(1); a.block_size = (int)k_cache.size(2);
+  TORCH_CHECK(k_cache.size(3) == q.size(2), "attention_fwd_paged: head_dim of q and caches differ");
+  a.b = (int)b; a.max_blocks = (int)block_tables.size(1);
+  a.q_strides[0] = q.stride(0); a.q_strides[1] = q.stride(1);
+  a.o_strides[0] = out.stride(0); a.o_strides[1] = a.d;
+  a.block_tables = block_tables.data_ptr<int>(); a.cu_q = cu_q.data_ptr<int>(); a.n_q = n_q.data_ptr<int>(); a.past = past.data_ptr<int>();
+  a.scale = (float)scale; a.dtype = dt_code(q);
+  if (lse.has_value() && lse->defined()) {
+    TORCH_CHECK(lse->device() == q.device() && lse->scalar_type() == at::kFloat && lse->is_contiguous() && lse->dim() == 2 && lse->size(0) == a.h &&
+                lse->size(1) == a.t, "attention_fwd_paged: lse must be fp32 [H, T]");
+    a.lse = lse->data_ptr<float>();
+  }
+  TORCH_CHECK(b200::attention_paged_prefill_supported(a), "attention_fwd_paged: unsupported operands (head_dim 128, fp16/bf16, H % Hkv == 0, "
+              "block_size in {16, 32, 64, 128, 256}, 16-byte aligned rows)");
+  c10::cuda::CUDAGuard guard(q.device());
+  Tensor scratch = torch::empty({b200::attention_paged_prefill_scratch_ints(a.t, a.b)}, q.options().dtype(at::kInt));
+  a.scratch = scratch.data_ptr<int>();
+  int rc = b200::attention_paged_prefill(a, cur_stream());
+  g_launches += 2;
+  check_err();
+  TORCH_CHECK(rc == 0, "paddle_b200.attention_fwd_paged launch failed rc=", rc);
+}
+
 static bool g_deterministic = false;     // FLAGS_cudnn_deterministic (the attention backward is order-independent as it is)
 
 // backward of attention_fwd: returns (dq [B,Sq,H,D], dk, dv [B,Sk,Hk,D]) in the input dtype
@@ -941,6 +985,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("attention_supported", &attention_supported);
   m.def("attention_fwd", traced("attention_fwd", &attention_fwd), pybind11::arg("q"), pybind11::arg("k"), pybind11::arg("v"), pybind11::arg("scale"), pybind11::arg("causal"),
         pybind11::arg("out_seq_major") = false, pybind11::arg("colmask") = pybind11::none());
+  m.def("attention_fwd_paged", traced("attention_fwd_paged", &attention_fwd_paged), pybind11::arg("q"), pybind11::arg("k_cache"),
+        pybind11::arg("v_cache"), pybind11::arg("block_tables"), pybind11::arg("cu_q"), pybind11::arg("n_q"), pybind11::arg("past"), pybind11::arg("scale"),
+        pybind11::arg("out"), pybind11::arg("lse") = pybind11::none());
   m.def("attention_bwd", traced("attention_bwd", &attention_bwd), pybind11::arg("q"), pybind11::arg("k"), pybind11::arg("v"), pybind11::arg("out"), pybind11::arg("lse"),
         pybind11::arg("d_out"), pybind11::arg("scale"), pybind11::arg("causal"), pybind11::arg("colmask") = pybind11::none());
   m.def("attention_bwd_packed", traced("attention_bwd_packed", &attention_bwd_packed), pybind11::arg("qkv"), pybind11::arg("nh"), pybind11::arg("nkv"), pybind11::arg("out"),

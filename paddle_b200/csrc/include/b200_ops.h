@@ -206,6 +206,25 @@ struct AttnArgs {
 };
 int attention_fwd_supported(const AttnArgs& a);
 int attention_fwd(const AttnArgs& a, cudaStream_t s);
+// Causal prefill over a paged KV cache: the queries are the n_q[i] new tokens of sequence i at packed rows cu_q[i] ..., its keys are the
+// past[i] + n_q[i] cached positions (the new K / V already written), read through block_tables [b, max_blocks]; key j is visible to new
+// row r iff j <= past[i] + r.  q: [t, H, D] rows (strides token, head); caches [num_blocks, Hk, block_size, D] contiguous, block_size
+// in {16, 32, 64, 128, 256}; o: [t, H, D] rows (strides token, head), written only at the new tokens' rows.  lse: fp32 [H, t] or
+// nullptr.  Sequences with n_q = 0 are skipped.  scratch: int32 [attention_paged_prefill_scratch_ints(t, b)], 8-byte aligned.
+// No host read of the lengths: the work list is built on the device.
+struct PagedAttnArgs {
+  const void* q; const void* k_cache; const void* v_cache; void* o; float* lse;
+  int t, h, hk, d, b, num_blocks, block_size, max_blocks;
+  int64_t q_strides[2], o_strides[2];
+  const int* block_tables; const int* cu_q; const int* n_q; const int* past;
+  int* scratch;
+  float scale;
+  int dtype;
+};
+int attention_paged_prefill_slots(int t, int b);
+int attention_paged_prefill_scratch_ints(int t, int b);
+int attention_paged_prefill_supported(const PagedAttnArgs& a);
+int attention_paged_prefill(const PagedAttnArgs& a, cudaStream_t s);
 // Backward (attention_bwd_sm100.cu). fwd: the forward's arguments with o (contiguous [B,Sq,H,D]) and lse filled in.
 // d_o: contiguous [B,Sq,H,D]; delta: fp32 scratch [B,H,Sq]; dq: fp32 [B,Sq,H,D], every element written; dk/dv: [B,Sk,Hk,D] views (dkv_strides).
 struct AttnBwdArgs {

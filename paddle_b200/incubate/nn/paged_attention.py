@@ -13,25 +13,33 @@ def _raw(t):
     return t.as_subclass(torch.Tensor) if isinstance(t, torch.Tensor) and type(t) is not torch.Tensor else t
 
 
-def _paged_kernels_ok(qkv, kc, d):
+_PREFILL_BLOCK_SIZES = (16, 32, 64, 128, 256)
+
+
+def _paged_kernels_ok(qkv, kc, d, block_size):
     from ...framework.flags import flag
 
-    return qkv.is_cuda and kc.is_cuda and d == 128 and qkv.dtype in (torch.float16, torch.bfloat16) and kc.dtype == qkv.dtype and flag("FLAGS_use_fused_kernels", True)
+    return (qkv.is_cuda and kc.is_cuda and d == 128 and qkv.dtype in (torch.float16, torch.bfloat16) and kc.dtype == qkv.dtype
+            and int(block_size) in _PREFILL_BLOCK_SIZES and flag("FLAGS_use_fused_kernels", True))
 
 
 def block_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_decoder, seq_lens_this_time, cu_seqlens_q, block_tables, block_size):
     """qkv: [total_tokens, (H + 2*H_kv) * D] packed over the batch; caches [num_blocks, H_kv, block_size, D].
 
-    CUDA path (head_dim 128, fp16 / bf16): the new K / V rows of EVERY sequence are scattered into the paged caches with one indexed write
-    (block and row computed on the device from the block table - no per-token Python loop); sequences that decode one token attend to their
-    cache through `decode_attention_paged` (csrc/decode_attention.cu: one table lookup per cached row, split-K over the positions), the
-    prefill sequences run as ONE packed variable-length causal attention on the tcgen05 kernels (kernels/attention.py column mask)."""
+    A sequence prefills when seq_lens_encoder > 0 (a fresh prompt) or when it brings more than one token on top of seq_lens_decoder cached
+    ones (a continuing chunk); it decodes when it brings exactly one token and seq_lens_encoder == 0.
+
+    CUDA path (head_dim 128, fp16 / bf16, block_size 16 / 32 / 64 / 128 / 256): the new K / V rows of EVERY sequence are scattered into the
+    paged caches with one indexed write (block and row computed on the device from the block table - no per-token Python loop); decode
+    sequences attend to their cache through `decode_attention_paged` (csrc/decode_attention.cu: one table lookup per cached row, split-K
+    over the positions); all prefill sequences run in ONE launch of `attention_fwd_paged` (csrc/attention_sm100.cu): causal wgmma flash
+    attention of each sequence's new tokens over its whole cached prefix, K / V read in place through the block table, q read and the
+    output written in place at the tokens' rows.  Other block sizes and devices take `_block_attention_ref`."""
     qkv, kc, vc = _raw(qkv), _raw(key_cache), _raw(value_cache)
     nkv, d = kc.shape[1], kc.shape[3]
-    if not _paged_kernels_ok(qkv, kc, d):
+    if not _paged_kernels_ok(qkv, kc, d, block_size):
         return _block_attention_ref(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_decoder, seq_lens_this_time, cu_seqlens_q, block_tables, block_size)
     from ..._build import ext
-    from ...kernels import attention as KAT
 
     dev = qkv.device
     nh = qkv.shape[1] // d - 2 * nkv
@@ -59,37 +67,18 @@ def block_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_deco
     scale = 1.0 / math.sqrt(d)
     is_dec = (now == 1) & (enc == 0)
     is_pre = (now > 0) & ~is_dec
+    any_dec, any_pre = torch.stack([is_dec.any(), is_pre.any()]).tolist()
     # ---- decode sequences: one query token against the paged cache
-    if bool(is_dec.any()):
+    if any_dec:
         ids = is_dec.nonzero().reshape(-1)
         qd = q[cu[ids]].contiguous()                                        # [Bd, H, D]
         lens = (dec[ids] + 1).to(torch.int32).contiguous()
         od = ext().decode_attention_paged(qd, kc, vc, lens, bt[ids].contiguous(), scale)
         out[cu[ids]] = od.reshape(ids.numel(), nh * d)
-    # ---- prefill sequences: packed varlen causal attention over their new tokens (+ any cached prefix gathered once)
-    if bool(is_pre.any()):
-        ids = is_pre.nonzero().reshape(-1)
-        if bool((past[ids] > 0).any()):       # chunked prefill on top of a cached prefix: rare, keep the simple reference for those
-            ref_out, _, _, _ = _block_attention_ref(qkv, kc, vc, seq_lens_encoder, seq_lens_decoder, seq_lens_this_time, cu_seqlens_q, block_tables, block_size)
-            sel_tok = (is_pre[seq_of] & valid).nonzero().reshape(-1)
-            out[sel_tok] = _raw(ref_out)[sel_tok]
-        else:
-            sel_tok = (is_pre[seq_of] & valid).nonzero().reshape(-1)
-            lens_p = now[ids]
-            cu_p = torch.zeros(ids.numel() + 1, dtype=torch.int64, device=dev)
-            cu_p[1:] = torch.cumsum(lens_p, 0)
-            tot = int(sel_tok.numel())
-            pad = (-tot) % 128                                              # the kernels tile 128 rows: pad the packed batch, padded rows are masked out
-            qp = torch.cat([q[sel_tok], q.new_zeros(pad, nh, d)]).unsqueeze(0)
-            kp = torch.cat([k[sel_tok], k.new_zeros(pad, nkv, d)]).unsqueeze(0)
-            vp = torch.cat([v[sel_tok], v.new_zeros(pad, nkv, d)]).unsqueeze(0)
-            cm = KAT.colmask_from_cu_seqlens(cu_p, cu_p, tot + pad)
-            op = KAT.attention_colmask(qp, kp, vp, cm, causal=True, scale=scale)
-            if op is None:
-                ref_out, _, _, _ = _block_attention_ref(qkv, kc, vc, seq_lens_encoder, seq_lens_decoder, seq_lens_this_time, cu_seqlens_q, block_tables, block_size)
-                out[sel_tok] = _raw(ref_out)[sel_tok]
-            else:
-                out[sel_tok] = _raw(op)[0, :tot].reshape(tot, nh * d)
+    # ---- prefill sequences (fresh prompts and continuing chunks): new tokens over their whole cached prefix, one launch for all
+    if any_pre:
+        i32 = lambda t: t.to(torch.int32).contiguous()                      # noqa: E731
+        ext().attention_fwd_paged(q, kc, vc, bt, i32(cu[:nseq]), i32(torch.where(is_pre, now, 0)), i32(past), scale, out)
     return out.as_subclass(Tensor), qkv.as_subclass(Tensor), kc.as_subclass(Tensor), vc.as_subclass(Tensor)
 
 

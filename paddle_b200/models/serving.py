@@ -8,7 +8,12 @@ preempted (its blocks go back to the pool; it is re-prefilled later from prompt 
 Every step packs the tokens of all scheduled sequences into ONE [tokens, hidden] batch: whole prompts for the sequences being prefilled,
 one token for the sequences being decoded.  The decoder layers run on the packed batch with the model's own sublayers; attention is
 `incubate.nn.paged_attention.block_attention` - on CUDA (head_dim 128, fp16 / bf16) one indexed scatter of the new K / V rows into the
-block pool, `decode_attention_paged` for the decode rows and one packed variable-length wgmma attention for the prefill rows.
+block pool, `decode_attention_paged` for the decode rows and one paged wgmma prefill attention (`attention_fwd_paged`) for the prefill rows.
+
+Chunked prefill (`max_prefill_chunk=N`): an admitted prompt still gets the blocks for its whole length, but is fed over successive steps,
+at most N tokens (and no more than the step's remaining token budget) at a time, each chunk attending to the chunks already cached.  Decode
+rows are scheduled first, so long prompts no longer stall running sequences, and a prompt longer than `max_batch_tokens` can be served.
+A sequence samples its first token after its last chunk.
 """
 from __future__ import annotations
 
@@ -44,6 +49,7 @@ class Sequence:
         self.id, self.prompt, self.max_new_tokens, self.eos = seq_id, [int(t) for t in prompt], int(max_new_tokens), eos_token_id
         self.do_sample, self.temperature, self.top_k, self.top_p = do_sample, temperature, top_k, top_p
         self.generated, self.blocks, self.cached, self.status, self.preemptions = [], [], 0, Sequence.WAITING, 0
+        self.target = 0                            # tokens to prefill since admission: the sequence samples once cached reaches it
 
     def tokens(self):
         return self.prompt + self.generated
@@ -55,7 +61,7 @@ class Sequence:
 class LLMEngine:
     """add_request() any time; step() runs one scheduler iteration (admit / preempt, one packed forward, one token per running sequence)."""
 
-    def __init__(self, model, num_blocks=256, block_size=16, max_running=64, max_batch_tokens=8192):
+    def __init__(self, model, num_blocks=256, block_size=16, max_running=64, max_batch_tokens=8192, max_prefill_chunk=None):
         from .generation import make_adapter
 
         model.eval()
@@ -63,6 +69,9 @@ class LLMEngine:
         self.ad, self.model, self.cfg, self.layers = ad, model, ad.cfg, ad.layers
         self.nh, self.nkv, self.hd = ad.nh, ad.nkv, ad.hd
         self.block_size, self.max_running, self.max_batch_tokens = int(block_size), int(max_running), int(max_batch_tokens)
+        if max_prefill_chunk is not None and int(max_prefill_chunk) < 1:
+            raise ValueError(f"max_prefill_chunk must be a positive number of tokens or None, got {max_prefill_chunk}")
+        self.max_prefill_chunk = None if max_prefill_chunk is None else int(max_prefill_chunk)
         p0 = _raw(next(iter(model.parameters())))
         self.device, self.dtype = p0.device, p0.dtype
         self.alloc = BlockAllocator(num_blocks)
@@ -100,11 +109,12 @@ class LLMEngine:
         self.waiting.insert(0, s)              # first in line when blocks come back
 
     def _schedule(self):
-        """Returns (decode sequences, prefill sequences).  Running sequences get their next slot first (newest ones are preempted when the
-        pool runs dry); then waiting sequences are admitted while blocks, the running limit and the token budget allow."""
+        """Returns (decode sequences, [(prefill sequence, tokens this step)]).  Running sequences get their next slot first (newest ones are
+        preempted when the pool runs dry); then half-prefilled sequences get their next chunk; then waiting sequences are admitted while
+        blocks, the running limit and the token budget allow (whole prompts, or a first chunk with max_prefill_chunk)."""
         decode = []
         for s in list(self.running):
-            if s not in self.running:
+            if s not in self.running or s.cached < s.target:     # gone, or still prefilling (its blocks are already allocated)
                 continue
             if self._blocks_for(s.cached + 1) > len(s.blocks):
                 while self.alloc.num_free() == 0:
@@ -120,16 +130,26 @@ class LLMEngine:
                 s.blocks.append(self.alloc.alloc())
             decode.append(s)
         budget = self.max_batch_tokens - len(decode)
+        chunk = self.max_prefill_chunk
         prefill = []
-        while self.waiting and len(self.running) + len(prefill) < self.max_running:
+        for s in self.running:
+            if s.cached < s.target and budget > 0:
+                n = min(chunk, s.target - s.cached, budget)
+                prefill.append((s, n))
+                budget -= n
+        admitted = 0
+        while self.waiting and len(self.running) + admitted < self.max_running:
             s = self.waiting[0]
-            n = len(s.tokens())
-            need = self._blocks_for(n + 1)
-            if n > budget or need > self.alloc.num_free():
+            total = len(s.tokens())
+            n = total if chunk is None else min(chunk, total, budget)
+            need = self._blocks_for(total + 1)
+            if n > budget or (chunk is not None and budget == 0) or need > self.alloc.num_free():
                 break
             self.waiting.pop(0)
             s.blocks = [self.alloc.alloc() for _ in range(need)]
-            prefill.append(s)
+            s.target = total
+            prefill.append((s, n))
+            admitted += 1
             budget -= n
         return decode, prefill
 
@@ -140,7 +160,7 @@ class LLMEngine:
         toks, pos = [], []
         for s, n in zip(seqs, n_new):
             all_t = s.tokens()
-            toks += all_t[len(all_t) - n:]
+            toks += all_t[s.cached:s.cached + n]
             pos += list(range(s.cached, s.cached + n))
         ids = torch.tensor(toks, dtype=torch.int64, device=dev).unsqueeze(0)                 # [1, T]
         position_ids = torch.tensor(pos, dtype=torch.int64, device=dev).unsqueeze(0)
@@ -166,14 +186,14 @@ class LLMEngine:
     def step(self):
         """One iteration.  Returns [(request id, new token, finished)] for every sequence that produced a token."""
         decode, prefill = self._schedule()
-        seqs = decode + prefill
+        seqs = decode + [s for s, _ in prefill]
         if not seqs:
             if self.waiting and not self.running:
                 raise MemoryError("the KV-cache pool cannot hold the next waiting request")
             return []
-        n_new = [1] * len(decode) + [len(s.tokens()) for s in prefill]
-        enc = [0] * len(decode) + [len(s.tokens()) for s in prefill]
-        dec = [s.cached for s in decode] + [0] * len(prefill)
+        n_new = [1] * len(decode) + [n for _, n in prefill]
+        enc = [0] * len(decode) + [n if s.cached == 0 else 0 for s, n in prefill]     # a continuing chunk attends to its cached prefix
+        dec = [s.cached for s in decode] + [s.cached for s, _ in prefill]
         logits = self._forward(seqs, n_new, enc, dec)
         self.stats["steps"] += 1
         self.stats["decode_tokens"] += len(decode)
@@ -184,6 +204,8 @@ class LLMEngine:
             if s.status != Sequence.RUNNING:
                 s.status = Sequence.RUNNING
                 self.running.append(s)
+            if s.cached < s.target:                # more chunks to come: nothing to sample yet
+                continue
             tok = int(_sample(logits[i: i + 1], s.do_sample, s.temperature, s.top_k, s.top_p)[0])
             s.generated.append(tok)
             fin = len(s.generated) >= s.max_new_tokens or (s.eos is not None and tok == s.eos)
