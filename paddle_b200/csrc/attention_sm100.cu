@@ -15,6 +15,12 @@
 // 128-row query tile) from a work list built on the device (heaviest tiles first) and walks only its own sequence's key tiles up to the
 // bottom-right causal limit.  A 128-key tile is assembled from {64 d, min(block_size, 64) rows} boxes, each at a 1024-byte multiple of
 // the tile, so the 128B-swizzled shared tile is byte-for-byte what one dense box would have written and the MMA code is unchanged.
+//
+// PAGED over 8-bit caches (KV = kv8::I8 / kv8::E4M3; q and o stay fp16 / bf16): a converter warpgroup (warps 8-11, 384 threads) takes
+// the TMA producer's place for K and V.  Its threads read the 8-bit rows through the block table with 16-byte loads, convert them
+// exactly to 16 bits and store them into the same swizzled K / V tiles, then fence.proxy.async and arrive on the tiles' mbarriers; keys
+// past the sequence are written as zeros, so stale or NaN cache rows never reach the MMAs.  The K dequant scale is folded into the exp2
+// scale and the V dequant scale into the epilogue's 1 / l, so the MMA and softmax code is the 16-bit kernel's.
 #include <cuda.h>
 #include <algorithm>
 #include <cstdio>
@@ -22,6 +28,7 @@
 #include <type_traits>
 
 #include "include/b200_common.cuh"
+#include "include/b200_kv8.cuh"
 #include "include/b200_ops.h"
 #include "include/b200_ptx.cuh"
 
@@ -31,6 +38,7 @@ using namespace ptx;
 
 constexpr int BM = 128, BN = 128, HD = 128;
 constexpr int kThreads = 288;   // warps 0-7: two MMA / softmax warpgroups, warp 8: TMA producer
+constexpr int kThreadsQ8 = 384; // 8-bit paged caches: warps 8-11 convert K / V (warp 8 lane 0 also loads Q)
 constexpr uint32_t TILE_BYTES = 128 * 128 * 2;   // 32 KB: every operand tile (Q, K, V)
 constexpr uint32_t HALF_BYTES = TILE_BYTES / 2;  // one 64-wide K-block of a tile
 constexpr uint32_t SMEM_BYTES = 5 * TILE_BYTES + 1024 /*align*/ + 256 /*barriers*/;   // Q, 2x K, 2x V
@@ -65,6 +73,13 @@ struct PagedParams : Params {
   const int* block_tables;    // [b, max_blocks]
   int max_blocks, block_size;
 };
+// 8-bit paged caches: the caches are read by the converter warpgroup, not through tensor maps.
+struct QuantPagedParams : PagedParams {
+  const uint8_t* k_cache;     // [num_blocks, hk, block_size, D]
+  const uint8_t* v_cache;
+  const float* k_dq;          // [hk] dequant scales
+  const float* v_dq;
+};
 
 __device__ __forceinline__ void st_shared_zero16(uint32_t addr) {
   asm volatile("st.shared.v4.u32 [%0], {%1, %1, %1, %1};" ::"r"(addr), "r"(0) : "memory");
@@ -72,11 +87,14 @@ __device__ __forceinline__ void st_shared_zero16(uint32_t addr) {
 
 // MASKED: column-wise row-range mask (flashmask / varlen) compiled in; the dense instantiation carries none of its code or registers
 // PAGED: queries = new tokens of each sequence, K / V read through the block table (see the file header); always causal, never MASKED
-template <typename T, bool MASKED, bool PAGED = false>
-__global__ void __launch_bounds__(kThreads, 1)
-fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
-           const __grid_constant__ CUtensorMap map_v, const std::conditional_t<PAGED, PagedParams, Params> p) {
+// KV: the cache element type; kv8::I8 / kv8::E4M3 (PAGED only) select the converter warpgroup and QuantPagedParams
+template <typename T, bool MASKED, bool PAGED = false, typename KV = T>
+__global__ void __launch_bounds__(std::is_same<KV, T>::value ? kThreads : kThreadsQ8, 1)
+fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
+           const std::conditional_t<PAGED, std::conditional_t<std::is_same<KV, T>::value, PagedParams, QuantPagedParams>, Params> p) {
   constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
+  constexpr bool Q8 = !std::is_same<KV, T>::value;
+  static_assert(!Q8 || (PAGED && !MASKED), "8-bit caches are paged only");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sQ = base;
@@ -114,17 +132,82 @@ fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CU
 
   if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&map_q);
-    tma_prefetch_desc(&map_k);
-    tma_prefetch_desc(&map_v);
+    if constexpr (!Q8) {
+      tma_prefetch_desc(&map_k);
+      tma_prefetch_desc(&map_v);
+    }
     mbar_init(q_full, 1);
-    for (int s = 0; s < 2; ++s) { mbar_init(k_full(s), 1); mbar_init(v_full(s), 1); mbar_init(k_empty(s), 8); mbar_init(v_empty(s), 8); }
+    constexpr uint32_t kv_arrivals = Q8 ? 4 : 1;   // converter warps, or the producer's expect_tx
+    for (int s = 0; s < 2; ++s) {
+      mbar_init(k_full(s), kv_arrivals); mbar_init(v_full(s), kv_arrivals); mbar_init(k_empty(s), 8); mbar_init(v_empty(s), 8);
+    }
     fence_barrier_init();
     fence_proxy_async();
   }
   __syncthreads();
 
-  if (warp == 8) {
-    if constexpr (PAGED) {
+  if (Q8 ? warp >= 8 : warp == 8) {
+    if constexpr (Q8) {
+      if (n_tiles > 0) {
+        // ================= converter warpgroup: thread c of 8 takes d [16c, 16c + 16) of key rows (tid / 8) + 16 i, i < 8 =================
+        const int tid = threadIdx.x - 256, c = tid & 7, r0 = tid >> 3;
+        if (tid == 0) {
+          mbar_expect_tx(q_full, TILE_BYTES);
+          tma_load_4d(sQ, &map_q, q_full, 0, q0 + m0, head, 0);
+          tma_load_4d(sQ + HALF_BYTES, &map_q, q_full, 64, q0 + m0, head, 0);
+        }
+        const int bsz = p.block_size, bshift = __ffs(bsz) - 1;
+        const int* bt = p.block_tables + (int64_t)batch * p.max_blocks;
+        const int64_t blk_stride = (int64_t)p.hk * bsz * HD;
+        const uint8_t* kcache = p.k_cache + (int64_t)kv_head * bsz * HD + c * 16;
+        const uint8_t* vcache = p.v_cache + (int64_t)kv_head * bsz * HD + c * 16;
+        // 16 converted values (16-byte chunks 2c, 2c + 1 of a 128-column row) -> the swizzled 16-bit tile row at `row_addr`
+        auto store_row = [&](const uint4& raw, uint32_t row_addr, int r) {
+          float f[16];
+          kv8::to_float16<KV>(raw, f);
+          uint32_t w[8];
+#pragma unroll
+          for (int i = 0; i < 8; ++i) w[i] = pack2<T>(f[2 * i], f[2 * i + 1]);
+#pragma unroll
+          for (int hc = 0; hc < 2; ++hc)
+            asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(row_addr + ((((2 * c + hc) & 7) ^ (r & 7)) << 4)),
+                         "r"(w[4 * hc]), "r"(w[4 * hc + 1]), "r"(w[4 * hc + 2]), "r"(w[4 * hc + 3]) : "memory");
+        };
+        for (int j = 0; j < n_tiles; ++j) {
+          const int s = j & 1;
+          const uint32_t ph = ((j >> 1) & 1) ^ 1;
+          uint4 kr[8], vr[8];
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {   // both tiles' loads in flight before the first wait
+            const int key = j * BN + i * 16 + r0;
+            kr[i] = vr[i] = make_uint4(0, 0, 0, 0);
+            if (key < sk) {
+              const int64_t off = __ldg(bt + (key >> bshift)) * blk_stride + (int64_t)(key & (bsz - 1)) * HD;
+              kr[i] = __ldg(reinterpret_cast<const uint4*>(kcache + off));
+              vr[i] = __ldg(reinterpret_cast<const uint4*>(vcache + off));
+            }
+          }
+          mbar_wait(k_empty(s), ph);
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {   // K tile: key rows of 128 bytes, d-half c / 4 at HALF_BYTES
+            const int r = i * 16 + r0;
+            store_row(kr[i], sK(s) + (c >> 2) * HALF_BYTES + r * 128, r);
+          }
+          fence_proxy_async();           // generic-proxy stores before the wgmma (async proxy) reads them
+          __syncwarp();
+          if (lane == 0) mbar_arrive(k_full(s));
+          mbar_wait(v_empty(s), ph);
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {   // V tile: 64-key blocks at HALF_BYTES, d-halves 8192 B apart
+            const int r = i * 16 + r0;
+            store_row(vr[i], sV(s) + (r >> 6) * HALF_BYTES + (c >> 2) * 8192 + (r & 63) * 128, r);
+          }
+          fence_proxy_async();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(v_full(s));
+        }
+      }
+    } else if constexpr (PAGED) {
       if (n_tiles > 0) {
         // ================= TMA producer, paged: lane l loads box l % C of K half / V d-half l / C =================
         const int bsz = p.block_size, R = min(bsz, 64), C = BN / R;   // C boxes of R key rows per 128-key K half and per 64-d V half
@@ -178,6 +261,8 @@ fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CU
     // ================= MMA + softmax + epilogue: warpgroup wg owns query rows [64 wg, 64 wg + 64) =================
     const int wg = warp >> 2, q = lane & 3;
     const int rl = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's rows: rl and rl + 8
+    float scale_log2 = p.scale_log2;
+    if constexpr (Q8) scale_log2 *= __ldg(p.k_dq + kv_head);  // S is computed on the quantized K
     float o_acc[HD / 2];
 #pragma unroll
     for (int i = 0; i < HD / 2; ++i) o_acc[i] = 0.f;
@@ -240,7 +325,7 @@ fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CU
         for (int jn = 0; jn < BN / 8; ++jn) mx = fmaxf(mx, fmaxf(sv[jn * 4 + h * 2], sv[jn * 4 + h * 2 + 1]));
         mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
         mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-        float m_new = fmaxf(m_i[h], mx * p.scale_log2);     // scale > 0
+        float m_new = fmaxf(m_i[h], mx * scale_log2);     // scale > 0
         if (m_new == -INFINITY) m_new = 0.f;                // fully masked so far: keep exp2 finite
         const float alpha = ex2(m_i[h] - m_new);
         m_i[h] = m_new;
@@ -249,7 +334,7 @@ fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CU
         for (int jn = 0; jn < BN / 8; ++jn)
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
-            const float pv = ex2(fmaf(sv[jn * 4 + h * 2 + e], p.scale_log2, -m_new));
+            const float pv = ex2(fmaf(sv[jn * 4 + h * 2 + e], scale_log2, -m_new));
             sv[jn * 4 + h * 2 + e] = pv;
             sum += pv;
           }
@@ -267,7 +352,7 @@ fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CU
         pa[ks][3] = pack2<T>(sv[ks * 8 + 6], sv[ks * 8 + 7]);
       }
       mbar_wait(v_full(s), ph);
-      if constexpr (PAGED) {
+      if constexpr (PAGED && !Q8) {   // (the converter writes zeros past the sequence)
         if (j * BN + BN > sk) {   // V rows past the sequence hold stale cache contents (possibly NaN) and P = 0 does not cancel NaN: zero them
           const int tid = threadIdx.x & 127;
           for (int e = (sk - j * BN) * 16 + tid; e < BN * 16; e += 128) {   // 16-byte chunks: key row e / 16, d-half (e / 8) & 1
@@ -299,7 +384,8 @@ fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CU
       float l = l_i[h];
       l += __shfl_xor_sync(0xffffffffu, l, 1);
       l += __shfl_xor_sync(0xffffffffu, l, 2);
-      const float inv = l > 0.f ? 1.f / l : 0.f;
+      float inv = l > 0.f ? 1.f / l : 0.f;
+      if constexpr (Q8) inv *= __ldg(p.v_dq + kv_head);   // O is accumulated on the quantized V
       const int row = m0 + rl + h * 8;
       if (row < nrows) {
         T* orow = reinterpret_cast<T*>(p.o) + (PAGED ? 0 : (int64_t)batch * p.o_sb) + (int64_t)(q0 + row) * p.o_ss + (int64_t)head * p.o_sh;
@@ -450,6 +536,7 @@ int attention_paged_prefill_scratch_ints(int t, int b) { return 3 * attention_pa
 
 int attention_paged_prefill_supported(const PagedAttnArgs& a) {
   if (a.d != 128 || (a.dtype != kBF16 && a.dtype != kF16)) return 0;
+  if (a.kv_dtype != -1 && ((a.kv_dtype != kI8 && a.kv_dtype != kE4M3) || !a.k_dq || !a.v_dq)) return 0;
   if (a.hk <= 0 || a.h % a.hk) return 0;
   if (a.block_size != 16 && a.block_size != 32 && a.block_size != 64 && a.block_size != 128 && a.block_size != 256) return 0;
   if (a.q_strides[0] % 8 || a.q_strides[1] % 8 || a.o_strides[0] % 8 || a.o_strides[1] % 8) return 0;   // 16-byte rows
@@ -468,9 +555,38 @@ int attention_paged_prefill(const PagedAttnArgs& a, cudaStream_t s) {
   CUtensorMap mq, mk, mv;
   // q: {d, token, head, 1} over the strided [T, H, D] view; caches: {d, row in block, kv head, block}
   if (!make_map4(&mq, a.q, a.d, a.t, a.h, 1, a.q_strides[0], a.q_strides[1], a.q_strides[0] * a.t, BM, a.dtype)) return 2;
+  int2* work = reinterpret_cast<int2*>(a.scratch);
+  if (a.kv_dtype != -1) {   // 8-bit caches: no tensor maps over them (the converter warpgroup reads them)
+    paged_work_kernel<<<1, 1024, 0, s>>>(a.n_q, a.past, a.b, slots, a.scratch + 2 * slots, work);
+    QuantPagedParams p = {};
+    p.b = a.b; p.sq = a.t; p.sk = 0; p.h = a.h; p.hk = a.hk;
+    p.scale_log2 = a.scale * 1.4426950408889634f;
+    p.causal = 1; p.causal_off = 0;
+    p.o = a.o; p.lse = a.lse;
+    p.o_sb = 0; p.o_ss = a.o_strides[0]; p.o_sh = a.o_strides[1];
+    p.colmask = nullptr; p.mask_heads = 1;
+    p.work = work; p.cu_q = a.cu_q; p.n_q = a.n_q; p.past = a.past;
+    p.block_tables = a.block_tables; p.max_blocks = a.max_blocks; p.block_size = a.block_size;
+    p.k_cache = reinterpret_cast<const uint8_t*>(a.k_cache); p.v_cache = reinterpret_cast<const uint8_t*>(a.v_cache);
+    p.k_dq = a.k_dq; p.v_dq = a.v_dq;
+    dim3 grid(a.h, slots);
+    auto launch = [&](auto kern, bool& attr) {
+      if (!attr) { B200_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES)); attr = true; }
+      kern<<<grid, kThreadsQ8, SMEM_BYTES, s>>>(mq, mq, mq, p);
+    };
+    static bool attr[4] = {};
+    const bool i8 = a.kv_dtype == kI8;
+    if (a.dtype == kBF16) {
+      if (i8) launch(fwd_kernel<__nv_bfloat16, false, true, kv8::I8>, attr[0]); else launch(fwd_kernel<__nv_bfloat16, false, true, kv8::E4M3>, attr[1]);
+    } else {
+      if (i8) launch(fwd_kernel<__half, false, true, kv8::I8>, attr[2]); else launch(fwd_kernel<__half, false, true, kv8::E4M3>, attr[3]);
+    }
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }
+    return 0;
+  }
   if (!make_map4(&mk, a.k_cache, a.d, a.block_size, a.hk, a.num_blocks, a.d, blk, blk * a.hk, rows, a.dtype)) return 2;
   if (!make_map4(&mv, a.v_cache, a.d, a.block_size, a.hk, a.num_blocks, a.d, blk, blk * a.hk, rows, a.dtype)) return 2;
-  int2* work = reinterpret_cast<int2*>(a.scratch);
   paged_work_kernel<<<1, 1024, 0, s>>>(a.n_q, a.past, a.b, slots, a.scratch + 2 * slots, work);
   PagedParams p = {};
   p.b = a.b; p.sq = a.t; p.sk = 0; p.h = a.h; p.hk = a.hk;

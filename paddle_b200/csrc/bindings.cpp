@@ -743,8 +743,28 @@ Tensor decode_attention(const Tensor& q, const Tensor& k_cache, const Tensor& v_
   return out;
 }
 
-// paged KV cache: q [B,H,D], caches [num_blocks,Hkv,block_size,D], lens int32 [B] (positions valid per sequence), block_tables int32 [B,max_blocks]
-Tensor decode_attention_paged(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& lens, const Tensor& block_tables, double scale) {
+// 8-bit KV caches (int8 / fp8 e4m3): the cache dtype code, after checking that k and v caches share it and that the dequant scales are
+// fp32 [Hkv] on q's device; -1 when no scales are given (the caches must then be of q's dtype, checked by the caller).
+constexpr int kKvI8 = 3, kKvE4M3 = 4;   // b200::DType codes of the 8-bit cache formats
+int kv8_code(const char* op, const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const OptT& k_dq, const OptT& v_dq) {
+  const bool has_k = k_dq.has_value() && k_dq->defined(), has_v = v_dq.has_value() && v_dq->defined();
+  TORCH_CHECK(has_k == has_v, op, ": k_dequant_scales and v_dequant_scales go together");
+  if (!has_k) return -1;
+  const auto st = k_cache.scalar_type();
+  TORCH_CHECK(v_cache.scalar_type() == st && (st == at::kChar || st == at::kFloat8_e4m3fn),
+              op, ": dequant scales need int8 or float8_e4m3fn caches of one dtype, got ", st, " and ", v_cache.scalar_type());
+  TORCH_CHECK(q.scalar_type() == at::kHalf || q.scalar_type() == at::kBFloat16, op, ": q must be fp16 or bf16 with 8-bit caches");
+  const int64_t hkv = k_cache.size(1);
+  for (const Tensor* t : {&*k_dq, &*v_dq})
+    TORCH_CHECK(t->scalar_type() == at::kFloat && t->device() == q.device() && t->is_contiguous() && t->dim() == 1 && t->size(0) == hkv,
+                op, ": dequant scales must be fp32 [Hkv] = [", hkv, "] on the device of q");
+  return st == at::kChar ? kKvI8 : kKvE4M3;
+}
+
+// paged KV cache: q [B,H,D], caches [num_blocks,Hkv,block_size,D], lens int32 [B] (positions valid per sequence), block_tables int32 [B,max_blocks];
+// int8 / fp8 e4m3 caches take fp32 [Hkv] k_dequant_scales / v_dequant_scales
+Tensor decode_attention_paged(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& lens, const Tensor& block_tables, double scale,
+                              const OptT& k_dequant_scales, const OptT& v_dequant_scales) {
   TORCH_CHECK(q.is_cuda() && q.dim() == 3 && k_cache.dim() == 4 && v_cache.dim() == 4 && q.is_contiguous() && k_cache.is_contiguous() && v_cache.is_contiguous(),
               "decode_attention_paged: q [B,H,D], caches [num_blocks,Hkv,block_size,D] contiguous");
   TORCH_CHECK(lens.scalar_type() == at::kInt && lens.is_contiguous() && lens.numel() == q.size(0), "decode_attention_paged: lens must be int32 [B]");
@@ -756,6 +776,19 @@ Tensor decode_attention_paged(const Tensor& q, const Tensor& k_cache, const Tens
   Tensor out = torch::empty_like(q);
   Tensor pacc = torch::empty({b, h, splits, d}, q.options().dtype(at::kFloat));
   Tensor pml = torch::empty({b, h, splits, 2}, q.options().dtype(at::kFloat));
+  const int kv = kv8_code("decode_attention_paged", q, k_cache, v_cache, k_dequant_scales, v_dequant_scales);
+  if (kv != -1) {
+    TORCH_CHECK(k_cache.device() == q.device() && v_cache.device() == q.device() && k_cache.sizes() == v_cache.sizes(),
+                "decode_attention_paged: caches must be of one shape on the device of q");
+    int rc = b200::decode_attention_paged_q8(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), lens.data_ptr<int>(), out.data_ptr(),
+                                             pacc.data_ptr<float>(), pml.data_ptr<float>(), b, h, hkv, d, splits, (float)scale, dt_code(q), kv,
+                                             k_dequant_scales->data_ptr<float>(), v_dequant_scales->data_ptr<float>(), block_tables.data_ptr<int>(),
+                                             mb, bs, cur_stream());
+    g_launches += 2;
+    check_err();
+    TORCH_CHECK(rc == 0, "paddle_b200.decode_attention_paged: unsupported shape (head_dim 128, H % Hkv == 0) rc=", rc);
+    return out;
+  }
   int rc = b200::decode_attention(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), lens.data_ptr<int>(), out.data_ptr(), pacc.data_ptr<float>(),
                                   pml.data_ptr<float>(), b, h, hkv, mb * bs, d, splits, (float)scale, dt_code(q), cur_stream(), block_tables.data_ptr<int>(), mb, bs);
   g_launches += 2;
@@ -817,13 +850,17 @@ std::vector<Tensor> attention_fwd(const Tensor& q, const Tensor& k, const Tensor
 // Causal prefill over the paged KV cache (new K / V already written to the caches): q [T,H,D] view of the packed qkv rows, caches
 // [num_blocks,Hkv,block_size,D], block_tables int32 [B,max_blocks], cu_q / n_q / past int32 [B] (n_q = 0: sequence skipped); writes
 // out [T,H*D] at the new tokens' rows only, and lse fp32 [H,T] at the same rows when given.  No host read of the lengths.
+// int8 / fp8 e4m3 caches take fp32 [Hkv] k_dequant_scales / v_dequant_scales.
 void attention_fwd_paged(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& block_tables, const Tensor& cu_q,
-                         const Tensor& n_q, const Tensor& past, double scale, const Tensor& out, const OptT& lse) {
+                         const Tensor& n_q, const Tensor& past, double scale, const Tensor& out, const OptT& lse, const OptT& k_dequant_scales,
+                         const OptT& v_dequant_scales) {
   TORCH_CHECK(q.is_cuda() && q.dim() == 3 && q.stride(2) == 1, "attention_fwd_paged: q must be a CUDA [T,H,D] view with unit head_dim stride");
   TORCH_CHECK(k_cache.dim() == 4 && v_cache.dim() == 4 && k_cache.is_contiguous() && v_cache.is_contiguous() && k_cache.sizes() == v_cache.sizes(),
               "attention_fwd_paged: caches must be contiguous [num_blocks,Hkv,block_size,D] of one shape");
-  TORCH_CHECK(k_cache.scalar_type() == q.scalar_type() && v_cache.scalar_type() == q.scalar_type(), "attention_fwd_paged: q and caches must share a dtype");
   TORCH_CHECK(k_cache.device() == q.device() && v_cache.device() == q.device(), "attention_fwd_paged: q and caches must be on one device");
+  const int kv = kv8_code("attention_fwd_paged", q, k_cache, v_cache, k_dequant_scales, v_dequant_scales);
+  if (kv == -1)
+    TORCH_CHECK(k_cache.scalar_type() == q.scalar_type() && v_cache.scalar_type() == q.scalar_type(), "attention_fwd_paged: q and caches must share a dtype");
   TORCH_CHECK(block_tables.device() == q.device() && block_tables.scalar_type() == at::kInt && block_tables.is_contiguous() && block_tables.dim() == 2,
               "attention_fwd_paged: block_tables must be int32 [B, max_blocks] on the device");
   const int64_t b = block_tables.size(0);
@@ -842,6 +879,7 @@ void attention_fwd_paged(const Tensor& q, const Tensor& k_cache, const Tensor& v
   a.o_strides[0] = out.stride(0); a.o_strides[1] = a.d;
   a.block_tables = block_tables.data_ptr<int>(); a.cu_q = cu_q.data_ptr<int>(); a.n_q = n_q.data_ptr<int>(); a.past = past.data_ptr<int>();
   a.scale = (float)scale; a.dtype = dt_code(q);
+  if (kv != -1) { a.kv_dtype = kv; a.k_dq = k_dequant_scales->data_ptr<float>(); a.v_dq = v_dequant_scales->data_ptr<float>(); }
   if (lse.has_value() && lse->defined()) {
     TORCH_CHECK(lse->device() == q.device() && lse->scalar_type() == at::kFloat && lse->is_contiguous() && lse->dim() == 2 && lse->size(0) == a.h &&
                 lse->size(1) == a.t, "attention_fwd_paged: lse must be fp32 [H, T]");
@@ -856,6 +894,55 @@ void attention_fwd_paged(const Tensor& q, const Tensor& k_cache, const Tensor& v
   g_launches += 2;
   check_err();
   TORCH_CHECK(rc == 0, "paddle_b200.attention_fwd_paged launch failed rc=", rc);
+}
+
+// Quantizing write of every sequence's new K / V rows into paged int8 / fp8 e4m3 caches: qkv [T, (H + 2 Hkv) * D] packed rows (unit
+// inner stride), caches [num_blocks, Hkv, block_size, D], cu_q int32 [B + 1], seq_lens_encoder / seq_lens_decoder int32 [B], block_tables
+// int32 [B, max_blocks], quant scales fp32 [Hkv]; y = (max_bound * scale) * x rounded (round_type 0: rint, 1: roundf) and clamped to the bounds.
+void paged_kv_cache_write(const Tensor& qkv, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cu_q, const Tensor& seq_lens_encoder,
+                          const Tensor& seq_lens_decoder, const Tensor& block_tables, const Tensor& k_quant_scales, const Tensor& v_quant_scales,
+                          int64_t round_type, double max_bound, double min_bound) {
+  TORCH_CHECK(qkv.is_cuda() && qkv.dim() == 2 && qkv.stride(1) == 1 && (qkv.scalar_type() == at::kHalf || qkv.scalar_type() == at::kBFloat16),
+              "paged_kv_cache_write: qkv must be a CUDA fp16 / bf16 [T, (H + 2 Hkv) * D] tensor with unit inner stride");
+  TORCH_CHECK(k_cache.dim() == 4 && k_cache.is_contiguous() && v_cache.is_contiguous() && k_cache.sizes() == v_cache.sizes() &&
+              k_cache.device() == qkv.device() && v_cache.device() == qkv.device(),
+              "paged_kv_cache_write: caches must be contiguous [num_blocks, Hkv, block_size, D] of one shape on the device of qkv");
+  const auto st = k_cache.scalar_type();
+  TORCH_CHECK(v_cache.scalar_type() == st && (st == at::kChar || st == at::kFloat8_e4m3fn), "paged_kv_cache_write: caches must both be int8 or float8_e4m3fn");
+  TORCH_CHECK(round_type == 0 || round_type == 1, "paged_kv_cache_write: round_type must be 0 (rint) or 1 (round half away from zero)");
+  TORCH_CHECK(min_bound <= max_bound, "paged_kv_cache_write: min_bound must not exceed max_bound");
+  if (st == at::kFloat8_e4m3fn) {
+    TORCH_CHECK(max_bound <= 448.0 && min_bound >= -448.0, "paged_kv_cache_write: fp8 e4m3 bounds must lie within [-448, 448]");
+  } else {
+    TORCH_CHECK(max_bound <= 127.0 && min_bound >= -128.0, "paged_kv_cache_write: int8 bounds must lie within [-128, 127]");
+  }
+  const int64_t hkv = k_cache.size(1), d = k_cache.size(3);
+  TORCH_CHECK(qkv.size(1) % d == 0 && qkv.size(1) / d > 2 * hkv, "paged_kv_cache_write: qkv row width must be (H + 2 Hkv) * D");
+  TORCH_CHECK(qkv.stride(0) % 4 == 0 && reinterpret_cast<uintptr_t>(qkv.data_ptr()) % 8 == 0, "paged_kv_cache_write: qkv rows must be 8-byte aligned");
+  TORCH_CHECK(block_tables.device() == qkv.device() && block_tables.scalar_type() == at::kInt && block_tables.is_contiguous() && block_tables.dim() == 2,
+              "paged_kv_cache_write: block_tables must be int32 [B, max_blocks] on the device");
+  const int64_t b = block_tables.size(0);
+  TORCH_CHECK(cu_q.device() == qkv.device() && cu_q.scalar_type() == at::kInt && cu_q.is_contiguous() && cu_q.numel() == b + 1,
+              "paged_kv_cache_write: cu_q must be int32 [B + 1] on the device");
+  for (const Tensor* t : {&seq_lens_encoder, &seq_lens_decoder})
+    TORCH_CHECK(t->device() == qkv.device() && t->scalar_type() == at::kInt && t->is_contiguous() && t->numel() == b,
+                "paged_kv_cache_write: seq_lens_encoder / seq_lens_decoder must be int32 [B] on the device");
+  for (const Tensor* t : {&k_quant_scales, &v_quant_scales})
+    TORCH_CHECK(t->device() == qkv.device() && t->scalar_type() == at::kFloat && t->is_contiguous() && t->dim() == 1 && t->size(0) == hkv,
+                "paged_kv_cache_write: quant scales must be fp32 [Hkv] on the device");
+  b200::PagedKvWriteArgs a;
+  a.qkv = qkv.data_ptr(); a.k_cache = k_cache.data_ptr(); a.v_cache = v_cache.data_ptr(); a.row_stride = qkv.stride(0);
+  a.t = (int)qkv.size(0); a.hkv = (int)hkv; a.d = (int)d; a.h = (int)(qkv.size(1) / d - 2 * hkv); a.b = (int)b;
+  a.block_size = (int)k_cache.size(2); a.max_blocks = (int)block_tables.size(1);
+  a.cu_q = cu_q.data_ptr<int>(); a.enc = seq_lens_encoder.data_ptr<int>(); a.dec = seq_lens_decoder.data_ptr<int>(); a.block_tables = block_tables.data_ptr<int>();
+  a.k_quant_scales = k_quant_scales.data_ptr<float>(); a.v_quant_scales = v_quant_scales.data_ptr<float>();
+  a.round_type = (int)round_type; a.max_bound = (float)max_bound; a.min_bound = (float)min_bound;
+  a.dtype = dt_code(qkv); a.kv_dtype = st == at::kChar ? kKvI8 : kKvE4M3;
+  c10::cuda::CUDAGuard guard(qkv.device());
+  int rc = b200::paged_kv_cache_write(a, cur_stream());
+  g_launches += 1;
+  check_err();
+  TORCH_CHECK(rc == 0, "paddle_b200.paged_kv_cache_write: unsupported operands (head_dim 128) rc=", rc);
 }
 
 static bool g_deterministic = false;     // FLAGS_cudnn_deterministic (the attention backward is order-independent as it is)
@@ -981,13 +1068,20 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("set_deterministic", [](bool on) { g_deterministic = on; });
   m.def("deterministic", []() { return g_deterministic; });
   m.def("decode_attention", traced("decode_attention", &decode_attention));
-  m.def("decode_attention_paged", traced("decode_attention_paged", &decode_attention_paged));
+  m.def("decode_attention_paged", traced("decode_attention_paged", &decode_attention_paged), pybind11::arg("q"), pybind11::arg("k_cache"),
+        pybind11::arg("v_cache"), pybind11::arg("lens"), pybind11::arg("block_tables"), pybind11::arg("scale"),
+        pybind11::arg("k_dequant_scales") = pybind11::none(), pybind11::arg("v_dequant_scales") = pybind11::none());
+  m.def("paged_kv_cache_write", traced("paged_kv_cache_write", &paged_kv_cache_write), pybind11::arg("qkv"), pybind11::arg("k_cache"),
+        pybind11::arg("v_cache"), pybind11::arg("cu_q"), pybind11::arg("seq_lens_encoder"), pybind11::arg("seq_lens_decoder"),
+        pybind11::arg("block_tables"), pybind11::arg("k_quant_scales"), pybind11::arg("v_quant_scales"), pybind11::arg("round_type") = 1,
+        pybind11::arg("max_bound") = 127.0, pybind11::arg("min_bound") = -127.0);
   m.def("attention_supported", &attention_supported);
   m.def("attention_fwd", traced("attention_fwd", &attention_fwd), pybind11::arg("q"), pybind11::arg("k"), pybind11::arg("v"), pybind11::arg("scale"), pybind11::arg("causal"),
         pybind11::arg("out_seq_major") = false, pybind11::arg("colmask") = pybind11::none());
   m.def("attention_fwd_paged", traced("attention_fwd_paged", &attention_fwd_paged), pybind11::arg("q"), pybind11::arg("k_cache"),
         pybind11::arg("v_cache"), pybind11::arg("block_tables"), pybind11::arg("cu_q"), pybind11::arg("n_q"), pybind11::arg("past"), pybind11::arg("scale"),
-        pybind11::arg("out"), pybind11::arg("lse") = pybind11::none());
+        pybind11::arg("out"), pybind11::arg("lse") = pybind11::none(), pybind11::arg("k_dequant_scales") = pybind11::none(),
+        pybind11::arg("v_dequant_scales") = pybind11::none());
   m.def("attention_bwd", traced("attention_bwd", &attention_bwd), pybind11::arg("q"), pybind11::arg("k"), pybind11::arg("v"), pybind11::arg("out"), pybind11::arg("lse"),
         pybind11::arg("d_out"), pybind11::arg("scale"), pybind11::arg("causal"), pybind11::arg("colmask") = pybind11::none());
   m.def("attention_bwd_packed", traced("attention_bwd_packed", &attention_bwd_packed), pybind11::arg("qkv"), pybind11::arg("nh"), pybind11::arg("nkv"), pybind11::arg("out"),

@@ -8,7 +8,7 @@
 
 namespace b200 {
 
-enum DType : int { kF32 = 0, kF16 = 1, kBF16 = 2 };
+enum DType : int { kF32 = 0, kF16 = 1, kBF16 = 2, kI8 = 3, kE4M3 = 4 };   // kI8 / kE4M3: quantized KV caches only
 
 #define B200_CUDA_CHECK(expr)                                                                  \
   do {                                                                                         \

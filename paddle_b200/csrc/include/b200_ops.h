@@ -187,6 +187,26 @@ int decode_attention_splits(int b, int h, int smax);
 int decode_attention(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* out, float* part_acc, float* part_ml, int b,
                      int h, int hkv, int smax, int d, int splits, float scale, int dtype, cudaStream_t s, const int* block_tables = nullptr,
                      int max_blocks = 0, int block_size = 0);   // block_tables: paged caches [num_blocks, Hkv, block_size, D]
+// The same over paged 8-bit caches (kv_dtype kI8 / kE4M3, q fp16 / bf16): k_dq / v_dq fp32 [Hkv] dequant scales on the device.
+int decode_attention_paged_q8(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* out, float* part_acc, float* part_ml,
+                              int b, int h, int hkv, int d, int splits, float scale, int dtype, int kv_dtype, const float* k_dq, const float* v_dq,
+                              const int* block_tables, int max_blocks, int block_size, cudaStream_t s);
+
+// ---- kv_cache_quant.cu ----------------------------------------------------------------------------------------
+// Quantizing write of every sequence's new K / V rows (read in place from the packed qkv [t, (h + 2 hkv) * 128] rows, row stride in
+// elements) into paged 8-bit caches [num_blocks, hkv, block_size, 128].  cu_q int32 [b + 1]; enc / dec int32 [b] (a sequence with
+// enc > 0 starts at position 0, otherwise at dec); quant scales fp32 [hkv].  See include/b200_kv8.cuh for the rounding rules.
+struct PagedKvWriteArgs {
+  const void* qkv; void* k_cache; void* v_cache;
+  int64_t row_stride;
+  int t, h, hkv, d, b, block_size, max_blocks;
+  const int* cu_q; const int* enc; const int* dec; const int* block_tables;
+  const float* k_quant_scales; const float* v_quant_scales;
+  int round_type;
+  float max_bound, min_bound;
+  int dtype, kv_dtype;
+};
+int paged_kv_cache_write(const PagedKvWriteArgs& a, cudaStream_t s);
 
 // ---- attention_sm100.cu ---------------------------------------------------------------------------------------
 // Flash-attention forward (head_dim 128, fp16/bf16). q [B,Sq,H,D], k/v [B,Sk,Hk,D], o [B,Sq,H,D] as strided views (element
@@ -220,6 +240,10 @@ struct PagedAttnArgs {
   int* scratch;
   float scale;
   int dtype;
+  // 8-bit caches: kv_dtype kI8 / kE4M3 with fp32 [hk] dequant scales on the device (q and o stay fp16 / bf16); -1: caches of `dtype`
+  int kv_dtype = -1;
+  const float* k_dq = nullptr;
+  const float* v_dq = nullptr;
 };
 int attention_paged_prefill_slots(int t, int b);
 int attention_paged_prefill_scratch_ints(int t, int b);

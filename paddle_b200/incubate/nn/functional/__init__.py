@@ -314,11 +314,22 @@ def variable_length_memory_efficient_attention(query, key, value, seq_lens, kv_s
 
 
 def block_multihead_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_decoder, seq_lens_this_time, padding_offsets, cum_offsets,
-                              cu_seqlens_q, cu_seqlens_k, block_tables, *args, max_seq_len=-1, block_size=64, use_neox_style=False, **kwargs):
-    """Paged-KV attention (prefill + decode). Parity: block_multihead_attention.py. key/value_cache: [num_blocks, H_kv, block_size, D]."""
+                              cu_seqlens_q, cu_seqlens_k, block_tables, pre_key_cache=None, pre_value_cache=None, cache_k_quant_scales=None,
+                              cache_v_quant_scales=None, cache_k_dequant_scales=None, cache_v_dequant_scales=None, qkv_out_scale=None, qkv_bias=None,
+                              out_shift=None, out_smooth=None, max_enc_len_this_time=None, max_dec_len_this_time=None, rope_emb=None, mask=None,
+                              tgt_mask=None, max_seq_len=-1, block_size=64, use_neox_style=False, use_dynamic_cachekv_quant=False, quant_round_type=1,
+                              quant_max_bound=127.0, quant_min_bound=-127.0, out_scale=-1, compute_dtype="default", rope_theta=10000.0):
+    """Paged-KV attention (prefill + decode). Parity: block_multihead_attention.py. key/value_cache: [num_blocks, H_kv, block_size, D].
+
+    int8 / float8_e4m3fn caches take static per-KV-head cache_{k,v}_{quant,dequant}_scales (fp32 [H_kv]) with quant_round_type and the
+    quant bounds (see incubate.nn.paged_attention).  Dynamic cache quantization raises NotImplementedError; scales with a 16-bit cache, or an
+    8-bit cache without them, raise ValueError.  The pre-caches, rope_emb, masks, qkv_out_scale / bias, out_shift / smooth and out_scale
+    are not applied."""
     from ....incubate.nn.paged_attention import block_attention
 
-    return block_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_decoder, seq_lens_this_time, cu_seqlens_q, block_tables, block_size)
+    return block_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_decoder, seq_lens_this_time, cu_seqlens_q, block_tables, block_size,
+                           cache_k_quant_scales, cache_v_quant_scales, cache_k_dequant_scales, cache_v_dequant_scales, use_dynamic_cachekv_quant,
+                           quant_round_type, quant_max_bound, quant_min_bound)
 
 
 def blha_get_max_len(seq_lens_encoder, seq_lens_decoder, batch_size):

@@ -4,7 +4,7 @@ from .gpt import GPTConfig, GPTForCausalLM, GPTModel, gpt3_1p3b, gpt3_6p7b, gpt_
 from .mixtral import MixtralConfig, MixtralForCausalLM, mixtral_8x7b, mixtral_tiny  # noqa: F401,E402
 from .mlp import MnistMLP  # noqa: F401,E402
 from .generation import KVCache, LlamaGenerator, generate  # noqa: F401,E402
-from .serving import BlockAllocator, LLMEngine  # noqa: F401,E402
+from .serving import BlockAllocator, LLMEngine, calibrate_kv_cache  # noqa: F401,E402
 
 
 def resnet50(**kw):

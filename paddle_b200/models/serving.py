@@ -14,6 +14,11 @@ Chunked prefill (`max_prefill_chunk=N`): an admitted prompt still gets the block
 at most N tokens (and no more than the step's remaining token budget) at a time, each chunk attending to the chunks already cached.  Decode
 rows are scheduled first, so long prompts no longer stall running sequences, and a prompt longer than `max_batch_tokens` can be served.
 A sequence samples its first token after its last chunk.
+
+Quantized KV cache (`kv_cache_dtype="int8"` or `"float8_e4m3fn"`): the block pool stores one byte per element, so the same memory holds
+twice the tokens of a 16-bit cache and decode reads half the bytes.  The scales are static, one per KV head and layer, derived from a
+calibrated absmax `kv_cache_absmax` [num_layers, 2, H_kv] (see `calibrate_kv_cache`): quant_scale = 1 / absmax and dequant_scale =
+absmax / bound, with bound 127 (int8) or 448 (fp8).  Static scales make chunked prefill and preemption work unchanged.
 """
 from __future__ import annotations
 
@@ -58,10 +63,14 @@ class Sequence:
         return self.status == Sequence.FINISHED
 
 
+_KV_CACHE_DTYPES = {"int8": (torch.int8, 127.0), "float8_e4m3fn": (torch.float8_e4m3fn, 448.0)}
+
+
 class LLMEngine:
     """add_request() any time; step() runs one scheduler iteration (admit / preempt, one packed forward, one token per running sequence)."""
 
-    def __init__(self, model, num_blocks=256, block_size=16, max_running=64, max_batch_tokens=8192, max_prefill_chunk=None):
+    def __init__(self, model, num_blocks=256, block_size=16, max_running=64, max_batch_tokens=8192, max_prefill_chunk=None, kv_cache_dtype=None,
+                 kv_cache_absmax=None):
         from .generation import make_adapter
 
         model.eval()
@@ -75,12 +84,36 @@ class LLMEngine:
         p0 = _raw(next(iter(model.parameters())))
         self.device, self.dtype = p0.device, p0.dtype
         self.alloc = BlockAllocator(num_blocks)
+        self._kv_quant = [{} for _ in self.layers]       # per layer: block_attention's cache quantization arguments
+        cache_dtype = self.dtype
+        if kv_cache_dtype is not None:
+            cache_dtype, self._kv_quant = self._static_kv_quant(kv_cache_dtype, kv_cache_absmax)
+        elif kv_cache_absmax is not None:
+            raise ValueError("kv_cache_absmax is only used with kv_cache_dtype='int8' or 'float8_e4m3fn'")
+        self.kv_cache_dtype = cache_dtype
         shape = (num_blocks, self.nkv, self.block_size, self.hd)
-        self.key_cache = [torch.zeros(shape, dtype=self.dtype, device=self.device) for _ in self.layers]
-        self.value_cache = [torch.zeros(shape, dtype=self.dtype, device=self.device) for _ in self.layers]
+        self.key_cache = [torch.zeros(shape, dtype=cache_dtype, device=self.device) for _ in self.layers]
+        self.value_cache = [torch.zeros(shape, dtype=cache_dtype, device=self.device) for _ in self.layers]
+        self._observe = None                             # calibrate_kv_cache: called with (layer index, packed qkv rows) every forward
         self.waiting, self.running, self.done = [], [], {}
         self._next_id = 0
         self.stats = {"steps": 0, "prefill_tokens": 0, "decode_tokens": 0, "preemptions": 0, "max_running": 0}
+
+    def _static_kv_quant(self, kv_cache_dtype, absmax):
+        name = str(kv_cache_dtype).replace("torch.", "")
+        if name not in _KV_CACHE_DTYPES:
+            raise ValueError(f"kv_cache_dtype must be None, 'int8' or 'float8_e4m3fn', got {kv_cache_dtype!r}")
+        dtype, bound = _KV_CACHE_DTYPES[name]
+        shape = (len(self.layers), 2, self.nkv)
+        if absmax is None or tuple(_raw(absmax).shape) != shape:
+            raise ValueError(f"kv_cache_dtype={name!r} needs kv_cache_absmax of shape [num_layers, 2, H_kv] = {list(shape)} "
+                             "(models.calibrate_kv_cache computes it)")
+        am = _raw(absmax).to(self.device, torch.float32)
+        am = torch.where(am > 0, am, torch.ones_like(am))   # a head whose rows are all zero: any scale stores them exactly
+        qs, dq = 1.0 / am, am / bound
+        quant = [{"cache_k_quant_scales": qs[li, 0], "cache_v_quant_scales": qs[li, 1], "cache_k_dequant_scales": dq[li, 0],
+                  "cache_v_dequant_scales": dq[li, 1], "quant_max_bound": bound, "quant_min_bound": -bound} for li in range(len(self.layers))]
+        return dtype, quant
 
     # ---- requests ---------------------------------------------------------------------------------------------------------------
     def add_request(self, prompt_ids, max_new_tokens=32, eos_token_id=None, do_sample=False, temperature=1.0, top_k=0, top_p=1.0):
@@ -178,7 +211,10 @@ class LLMEngine:
         for li, layer in enumerate(self.layers):
             qkv = self.ad.attn_in(layer, h, position_ids)
             t = qkv.shape[1]
-            out, _, _, _ = block_attention(qkv.reshape(t, (nh + 2 * nkv) * hd), self.key_cache[li], self.value_cache[li], enc_t, dec_t, now_t, cu, bt, self.block_size)
+            if self._observe is not None:
+                self._observe(li, qkv.reshape(t, (nh + 2 * nkv) * hd))
+            out, _, _, _ = block_attention(qkv.reshape(t, (nh + 2 * nkv) * hd), self.key_cache[li], self.value_cache[li], enc_t, dec_t, now_t, cu, bt,
+                                           self.block_size, **self._kv_quant[li])
             h = self.ad.attn_out(layer, h, _raw(out).reshape(1, t, nh * hd))
         last = (cu[1:].long() - 1)
         return self.ad.logits(_raw(h)[:, last])[0]                                     # [num_seqs, vocab]
@@ -229,3 +265,26 @@ class LLMEngine:
     def result(self, request_id):
         s = self.done.get(request_id)
         return None if s is None else _w(torch.tensor(s.generated, dtype=torch.int64))
+
+
+@torch.no_grad()
+def calibrate_kv_cache(model, prompts, block_size=16):
+    """absmax [num_layers, 2, H_kv] (fp32) of exactly the rows LLMEngine writes into its KV cache when it prefills `prompts`: K after
+    rotary, and V, per layer and KV head.  Pass it as LLMEngine(kv_cache_dtype=..., kv_cache_absmax=...)."""
+    prompts = [_raw(p).reshape(-1).tolist() if isinstance(p, torch.Tensor) else list(p) for p in prompts]
+    longest = max(len(p) for p in prompts)
+    eng = LLMEngine(model, num_blocks=(longest + 1 + block_size - 1) // block_size, block_size=block_size, max_running=1,
+                    max_batch_tokens=longest + 1)
+    nh, nkv, hd = eng.nh, eng.nkv, eng.hd
+    amax = torch.zeros(len(eng.layers), 2, nkv, dtype=torch.float32, device=eng.device)
+
+    def observe(li, qkv):
+        rows = qkv.reshape(qkv.shape[0], nh + 2 * nkv, hd).float()
+        amax[li, 0] = torch.maximum(amax[li, 0], rows[:, nh:nh + nkv].abs().amax(dim=(0, 2)))
+        amax[li, 1] = torch.maximum(amax[li, 1], rows[:, nh + nkv:].abs().amax(dim=(0, 2)))
+
+    eng._observe = observe
+    for p in prompts:
+        eng.add_request(p, max_new_tokens=1)     # the first token is sampled from the prefill; its own row is never written
+    eng.run_until_done()
+    return amax
