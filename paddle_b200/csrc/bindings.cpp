@@ -896,6 +896,53 @@ void attention_fwd_paged(const Tensor& q, const Tensor& k_cache, const Tensor& v
   TORCH_CHECK(rc == 0, "paddle_b200.attention_fwd_paged launch failed rc=", rc);
 }
 
+// Multi-token decode over the paged KV cache (the verify rows of speculative decoding; new K / V already written): q [T,H,D] view of the
+// packed qkv rows, caches [num_blocks,Hkv,block_size,D], block_tables int32 [B,max_blocks], cu_q / n_q / past int32 [B] (n_q = 0: sequence
+// skipped); writes out [T, H*D] at the new tokens' rows only.  n_q * (H / Hkv) may not exceed 64 (a sequence beyond it gets NaN rows: the
+// lengths are not read on the host).  int8 / fp8 e4m3 caches take fp32 [Hkv] k_dequant_scales / v_dequant_scales.
+void decode_attention_paged_multi(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& block_tables, const Tensor& cu_q,
+                                  const Tensor& n_q, const Tensor& past, double scale, const Tensor& out, const OptT& k_dequant_scales,
+                                  const OptT& v_dequant_scales) {
+  TORCH_CHECK(q.is_cuda() && q.dim() == 3 && q.stride(2) == 1, "decode_attention_paged_multi: q must be a CUDA [T,H,D] view with unit head_dim stride");
+  TORCH_CHECK(q.scalar_type() == at::kHalf || q.scalar_type() == at::kBFloat16, "decode_attention_paged_multi: q must be fp16 or bf16");
+  TORCH_CHECK(k_cache.dim() == 4 && v_cache.dim() == 4 && k_cache.is_contiguous() && v_cache.is_contiguous() && k_cache.sizes() == v_cache.sizes(),
+              "decode_attention_paged_multi: caches must be contiguous [num_blocks,Hkv,block_size,D] of one shape");
+  TORCH_CHECK(k_cache.device() == q.device() && v_cache.device() == q.device(), "decode_attention_paged_multi: q and caches must be on one device");
+  const int kv = kv8_code("decode_attention_paged_multi", q, k_cache, v_cache, k_dequant_scales, v_dequant_scales);
+  if (kv == -1)
+    TORCH_CHECK(k_cache.scalar_type() == q.scalar_type() && v_cache.scalar_type() == q.scalar_type(),
+                "decode_attention_paged_multi: q and caches must share a dtype");
+  TORCH_CHECK(block_tables.device() == q.device() && block_tables.scalar_type() == at::kInt && block_tables.is_contiguous() && block_tables.dim() == 2
+              && block_tables.size(1) > 0, "decode_attention_paged_multi: block_tables must be int32 [B, max_blocks] on the device");
+  const int64_t b = block_tables.size(0);
+  for (const Tensor* t : {&cu_q, &n_q, &past})
+    TORCH_CHECK(t->device() == q.device() && t->scalar_type() == at::kInt && t->is_contiguous() && t->numel() == b,
+                "decode_attention_paged_multi: cu_q / n_q / past must be int32 [B] on the device");
+  TORCH_CHECK(out.device() == q.device() && out.scalar_type() == q.scalar_type() && out.dim() == 2 && out.size(0) == q.size(0) &&
+              out.size(1) == q.size(1) * q.size(2) && out.stride(1) == 1, "decode_attention_paged_multi: out must be [T, H*D] with unit inner stride");
+  TORCH_CHECK(q.size(2) == 128 && k_cache.size(3) == 128, "decode_attention_paged_multi: head_dim must be 128");
+  const int64_t hkv = k_cache.size(1);
+  TORCH_CHECK(hkv > 0 && q.size(1) % hkv == 0 && q.size(1) / hkv <= 64, "decode_attention_paged_multi: H must be a multiple of Hkv with H / Hkv <= 64, "
+              "and n_q * (H / Hkv) <= 64 per sequence");
+  b200::PagedMultiArgs a;
+  a.q = q.data_ptr(); a.k_cache = k_cache.data_ptr(); a.v_cache = v_cache.data_ptr(); a.out = out.data_ptr();
+  a.block_tables = block_tables.data_ptr<int>(); a.cu_q = cu_q.data_ptr<int>(); a.n_q = n_q.data_ptr<int>(); a.past = past.data_ptr<int>();
+  a.q_st = q.stride(0); a.q_sh = q.stride(1); a.o_st = out.stride(0);
+  a.b = (int)b; a.h = (int)q.size(1); a.hkv = (int)hkv; a.d = (int)q.size(2);
+  a.max_blocks = (int)block_tables.size(1); a.block_size = (int)k_cache.size(2);
+  a.splits = b200::decode_attention_splits(a.b, a.hkv, a.max_blocks * a.block_size);
+  a.scale = (float)scale; a.dtype = dt_code(q);
+  if (kv != -1) { a.kv_dtype = kv; a.k_dq = k_dequant_scales->data_ptr<float>(); a.v_dq = v_dequant_scales->data_ptr<float>(); }
+  c10::cuda::CUDAGuard guard(q.device());
+  Tensor pacc = torch::empty({b, hkv, a.splits, 64, 128}, q.options().dtype(at::kFloat));
+  Tensor pml = torch::empty({b, hkv, a.splits, 64, 2}, q.options().dtype(at::kFloat));
+  a.part_acc = pacc.data_ptr<float>(); a.part_ml = pml.data_ptr<float>();
+  int rc = b200::decode_attention_paged_multi(a, cur_stream());
+  g_launches += 2;
+  check_err();
+  TORCH_CHECK(rc == 0, "paddle_b200.decode_attention_paged_multi: unsupported operands (16-byte aligned rows and caches) rc=", rc);
+}
+
 // Quantizing write of every sequence's new K / V rows into paged int8 / fp8 e4m3 caches: qkv [T, (H + 2 Hkv) * D] packed rows (unit
 // inner stride), caches [num_blocks, Hkv, block_size, D], cu_q int32 [B + 1], seq_lens_encoder / seq_lens_decoder int32 [B], block_tables
 // int32 [B, max_blocks], quant scales fp32 [Hkv]; y = (max_bound * scale) * x rounded (round_type 0: rint, 1: roundf) and clamped to the bounds.
@@ -1081,6 +1128,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("attention_fwd_paged", traced("attention_fwd_paged", &attention_fwd_paged), pybind11::arg("q"), pybind11::arg("k_cache"),
         pybind11::arg("v_cache"), pybind11::arg("block_tables"), pybind11::arg("cu_q"), pybind11::arg("n_q"), pybind11::arg("past"), pybind11::arg("scale"),
         pybind11::arg("out"), pybind11::arg("lse") = pybind11::none(), pybind11::arg("k_dequant_scales") = pybind11::none(),
+        pybind11::arg("v_dequant_scales") = pybind11::none());
+  m.def("decode_attention_paged_multi", traced("decode_attention_paged_multi", &decode_attention_paged_multi), pybind11::arg("q"),
+        pybind11::arg("k_cache"), pybind11::arg("v_cache"), pybind11::arg("block_tables"), pybind11::arg("cu_q"), pybind11::arg("n_q"),
+        pybind11::arg("past"), pybind11::arg("scale"), pybind11::arg("out"), pybind11::arg("k_dequant_scales") = pybind11::none(),
         pybind11::arg("v_dequant_scales") = pybind11::none());
   m.def("attention_bwd", traced("attention_bwd", &attention_bwd), pybind11::arg("q"), pybind11::arg("k"), pybind11::arg("v"), pybind11::arg("out"), pybind11::arg("lse"),
         pybind11::arg("d_out"), pybind11::arg("scale"), pybind11::arg("causal"), pybind11::arg("colmask") = pybind11::none());

@@ -16,6 +16,7 @@
 // Paged int8 / fp8 e4m3 caches (decode_split_q8_kernel): the same walk over 8-bit rows, dequantized with per-KV-head scales.
 #include <cuda.h>
 #include <cstdio>
+#include <type_traits>
 
 #include "include/b200_common.cuh"
 #include "include/b200_kv8.cuh"
@@ -199,6 +200,280 @@ __global__ void __launch_bounds__(D) decode_merge_kernel(const float* __restrict
 
 }  // namespace decode
 
+// Multi-token paged decode: the few new tokens of each sequence (the verify rows of speculative decoding) over its long cached prefix.
+// Grid = (splits, Hkv, B).  A CTA owns every query row of one (sequence, KV head): n_q tokens x G = H / Hkv heads, packed into one 64-row
+// tile (row r = token r / G, head kvh * G + r % G), so each cached K / V row is read from HBM once per call.  Its 4 warps own 16 rows each
+// and run mma.sync m16n8k16 (fp32 accumulate): S = Q K^T over 64-key tiles, P kept in registers as the A operand of P V.  K / V tiles come
+// through the block table by cp.async 16-byte copies, three stages deep; keys at or past the sequence's length are zero-filled without
+// reading their table entry, so NaN in a recycled block never reaches the MMAs.  Masking is bottom-right causal: token j sees keys
+// < past + j + 1.  Each split writes an unnormalized partial (m, l, acc) per row; multi_merge_kernel combines them like decode_merge_kernel.
+// 8-bit caches are copied raw and converted exactly to 16 bits in shared memory; K's dequant scale joins the softmax scale and V's scales
+// the split's partial, so with power-of-two scales the result is bit-identical to the 16-bit kernel on the dequantized cache.
+namespace decode_multi {
+
+constexpr int D = 128, BN = 64, kRows = 64, kThreads = 128, kStages = 3;
+constexpr int kTile16 = BN * D * 2, kTile8 = BN * D;   // one K or V tile of 64 keys: 16 KB in 16 bits, 8 KB in 8 bits
+
+struct Params {
+  const void* q; const void* k_cache; const void* v_cache;
+  void* out; float* part_acc; float* part_ml;
+  const int* block_tables; const int* cu_q; const int* n_q; const int* past;
+  const float* k_dq; const float* v_dq;
+  int64_t q_st, q_sh, o_st;   // element strides: q (token, head), out (token; heads are D apart)
+  int h, hkv, splits, max_blocks, block_size;
+  float scale_log2;
+};
+
+// shared memory: Q tile [64][128] 16-bit | K, V 16-bit tiles (kStages, or 1 for 8-bit caches) | 8-bit caches: raw K, V tiles (kStages).
+// Two tiles stay in flight while one is computed; two CTAs fit on an SM.
+template <bool Q8> struct Smem {
+  static constexpr int kKV = kRows * D * 2;
+  static constexpr int kRaw = kKV + (Q8 ? 1 : kStages) * 2 * kTile16;
+  static constexpr int kBytes = kRaw + (Q8 ? kStages * 2 * kTile8 : 0);
+};
+
+// byte offset of 16-byte chunk c (0..15) of row `row` in a [rows][128] 16-bit tile; the XOR spreads 8 consecutive rows over all banks
+__device__ __forceinline__ uint32_t swz(int row, int c) { return (uint32_t)(row * (D * 2) + ((c ^ (row & 7)) << 4)); }
+
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool valid) {   // !valid: zero-fill, nothing is read
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
+__device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], uint32_t addr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
+}
+__device__ __forceinline__ void ldsm_x4_t(uint32_t (&r)[4], uint32_t addr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
+}
+
+template <typename T> __device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1);
+template <> __device__ __forceinline__ void mma16816<__nv_bfloat16>(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+template <> __device__ __forceinline__ void mma16816<__half>(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+
+template <typename T> __device__ __forceinline__ uint32_t pack2(float lo, float hi);
+template <> __device__ __forceinline__ uint32_t pack2<__nv_bfloat16>(float lo, float hi) {
+  const __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
+  return *reinterpret_cast<const uint32_t*>(&v);
+}
+template <> __device__ __forceinline__ uint32_t pack2<__half>(float lo, float hi) {
+  const __half2 v = __floats2half2_rn(lo, hi);
+  return *reinterpret_cast<const uint32_t*>(&v);
+}
+
+// KV = T: 16-bit caches; KV = kv8::I8 / kv8::E4M3: 8-bit caches with fp32 [Hkv] dequant scales
+template <typename T, typename KV>
+__global__ void __launch_bounds__(kThreads) multi_split_kernel(const Params p) {
+  constexpr bool Q8 = !std::is_same<T, KV>::value;
+  using S = Smem<Q8>;
+  const int split = blockIdx.x, kvh = blockIdx.y, b = blockIdx.z;
+  const int nq = p.n_q[b], g_size = p.h / p.hkv, nrows = nq * g_size;
+  if (nq <= 0 || nrows > kRows) return;                      // skipped, or past the row limit (multi_merge_kernel writes NaN)
+  const int past = p.past[b];
+  const int len = min(past + nq, p.max_blocks * p.block_size);
+  const int ntiles = (len + BN - 1) / BN, per = (ntiles + p.splits - 1) / p.splits;
+  const int t0 = split * per, t1 = min(ntiles, t0 + per);
+  extern __shared__ __align__(128) uint8_t smem[];
+  const uint32_t sbase = (uint32_t)__cvta_generic_to_shared(smem);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int* bt = p.block_tables + (int64_t)b * p.max_blocks;
+  const int cu = p.cu_q[b];
+
+  // Q tile: rows past nrows are zero
+#pragma unroll
+  for (int i = 0; i < kRows * D / 8 / kThreads; ++i) {
+    const int row = i * (kThreads / 16) + (tid >> 4), c = tid & 15;
+    const bool ok = row < nrows;
+    const T* src = reinterpret_cast<const T*>(p.q);
+    if (ok) src += (int64_t)(cu + row / g_size) * p.q_st + (int64_t)(kvh * g_size + row % g_size) * p.q_sh + c * 8;
+    cp_async16(sbase + swz(row, c), src, ok);
+  }
+  // cached K / V rows of key tile `tile` into stage `st`; keys at or past len are zero-filled
+  auto load_kv = [&](int tile, int st) {
+    constexpr int kEl = Q8 ? 16 : 8;                         // elements per 16-byte chunk
+    constexpr int kChunks = D / kEl;
+#pragma unroll
+    for (int i = 0; i < BN * kChunks / kThreads; ++i) {
+      const int row = i * (kThreads / kChunks) + tid / kChunks, c = tid % kChunks;
+      const int pos = tile * BN + row;
+      const bool ok = pos < len;
+      int64_t off = 0;
+      if (ok) off = (((int64_t)bt[pos / p.block_size] * p.hkv + kvh) * p.block_size + pos % p.block_size) * D + c * kEl;
+      if constexpr (Q8) {
+        const uint32_t dst = sbase + S::kRaw + st * 2 * kTile8 + row * D + c * 16;
+        cp_async16(dst, reinterpret_cast<const uint8_t*>(p.k_cache) + off, ok);
+        cp_async16(dst + kTile8, reinterpret_cast<const uint8_t*>(p.v_cache) + off, ok);
+      } else {
+        const uint32_t dst = sbase + S::kKV + st * 2 * kTile16 + swz(row, c);
+        cp_async16(dst, reinterpret_cast<const T*>(p.k_cache) + off, ok);
+        cp_async16(dst + kTile16, reinterpret_cast<const T*>(p.v_cache) + off, ok);
+      }
+    }
+  };
+  if (t0 < t1) load_kv(t0, 0);
+  cp_async_commit();
+  if (t0 + 1 < t1) load_kv(t0 + 1, 1);
+  cp_async_commit();
+
+  float qk_scale = p.scale_log2, v_scale = 1.f;
+  if constexpr (Q8) { qk_scale *= __ldg(p.k_dq + kvh); v_scale = __ldg(p.v_dq + kvh); }
+  const bool active = warp * 16 < nrows;
+  const int r_lo = warp * 16 + (lane >> 2);                  // this lane's two rows: r_lo and r_lo + 8
+  int limit[2];                                              // keys < limit are visible to the row
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) limit[hh] = min(len, past + (r_lo + hh * 8) / g_size + 1);
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  float acc[D / 8][4];
+#pragma unroll
+  for (int n = 0; n < D / 8; ++n) acc[n][0] = acc[n][1] = acc[n][2] = acc[n][3] = 0.f;
+  uint32_t qf[D / 16][4];
+
+  for (int t = t0; t < t1; ++t) {
+    const int st = (t - t0) % kStages;
+    cp_async_wait<1>();                                      // tile t has landed (only tile t + 1 may still be in flight)
+    __syncthreads();                                         // ... for every thread, and nobody still reads the stage refilled next
+    if (t + 2 < t1) load_kv(t + 2, (st + 2) % kStages);
+    cp_async_commit();
+    if (t == t0 && active) {
+#pragma unroll
+      for (int kk = 0; kk < D / 16; ++kk) ldsm_x4(qf[kk], sbase + swz(warp * 16 + (lane & 15), kk * 2 + (lane >> 4)));
+    }
+    uint32_t kv16 = sbase + S::kKV + st * 2 * kTile16;
+    if constexpr (Q8) {                                      // raw 8-bit tiles -> the 16-bit tiles, exactly
+      kv16 = sbase + S::kKV;
+#pragma unroll
+      for (int i = 0; i < 2 * BN * (D / 16) / kThreads; ++i) {
+        const int id = i * kThreads + tid, kv = id / (BN * 8), row = (id / 8) % BN, c = id % 8;
+        const uint4 raw = *reinterpret_cast<const uint4*>(smem + S::kRaw + st * 2 * kTile8 + kv * kTile8 + row * D + c * 16);
+        float f[16];
+        kv8::to_float16<KV>(raw, f);
+        uint32_t w[8];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) w[e] = pack2<T>(f[2 * e], f[2 * e + 1]);
+        uint8_t* dst = smem + S::kKV + kv * kTile16;
+        *reinterpret_cast<uint4*>(dst + swz(row, 2 * c)) = make_uint4(w[0], w[1], w[2], w[3]);
+        *reinterpret_cast<uint4*>(dst + swz(row, 2 * c + 1)) = make_uint4(w[4], w[5], w[6], w[7]);
+      }
+      __syncthreads();
+    }
+    if (active) {
+      // S = Q K^T: 16 rows x 64 keys per warp
+      float s[BN / 8][4];
+#pragma unroll
+      for (int n = 0; n < BN / 8; ++n) s[n][0] = s[n][1] = s[n][2] = s[n][3] = 0.f;
+#pragma unroll
+      for (int kk = 0; kk < D / 16; ++kk) {
+#pragma unroll
+        for (int np = 0; np < BN / 16; ++np) {
+          uint32_t bf[4];
+          ldsm_x4(bf, kv16 + swz(np * 16 + (lane & 7) + ((lane >> 4) << 3), kk * 2 + ((lane >> 3) & 1)));
+          mma16816<T>(s[2 * np], qf[kk], bf[0], bf[1]);
+          mma16816<T>(s[2 * np + 1], qf[kk], bf[2], bf[3]);
+        }
+      }
+      // mask, online softmax (log2 domain); a row's 64 scores are spread over the 4 lanes of a quad
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        float mx = -INFINITY;
+#pragma unroll
+        for (int n = 0; n < BN / 8; ++n)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int key = t * BN + n * 8 + 2 * (lane & 3) + e;
+            float& v = s[n][hh * 2 + e];
+            v = key < limit[hh] ? v * qk_scale : -INFINITY;
+            mx = fmaxf(mx, v);
+          }
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+        const float m_new = fmaxf(m[hh], mx);
+        const float base = m_new == -INFINITY ? 0.f : m_new;   // a row with no visible key yet keeps p = 0 (never exp2(-inf + inf))
+        const float alpha = exp2f(m[hh] - base);
+        float sum = 0.f;
+#pragma unroll
+        for (int n = 0; n < BN / 8; ++n)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            float& v = s[n][hh * 2 + e];
+            v = exp2f(v - base);
+            sum += v;
+          }
+        l[hh] = l[hh] * alpha + sum;
+        m[hh] = m_new;
+#pragma unroll
+        for (int n = 0; n < D / 8; ++n) { acc[n][hh * 2] *= alpha; acc[n][hh * 2 + 1] *= alpha; }
+      }
+      // O += P V: P's accumulator fragments are the A fragments of the next MMA
+#pragma unroll
+      for (int kk = 0; kk < BN / 16; ++kk) {
+        const uint32_t pa[4] = {pack2<T>(s[2 * kk][0], s[2 * kk][1]), pack2<T>(s[2 * kk][2], s[2 * kk][3]),
+                                pack2<T>(s[2 * kk + 1][0], s[2 * kk + 1][1]), pack2<T>(s[2 * kk + 1][2], s[2 * kk + 1][3])};
+#pragma unroll
+        for (int np = 0; np < D / 16; ++np) {
+          uint32_t bf[4];
+          ldsm_x4_t(bf, kv16 + kTile16 + swz(kk * 16 + (lane & 7) + (((lane >> 3) & 1) << 3), np * 2 + (lane >> 4)));
+          mma16816<T>(acc[2 * np], pa, bf[0], bf[1]);
+          mma16816<T>(acc[2 * np + 1], pa, bf[2], bf[3]);
+        }
+      }
+    }
+  }
+  cp_async_wait<0>();
+  if (!active) return;
+  // this split's partial for the warp's rows (an empty split writes m = -inf, l = 0, acc = 0)
+  const int64_t pbase = (((int64_t)b * p.hkv + kvh) * p.splits + split) * kRows;
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    float lq = l[hh];
+    lq += __shfl_xor_sync(0xffffffffu, lq, 1);
+    lq += __shfl_xor_sync(0xffffffffu, lq, 2);
+    const int r = r_lo + hh * 8;
+    if (r >= nrows) continue;
+    float* pa = p.part_acc + (pbase + r) * D + 2 * (lane & 3);
+#pragma unroll
+    for (int n = 0; n < D / 8; ++n) *reinterpret_cast<float2*>(pa + n * 8) = make_float2(acc[n][hh * 2] * v_scale, acc[n][hh * 2 + 1] * v_scale);
+    if ((lane & 3) == 0) { p.part_ml[(pbase + r) * 2] = m[hh]; p.part_ml[(pbase + r) * 2 + 1] = lq; }
+  }
+}
+
+// grid (64 rows, Hkv, B), D threads: combines the splits of one query row, as decode_merge_kernel does, and writes it in place.  A
+// sequence over the row limit gets NaN rows rather than a silently partial result.
+template <typename T>
+__global__ void __launch_bounds__(D) multi_merge_kernel(const Params p) {
+  const int r = blockIdx.x, kvh = blockIdx.y, b = blockIdx.z, tid = threadIdx.x;
+  const int nq = p.n_q[b], g_size = p.h / p.hkv, nrows = nq * g_size;
+  if (nq <= 0) return;
+  T* out = reinterpret_cast<T*>(p.out);
+  const int64_t cu = p.cu_q[b];
+  if (nrows > kRows) {
+    for (int rr = r; rr < nrows; rr += kRows)
+      out[(cu + rr / g_size) * p.o_st + (int64_t)(kvh * g_size + rr % g_size) * D + tid] = from_f<T>(__int_as_float(0x7fc00000));
+    return;
+  }
+  if (r >= nrows) return;
+  const int64_t pb = ((int64_t)b * p.hkv + kvh) * p.splits * kRows + r;
+  float mg = -INFINITY;
+  for (int s = 0; s < p.splits; ++s) mg = fmaxf(mg, p.part_ml[(pb + (int64_t)s * kRows) * 2]);
+  float l = 0.f, o = 0.f;
+  for (int s = 0; s < p.splits; ++s) {
+    const int64_t i = pb + (int64_t)s * kRows;
+    const float ms = p.part_ml[i * 2];
+    const float f = (ms == -INFINITY) ? 0.f : exp2f(ms - mg);
+    l += p.part_ml[i * 2 + 1] * f;
+    o += p.part_acc[i * D + tid] * f;
+  }
+  out[(cu + r / g_size) * p.o_st + (int64_t)(kvh * g_size + r % g_size) * D + tid] = from_f<T>(l > 0.f ? o / l : 0.f);
+}
+
+}  // namespace decode_multi
+
 int decode_attention_splits(int b, int h, int smax) {
   // enough CTAs to fill the machine, at least 256 positions per split
   int splits = (2 * sm_count() + b * h - 1) / (b * h);
@@ -248,6 +523,44 @@ int decode_attention_paged_q8(const void* q, const void* k_cache, const void* v_
     if (kv_dtype == kI8) launch(__nv_bfloat16(), kv8::I8()); else launch(__nv_bfloat16(), kv8::E4M3());
   } else {
     if (kv_dtype == kI8) launch(__half(), kv8::I8()); else launch(__half(), kv8::E4M3());
+  }
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) { set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }
+  return 0;
+}
+
+int decode_attention_paged_multi(const PagedMultiArgs& a, cudaStream_t s) {
+  using namespace decode_multi;
+  if (a.d != D || a.hkv <= 0 || a.h % a.hkv || a.h / a.hkv > kRows || (a.dtype != kBF16 && a.dtype != kF16)) return 1;
+  if (a.kv_dtype != -1 && ((a.kv_dtype != kI8 && a.kv_dtype != kE4M3) || !a.k_dq || !a.v_dq)) return 1;
+  if (a.max_blocks <= 0 || a.block_size <= 0 || a.splits < 1) return 1;
+  if (a.q_st % 8 || a.q_sh % 8 || a.o_st % 8 || ((reinterpret_cast<uintptr_t>(a.q) | reinterpret_cast<uintptr_t>(a.k_cache) |
+                                                  reinterpret_cast<uintptr_t>(a.v_cache)) & 15)) return 1;
+  if (a.b == 0) return 0;
+  Params p;
+  p.q = a.q; p.k_cache = a.k_cache; p.v_cache = a.v_cache; p.out = a.out; p.part_acc = a.part_acc; p.part_ml = a.part_ml;
+  p.block_tables = a.block_tables; p.cu_q = a.cu_q; p.n_q = a.n_q; p.past = a.past; p.k_dq = a.k_dq; p.v_dq = a.v_dq;
+  p.q_st = a.q_st; p.q_sh = a.q_sh; p.o_st = a.o_st;
+  p.h = a.h; p.hkv = a.hkv; p.splits = a.splits; p.max_blocks = a.max_blocks; p.block_size = a.block_size;
+  p.scale_log2 = a.scale * 1.4426950408889634f;
+  const dim3 grid(a.splits, a.hkv, a.b), mgrid(kRows, a.hkv, a.b);
+  auto launch = [&](auto tag_t, auto tag_kv) {
+    using T = decltype(tag_t);
+    using KV = decltype(tag_kv);
+    constexpr int smem = Smem<!std::is_same<T, KV>::value>::kBytes;
+    static bool attr = false;   // one flag per instantiation
+    if (!attr) { B200_CUDA_CHECK(cudaFuncSetAttribute(multi_split_kernel<T, KV>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); attr = true; }
+    multi_split_kernel<T, KV><<<grid, kThreads, smem, s>>>(p);
+    multi_merge_kernel<T><<<mgrid, D, 0, s>>>(p);
+  };
+  if (a.dtype == kBF16) {
+    if (a.kv_dtype == kI8) launch(__nv_bfloat16(), kv8::I8());
+    else if (a.kv_dtype == kE4M3) launch(__nv_bfloat16(), kv8::E4M3());
+    else launch(__nv_bfloat16(), __nv_bfloat16());
+  } else {
+    if (a.kv_dtype == kI8) launch(__half(), kv8::I8());
+    else if (a.kv_dtype == kE4M3) launch(__half(), kv8::E4M3());
+    else launch(__half(), __half());
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }

@@ -191,6 +191,25 @@ int decode_attention(const void* q, const void* k_cache, const void* v_cache, co
 int decode_attention_paged_q8(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* out, float* part_acc, float* part_ml,
                               int b, int h, int hkv, int d, int splits, float scale, int dtype, int kv_dtype, const float* k_dq, const float* v_dq,
                               const int* block_tables, int max_blocks, int block_size, cudaStream_t s);
+// Multi-token paged decode (verify rows of speculative decoding): sequence i brings n_q[i] new tokens at packed rows cu_q[i] ... over
+// past[i] cached positions (the new K / V already written); key j is visible to new token r iff j <= past[i] + r.  q: [t, h, 128] rows
+// (strides q_st, q_sh); out [t, h * 128] (row stride o_st), written only at the new tokens' rows; sequences with n_q = 0 are skipped.
+// n_q * (h / hkv) must not exceed 64: a sequence beyond that gets NaN rows.  Caches [num_blocks, hkv, block_size, 128] of q's dtype, or
+// int8 / fp8 e4m3 (kv_dtype kI8 / kE4M3) with fp32 [hkv] dequant scales.  part_acc: fp32 [b, hkv, splits, 64, 128] and part_ml: fp32
+// [b, hkv, splits, 64, 2] scratch.  No host read of the lengths.
+struct PagedMultiArgs {
+  const void* q; const void* k_cache; const void* v_cache; void* out;
+  float* part_acc; float* part_ml;
+  const int* block_tables; const int* cu_q; const int* n_q; const int* past;
+  int64_t q_st, q_sh, o_st;
+  int b, h, hkv, d, max_blocks, block_size, splits;
+  float scale;
+  int dtype;
+  int kv_dtype = -1;
+  const float* k_dq = nullptr;
+  const float* v_dq = nullptr;
+};
+int decode_attention_paged_multi(const PagedMultiArgs& a, cudaStream_t s);
 
 // ---- kv_cache_quant.cu ----------------------------------------------------------------------------------------
 // Quantizing write of every sequence's new K / V rows (read in place from the packed qkv [t, (h + 2 hkv) * 128] rows, row stride in

@@ -20,6 +20,9 @@ def _raw(t):
 
 
 _PREFILL_BLOCK_SIZES = (16, 32, 64, 128, 256)
+# Longest continuing chunk (seq_lens_encoder == 0) that block_attention sends to `decode_attention_paged_multi` rather than
+# `attention_fwd_paged`; also capped so that now * (H / H_kv) <= 64.  Set from scripts/bench_spec_verify.py (DESIGN.md section 4).
+VERIFY_MAX = 16
 _KV8_DTYPES = (torch.int8, torch.float8_e4m3fn)
 _KV8_LIMITS = {torch.int8: (-128.0, 127.0), torch.float8_e4m3fn: (-448.0, 448.0)}
 
@@ -102,17 +105,21 @@ def block_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_deco
     """qkv: [total_tokens, (H + 2*H_kv) * D] packed over the batch; caches [num_blocks, H_kv, block_size, D].
 
     A sequence prefills when seq_lens_encoder > 0 (a fresh prompt) or when it brings more than one token on top of seq_lens_decoder cached
-    ones (a continuing chunk); it decodes when it brings exactly one token and seq_lens_encoder == 0.
+    ones (a continuing chunk); it decodes when it brings exactly one token and seq_lens_encoder == 0.  A continuing chunk of 2 ..
+    VERIFY_MAX tokens with now * (H / H_kv) <= 64 - the verify rows of speculative decoding - is a short chunk.
 
     CUDA path (head_dim 128, fp16 / bf16, block_size 16 / 32 / 64 / 128 / 256): the new K / V rows of EVERY sequence are scattered into the
     paged caches with one indexed write (block and row computed on the device from the block table - no per-token Python loop); decode
     sequences attend to their cache through `decode_attention_paged` (csrc/decode_attention.cu: one table lookup per cached row, split-K
     over the positions); all prefill sequences run in ONE launch of `attention_fwd_paged` (csrc/attention_sm100.cu): causal wgmma flash
     attention of each sequence's new tokens over its whole cached prefix, K / V read in place through the block table, q read and the
-    output written in place at the tokens' rows.  Other block sizes and devices take `_block_attention_ref`.
+    output written in place at the tokens' rows; all short chunks run in ONE launch of `decode_attention_paged_multi`
+    (csrc/decode_attention.cu: split-K over the cached positions, every query row of a KV head in one tensor-core tile, q and the output in
+    place as for prefill).  The three row kinds are told apart with one host read.  Other block sizes and devices take
+    `_block_attention_ref`.
 
     int8 / float8_e4m3fn caches (static scales, see the module docstring): the new rows are quantized into the caches by one launch of
-    `paged_kv_cache_write` (csrc/kv_cache_quant.cu), and both attention kernels read the 8-bit rows and dequantize them on the fly."""
+    `paged_kv_cache_write` (csrc/kv_cache_quant.cu), and the attention kernels read the 8-bit rows and dequantize them on the fly."""
     qkv, kc, vc = _raw(qkv), _raw(key_cache), _raw(value_cache)
     nkv, d = kc.shape[1], kc.shape[3]
     quant = kv_quant_params(kc, vc, cache_k_quant_scales, cache_v_quant_scales, cache_k_dequant_scales, cache_v_dequant_scales,
@@ -155,8 +162,9 @@ def block_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_deco
     out = qkv.new_zeros((total_tokens, nh * d))
     scale = 1.0 / math.sqrt(d)
     is_dec = (now == 1) & (enc == 0)
-    is_pre = (now > 0) & ~is_dec
-    any_dec, any_pre = torch.stack([is_dec.any(), is_pre.any()]).tolist()
+    is_ver = (enc == 0) & (now >= 2) & (now <= min(VERIFY_MAX, 64 // (nh // nkv)))
+    is_pre = (now > 0) & ~is_dec & ~is_ver
+    any_dec, any_ver, any_pre = torch.stack([is_dec.any(), is_ver.any(), is_pre.any()]).tolist()
     # ---- decode sequences: one query token against the paged cache
     if any_dec:
         ids = is_dec.nonzero().reshape(-1)
@@ -164,7 +172,10 @@ def block_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_deco
         lens = (dec[ids] + 1).to(torch.int32).contiguous()
         od = ext().decode_attention_paged(qd, kc, vc, lens, bt[ids].contiguous(), scale, **dq)
         out[cu[ids]] = od.reshape(ids.numel(), nh * d)
-    # ---- prefill sequences (fresh prompts and continuing chunks): new tokens over their whole cached prefix, one launch for all
+    # ---- short chunks (verify rows): a few new tokens over a long cached prefix, one launch for all
+    if any_ver:
+        ext().decode_attention_paged_multi(q, kc, vc, bt, i32(cu[:nseq]), i32(torch.where(is_ver, now, 0)), i32(past), scale, out, **dq)
+    # ---- prefill sequences (fresh prompts and longer continuing chunks): new tokens over their whole cached prefix, one launch for all
     if any_pre:
         ext().attention_fwd_paged(q, kc, vc, bt, i32(cu[:nseq]), i32(torch.where(is_pre, now, 0)), i32(past), scale, out, **dq)
     return out.as_subclass(Tensor), qkv.as_subclass(Tensor), kc.as_subclass(Tensor), vc.as_subclass(Tensor)
