@@ -3,8 +3,10 @@
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
 
+#include <algorithm>
 #include <atomic>
 #include <optional>
+#include <vector>
 
 #include "include/b200_ops.h"
 #include "runtime/runtime.h"
@@ -943,6 +945,119 @@ void decode_attention_paged_multi(const Tensor& q, const Tensor& k_cache, const 
   TORCH_CHECK(rc == 0, "paddle_b200.decode_attention_paged_multi: unsupported operands (16-byte aligned rows and caches) rc=", rc);
 }
 
+// Shared-prefix decode over the paged KV cache (new K / V already written): q [T,H,D] view of the packed qkv rows, caches
+// [num_blocks,Hkv,block_size,D], block_tables int32 [B,max_blocks], cu_q / lens int32 [B] on the device (lens: keys including the new
+// token).  Groups on the host: cu_groups int32 [G+1], group_seqs int32 [n] (distinct batch indices), prefix_len int32 [G] (positive
+// multiples of block_size); every member of group g shares its first prefix_len[g] / block_size table entries with the others.  Writes
+// out [T, H*D] at the members' rows only.  The host builds the task list (prefix tiles of up to 64 / (H / Hkv) members, one suffix task
+// per member, split counts) and copies it to the device; no device value is read.  A member breaking the contract gets NaN rows.
+void decode_attention_paged_shared(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& block_tables, const Tensor& cu_q,
+                                   const Tensor& lens, const Tensor& cu_groups, const Tensor& group_seqs, const Tensor& prefix_len, double scale,
+                                   const Tensor& out, const OptT& k_dequant_scales, const OptT& v_dequant_scales) {
+  const char* fn = "decode_attention_paged_shared";
+  TORCH_CHECK(q.is_cuda() && q.dim() == 3 && q.stride(2) == 1, fn, ": q must be a CUDA [T,H,D] view with unit head_dim stride");
+  TORCH_CHECK(q.scalar_type() == at::kHalf || q.scalar_type() == at::kBFloat16, fn, ": q must be fp16 or bf16");
+  TORCH_CHECK(k_cache.dim() == 4 && v_cache.dim() == 4 && k_cache.is_contiguous() && v_cache.is_contiguous() && k_cache.sizes() == v_cache.sizes(),
+              fn, ": caches must be contiguous [num_blocks,Hkv,block_size,D] of one shape");
+  TORCH_CHECK(k_cache.device() == q.device() && v_cache.device() == q.device(), fn, ": q and caches must be on one device");
+  const int kv = kv8_code(fn, q, k_cache, v_cache, k_dequant_scales, v_dequant_scales);
+  if (kv == -1)
+    TORCH_CHECK(k_cache.scalar_type() == q.scalar_type() && v_cache.scalar_type() == q.scalar_type(), fn, ": q and caches must share a dtype");
+  TORCH_CHECK(block_tables.device() == q.device() && block_tables.scalar_type() == at::kInt && block_tables.is_contiguous() && block_tables.dim() == 2
+              && block_tables.size(1) > 0, fn, ": block_tables must be int32 [B, max_blocks] on the device");
+  const int64_t b = block_tables.size(0);
+  for (const Tensor* t : {&cu_q, &lens})
+    TORCH_CHECK(t->device() == q.device() && t->scalar_type() == at::kInt && t->is_contiguous() && t->numel() == b, fn, ": cu_q / lens must be int32 [B] on the device");
+  for (const Tensor* t : {&cu_groups, &group_seqs, &prefix_len})
+    TORCH_CHECK(t->device().is_cpu() && t->scalar_type() == at::kInt && t->is_contiguous() && t->dim() == 1, fn,
+                ": cu_groups / group_seqs / prefix_len must be int32 1-D tensors on the host");
+  TORCH_CHECK(out.device() == q.device() && out.scalar_type() == q.scalar_type() && out.dim() == 2 && out.size(0) == q.size(0) &&
+              out.size(1) == q.size(1) * q.size(2) && out.stride(1) == 1, fn, ": out must be [T, H*D] with unit inner stride");
+  TORCH_CHECK(q.size(2) == 128 && k_cache.size(3) == 128, fn, ": head_dim must be 128");
+  const int64_t hkv = k_cache.size(1), h = q.size(1), bs = k_cache.size(2), max_blocks = block_tables.size(1);
+  TORCH_CHECK(hkv > 0 && h % hkv == 0 && h / hkv <= 64, fn, ": H must be a multiple of Hkv with H / Hkv <= 64");
+  const int64_t g_size = h / hkv, ng = prefix_len.numel(), n = group_seqs.numel();
+  const int* cg = cu_groups.data_ptr<int>();
+  const int* gs = group_seqs.data_ptr<int>();
+  const int* pl = prefix_len.data_ptr<int>();
+  TORCH_CHECK(cu_groups.numel() == ng + 1 && cg[0] == 0 && cg[ng] == n, fn, ": cu_groups must be [G + 1] from 0 to len(group_seqs)");
+  std::vector<char> seen(b, 0);
+  for (int64_t g = 0; g < ng; ++g) {
+    TORCH_CHECK(cg[g + 1] > cg[g], fn, ": every group needs at least one member (cu_groups must rise strictly)");
+    // messages take std::to_string: a number streamed into TORCH_CHECK's ostringstream crashes this extension (DESIGN.md section 2)
+    TORCH_CHECK(pl[g] > 0 && pl[g] % bs == 0 && pl[g] / bs <= max_blocks, fn, ": prefix_len must be a positive multiple of block_size ",
+                std::to_string(bs), " within the block table, got ", std::to_string(pl[g]));
+  }
+  for (int64_t i = 0; i < n; ++i) {
+    TORCH_CHECK(gs[i] >= 0 && gs[i] < b, fn, ": group_seqs holds batch index ", std::to_string(gs[i]), " outside [0, ", std::to_string(b), ")");
+    TORCH_CHECK(!seen[gs[i]], fn, ": sequence ", std::to_string(gs[i]), " is in more than one group");
+    seen[gs[i]] = 1;
+  }
+  if (n == 0) return;
+  // task list: every group's prefix tiles (split over its prefix), then one suffix task per member (split over the longest possible suffix)
+  const int sm = at::cuda::getDeviceProperties(q.device().index())->multiProcessorCount;
+  const int64_t per_tile = 64 / g_size;
+  int64_t n_tiles = 0;
+  for (int64_t g = 0; g < ng; ++g) n_tiles += (cg[g + 1] - cg[g] + per_tile - 1) / per_tile;
+  auto splits_for = [&](int64_t ctas, int64_t keys) {
+    int64_t s = (2 * sm + ctas * hkv - 1) / (ctas * hkv);
+    s = std::min(s, std::max<int64_t>((keys + 255) / 256, 1));
+    return (int)std::max<int64_t>(1, std::min<int64_t>(s, 64));
+  };
+  int min_plen = pl[0];
+  for (int64_t g = 1; g < ng; ++g) min_plen = std::min(min_plen, pl[g]);
+  const int suf_splits = splits_for(n, max_blocks * bs - min_plen);
+  std::vector<int> tasks, members(n * b200::kSharedMemberInts);
+  int64_t rows = 0;
+  auto add_task = [&](int tb, int m0, int cnt, int lo, int hi, int splits) {
+    const int64_t t0 = (int64_t)tasks.size() / b200::kSharedTaskInts;
+    for (int s = 0; s < splits; ++s) {
+      tasks.insert(tasks.end(), {tb, m0, cnt, lo, hi, s, splits, (int)rows});
+      rows += cnt * g_size;
+    }
+    return (int)t0;
+  };
+  for (int64_t g = 0; g < ng; ++g) {
+    const int splits = splits_for(n_tiles, pl[g]);
+    for (int m0 = cg[g]; m0 < cg[g + 1]; m0 += per_tile) {
+      const int cnt = std::min<int>(per_tile, cg[g + 1] - m0);
+      const int t0 = add_task(gs[cg[g]], m0, cnt, 0, pl[g], splits);
+      for (int i = m0; i < m0 + cnt; ++i) {
+        int* mi = members.data() + (int64_t)i * b200::kSharedMemberInts;
+        mi[0] = t0; mi[1] = (int)((i - m0) * g_size); mi[3] = gs[cg[g]]; mi[4] = pl[g]; mi[5] = gs[i];
+      }
+    }
+  }
+  for (int64_t g = 0; g < ng; ++g)
+    for (int i = cg[g]; i < cg[g + 1]; ++i) members[(int64_t)i * b200::kSharedMemberInts + 2] = add_task(gs[i], i, 1, pl[g], -1, suf_splits);
+  const int64_t n_tasks = (int64_t)tasks.size() / b200::kSharedTaskInts;
+  TORCH_CHECK(rows < INT32_MAX && n_tasks < INT32_MAX, fn, ": too many tasks");
+  c10::cuda::CUDAGuard guard(q.device());
+  // one pinned host buffer (group_seqs | tasks | members), one asynchronous copy
+  Tensor host = torch::empty({n + (int64_t)tasks.size() + (int64_t)members.size()}, at::TensorOptions().dtype(at::kInt).pinned_memory(true));
+  int* hp = host.data_ptr<int>();
+  std::copy(gs, gs + n, hp);
+  std::copy(tasks.begin(), tasks.end(), hp + n);
+  std::copy(members.begin(), members.end(), hp + n + tasks.size());
+  Tensor dev = host.to(q.device(), /*non_blocking=*/true);
+  b200::PagedSharedArgs a;
+  a.q = q.data_ptr(); a.k_cache = k_cache.data_ptr(); a.v_cache = v_cache.data_ptr(); a.out = out.data_ptr();
+  a.block_tables = block_tables.data_ptr<int>(); a.cu_q = cu_q.data_ptr<int>(); a.lens = lens.data_ptr<int>();
+  a.group_seqs = dev.data_ptr<int>(); a.tasks = a.group_seqs + n; a.members = a.tasks + tasks.size();
+  a.q_st = q.stride(0); a.q_sh = q.stride(1); a.o_st = out.stride(0);
+  a.n_tasks = (int)n_tasks; a.n_members = (int)n; a.rows = (int)rows;
+  a.h = (int)h; a.hkv = (int)hkv; a.d = (int)q.size(2); a.max_blocks = (int)max_blocks; a.block_size = (int)bs;
+  a.scale = (float)scale; a.dtype = dt_code(q);
+  if (kv != -1) { a.kv_dtype = kv; a.k_dq = k_dequant_scales->data_ptr<float>(); a.v_dq = v_dequant_scales->data_ptr<float>(); }
+  Tensor pacc = torch::empty({hkv, rows, 128}, q.options().dtype(at::kFloat));
+  Tensor pml = torch::empty({hkv, rows, 2}, q.options().dtype(at::kFloat));
+  a.part_acc = pacc.data_ptr<float>(); a.part_ml = pml.data_ptr<float>();
+  int rc = b200::decode_attention_paged_shared(a, cur_stream());
+  g_launches += 2;
+  check_err();
+  TORCH_CHECK(rc == 0, "paddle_b200.decode_attention_paged_shared: unsupported operands (16-byte aligned rows and caches) rc=", std::to_string(rc));
+}
+
 // Quantizing write of every sequence's new K / V rows into paged int8 / fp8 e4m3 caches: qkv [T, (H + 2 Hkv) * D] packed rows (unit
 // inner stride), caches [num_blocks, Hkv, block_size, D], cu_q int32 [B + 1], seq_lens_encoder / seq_lens_decoder int32 [B], block_tables
 // int32 [B, max_blocks], quant scales fp32 [Hkv]; y = (max_bound * scale) * x rounded (round_type 0: rint, 1: roundf) and clamped to the bounds.
@@ -1133,6 +1248,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         pybind11::arg("k_cache"), pybind11::arg("v_cache"), pybind11::arg("block_tables"), pybind11::arg("cu_q"), pybind11::arg("n_q"),
         pybind11::arg("past"), pybind11::arg("scale"), pybind11::arg("out"), pybind11::arg("k_dequant_scales") = pybind11::none(),
         pybind11::arg("v_dequant_scales") = pybind11::none());
+  m.def("decode_attention_paged_shared", traced("decode_attention_paged_shared", &decode_attention_paged_shared), pybind11::arg("q"),
+        pybind11::arg("k_cache"), pybind11::arg("v_cache"), pybind11::arg("block_tables"), pybind11::arg("cu_q"), pybind11::arg("lens"),
+        pybind11::arg("cu_groups"), pybind11::arg("group_seqs"), pybind11::arg("prefix_len"), pybind11::arg("scale"), pybind11::arg("out"),
+        pybind11::arg("k_dequant_scales") = pybind11::none(), pybind11::arg("v_dequant_scales") = pybind11::none());
   m.def("attention_bwd", traced("attention_bwd", &attention_bwd), pybind11::arg("q"), pybind11::arg("k"), pybind11::arg("v"), pybind11::arg("out"), pybind11::arg("lse"),
         pybind11::arg("d_out"), pybind11::arg("scale"), pybind11::arg("causal"), pybind11::arg("colmask") = pybind11::none());
   m.def("attention_bwd_packed", traced("attention_bwd_packed", &attention_bwd_packed), pybind11::arg("qkv"), pybind11::arg("nh"), pybind11::arg("nkv"), pybind11::arg("out"),

@@ -210,6 +210,27 @@ struct PagedMultiArgs {
   const float* v_dq = nullptr;
 };
 int decode_attention_paged_multi(const PagedMultiArgs& a, cudaStream_t s);
+// Shared-prefix decode over the paged KV cache: single-token decode rows (query row cu_q[b], lens[b] keys including the new one) of
+// sequences grouped so that a group's members share their first prefix_len table entries.  The host-built task list, on the device:
+//   tasks [n_tasks][kSharedTaskInts]: {table row, first index into group_seqs, members, first key, key end (prefix_len) or -1 (the
+//     sequence's length), split, splits, first row in the partial buffer}; one CTA per (task, KV head);
+//   members [n_members][kSharedMemberInts]: {first prefix task, row offset in it, first suffix task, group's first sequence,
+//     prefix_len, sequence}.
+// part_acc fp32 [hkv, rows, 128] and part_ml fp32 [hkv, rows, 2] scratch.  A member breaking the group contract gets NaN rows.
+constexpr int kSharedTaskInts = 8, kSharedMemberInts = 6;
+struct PagedSharedArgs {
+  const void* q; const void* k_cache; const void* v_cache; void* out;
+  float* part_acc; float* part_ml;
+  const int* block_tables; const int* cu_q; const int* lens; const int* group_seqs; const int* tasks; const int* members;
+  int64_t q_st, q_sh, o_st;
+  int n_tasks, n_members, rows, h, hkv, d, max_blocks, block_size;
+  float scale;
+  int dtype;
+  int kv_dtype = -1;
+  const float* k_dq = nullptr;
+  const float* v_dq = nullptr;
+};
+int decode_attention_paged_shared(const PagedSharedArgs& a, cudaStream_t s);
 
 // ---- kv_cache_quant.cu ----------------------------------------------------------------------------------------
 // Quantizing write of every sequence's new K / V rows (read in place from the packed qkv [t, (h + 2 hkv) * 128] rows, row stride in

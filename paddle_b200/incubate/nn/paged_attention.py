@@ -23,6 +23,14 @@ _PREFILL_BLOCK_SIZES = (16, 32, 64, 128, 256)
 # Longest continuing chunk (seq_lens_encoder == 0) that block_attention sends to `decode_attention_paged_multi` rather than
 # `attention_fwd_paged`; also capped so that now * (H / H_kv) <= 64.  Set from scripts/bench_spec_verify.py (DESIGN.md section 4).
 VERIFY_MAX = 16
+# Decode rows that share a cached prefix run on `decode_attention_paged_shared` only in groups of at least SHARED_PREFIX_MIN_GROUP
+# sequences sharing at least SHARED_PREFIX_MIN_TOKENS prefix tokens; smaller groups stay on `decode_attention_paged`.  Set from
+# scripts/bench_prefix_caching.py (DESIGN.md section 4).
+SHARED_PREFIX_MIN_GROUP = 4
+SHARED_PREFIX_MIN_TOKENS = 4096
+# ... or of at least SHARED_PREFIX_LARGE_GROUP sequences sharing at least SHARED_PREFIX_LARGE_GROUP_MIN_TOKENS.
+SHARED_PREFIX_LARGE_GROUP = 16
+SHARED_PREFIX_LARGE_GROUP_MIN_TOKENS = 512
 _KV8_DTYPES = (torch.int8, torch.float8_e4m3fn)
 _KV8_LIMITS = {torch.int8: (-128.0, 127.0), torch.float8_e4m3fn: (-448.0, 448.0)}
 
@@ -91,6 +99,41 @@ def dequantize_kv(q, dequant_scale):
     return q.float() * dequant_scale.to(q.device, torch.float32)[:, None, None]
 
 
+def shared_prefix_pays(group_size, prefix_len, heads_per_kv):
+    """Whether a group of `group_size` decode rows sharing `prefix_len` cached tokens is worth `decode_attention_paged_shared`.  On an H100
+    (DESIGN.md section 4) it lost to `decode_attention_paged` in groups of 2 at every prefix with 32 / 32 heads and an int8 cache, and in
+    groups of 2 and 4 at 512 - 1024 prefix tokens; it won in every measured group of 4 from 4096 tokens and of 16 from 512.  heads_per_kv
+    (H / H_kv) is not used: those break-even points held for 32 / 8 and 32 / 32 heads alike."""
+    return ((group_size >= SHARED_PREFIX_MIN_GROUP and prefix_len >= SHARED_PREFIX_MIN_TOKENS)
+            or (group_size >= SHARED_PREFIX_LARGE_GROUP and prefix_len >= SHARED_PREFIX_LARGE_GROUP_MIN_TOKENS))
+
+
+def _shared_prefix_groups(shared_prefix, nseq, block_size):
+    """Validates the host-visible part of block_attention's shared_prefix = (cu_groups [G+1], group_seqs [n], prefix_len [G]) (host
+    lists or CPU integer tensors) and returns them as int lists.  Raises ValueError."""
+    def as_list(v, name):
+        if isinstance(v, torch.Tensor):
+            v = _raw(v)
+            if v.device.type != "cpu" or v.dtype not in (torch.int32, torch.int64) or v.dim() != 1:
+                raise ValueError(f"shared_prefix: {name} must be a host list or a 1-D CPU integer tensor")
+            return v.tolist()
+        return [int(x) for x in v]
+
+    try:
+        cu, seqs, plen = shared_prefix
+    except (TypeError, ValueError):
+        raise ValueError("shared_prefix must be (cu_groups, group_seqs, prefix_len)") from None
+    cu, seqs, plen = as_list(cu, "cu_groups"), as_list(seqs, "group_seqs"), as_list(plen, "prefix_len")
+    if len(cu) != len(plen) + 1 or not cu or cu[0] != 0 or cu[-1] != len(seqs) or any(b <= a for a, b in zip(cu, cu[1:])):
+        raise ValueError(f"shared_prefix: cu_groups must rise strictly from 0 to len(group_seqs) = {len(seqs)} in len(prefix_len) + 1 "
+                         f"steps, got {cu}")
+    if any(not 0 <= b < nseq for b in seqs) or len(set(seqs)) != len(seqs):
+        raise ValueError(f"shared_prefix: group_seqs must be distinct batch indices in [0, {nseq}), got {seqs}")
+    if any(p <= 0 or p % int(block_size) for p in plen):
+        raise ValueError(f"shared_prefix: every prefix_len must be a positive multiple of block_size {block_size}, got {plen}")
+    return cu, seqs, plen
+
+
 def _paged_kernels_ok(qkv, kc, d, block_size, quant=None):
     from ...framework.flags import flag
 
@@ -101,7 +144,7 @@ def _paged_kernels_ok(qkv, kc, d, block_size, quant=None):
 
 def block_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_decoder, seq_lens_this_time, cu_seqlens_q, block_tables, block_size,
                     cache_k_quant_scales=None, cache_v_quant_scales=None, cache_k_dequant_scales=None, cache_v_dequant_scales=None,
-                    use_dynamic_cachekv_quant=False, quant_round_type=1, quant_max_bound=127.0, quant_min_bound=-127.0):
+                    use_dynamic_cachekv_quant=False, quant_round_type=1, quant_max_bound=127.0, quant_min_bound=-127.0, shared_prefix=None):
     """qkv: [total_tokens, (H + 2*H_kv) * D] packed over the batch; caches [num_blocks, H_kv, block_size, D].
 
     A sequence prefills when seq_lens_encoder > 0 (a fresh prompt) or when it brings more than one token on top of seq_lens_decoder cached
@@ -119,14 +162,21 @@ def block_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_deco
     `_block_attention_ref`.
 
     int8 / float8_e4m3fn caches (static scales, see the module docstring): the new rows are quantized into the caches by one launch of
-    `paged_kv_cache_write` (csrc/kv_cache_quant.cu), and the attention kernels read the 8-bit rows and dequantize them on the fly."""
+    `paged_kv_cache_write` (csrc/kv_cache_quant.cu), and the attention kernels read the 8-bit rows and dequantize them on the fly.
+
+    shared_prefix = (cu_groups [G+1], group_seqs [n], prefix_len [G]), host lists or CPU int tensors: group g's members, the batch indices
+    group_seqs[cu_groups[g]:cu_groups[g+1]], are decode rows whose first prefix_len[g] / block_size table entries are the same blocks
+    (prefix_len a positive multiple of block_size, at most each member's cached length).  Their rows run in ONE launch pair of
+    `decode_attention_paged_shared` (csrc/decode_attention.cu), which reads each group's prefix once per 64-row tile of members instead of
+    once per member.  A grouped row that is not a decode row raises ValueError; a member whose table or length breaks the contract gets
+    NaN rows (the device data is not read on the host).  Every other row takes its usual path.  None: no grouping."""
     qkv, kc, vc = _raw(qkv), _raw(key_cache), _raw(value_cache)
     nkv, d = kc.shape[1], kc.shape[3]
     quant = kv_quant_params(kc, vc, cache_k_quant_scales, cache_v_quant_scales, cache_k_dequant_scales, cache_v_dequant_scales,
                             use_dynamic_cachekv_quant, quant_round_type, quant_max_bound, quant_min_bound)
     if not _paged_kernels_ok(qkv, kc, d, block_size, quant):
         return _block_attention_ref(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_decoder, seq_lens_this_time, cu_seqlens_q, block_tables,
-                                    block_size, quant=quant)
+                                    block_size, quant=quant, shared_prefix=shared_prefix)
     from ..._build import ext
 
     dev = qkv.device
@@ -164,7 +214,21 @@ def block_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_deco
     is_dec = (now == 1) & (enc == 0)
     is_ver = (enc == 0) & (now >= 2) & (now <= min(VERIFY_MAX, 64 // (nh // nkv)))
     is_pre = (now > 0) & ~is_dec & ~is_ver
-    any_dec, any_ver, any_pre = torch.stack([is_dec.any(), is_ver.any(), is_pre.any()]).tolist()
+    if shared_prefix is None:
+        any_dec, any_ver, any_pre = torch.stack([is_dec.any(), is_ver.any(), is_pre.any()]).tolist()
+    else:
+        groups = _shared_prefix_groups(shared_prefix, nseq, block_size)
+        in_group = torch.zeros(nseq, dtype=torch.bool)
+        in_group[groups[1]] = True
+        in_group = in_group.pin_memory().to(dev, non_blocking=True)        # a pinned copy: the host does not wait for the stream
+        bad = in_group & ~is_dec
+        is_dec = is_dec & ~in_group
+        any_dec, any_ver, any_pre, any_bad = torch.stack([is_dec.any(), is_ver.any(), is_pre.any(), bad.any()]).tolist()
+        if any_bad:
+            raise ValueError("block_attention: shared_prefix groups may only hold decode rows (seq_lens_this_time 1, seq_lens_encoder 0)")
+        # ---- grouped decode rows: each group's prefix read once per tile of members, then every member's own keys
+        ext().decode_attention_paged_shared(q, kc, vc, bt, i32(cu[:nseq]), i32(dec + 1), *(torch.tensor(v, dtype=torch.int32) for v in groups),
+                                            scale, out, **dq)
     # ---- decode sequences: one query token against the paged cache
     if any_dec:
         ids = is_dec.nonzero().reshape(-1)
@@ -183,9 +247,11 @@ def block_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_deco
 
 def _block_attention_ref(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_decoder, seq_lens_this_time, cu_seqlens_q, block_tables, block_size,
                          cache_k_quant_scales=None, cache_v_quant_scales=None, cache_k_dequant_scales=None, cache_v_dequant_scales=None,
-                         use_dynamic_cachekv_quant=False, quant_round_type=1, quant_max_bound=127.0, quant_min_bound=-127.0, quant=None):
+                         use_dynamic_cachekv_quant=False, quant_round_type=1, quant_max_bound=127.0, quant_min_bound=-127.0, quant=None,
+                         shared_prefix=None):
     """qkv: [total_tokens, (H + 2*H_kv) * D] packed over the batch; caches [num_blocks, H_kv, block_size, D].  `quant`: an already
-    validated KVQuant (otherwise it is built from the scale / round / bound arguments)."""
+    validated KVQuant (otherwise it is built from the scale / round / bound arguments).  `shared_prefix`: as in block_attention; its whole
+    contract is checked here (ValueError on a violation), and it does not change the math."""
     qkv, kc, vc = _raw(qkv), _raw(key_cache), _raw(value_cache)
     if quant is None:
         quant = kv_quant_params(kc, vc, cache_k_quant_scales, cache_v_quant_scales, cache_k_dequant_scales, cache_v_dequant_scales,
@@ -195,6 +261,8 @@ def _block_attention_ref(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens
     enc, dec, now = _raw(seq_lens_encoder).reshape(-1).tolist(), _raw(seq_lens_decoder).reshape(-1).tolist(), _raw(seq_lens_this_time).reshape(-1).tolist()
     cu = _raw(cu_seqlens_q).reshape(-1).tolist()
     bt = _raw(block_tables)
+    if shared_prefix is not None:
+        _check_shared_prefix(shared_prefix, enc, dec, now, bt, block_size)
     out = qkv.new_zeros((qkv.shape[0], nh * d))
     for b in range(len(now)):
         n = now[b]
@@ -228,3 +296,19 @@ def _block_attention_ref(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens
         o = torch.einsum("hns,hsd->nhd", torch.softmax(s, -1), V.float())
         out[cu[b]:cu[b] + n] = o.reshape(n, nh * d).to(out.dtype)
     return out.as_subclass(Tensor), qkv.as_subclass(Tensor), kc.as_subclass(Tensor), vc.as_subclass(Tensor)
+
+
+def _check_shared_prefix(shared_prefix, enc, dec, now, block_tables, block_size):
+    """The full shared_prefix contract over host copies of the lengths and tables: ValueError on the first violation."""
+    cu, seqs, plen = _shared_prefix_groups(shared_prefix, len(now), block_size)
+    bt = block_tables.cpu()
+    for g, p in enumerate(plen):
+        idx = seqs[cu[g]:cu[g + 1]]
+        nb = p // int(block_size)
+        for b in idx:
+            if now[b] != 1 or enc[b] != 0:
+                raise ValueError(f"shared_prefix: sequence {b} is not a decode row (seq_lens_this_time {now[b]}, seq_lens_encoder {enc[b]})")
+            if p > dec[b]:
+                raise ValueError(f"shared_prefix: prefix_len {p} of group {g} exceeds the {dec[b]} cached tokens of sequence {b}")
+            if nb > bt.shape[1] or not torch.equal(bt[b, :nb], bt[idx[0], :nb]):
+                raise ValueError(f"shared_prefix: sequence {b} does not share the first {nb} blocks of group {g}")

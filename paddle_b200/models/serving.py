@@ -28,12 +28,27 @@ then runs k_s - 1 single-token forwards, proposing its argmax each time.  One ta
 now = 1 + k_s tokens (block_attention sends those rows to `decode_attention_paged_multi`); the longest prefix of proposals equal to
 the target's argmax is accepted, followed by the target's own token at the first mismatch (or the bonus token after a full match),
 so greedy outputs equal non-speculative decoding.  Sampling requests decode one token per step as without a draft.
+
+Prefix caching (`enable_prefix_caching=True`, off by default): a memory policy - cached blocks stay resident until they are evicted.  A full
+block is registered once all its positions are in the cache, under a BlockKey (the previous block's key, its token ids); prompt and
+generated-token blocks alike, so a preempted sequence finds its own blocks when it is readmitted.  Admission matches the longest chain of
+registered blocks covering tokens[:total - 1] (the last token is always computed: its logits give the first sample), so the first computed
+position is a block boundary and no sequence ever writes into a shared block.  The sequence starts with cached = the matched tokens; its
+prefill is an ordinary continuing chunk, charged only the unmatched tokens.  Blocks are reference-counted (PrefixCachingAllocator): a
+registered block nobody holds is evictable - still matchable, in LRU order, a finished sequence's chain joining tail first - and alloc()
+takes a free block before evicting one; num_free() counts both.  A key already registered by another block (identical prompts admitted in
+one step) leaves the block private.  With a draft model a block registers only once both caches hold it (min(cached, draft_cached) >= its
+end), and a sampling request's blocks never register, since the draft writes rows for greedy sequences only; a hit sets draft_cached =
+cached.  Each step the plain decode rows are grouped by their first block id; a group's prefix is its members' longest common run of
+leading block ids, and groups that `paged_attention.shared_prefix_pays` accepts run on `decode_attention_paged_shared`, which reads that
+prefix once per tile of members.  stats gains prefix_hit_tokens.  Not covered: multi-level (tree) prefixes, grouping verify rows, parallel
+sampling (n > 1) and copy-on-write of partial blocks.
 """
 from __future__ import annotations
 
 import torch
 
-from ..incubate.nn.paged_attention import block_attention
+from ..incubate.nn.paged_attention import block_attention, shared_prefix_pays
 from .generation import _raw, _sample, _w
 
 
@@ -56,6 +71,92 @@ class BlockAllocator:
         self._free.extend(reversed(blocks))
 
 
+class BlockKey:
+    """Identity of a full block's contents: the key of the block before it in its sequence (None for the first) and its block_size token
+    ids.  The chain fixes the block's position, so equal keys mean equal K / V under static cache scales.  Equality compares token ids
+    exactly (a hash collision never matches); the hash is computed once."""
+    __slots__ = ("parent", "tokens", "_hash")
+
+    def __init__(self, parent, tokens):
+        self.parent, self.tokens = parent, tuple(tokens)
+        self._hash = hash((None if parent is None else parent._hash, self.tokens))
+
+    def __hash__(self):
+        return self._hash
+
+    def __eq__(self, other):
+        return self is other or (isinstance(other, BlockKey) and self._hash == other._hash and self.tokens == other.tokens
+                                 and self.parent == other.parent)
+
+
+class PrefixCachingAllocator(BlockAllocator):
+    """BlockAllocator with reference counts and a table of registered full blocks (LLMEngine(enable_prefix_caching=True)).
+
+    A block is free, evictable (registered, no reference: still matchable, in LRU order) or referenced.  free() drops one reference per
+    block; a registered block that reaches zero becomes the most recently used evictable block, any other goes back to the free list.
+    alloc() takes a free block first, then evicts the least recently used evictable one (its key is dropped).  num_free() counts free plus
+    evictable blocks: both can be handed out."""
+
+    def __init__(self, num_blocks):
+        super().__init__(num_blocks)
+        self.ref = {}                  # block -> number of sequences holding it
+        self.key_of = {}               # registered block -> its BlockKey
+        self.table = {}                # BlockKey -> registered block
+        self.evictable = {}            # registered blocks without a reference, least recently used first (dicts keep insertion order)
+
+    def num_free(self):
+        return len(self._free) + len(self.evictable)
+
+    def alloc(self):
+        if self._free:
+            blk = self._free.pop()
+        elif self.evictable:
+            blk = next(iter(self.evictable))
+            del self.evictable[blk]
+            del self.table[self.key_of.pop(blk)]
+        else:
+            raise MemoryError("KV-cache block pool is exhausted")
+        self.ref[blk] = 1
+        return blk
+
+    def free(self, blocks):
+        for blk in reversed(blocks):  # tail first: a chain's end becomes evictable before its start
+            self.ref[blk] -= 1
+            if self.ref[blk] == 0:
+                del self.ref[blk]
+                if blk in self.key_of:
+                    self.evictable[blk] = None
+                else:
+                    self._free.append(blk)
+
+    def match(self, tokens, block_size):
+        """(blocks, keys) of the longest chain of registered blocks that covers tokens[:k * block_size], k as large as possible."""
+        blocks, keys, parent = [], [], None
+        for j in range(len(tokens) // block_size):
+            blk = self.table.get(BlockKey(parent, tokens[j * block_size:(j + 1) * block_size]))
+            if blk is None:
+                break
+            parent = self.key_of[blk]            # the registered object: the next lookup compares parents by identity
+            blocks.append(blk)
+            keys.append(parent)
+        return blocks, keys
+
+    def acquire(self, blocks):
+        """One more reference to each (registered) block; an evictable one leaves the eviction order."""
+        for blk in blocks:
+            self.evictable.pop(blk, None)
+            self.ref[blk] = self.ref.get(blk, 0) + 1
+
+    def register(self, blk, key):
+        """Makes `blk` matchable under `key` and returns the registered key object, unless another block already holds the key: then
+        `blk` stays private and that block's key is returned (children chain to it)."""
+        have = self.table.get(key)
+        if have is not None:
+            return self.key_of[have]
+        self.table[key], self.key_of[blk] = blk, key
+        return key
+
+
 class Sequence:
     WAITING, RUNNING, FINISHED = "waiting", "running", "finished"
 
@@ -65,6 +166,7 @@ class Sequence:
         self.generated, self.blocks, self.cached, self.status, self.preemptions = [], [], 0, Sequence.WAITING, 0
         self.target = 0                            # tokens to prefill since admission: the sequence samples once cached reaches it
         self.draft_cached, self.spec = 0, 0        # speculative decoding: positions in the draft's cache, proposals this step
+        self.keys = []                             # prefix caching: BlockKeys of the leading full blocks already keyed
 
     def tokens(self):
         return self.prompt + self.generated
@@ -81,7 +183,7 @@ class LLMEngine:
     with a draft model, up to num_speculative_tokens + 1 tokens per greedy decode sequence)."""
 
     def __init__(self, model, num_blocks=256, block_size=16, max_running=64, max_batch_tokens=8192, max_prefill_chunk=None, kv_cache_dtype=None,
-                 kv_cache_absmax=None, draft_model=None, num_speculative_tokens=0):
+                 kv_cache_absmax=None, draft_model=None, num_speculative_tokens=0, enable_prefix_caching=False):
         from .generation import make_adapter
 
         model.eval()
@@ -94,7 +196,8 @@ class LLMEngine:
         self.max_prefill_chunk = None if max_prefill_chunk is None else int(max_prefill_chunk)
         p0 = _raw(next(iter(model.parameters())))
         self.device, self.dtype = p0.device, p0.dtype
-        self.alloc = BlockAllocator(num_blocks)
+        self.enable_prefix_caching = bool(enable_prefix_caching)
+        self.alloc = PrefixCachingAllocator(num_blocks) if self.enable_prefix_caching else BlockAllocator(num_blocks)
         self._kv_quant = [{} for _ in self.layers]       # per layer: block_attention's cache quantization arguments
         cache_dtype = self.dtype
         if kv_cache_dtype is not None:
@@ -113,6 +216,8 @@ class LLMEngine:
         self.num_speculative_tokens, self._draft = self._draft_setup(draft_model, num_speculative_tokens, num_blocks)
         if self.num_speculative_tokens:
             self.stats.update(draft_tokens=0, accepted_tokens=0)
+        if self.enable_prefix_caching:
+            self.stats["prefix_hit_tokens"] = 0
 
     def _draft_setup(self, draft_model, k, num_blocks):
         """(k, (adapter, key caches, value caches, no quantization)) of the draft model, or (0, None) without one."""
@@ -170,7 +275,7 @@ class LLMEngine:
 
     def _preempt(self, s):
         self.alloc.free(s.blocks)
-        s.blocks, s.cached, s.draft_cached, s.status = [], 0, 0, Sequence.WAITING
+        s.blocks, s.cached, s.draft_cached, s.status, s.keys = [], 0, 0, Sequence.WAITING, []
         s.preemptions += 1
         self.stats["preemptions"] += 1
         self.running.remove(s)
@@ -210,13 +315,25 @@ class LLMEngine:
         admitted = 0
         while self.waiting and len(self.running) + admitted < self.max_running:
             s = self.waiting[0]
-            total = len(s.tokens())
-            n = total if chunk is None else min(chunk, total, budget)
-            need = self._blocks_for(total + 1)
-            if n > budget or (chunk is not None and budget == 0) or need > self.alloc.num_free():
+            toks = s.tokens()
+            total = len(toks)
+            hits, keys = [], []
+            if self.enable_prefix_caching:           # at least the last token is computed: its logits give the first sample
+                hits, keys = self.alloc.match(toks[:total - 1], self.block_size)
+            m = len(hits) * self.block_size
+            n = total - m if chunk is None else min(chunk, total - m, budget)
+            need = self._blocks_for(total + 1) - len(hits)
+            held = sum(1 for b in hits if b in self.alloc.evictable) if hits else 0   # matched evictable blocks stop being available
+            if n > budget or (chunk is not None and budget == 0) or need > self.alloc.num_free() - held:
                 break
             self.waiting.pop(0)
-            s.blocks = [self.alloc.alloc() for _ in range(need)]
+            if hits:
+                self.alloc.acquire(hits)
+                self.stats["prefix_hit_tokens"] += m
+            s.blocks = hits + [self.alloc.alloc() for _ in range(need)]
+            s.keys, s.cached = keys, m
+            if self.num_speculative_tokens:
+                s.draft_cached = m                   # registered blocks hold their rows in both caches
             s.target = total
             prefill.append((s, n))
             admitted += 1
@@ -235,6 +352,44 @@ class LLMEngine:
             budget -= k
         return budget
 
+    # ---- prefix caching -----------------------------------------------------------------------------------------------------------
+    def _register(self, s, toks):
+        """Keys and registers s's full blocks whose positions are all in the cache (with a draft: in both caches; a sampling request's
+        draft cache is never written, so its blocks never register then).  toks: s's tokens, at least up to s.cached."""
+        if not self.enable_prefix_caching or (self.num_speculative_tokens and s.do_sample):
+            return
+        end = min(s.cached, s.draft_cached) if self.num_speculative_tokens else s.cached
+        bs = self.block_size
+        for j in range(len(s.keys), end // bs):
+            key = BlockKey(s.keys[-1] if s.keys else None, toks[j * bs:(j + 1) * bs])
+            s.keys.append(self.alloc.register(s.blocks[j], key))
+
+    def _shared_prefix_groups(self, seqs, n_new):
+        """block_attention's shared_prefix argument for the plain decode rows among seqs (the first len(decode) of them, one new token and
+        no speculation): rows are grouped by their first block id, a group's prefix is the longest run of leading block ids common to all
+        its members, and only groups that paged_attention.shared_prefix_pays() accepts are passed.  None when there are none."""
+        if not self.enable_prefix_caching:
+            return None
+        by_first = {}
+        for i, (s, n) in enumerate(zip(seqs, n_new)):
+            if n == 1 and s.cached >= s.target and s.keys:     # a decode row with at least one registered (or shared) full block
+                by_first.setdefault(s.blocks[0], []).append(i)
+        cu, members, plen = [0], [], []
+        for idx in by_first.values():
+            if len(idx) < 2:
+                continue
+            first = seqs[idx[0]].blocks
+            k = min(len(seqs[i].keys) for i in idx)
+            for i in idx[1:]:
+                b = seqs[i].blocks
+                k = next((j for j in range(k) if b[j] != first[j]), k)
+            if not shared_prefix_pays(len(idx), k * self.block_size, self.nh // self.nkv):
+                continue
+            members += idx
+            cu.append(len(members))
+            plen.append(k * self.block_size)
+        return (cu, members, plen) if plen else None
+
     # ---- one packed forward -------------------------------------------------------------------------------------------------------
     def _forward(self, seqs, n_new, enc, dec):
         """The target model over this step's rows (s.tokens() from s.cached); logits of each sequence's last row [num_seqs, vocab]."""
@@ -244,7 +399,7 @@ class LLMEngine:
     def _run(self, net, seqs, n_new, enc, dec, toks=None, rows=None):
         """One packed forward of `net` = (adapter, key caches, value caches, quantization args) over the sequences' blocks: n_new[i] tokens
         at positions dec[i] ... (toks[i], by default taken from s.tokens()).  Returns the logits of packed rows `rows` (default: each
-        sequence's last row)."""
+        sequence's last row).  Target forwards pass the shared-prefix groups of their decode rows to block_attention."""
         ad, key_cache, value_cache, kv_quant = net
         dev = self.device
         if toks is None:
@@ -263,6 +418,7 @@ class LLMEngine:
         dec_t = torch.tensor(dec, dtype=torch.int32, device=dev)
         now_t = torch.tensor(n_new, dtype=torch.int32, device=dev)
         nh, nkv, hd = ad.nh, ad.nkv, ad.hd
+        shared = self._shared_prefix_groups(seqs, n_new) if net is self._target else None
         h = ad.embed_tokens(ids, position_ids)
         for li, layer in enumerate(ad.layers):
             qkv = ad.attn_in(layer, h, position_ids)
@@ -270,7 +426,7 @@ class LLMEngine:
             if self._observe is not None and net is self._target:
                 self._observe(li, qkv.reshape(t, (nh + 2 * nkv) * hd))
             out, _, _, _ = block_attention(qkv.reshape(t, (nh + 2 * nkv) * hd), key_cache[li], value_cache[li], enc_t, dec_t, now_t, cu, bt,
-                                           self.block_size, **kv_quant[li])
+                                           self.block_size, **kv_quant[li], shared_prefix=shared)
             h = ad.attn_out(layer, h, _raw(out).reshape(1, t, nh * hd))
         rows = (cu[1:].long() - 1) if rows is None else torch.tensor(rows, dtype=torch.int64, device=dev)
         return ad.logits(_raw(h)[:, rows])[0]                                          # [len(rows), vocab]
@@ -307,6 +463,7 @@ class LLMEngine:
         out = []
         for i, (s, n) in enumerate(zip(seqs, n_new)):
             s.cached += n
+            self._register(s, s.tokens())
             if s.status != Sequence.RUNNING:
                 s.status = Sequence.RUNNING
                 self.running.append(s)
@@ -370,6 +527,7 @@ class LLMEngine:
             r += k + 1
             s.cached += len(emit)               # the last token and the accepted proposals are now in the target's cache
             s.draft_cached = min(s.draft_cached, s.cached)
+            self._register(s, s.tokens() + emit)
             for tok in emit:
                 fin = self._finish_token(s, tok)
                 out.append((s.id, tok, fin))
@@ -384,6 +542,7 @@ class LLMEngine:
             i = r
             r += 1
             s.cached += n
+            self._register(s, s.tokens())
             if s.status != Sequence.RUNNING:
                 s.status = Sequence.RUNNING
                 self.running.append(s)
