@@ -1058,28 +1058,46 @@ void decode_attention_paged_shared(const Tensor& q, const Tensor& k_cache, const
   TORCH_CHECK(rc == 0, "paddle_b200.decode_attention_paged_shared: unsupported operands (16-byte aligned rows and caches) rc=", std::to_string(rc));
 }
 
-// Quantizing write of every sequence's new K / V rows into paged int8 / fp8 e4m3 caches: qkv [T, (H + 2 Hkv) * D] packed rows (unit
-// inner stride), caches [num_blocks, Hkv, block_size, D], cu_q int32 [B + 1], seq_lens_encoder / seq_lens_decoder int32 [B], block_tables
-// int32 [B, max_blocks], quant scales fp32 [Hkv]; y = (max_bound * scale) * x rounded (round_type 0: rint, 1: roundf) and clamped to the bounds.
+// Write of every sequence's new K / V rows into the paged caches: qkv [T, (H + 2 Hkv) * D] packed rows (unit inner stride), caches
+// [num_blocks, Hkv, block_size, D], cu_q int32 [B + 1], seq_lens_encoder / seq_lens_decoder int32 [B], block_tables int32 [B, max_blocks].
+// int8 / fp8 e4m3 caches take quant scales fp32 [Hkv]: y = (max_bound * scale) * x rounded (round_type 0: rint, 1: roundf) and clamped to
+// the bounds; 16-bit caches (the compute type) take a copy.  The optional rest is block_multihead_attention's qkv prologue, applied to
+// each row first (csrc/kv_cache_quant.cu): int32 qkv with qkv_out_scale fp32 [W]; qkv_bias [W] of the compute type; rope_cos / rope_sin
+// fp32 [S, 64] (interleaved pairs) or [S, 128] (neox halves, neox = true), every new token's position < S; qkv_out [T, W] of the
+// compute type receives the processed rows (it may be qkv itself).  The compute type is qkv's dtype, or qkv_out's for int32 qkv.
 void paged_kv_cache_write(const Tensor& qkv, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cu_q, const Tensor& seq_lens_encoder,
-                          const Tensor& seq_lens_decoder, const Tensor& block_tables, const Tensor& k_quant_scales, const Tensor& v_quant_scales,
-                          int64_t round_type, double max_bound, double min_bound) {
-  TORCH_CHECK(qkv.is_cuda() && qkv.dim() == 2 && qkv.stride(1) == 1 && (qkv.scalar_type() == at::kHalf || qkv.scalar_type() == at::kBFloat16),
-              "paged_kv_cache_write: qkv must be a CUDA fp16 / bf16 [T, (H + 2 Hkv) * D] tensor with unit inner stride");
+                          const Tensor& seq_lens_decoder, const Tensor& block_tables, const OptT& k_quant_scales, const OptT& v_quant_scales,
+                          int64_t round_type, double max_bound, double min_bound, const OptT& qkv_out, const OptT& qkv_out_scale,
+                          const OptT& qkv_bias, const OptT& rope_cos, const OptT& rope_sin, bool neox) {
+  const bool i32 = qkv.scalar_type() == at::kInt;
+  TORCH_CHECK(qkv.is_cuda() && qkv.dim() == 2 && qkv.stride(1) == 1 && (qkv.scalar_type() == at::kHalf || qkv.scalar_type() == at::kBFloat16 || i32),
+              "paged_kv_cache_write: qkv must be a CUDA fp16 / bf16 / int32 [T, (H + 2 Hkv) * D] tensor with unit inner stride");
+  const bool has_out = qkv_out.has_value() && qkv_out->defined();
+  TORCH_CHECK(!i32 || has_out, "paged_kv_cache_write: int32 qkv needs qkv_out, whose dtype is the compute type");
+  const auto ct = i32 ? qkv_out->scalar_type() : qkv.scalar_type();
+  TORCH_CHECK(ct == at::kHalf || ct == at::kBFloat16, "paged_kv_cache_write: the compute type must be fp16 or bf16");
   TORCH_CHECK(k_cache.dim() == 4 && k_cache.is_contiguous() && v_cache.is_contiguous() && k_cache.sizes() == v_cache.sizes() &&
               k_cache.device() == qkv.device() && v_cache.device() == qkv.device(),
               "paged_kv_cache_write: caches must be contiguous [num_blocks, Hkv, block_size, D] of one shape on the device of qkv");
   const auto st = k_cache.scalar_type();
-  TORCH_CHECK(v_cache.scalar_type() == st && (st == at::kChar || st == at::kFloat8_e4m3fn), "paged_kv_cache_write: caches must both be int8 or float8_e4m3fn");
-  TORCH_CHECK(round_type == 0 || round_type == 1, "paged_kv_cache_write: round_type must be 0 (rint) or 1 (round half away from zero)");
-  TORCH_CHECK(min_bound <= max_bound, "paged_kv_cache_write: min_bound must not exceed max_bound");
-  if (st == at::kFloat8_e4m3fn) {
-    TORCH_CHECK(max_bound <= 448.0 && min_bound >= -448.0, "paged_kv_cache_write: fp8 e4m3 bounds must lie within [-448, 448]");
-  } else {
-    TORCH_CHECK(max_bound <= 127.0 && min_bound >= -128.0, "paged_kv_cache_write: int8 bounds must lie within [-128, 127]");
-  }
+  const bool kv16 = st == ct;
+  TORCH_CHECK(v_cache.scalar_type() == st && (st == at::kChar || st == at::kFloat8_e4m3fn || kv16),
+              "paged_kv_cache_write: caches must both be int8, float8_e4m3fn or of the compute type");
   const int64_t hkv = k_cache.size(1), d = k_cache.size(3);
-  TORCH_CHECK(qkv.size(1) % d == 0 && qkv.size(1) / d > 2 * hkv, "paged_kv_cache_write: qkv row width must be (H + 2 Hkv) * D");
+  if (!kv16) {
+    TORCH_CHECK(round_type == 0 || round_type == 1, "paged_kv_cache_write: round_type must be 0 (rint) or 1 (round half away from zero)");
+    TORCH_CHECK(min_bound <= max_bound, "paged_kv_cache_write: min_bound must not exceed max_bound");
+    if (st == at::kFloat8_e4m3fn) {
+      TORCH_CHECK(max_bound <= 448.0 && min_bound >= -448.0, "paged_kv_cache_write: fp8 e4m3 bounds must lie within [-448, 448]");
+    } else {
+      TORCH_CHECK(max_bound <= 127.0 && min_bound >= -128.0, "paged_kv_cache_write: int8 bounds must lie within [-128, 127]");
+    }
+    for (const OptT* t : {&k_quant_scales, &v_quant_scales})
+      TORCH_CHECK(t->has_value() && (*t)->device() == qkv.device() && (*t)->scalar_type() == at::kFloat && (*t)->is_contiguous() && (*t)->dim() == 1 &&
+                  (*t)->size(0) == hkv, "paged_kv_cache_write: quant scales must be fp32 [Hkv] on the device");
+  }
+  const int64_t w = qkv.size(1);
+  TORCH_CHECK(w % d == 0 && w / d > 2 * hkv, "paged_kv_cache_write: qkv row width must be (H + 2 Hkv) * D");
   TORCH_CHECK(qkv.stride(0) % 4 == 0 && reinterpret_cast<uintptr_t>(qkv.data_ptr()) % 8 == 0, "paged_kv_cache_write: qkv rows must be 8-byte aligned");
   TORCH_CHECK(block_tables.device() == qkv.device() && block_tables.scalar_type() == at::kInt && block_tables.is_contiguous() && block_tables.dim() == 2,
               "paged_kv_cache_write: block_tables must be int32 [B, max_blocks] on the device");
@@ -1089,22 +1107,88 @@ void paged_kv_cache_write(const Tensor& qkv, const Tensor& k_cache, const Tensor
   for (const Tensor* t : {&seq_lens_encoder, &seq_lens_decoder})
     TORCH_CHECK(t->device() == qkv.device() && t->scalar_type() == at::kInt && t->is_contiguous() && t->numel() == b,
                 "paged_kv_cache_write: seq_lens_encoder / seq_lens_decoder must be int32 [B] on the device");
-  for (const Tensor* t : {&k_quant_scales, &v_quant_scales})
-    TORCH_CHECK(t->device() == qkv.device() && t->scalar_type() == at::kFloat && t->is_contiguous() && t->dim() == 1 && t->size(0) == hkv,
-                "paged_kv_cache_write: quant scales must be fp32 [Hkv] on the device");
+  auto aligned16 = [](const Tensor& t) { return reinterpret_cast<uintptr_t>(t.data_ptr()) % 16 == 0; };
+  const bool has_scale = qkv_out_scale.has_value() && qkv_out_scale->defined(), has_bias = qkv_bias.has_value() && qkv_bias->defined();
+  const bool has_cos = rope_cos.has_value() && rope_cos->defined(), has_sin = rope_sin.has_value() && rope_sin->defined();
+  const bool prologue = i32 || has_out || has_scale || has_bias || has_cos || has_sin || kv16;
+  if (prologue) {
+    TORCH_CHECK((qkv.stride(0) * qkv.element_size()) % 16 == 0 && aligned16(qkv), "paged_kv_cache_write: qkv rows must be 16-byte aligned");
+    TORCH_CHECK(i32 == has_scale, "paged_kv_cache_write: qkv_out_scale goes with int32 qkv, and only with it");
+    if (has_scale)
+      TORCH_CHECK(qkv_out_scale->device() == qkv.device() && qkv_out_scale->scalar_type() == at::kFloat && qkv_out_scale->is_contiguous() &&
+                  qkv_out_scale->numel() == w && aligned16(*qkv_out_scale), "paged_kv_cache_write: qkv_out_scale must be fp32 [W] on the device");
+    if (has_bias)
+      TORCH_CHECK(qkv_bias->device() == qkv.device() && qkv_bias->scalar_type() == ct && qkv_bias->is_contiguous() && qkv_bias->numel() == w &&
+                  aligned16(*qkv_bias), "paged_kv_cache_write: qkv_bias must be [W] of the compute type on the device");
+    TORCH_CHECK(has_cos == has_sin, "paged_kv_cache_write: rope_cos and rope_sin go together");
+    if (has_cos)
+      for (const OptT* t : {&rope_cos, &rope_sin})
+        TORCH_CHECK((*t)->device() == qkv.device() && (*t)->scalar_type() == at::kFloat && (*t)->is_contiguous() && (*t)->dim() == 2 &&
+                    (*t)->sizes() == rope_cos->sizes() && (*t)->size(1) == (neox ? d : d / 2) && aligned16(**t),
+                    "paged_kv_cache_write: rope_cos / rope_sin must be fp32 [S, D / 2] (neox: [S, D]) on the device");
+    if (has_out)
+      TORCH_CHECK(qkv_out->device() == qkv.device() && qkv_out->scalar_type() == ct && qkv_out->dim() == 2 && qkv_out->size(0) == qkv.size(0) && qkv_out->size(1) == w &&
+                  qkv_out->stride(1) == 1 && (qkv_out->stride(0) * qkv_out->element_size()) % 16 == 0 && aligned16(*qkv_out),
+                  "paged_kv_cache_write: qkv_out must be [T, W] of the compute type with 16-byte aligned rows");
+  }
   b200::PagedKvWriteArgs a;
   a.qkv = qkv.data_ptr(); a.k_cache = k_cache.data_ptr(); a.v_cache = v_cache.data_ptr(); a.row_stride = qkv.stride(0);
-  a.t = (int)qkv.size(0); a.hkv = (int)hkv; a.d = (int)d; a.h = (int)(qkv.size(1) / d - 2 * hkv); a.b = (int)b;
+  a.t = (int)qkv.size(0); a.hkv = (int)hkv; a.d = (int)d; a.h = (int)(w / d - 2 * hkv); a.b = (int)b;
   a.block_size = (int)k_cache.size(2); a.max_blocks = (int)block_tables.size(1);
   a.cu_q = cu_q.data_ptr<int>(); a.enc = seq_lens_encoder.data_ptr<int>(); a.dec = seq_lens_decoder.data_ptr<int>(); a.block_tables = block_tables.data_ptr<int>();
-  a.k_quant_scales = k_quant_scales.data_ptr<float>(); a.v_quant_scales = v_quant_scales.data_ptr<float>();
+  a.k_quant_scales = kv16 ? nullptr : k_quant_scales->data_ptr<float>(); a.v_quant_scales = kv16 ? nullptr : v_quant_scales->data_ptr<float>();
   a.round_type = (int)round_type; a.max_bound = (float)max_bound; a.min_bound = (float)min_bound;
-  a.dtype = dt_code(qkv); a.kv_dtype = st == at::kChar ? kKvI8 : kKvE4M3;
+  a.dtype = dt_code(ct); a.kv_dtype = kv16 ? a.dtype : st == at::kChar ? kKvI8 : kKvE4M3;
+  if (prologue) {
+    a.qkv_int32 = i32 ? 1 : 0;
+    a.col_scale = has_scale ? qkv_out_scale->data_ptr<float>() : nullptr;
+    a.bias = has_bias ? qkv_bias->data_ptr() : nullptr;
+    a.rope = has_cos ? (neox ? 2 : 1) : 0;
+    a.rope_cos = has_cos ? rope_cos->data_ptr<float>() : nullptr; a.rope_sin = has_cos ? rope_sin->data_ptr<float>() : nullptr;
+    a.rope_stride = has_cos ? (int)rope_cos->size(1) : 0;
+    a.out = has_out ? qkv_out->data_ptr() : nullptr; a.out_stride = has_out ? qkv_out->stride(0) : 0;
+  }
   c10::cuda::CUDAGuard guard(qkv.device());
   int rc = b200::paged_kv_cache_write(a, cur_stream());
   g_launches += 1;
   check_err();
   TORCH_CHECK(rc == 0, "paddle_b200.paged_kv_cache_write: unsupported operands (head_dim 128) rc=", rc);
+}
+
+// Output quantization of block_multihead_attention (out_scale > 0): x [rows, cols] fp16 / bf16 contiguous -> y int8 / float8_e4m3fn of the
+// same shape, y = quantize(max_bound * out_scale * x) under the cache rounding rules; shift / smooth [cols] of x's dtype, both or neither:
+// x is first replaced by ((x + shift) * smooth), each step rounded to x's dtype.
+void attention_out_quant(const Tensor& x, const Tensor& y, double out_scale, const OptT& shift, const OptT& smooth, int64_t round_type,
+                         double max_bound, double min_bound) {
+  TORCH_CHECK(x.is_cuda() && x.dim() == 2 && x.is_contiguous() && (x.scalar_type() == at::kHalf || x.scalar_type() == at::kBFloat16) &&
+              reinterpret_cast<uintptr_t>(x.data_ptr()) % 16 == 0 && x.size(1) % 8 == 0,
+              "attention_out_quant: x must be a contiguous CUDA fp16 / bf16 [rows, cols] tensor, cols a multiple of 8, 16-byte aligned");
+  TORCH_CHECK(y.device() == x.device() && y.is_contiguous() && y.sizes() == x.sizes() && (y.scalar_type() == at::kChar || y.scalar_type() == at::kFloat8_e4m3fn) &&
+              reinterpret_cast<uintptr_t>(y.data_ptr()) % 8 == 0, "attention_out_quant: y must be a contiguous int8 / float8_e4m3fn tensor shaped like x");
+  TORCH_CHECK(round_type == 0 || round_type == 1, "attention_out_quant: round_type must be 0 (rint) or 1 (round half away from zero)");
+  TORCH_CHECK(min_bound <= max_bound, "attention_out_quant: min_bound must not exceed max_bound");
+  if (y.scalar_type() == at::kFloat8_e4m3fn) {
+    TORCH_CHECK(max_bound <= 448.0 && min_bound >= -448.0, "attention_out_quant: fp8 e4m3 bounds must lie within [-448, 448]");
+  } else {
+    TORCH_CHECK(max_bound <= 127.0 && min_bound >= -128.0, "attention_out_quant: int8 bounds must lie within [-128, 127]");
+  }
+  const bool has_shift = shift.has_value() && shift->defined(), has_smooth = smooth.has_value() && smooth->defined();
+  TORCH_CHECK(has_shift == has_smooth, "attention_out_quant: shift and smooth go together");
+  if (has_shift)
+    for (const OptT* t : {&shift, &smooth})
+      TORCH_CHECK((*t)->device() == x.device() && (*t)->scalar_type() == x.scalar_type() && (*t)->is_contiguous() && (*t)->numel() == x.size(1) &&
+                  reinterpret_cast<uintptr_t>((*t)->data_ptr()) % 16 == 0, "attention_out_quant: shift / smooth must be [cols] of x's dtype on the device");
+  b200::OutQuantArgs a;
+  a.x = x.data_ptr(); a.y = y.data_ptr(); a.rows = x.size(0); a.cols = (int)x.size(1);
+  a.shift = optp(shift); a.smooth = optp(smooth);
+  a.scale = (float)max_bound * (float)out_scale;
+  a.round_type = (int)round_type; a.max_bound = (float)max_bound; a.min_bound = (float)min_bound;
+  a.dtype = dt_code(x); a.out_dtype = y.scalar_type() == at::kChar ? kKvI8 : kKvE4M3;
+  c10::cuda::CUDAGuard guard(x.device());
+  int rc = b200::attention_out_quant(a, cur_stream());
+  g_launches += 1;
+  check_err();
+  TORCH_CHECK(rc == 0, "paddle_b200.attention_out_quant: unsupported operands rc=", rc);
 }
 
 static bool g_deterministic = false;     // FLAGS_cudnn_deterministic (the attention backward is order-independent as it is)
@@ -1236,6 +1320,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("paged_kv_cache_write", traced("paged_kv_cache_write", &paged_kv_cache_write), pybind11::arg("qkv"), pybind11::arg("k_cache"),
         pybind11::arg("v_cache"), pybind11::arg("cu_q"), pybind11::arg("seq_lens_encoder"), pybind11::arg("seq_lens_decoder"),
         pybind11::arg("block_tables"), pybind11::arg("k_quant_scales"), pybind11::arg("v_quant_scales"), pybind11::arg("round_type") = 1,
+        pybind11::arg("max_bound") = 127.0, pybind11::arg("min_bound") = -127.0, pybind11::arg("qkv_out") = pybind11::none(),
+        pybind11::arg("qkv_out_scale") = pybind11::none(), pybind11::arg("qkv_bias") = pybind11::none(), pybind11::arg("rope_cos") = pybind11::none(),
+        pybind11::arg("rope_sin") = pybind11::none(), pybind11::arg("neox") = false);
+  m.def("attention_out_quant", traced("attention_out_quant", &attention_out_quant), pybind11::arg("x"), pybind11::arg("y"), pybind11::arg("out_scale"),
+        pybind11::arg("shift") = pybind11::none(), pybind11::arg("smooth") = pybind11::none(), pybind11::arg("round_type") = 1,
         pybind11::arg("max_bound") = 127.0, pybind11::arg("min_bound") = -127.0);
   m.def("attention_supported", &attention_supported);
   m.def("attention_fwd", traced("attention_fwd", &attention_fwd), pybind11::arg("q"), pybind11::arg("k"), pybind11::arg("v"), pybind11::arg("scale"), pybind11::arg("causal"),

@@ -245,8 +245,38 @@ struct PagedKvWriteArgs {
   int round_type;
   float max_bound, min_bound;
   int dtype, kv_dtype;
+  // The qkv prologue of block_multihead_attention, applied to every new row before it is stored; with all of it at its default the call
+  // is the plain quantizing write above.  dtype is then the compute type T (kF16 / kBF16), and kv_dtype == dtype stores a 16-bit copy.
+  // qkv_int32: qkv holds int32 values, dequantized by col_scale fp32 [(h + 2 hkv) * 128].  bias: T [(h + 2 hkv) * 128] or nullptr.
+  // rope (kv_cache_quant.cu RopeStyle): 0 none, 1 interleaved pairs, 2 neox halves on the Q and K heads, with fp32 cos / sin tables
+  // [S, rope_stride] read at each token's position (the caller guarantees position < S).  out: T [t, (h + 2 hkv) * 128] rows (row
+  // stride out_stride) that receive every processed row, q, k and v; it may be qkv itself; nullptr: not written.
+  int qkv_int32 = 0;
+  const float* col_scale = nullptr;
+  const void* bias = nullptr;
+  int rope = 0;
+  const float* rope_cos = nullptr;
+  const float* rope_sin = nullptr;
+  int rope_stride = 0;
+  void* out = nullptr;
+  int64_t out_stride = 0;
 };
 int paged_kv_cache_write(const PagedKvWriteArgs& a, cudaStream_t s);
+// Output quantization of block_multihead_attention: x [rows, cols] T (kF16 / kBF16, contiguous) -> y [rows, cols] int8 / e4m3 (out_dtype
+// kI8 / kE4M3), y = quantize(x) with a = scale (max_bound * out_scale) under the cache rules of include/b200_kv8.cuh.  shift / smooth:
+// T [cols], both or neither; x is first replaced by ((x + shift) -> T) * smooth -> T.  cols a multiple of 8.
+struct OutQuantArgs {
+  const void* x; void* y;
+  int64_t rows;
+  int cols;
+  const void* shift = nullptr;
+  const void* smooth = nullptr;
+  float scale;
+  int round_type;
+  float max_bound, min_bound;
+  int dtype, out_dtype;
+};
+int attention_out_quant(const OutQuantArgs& a, cudaStream_t s);
 
 // ---- attention_sm100.cu ---------------------------------------------------------------------------------------
 // Flash-attention forward (head_dim 128, fp16/bf16). q [B,Sq,H,D], k/v [B,Sk,Hk,D], o [B,Sq,H,D] as strided views (element

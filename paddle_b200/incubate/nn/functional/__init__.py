@@ -323,13 +323,20 @@ def block_multihead_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq
 
     int8 / float8_e4m3fn caches take static per-KV-head cache_{k,v}_{quant,dequant}_scales (fp32 [H_kv]) with quant_round_type and the
     quant bounds (see incubate.nn.paged_attention).  Dynamic cache quantization raises NotImplementedError; scales with a 16-bit cache, or an
-    8-bit cache without them, raise ValueError.  The pre-caches, rope_emb, masks, qkv_out_scale / bias, out_shift / smooth and out_scale
-    are not applied."""
+    8-bit cache without them, raise ValueError.
+
+    The qkv prologue and the output quantization follow incubate.nn.paged_attention.block_attention: int32 qkv with qkv_out_scale and
+    compute_dtype 'bf16' / 'fp16' / 'fp32', qkv_bias, rope_emb [2, 1, S, 1, D / 2] (use_neox_style: [2, 1, S, 1, D], pairs (i, i + D / 2)),
+    and out_scale > 0 with optional out_shift / out_smooth, giving int8 output for quant_max_bound 127 and float8_e4m3fn for 448 (the
+    reference types int32-input output as int8 whatever the bound).  Decode rows take their rotary from rope_emb as prefill rows do;
+    rope_theta is accepted and not used.  Not applied: the pre-caches, mask and tgt_mask, and the padding / max-length arguments
+    (padding_offsets, cum_offsets, cu_seqlens_k, max_enc_len_this_time, max_dec_len_this_time, max_seq_len)."""
     from ....incubate.nn.paged_attention import block_attention
 
     return block_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_decoder, seq_lens_this_time, cu_seqlens_q, block_tables, block_size,
                            cache_k_quant_scales, cache_v_quant_scales, cache_k_dequant_scales, cache_v_dequant_scales, use_dynamic_cachekv_quant,
-                           quant_round_type, quant_max_bound, quant_min_bound)
+                           quant_round_type, quant_max_bound, quant_min_bound, qkv_out_scale=qkv_out_scale, qkv_bias=qkv_bias, rope_emb=rope_emb,
+                           use_neox_style=use_neox_style, out_shift=out_shift, out_smooth=out_smooth, out_scale=out_scale, compute_dtype=compute_dtype)
 
 
 def blha_get_max_len(seq_lens_encoder, seq_lens_decoder, batch_size):

@@ -78,6 +78,136 @@ def kv_quant_params(key_cache, value_cache, cache_k_quant_scales=None, cache_v_q
     return KVQuant(*f32, int(quant_round_type), float(quant_max_bound), float(quant_min_bound))
 
 
+class QKVPrologue(NamedTuple):
+    """Validated qkv prologue / output epilogue of block_multihead_attention (see block_attention), on qkv's device.  dtype: the compute type
+    T.  qkv_out_scale: fp32 [W] (int32 qkv only); qkv_bias: T [W]; rope_cos / rope_sin: fp32 [S_rope, R] with neox; out_dtype: int8 /
+    float8_e4m3fn when out_scale > 0, else None; out_shift / out_smooth: T [H * D]."""
+    dtype: torch.dtype
+    qkv_out_scale: torch.Tensor | None
+    qkv_bias: torch.Tensor | None
+    rope_cos: torch.Tensor | None
+    rope_sin: torch.Tensor | None
+    neox: bool
+    out_scale: float
+    out_dtype: torch.dtype | None
+    out_shift: torch.Tensor | None
+    out_smooth: torch.Tensor | None
+    round_type: int
+    max_bound: float
+    min_bound: float
+
+    @property
+    def has_prologue(self):
+        return self.qkv_out_scale is not None or self.qkv_bias is not None or self.rope_cos is not None
+
+
+_COMPUTE_DTYPES = {"bf16": torch.bfloat16, "fp16": torch.float16, "fp32": torch.float32}
+_OUT_DTYPES = {127.0: torch.int8, 448.0: torch.float8_e4m3fn}
+
+
+def qkv_prologue_params(qkv, num_heads, num_kv_heads, head_dim, qkv_out_scale=None, qkv_bias=None, rope_emb=None, use_neox_style=False,
+                        out_shift=None, out_smooth=None, out_scale=-1, compute_dtype="default", quant_round_type=1, quant_max_bound=127.0,
+                        quant_min_bound=-127.0):
+    """None when block_attention's qkv prologue and output epilogue have nothing to do (no int32 qkv, qkv_bias, rope_emb, and out_scale
+    <= 0), else a QKVPrologue.  Raises ValueError on inputs the op would otherwise get silently wrong."""
+    qkv = _raw(qkv)
+    qkv_out_scale, qkv_bias, rope_emb, out_shift, out_smooth = (_raw(t) for t in (qkv_out_scale, qkv_bias, rope_emb, out_shift, out_smooth))
+    dev, w = qkv.device, qkv.shape[1]
+    if compute_dtype != "default" and compute_dtype not in _COMPUTE_DTYPES:
+        raise ValueError(f"block_multihead_attention: compute_dtype must be 'default', 'bf16', 'fp16' or 'fp32', got {compute_dtype!r}")
+    if qkv.dtype == torch.int32:
+        if compute_dtype == "default":
+            raise ValueError("block_multihead_attention: int32 qkv needs compute_dtype 'bf16', 'fp16' or 'fp32'")
+        if qkv_out_scale is None:
+            raise ValueError("block_multihead_attention: int32 qkv needs qkv_out_scale (fp32 [W]) to dequantize it")
+        dtype = _COMPUTE_DTYPES[compute_dtype]
+        if qkv_out_scale.numel() != w:
+            raise ValueError(f"block_multihead_attention: qkv_out_scale must have W = {w} elements, got {list(qkv_out_scale.shape)}")
+        qkv_out_scale = qkv_out_scale.reshape(w).to(dev, torch.float32).contiguous()
+    else:
+        if qkv_out_scale is not None:
+            raise ValueError(f"block_multihead_attention: qkv_out_scale dequantizes int32 qkv; qkv is {qkv.dtype}")
+        if compute_dtype != "default" and _COMPUTE_DTYPES[compute_dtype] != qkv.dtype:
+            raise ValueError(f"block_multihead_attention: compute_dtype {compute_dtype!r} does not match the {qkv.dtype} qkv")
+        dtype = qkv.dtype
+    if qkv_bias is not None:
+        if qkv_bias.numel() != w:
+            raise ValueError(f"block_multihead_attention: qkv_bias must have W = {w} elements, got {list(qkv_bias.shape)}")
+        qkv_bias = qkv_bias.reshape(w).to(dev, dtype).contiguous()
+    cos = sin = None
+    if rope_emb is not None:
+        r = head_dim if use_neox_style else head_dim // 2
+        if rope_emb.dim() != 5 or rope_emb.shape[0] != 2 or rope_emb.shape[3] != 1:
+            raise ValueError(f"block_multihead_attention: rope_emb must be [2, 1, S, 1, {r}] (cos, sin), got {list(rope_emb.shape)}")
+        if rope_emb.shape[1] != 1:
+            raise ValueError(f"block_multihead_attention: rope_emb must have batch dimension 1 (one table for every sequence), got "
+                             f"{rope_emb.shape[1]}")
+        if rope_emb.shape[4] != r:
+            raise ValueError(f"block_multihead_attention: rope_emb's last dimension must be {r} (head_dim{'' if use_neox_style else ' / 2'} "
+                             f"with use_neox_style={bool(use_neox_style)}), got {rope_emb.shape[4]}")
+        t = rope_emb.to(dev, torch.float32)
+        cos, sin = t[0].reshape(-1, r).contiguous(), t[1].reshape(-1, r).contiguous()
+    out_dtype = None
+    if float(out_scale) > 0:
+        out_dtype = _OUT_DTYPES.get(float(quant_max_bound))
+        if out_dtype is None:
+            raise ValueError(f"block_multihead_attention: out_scale > 0 needs quant_max_bound 127 (int8 output) or 448 (float8_e4m3fn output), "
+                             f"got {quant_max_bound}")
+        lo, hi = _KV8_LIMITS[out_dtype]
+        if not (lo <= float(quant_min_bound) <= float(quant_max_bound)):
+            raise ValueError(f"block_multihead_attention: quant_min_bound {quant_min_bound} must lie within [{lo}, {quant_max_bound}]")
+        if int(quant_round_type) not in (0, 1):
+            raise ValueError(f"block_multihead_attention: quant_round_type must be 0 or 1, got {quant_round_type}")
+        if (out_shift is None) != (out_smooth is None):
+            raise ValueError("block_multihead_attention: out_shift and out_smooth go together")
+        if out_shift is not None:
+            if out_dtype != torch.int8:
+                raise ValueError("block_multihead_attention: out_shift / out_smooth apply to int8 output only (quant_max_bound 127)")
+            hd = num_heads * head_dim
+            if out_shift.numel() != hd or out_smooth.numel() != hd:
+                raise ValueError(f"block_multihead_attention: out_shift / out_smooth must have H * D = {hd} elements")
+            out_shift, out_smooth = out_shift.reshape(hd).to(dev, dtype).contiguous(), out_smooth.reshape(hd).to(dev, dtype).contiguous()
+    else:
+        out_shift = out_smooth = None                                          # as in the reference: not applied without out_scale
+    if qkv.dtype != torch.int32 and qkv_bias is None and cos is None and out_dtype is None:
+        return None
+    return QKVPrologue(dtype, qkv_out_scale, qkv_bias, cos, sin, bool(use_neox_style), float(out_scale), out_dtype, out_shift, out_smooth,
+                       int(quant_round_type), float(quant_max_bound), float(quant_min_bound))
+
+
+def _prologue_ref(x, pro, pos, nh, nkv, d):
+    """The qkv prologue op by op in torch: x [n, W] packed rows (int32 or T), pos [n] their positions -> processed rows [n, W] of T."""
+    if x.dtype == torch.int32:
+        x = (x.float() * pro.qkv_out_scale).to(pro.dtype)
+    if pro.qkv_bias is not None:
+        x = x + pro.qkv_bias
+    if pro.rope_cos is None:
+        return x
+    n = x.shape[0]
+    rows = x.reshape(n, nh + 2 * nkv, d)
+    qk = rows[:, :nh + nkv].float()
+    c, s = pro.rope_cos[pos][:, None, :d // 2], pro.rope_sin[pos][:, None, :d // 2]
+    if pro.neox:
+        l, r = qk[..., :d // 2], qk[..., d // 2:]
+    else:
+        l, r = qk[..., 0::2], qk[..., 1::2]
+    nl, nr = l * c - r * s, r * c + l * s
+    qk = torch.cat([nl, nr], -1) if pro.neox else torch.stack([nl, nr], -1).flatten(-2)
+    return torch.cat([qk.to(pro.dtype), rows[:, nh + nkv:]], 1).reshape(n, -1)
+
+
+def _out_quant_ref(o, pro):
+    """The out_scale epilogue op by op: o [T, H * D] of T -> int8 / float8_e4m3fn."""
+    if pro.out_shift is not None:
+        o = (o + pro.out_shift) * pro.out_smooth
+    a = torch.tensor(pro.max_bound, dtype=torch.float32, device=o.device) * torch.tensor(pro.out_scale, dtype=torch.float32, device=o.device)
+    y = a * o.float()
+    if pro.out_dtype == torch.int8:
+        y = torch.round(y) if pro.round_type == 0 else _round_half_away(y)
+        return y.clamp(pro.min_bound, pro.max_bound).to(torch.int8)
+    return y.clamp(pro.min_bound, pro.max_bound).to(pro.out_dtype)
+
+
 def _round_half_away(y):
     """roundf: ties away from zero.  y - trunc(y) is exact in fp32, so 0.49999997 stays below one half (floor(|y| + 0.5) rounds it up)."""
     t = torch.trunc(y)
@@ -134,17 +264,25 @@ def _shared_prefix_groups(shared_prefix, nseq, block_size):
     return cu, seqs, plen
 
 
-def _paged_kernels_ok(qkv, kc, d, block_size, quant=None):
+def _paged_kernels_ok(qkv, kc, d, block_size, quant=None, pro=None):
     from ...framework.flags import flag
 
-    cache_ok = kc.dtype == qkv.dtype or (quant is not None and kc.dtype in _KV8_DTYPES)
-    return (qkv.is_cuda and kc.is_cuda and d == 128 and qkv.dtype in (torch.float16, torch.bfloat16) and cache_ok
+    dtype = qkv.dtype if pro is None else pro.dtype                      # the compute type: int32 qkv is dequantized to it
+    cache_ok = kc.dtype == dtype or (quant is not None and kc.dtype in _KV8_DTYPES)
+    return (qkv.is_cuda and kc.is_cuda and d == 128 and dtype in (torch.float16, torch.bfloat16) and cache_ok
             and int(block_size) in _PREFILL_BLOCK_SIZES and flag("FLAGS_use_fused_kernels", True))
+
+
+def _check_rope_positions(pro, max_pos):
+    if pro is not None and pro.rope_cos is not None and max_pos >= pro.rope_cos.shape[0]:
+        raise ValueError(f"block_multihead_attention: a new token sits at position {max_pos}, past the {pro.rope_cos.shape[0]} rows of rope_emb")
 
 
 def block_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_decoder, seq_lens_this_time, cu_seqlens_q, block_tables, block_size,
                     cache_k_quant_scales=None, cache_v_quant_scales=None, cache_k_dequant_scales=None, cache_v_dequant_scales=None,
-                    use_dynamic_cachekv_quant=False, quant_round_type=1, quant_max_bound=127.0, quant_min_bound=-127.0, shared_prefix=None):
+                    use_dynamic_cachekv_quant=False, quant_round_type=1, quant_max_bound=127.0, quant_min_bound=-127.0, shared_prefix=None, *,
+                    qkv_out_scale=None, qkv_bias=None, rope_emb=None, use_neox_style=False, out_shift=None, out_smooth=None, out_scale=-1,
+                    compute_dtype="default"):
     """qkv: [total_tokens, (H + 2*H_kv) * D] packed over the batch; caches [num_blocks, H_kv, block_size, D].
 
     A sequence prefills when seq_lens_encoder > 0 (a fresh prompt) or when it brings more than one token on top of seq_lens_decoder cached
@@ -169,18 +307,34 @@ def block_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_deco
     (prefix_len a positive multiple of block_size, at most each member's cached length).  Their rows run in ONE launch pair of
     `decode_attention_paged_shared` (csrc/decode_attention.cu), which reads each group's prefix once per 64-row tile of members instead of
     once per member.  A grouped row that is not a decode row raises ValueError; a member whose table or length breaks the contract gets
-    NaN rows (the device data is not read on the host).  Every other row takes its usual path.  None: no grouping."""
+    NaN rows (the device data is not read on the host).  Every other row takes its usual path.  None: no grouping.
+
+    qkv prologue (each optional; T is the compute type: qkv's dtype, or compute_dtype 'bf16' / 'fp16' / 'fp32' for int32 qkv), applied to
+    every new row in this order, each step rounded to T: int32 qkv is dequantized, float(qkv) * qkv_out_scale (fp32 [W]); qkv_bias (T [W])
+    is added; rope_emb ([2, 1, S_rope, 1, R] cos, sin, read as fp32) rotates the Q and K heads at each token's position p: pairs (2i, 2i + 1)
+    with R = D / 2, or with use_neox_style pairs (i, i + D / 2) with R = D (entries i >= D / 2 are not read), l' = l cos - r sin,
+    r' = r cos + l sin, every product and sum rounded to fp32.  Decode rows read the table too (block_multihead_attention's rope_theta is
+    not used).  The processed K / V rows are what the caches receive.  A float qkv gets its processed rows (q, k and v) written back in
+    place; an int32 qkv is returned unchanged.  On the CUDA path the whole prologue and the cache write are ONE launch of
+    `paged_kv_cache_write` (csrc/kv_cache_quant.cu), positions found on the device; a position >= S_rope raises ValueError before it,
+    checked in the same host read that tells the row kinds apart.
+
+    out_scale > 0: the output is quantized to int8 (quant_max_bound 127) or float8_e4m3fn (448) by one launch of `attention_out_quant`
+    after the attention: y = max_bound * out_scale * o, rounded and clamped as the cache is (quant_round_type, bounds); out_shift /
+    out_smooth (T [H * D], int8 output only) first replace o by ((o + shift) -> T) * smooth -> T."""
     qkv, kc, vc = _raw(qkv), _raw(key_cache), _raw(value_cache)
     nkv, d = kc.shape[1], kc.shape[3]
     quant = kv_quant_params(kc, vc, cache_k_quant_scales, cache_v_quant_scales, cache_k_dequant_scales, cache_v_dequant_scales,
                             use_dynamic_cachekv_quant, quant_round_type, quant_max_bound, quant_min_bound)
-    if not _paged_kernels_ok(qkv, kc, d, block_size, quant):
+    nh = qkv.shape[1] // d - 2 * nkv
+    pro = qkv_prologue_params(qkv, nh, nkv, d, qkv_out_scale, qkv_bias, rope_emb, use_neox_style, out_shift, out_smooth, out_scale, compute_dtype,
+                              quant_round_type, quant_max_bound, quant_min_bound)
+    if not _paged_kernels_ok(qkv, kc, d, block_size, quant, pro):
         return _block_attention_ref(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_decoder, seq_lens_this_time, cu_seqlens_q, block_tables,
-                                    block_size, quant=quant, shared_prefix=shared_prefix)
+                                    block_size, quant=quant, shared_prefix=shared_prefix, prologue=pro)
     from ..._build import ext
 
     dev = qkv.device
-    nh = qkv.shape[1] // d - 2 * nkv
     enc = _raw(seq_lens_encoder).reshape(-1).to(dev, torch.int64)
     dec = _raw(seq_lens_decoder).reshape(-1).to(dev, torch.int64)
     now = _raw(seq_lens_this_time).reshape(-1).to(dev, torch.int64)
@@ -188,44 +342,44 @@ def block_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_deco
     bt = _raw(block_tables).to(dev, torch.int32).contiguous()
     nseq = now.numel()
     total_tokens = qkv.shape[0]
-    rows = qkv.reshape(total_tokens, nh + 2 * nkv, d)
-    q, k, v = rows[:, :nh], rows[:, nh:nh + nkv], rows[:, nh + nkv:]
     past = torch.where(enc > 0, torch.zeros_like(dec), dec)                  # prefill starts at position 0, decode continues after the cache
     i32 = lambda t: t.to(torch.int32).contiguous()                          # noqa: E731
-    if quant is None:
-        # ---- scatter the new K / V rows into the paged caches (all sequences at once)
-        tok = torch.arange(total_tokens, device=dev)
-        seq_of = torch.bucketize(tok, cu[1:nseq + 1], right=True).clamp(max=nseq - 1)
-        valid = tok < cu[nseq]
-        pos = past[seq_of] + (tok - cu[seq_of])
-        blk = bt.long()[seq_of, (pos // block_size).clamp(max=bt.shape[1] - 1)]
-        off = pos % block_size
-        sel = valid.nonzero().reshape(-1)
-        kc[blk[sel], :, off[sel]] = k[sel]
-        vc[blk[sel], :, off[sel]] = v[sel]
-        dq = {}
+    dq = {} if quant is None else {"k_dequant_scales": quant.k_dequant, "v_dequant_scales": quant.v_dequant}
+    if pro is not None:
+        # ---- the row kinds and the last new position in one host read, then the prologue and the cache write in one launch
+        kinds = _row_kinds(enc, now, nh, nkv, block_size, shared_prefix, torch.where(now > 0, past + now - 1, -1).max())
+        _check_rope_positions(pro, kinds[-1])
+        x = qkv if qkv.dtype != torch.int32 else torch.empty(qkv.shape, dtype=pro.dtype, device=dev)   # the processed rows
+        ext().paged_kv_cache_write(qkv, kc, vc, i32(cu[:nseq + 1]), i32(enc), i32(dec), bt, *((quant.k_quant, quant.v_quant, quant.round_type,
+                                   quant.max_bound, quant.min_bound) if quant is not None else (None, None, 1, 127.0, -127.0)),
+                                   qkv_out=x if pro.has_prologue else None,
+                                   qkv_out_scale=pro.qkv_out_scale, qkv_bias=pro.qkv_bias, rope_cos=pro.rope_cos, rope_sin=pro.rope_sin,
+                                   neox=pro.neox)
     else:
-        # ---- quantize the new K / V rows into the 8-bit caches: one launch, rows read in place from qkv
-        ext().paged_kv_cache_write(qkv.reshape(total_tokens, -1), kc, vc, i32(cu[:nseq + 1]), i32(enc), i32(dec), bt, quant.k_quant, quant.v_quant,
-                                   quant.round_type, quant.max_bound, quant.min_bound)
-        dq = {"k_dequant_scales": quant.k_dequant, "v_dequant_scales": quant.v_dequant}
-    out = qkv.new_zeros((total_tokens, nh * d))
+        x = qkv
+        if quant is None:
+            # ---- scatter the new K / V rows into the paged caches (all sequences at once)
+            rows = qkv.reshape(total_tokens, nh + 2 * nkv, d)
+            k, v = rows[:, nh:nh + nkv], rows[:, nh + nkv:]
+            tok = torch.arange(total_tokens, device=dev)
+            seq_of = torch.bucketize(tok, cu[1:nseq + 1], right=True).clamp(max=nseq - 1)
+            valid = tok < cu[nseq]
+            pos = past[seq_of] + (tok - cu[seq_of])
+            blk = bt.long()[seq_of, (pos // block_size).clamp(max=bt.shape[1] - 1)]
+            off = pos % block_size
+            sel = valid.nonzero().reshape(-1)
+            kc[blk[sel], :, off[sel]] = k[sel]
+            vc[blk[sel], :, off[sel]] = v[sel]
+        else:
+            # ---- quantize the new K / V rows into the 8-bit caches: one launch, rows read in place from qkv
+            ext().paged_kv_cache_write(qkv.reshape(total_tokens, -1), kc, vc, i32(cu[:nseq + 1]), i32(enc), i32(dec), bt, quant.k_quant, quant.v_quant,
+                                       quant.round_type, quant.max_bound, quant.min_bound)
+        kinds = _row_kinds(enc, now, nh, nkv, block_size, shared_prefix)
+    is_dec, is_ver, is_pre, groups, any_dec, any_ver, any_pre = kinds[:7]
+    q = x.reshape(total_tokens, nh + 2 * nkv, d)[:, :nh]
+    out = x.new_zeros((total_tokens, nh * d))
     scale = 1.0 / math.sqrt(d)
-    is_dec = (now == 1) & (enc == 0)
-    is_ver = (enc == 0) & (now >= 2) & (now <= min(VERIFY_MAX, 64 // (nh // nkv)))
-    is_pre = (now > 0) & ~is_dec & ~is_ver
-    if shared_prefix is None:
-        any_dec, any_ver, any_pre = torch.stack([is_dec.any(), is_ver.any(), is_pre.any()]).tolist()
-    else:
-        groups = _shared_prefix_groups(shared_prefix, nseq, block_size)
-        in_group = torch.zeros(nseq, dtype=torch.bool)
-        in_group[groups[1]] = True
-        in_group = in_group.pin_memory().to(dev, non_blocking=True)        # a pinned copy: the host does not wait for the stream
-        bad = in_group & ~is_dec
-        is_dec = is_dec & ~in_group
-        any_dec, any_ver, any_pre, any_bad = torch.stack([is_dec.any(), is_ver.any(), is_pre.any(), bad.any()]).tolist()
-        if any_bad:
-            raise ValueError("block_attention: shared_prefix groups may only hold decode rows (seq_lens_this_time 1, seq_lens_encoder 0)")
+    if groups is not None:
         # ---- grouped decode rows: each group's prefix read once per tile of members, then every member's own keys
         ext().decode_attention_paged_shared(q, kc, vc, bt, i32(cu[:nseq]), i32(dec + 1), *(torch.tensor(v, dtype=torch.int32) for v in groups),
                                             scale, out, **dq)
@@ -242,33 +396,79 @@ def block_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_deco
     # ---- prefill sequences (fresh prompts and longer continuing chunks): new tokens over their whole cached prefix, one launch for all
     if any_pre:
         ext().attention_fwd_paged(q, kc, vc, bt, i32(cu[:nseq]), i32(torch.where(is_pre, now, 0)), i32(past), scale, out, **dq)
+    if pro is not None and pro.out_dtype is not None:
+        # ---- output quantization: one launch over every row
+        y = torch.empty(out.shape, dtype=pro.out_dtype, device=dev)
+        ext().attention_out_quant(out, y, pro.out_scale, pro.out_shift, pro.out_smooth, pro.round_type, pro.max_bound, pro.min_bound)
+        out = y
     return out.as_subclass(Tensor), qkv.as_subclass(Tensor), kc.as_subclass(Tensor), vc.as_subclass(Tensor)
+
+
+def _row_kinds(enc, now, nh, nkv, block_size, shared_prefix, extra=None):
+    """Splits block_attention's rows into decode / verify / prefill rows with ONE host read: (is_dec, is_ver, is_pre, shared-prefix groups or
+    None, any_dec, any_ver, any_pre[, int(extra)]).  Grouped rows leave is_dec; a grouped row that is not a decode row raises ValueError."""
+    nseq, dev = now.numel(), now.device
+    is_dec = (now == 1) & (enc == 0)
+    is_ver = (enc == 0) & (now >= 2) & (now <= min(VERIFY_MAX, 64 // (nh // nkv)))
+    is_pre = (now > 0) & ~is_dec & ~is_ver
+    groups = bad = None
+    if shared_prefix is not None:
+        groups = _shared_prefix_groups(shared_prefix, nseq, block_size)
+        in_group = torch.zeros(nseq, dtype=torch.bool)
+        in_group[groups[1]] = True
+        in_group = in_group.pin_memory().to(dev, non_blocking=True)        # a pinned copy: the host does not wait for the stream
+        bad = in_group & ~is_dec
+        is_dec = is_dec & ~in_group
+    flags = [is_dec.any(), is_ver.any(), is_pre.any()] + ([] if bad is None else [bad.any()])
+    if extra is not None:
+        flags = [f.long() for f in flags] + [extra]
+    flags = torch.stack(flags).tolist()
+    if shared_prefix is not None and flags.pop(3):
+        raise ValueError("block_attention: shared_prefix groups may only hold decode rows (seq_lens_this_time 1, seq_lens_encoder 0)")
+    return (is_dec, is_ver, is_pre, groups, *(bool(f) for f in flags[:3]), *(int(f) for f in flags[3:]))
 
 
 def _block_attention_ref(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_decoder, seq_lens_this_time, cu_seqlens_q, block_tables, block_size,
                          cache_k_quant_scales=None, cache_v_quant_scales=None, cache_k_dequant_scales=None, cache_v_dequant_scales=None,
                          use_dynamic_cachekv_quant=False, quant_round_type=1, quant_max_bound=127.0, quant_min_bound=-127.0, quant=None,
-                         shared_prefix=None):
+                         shared_prefix=None, prologue=None, **prologue_args):
     """qkv: [total_tokens, (H + 2*H_kv) * D] packed over the batch; caches [num_blocks, H_kv, block_size, D].  `quant`: an already
     validated KVQuant (otherwise it is built from the scale / round / bound arguments).  `shared_prefix`: as in block_attention; its whole
-    contract is checked here (ValueError on a violation), and it does not change the math."""
+    contract is checked here (ValueError on a violation), and it does not change the math.  `prologue`: an already validated QKVPrologue
+    (otherwise it is built from block_attention's keyword arguments qkv_out_scale, qkv_bias, rope_emb, use_neox_style, out_shift,
+    out_smooth, out_scale and compute_dtype in `prologue_args`), applied op by op in torch."""
     qkv, kc, vc = _raw(qkv), _raw(key_cache), _raw(value_cache)
     if quant is None:
         quant = kv_quant_params(kc, vc, cache_k_quant_scales, cache_v_quant_scales, cache_k_dequant_scales, cache_v_dequant_scales,
                                 use_dynamic_cachekv_quant, quant_round_type, quant_max_bound, quant_min_bound)
     nkv, d = kc.shape[1], kc.shape[3]
     nh = qkv.shape[1] // d - 2 * nkv
+    pro = prologue
+    if pro is None:
+        pro = qkv_prologue_params(qkv, nh, nkv, d, **prologue_args, quant_round_type=quant_round_type, quant_max_bound=quant_max_bound,
+                                  quant_min_bound=quant_min_bound)
     enc, dec, now = _raw(seq_lens_encoder).reshape(-1).tolist(), _raw(seq_lens_decoder).reshape(-1).tolist(), _raw(seq_lens_this_time).reshape(-1).tolist()
     cu = _raw(cu_seqlens_q).reshape(-1).tolist()
     bt = _raw(block_tables)
     if shared_prefix is not None:
         _check_shared_prefix(shared_prefix, enc, dec, now, bt, block_size)
-    out = qkv.new_zeros((qkv.shape[0], nh * d))
+    x = qkv
+    if pro is not None:
+        starts = [0 if enc[b] > 0 else dec[b] for b in range(len(now))]
+        _check_rope_positions(pro, max([starts[b] + now[b] - 1 for b in range(len(now)) if now[b] > 0], default=-1))
+        if qkv.dtype == torch.int32:
+            x = torch.zeros(qkv.shape, dtype=pro.dtype, device=qkv.device)
+        if pro.has_prologue:
+            for b in range(len(now)):
+                if now[b] > 0:
+                    pos = torch.arange(starts[b], starts[b] + now[b], device=qkv.device)
+                    x[cu[b]:cu[b] + now[b]] = _prologue_ref(qkv[cu[b]:cu[b] + now[b]], pro, pos, nh, nkv, d)
+    out = x.new_zeros((qkv.shape[0], nh * d))
     for b in range(len(now)):
         n = now[b]
         if n == 0:
             continue
-        rows = qkv[cu[b]:cu[b] + n].reshape(n, nh + 2 * nkv, d)
+        rows = x[cu[b]:cu[b] + n].reshape(n, nh + 2 * nkv, d)
         q, k, v = rows[:, :nh], rows[:, nh:nh + nkv], rows[:, nh + nkv:]
         past = dec[b] if enc[b] == 0 else 0
         for t in range(n):  # append new K/V into the paged cache
@@ -295,6 +495,8 @@ def _block_attention_ref(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens
         s = s.masked_fill(kpos > qpos, float("-inf"))
         o = torch.einsum("hns,hsd->nhd", torch.softmax(s, -1), V.float())
         out[cu[b]:cu[b] + n] = o.reshape(n, nh * d).to(out.dtype)
+    if pro is not None and pro.out_dtype is not None:
+        out = _out_quant_ref(out, pro)
     return out.as_subclass(Tensor), qkv.as_subclass(Tensor), kc.as_subclass(Tensor), vc.as_subclass(Tensor)
 
 

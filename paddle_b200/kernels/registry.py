@@ -181,7 +181,7 @@ def _register_builtin(f):
     r("flash_attn", A, ("*",), "kernels.attention:attention_ref")
     r("flash_attn_qkvpacked", G, HALF, "kernels.attention:attention_packed", native="csrc/attention_sm100.cu (packed qkv)")
     r("masked_multihead_attention", G, HALF, "incubate.nn.functional:masked_multihead_attention", native="csrc/decode_attention.cu")
-    r("block_multihead_attention", G, HALF, "incubate.nn.paged_attention:block_attention", native="csrc/decode_attention.cu (paged), csrc/attention_sm100.cu (paged prefill), csrc/kv_cache_quant.cu (int8 / fp8 cache write)", priority=10)
+    r("block_multihead_attention", G, HALF, "incubate.nn.paged_attention:block_attention", native="csrc/decode_attention.cu (paged), csrc/attention_sm100.cu (paged prefill), csrc/kv_cache_quant.cu (int8 / fp8 cache write; qkv dequant / bias / rotary prologue fused into the cache write; out_scale output quantization)", priority=10)
     r("block_multihead_attention", A, ("*",), "incubate.nn.paged_attention:block_attention")
     # normalisation / activation / rotary / loss
     r("rms_norm", G, FLOAT, "kernels.norm:rms_norm", native="csrc/norm.cu::rms_norm_fwd / rms_norm_bwd", priority=10)
