@@ -604,11 +604,20 @@ Tensor moe_rows_dot(const Tensor& src, const Tensor& dest, const Tensor& g, int6
   return dw;
 }
 
-// x [M, K] bf16 / fp16, w int8 [N, K] (or int4 packed [N, K/2]), scale float [N], bias [N] or None -> [M, N]
-Tensor weight_only_gemm(const Tensor& x, const Tensor& w, const Tensor& scale, const OptT& bias, bool int4) {
+// x [M, K] bf16 / fp16, w int8 [N, K] (or int4 packed [N, K/2]), scale float [N] (group_size <= 0) or [K / group_size, N] (64 / 128),
+// bias [N] or None -> [M, N]
+Tensor weight_only_gemm(const Tensor& x, const Tensor& w, const Tensor& scale, const OptT& bias, bool int4, int64_t group_size) {
   TORCH_CHECK(x.is_cuda() && x.dim() == 2 && x.is_contiguous() && (x.scalar_type() == at::kBFloat16 || x.scalar_type() == at::kHalf), "weight_only_gemm: x [M, K] bf16 / fp16 contiguous");
   TORCH_CHECK(w.is_cuda() && w.dim() == 2 && w.is_contiguous() && w.scalar_type() == at::kChar && w.size(1) == (int4 ? x.size(1) / 2 : x.size(1)), "weight_only_gemm: w int8 [N, K] (int4: [N, K/2])");
-  TORCH_CHECK(scale.is_cuda() && scale.scalar_type() == at::kFloat && scale.numel() == w.size(0) && scale.is_contiguous(), "weight_only_gemm: scale float32 [N]");
+  if (group_size <= 0) {
+    TORCH_CHECK(scale.is_cuda() && scale.scalar_type() == at::kFloat && scale.numel() == w.size(0) && scale.is_contiguous(), "weight_only_gemm: scale float32 [N]");
+  } else {
+    // literal messages: with this extension's host toolchain a failing TORCH_CHECK that formats an integer aborts instead of raising
+    TORCH_CHECK(group_size == 64 || group_size == 128, "weight_only_gemm: group_size must be -1, 64 or 128");
+    TORCH_CHECK(x.size(1) % group_size == 0, "weight_only_gemm: K is not a multiple of group_size");
+    TORCH_CHECK(scale.is_cuda() && scale.scalar_type() == at::kFloat && scale.dim() == 2 && scale.size(0) == x.size(1) / group_size && scale.size(1) == w.size(0) && scale.is_contiguous(),
+                "weight_only_gemm: scale float32 [K / group_size, N] contiguous");
+  }
   c10::cuda::CUDAGuard guard(x.device());
   b200::WoGemmArgs g;
   g.m = (int)x.size(0); g.k = (int)x.size(1); g.n = (int)w.size(0);
@@ -617,10 +626,35 @@ Tensor weight_only_gemm(const Tensor& x, const Tensor& w, const Tensor& scale, c
   g.bias = nullptr;
   if (bias.has_value() && bias->defined()) { TORCH_CHECK(bias->scalar_type() == x.scalar_type() && bias->numel() == g.n && bias->is_contiguous(), "weight_only_gemm: bias [N] in x dtype"); g.bias = bias->data_ptr(); }
   g.int4 = int4 ? 1 : 0; g.bf16 = x.scalar_type() == at::kBFloat16 ? 1 : 0;
+  g.group_size = group_size > 0 ? (int)group_size : 0;
   int rc = b200::gemm_weight_only(g, cur_stream());
   g_launches += 1;
   check_err();
-  TORCH_CHECK(rc == 0, "paddle_b200.weight_only_gemm: unsupported shape (K multiple of 64, N multiple of 8) rc=", rc);
+  TORCH_CHECK(rc == 0, "paddle_b200.weight_only_gemm: unsupported shape (K multiple of 64, N multiple of 8, M <= 64, 16-byte aligned)");
+  return out;
+}
+
+// w int8 [N, K] (int4 packed [N, K/2]), scale float [N] or [K / group_size, N] -> [K, N] in out_dtype (bf16 / fp16 / fp32); one launch
+Tensor weight_dequantize(const Tensor& w, const Tensor& scale, bool int4, int64_t group_size, at::ScalarType out_dtype) {
+  TORCH_CHECK(w.is_cuda() && w.dim() == 2 && w.is_contiguous() && w.scalar_type() == at::kChar && w.numel() > 0, "weight_dequantize: w int8 [N, K] (int4: [N, K/2]) contiguous");
+  TORCH_CHECK(out_dtype == at::kBFloat16 || out_dtype == at::kHalf || out_dtype == at::kFloat, "weight_dequantize: out_dtype bf16 / fp16 / fp32");
+  const int64_t n = w.size(0), k = int4 ? 2 * w.size(1) : w.size(1);
+  TORCH_CHECK(n < (int64_t)1 << 31 && k < (int64_t)1 << 31, "weight_dequantize: dimensions too large");
+  if (group_size <= 0) {
+    TORCH_CHECK(scale.is_cuda() && scale.scalar_type() == at::kFloat && scale.numel() == n && scale.is_contiguous(), "weight_dequantize: scale float32 [N]");
+  } else {
+    TORCH_CHECK(k % group_size == 0, "weight_dequantize: K is not a multiple of group_size");
+    TORCH_CHECK(scale.is_cuda() && scale.scalar_type() == at::kFloat && scale.dim() == 2 && scale.size(0) == k / group_size && scale.size(1) == n && scale.is_contiguous(),
+                "weight_dequantize: scale float32 [K / group_size, N] contiguous");
+  }
+  TORCH_CHECK(scale.device() == w.device(), "weight_dequantize: w and scale on one device");
+  c10::cuda::CUDAGuard guard(w.device());
+  Tensor out = torch::empty({k, n}, w.options().dtype(out_dtype));
+  int rc = b200::weight_dequantize(w.data_ptr(), scale.data_ptr<float>(), out.data_ptr(), (int)n, (int)k, int4 ? 1 : 0, group_size > 0 ? (int)group_size : 0,
+                                   dt_code(out_dtype), cur_stream());
+  g_launches += 1;
+  check_err();
+  TORCH_CHECK(rc == 0, "paddle_b200.weight_dequantize: unsupported shape");
   return out;
 }
 
@@ -1300,7 +1334,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         pybind11::arg("topk") = 1);
   m.def("moe_rows_dot", traced("moe_rows_dot", &moe_rows_dot));
   m.def("weight_only_gemm", traced("weight_only_gemm", &weight_only_gemm), pybind11::arg("x"), pybind11::arg("w"), pybind11::arg("scale"), pybind11::arg("bias") = pybind11::none(),
-        pybind11::arg("int4") = false);
+        pybind11::arg("int4") = false, pybind11::arg("group_size") = -1);
+  m.def("weight_dequantize", traced("weight_dequantize", &weight_dequantize), pybind11::arg("w"), pybind11::arg("scale"), pybind11::arg("int4") = false,
+        pybind11::arg("group_size") = -1, pybind11::arg("out_dtype") = at::kBFloat16);
   m.def("gemm_grouped", traced("gemm_grouped", &gemm_grouped), pybind11::arg("a"), pybind11::arg("b"), pybind11::arg("tile_expert"), pybind11::arg("b_is_nk") = false,
         pybind11::arg("out") = pybind11::none());
   m.def("gemm_grouped_wgrad", traced("gemm_grouped_wgrad", &gemm_grouped_wgrad));

@@ -1,4 +1,5 @@
-// Weight-only quantised GEMM for sm_90a: out[M,N] = x[M,K] (bf16 / fp16) @ dequant(Wq[N,K] int8 | int4) * scale[N] (+ bias), M <= 64.
+// Weight-only quantised GEMM for sm_90a: out[M,N] = x[M,K] (bf16 / fp16) @ dequant(Wq[N,K] int8 | int4) (+ bias), M <= 64, with per-channel
+// scales scale[N] or group-wise scales scale[K / G, N] (G = 64 or 128 consecutive k of one channel share a scale).
 //
 // The int8 / int4 weights never exist as 16-bit values in HBM or in shared memory: TMA streams raw [128 channels x 128 B] boxes into a
 // ring, the two MMA warpgroups expand them IN REGISTERS straight into the A-operand fragment layout of wgmma (A from registers, B =
@@ -8,10 +9,16 @@
 // are split along K over a thread-block CLUSTER whose CTAs reduce their partial tiles through DSMEM - no workspace, no atomics, no
 // second kernel.
 //
+// Group-wise scales: each group's k-blocks accumulate into a separate group accumulator (the group's first wgmma has scale-d = 0); once
+// they retire, the thread folds acc += acc_g * s[g][channel] in fp32 (two scales per thread: rows r0 and r0 + 8).  The epilogue and the
+// split-K reduction then add only the bias.  A second kernel expands the quantised weight to 16-bit / fp32 in one pass for the batches
+// that run the dense GEMM instead.
+//
 // Parity: paddle/phi/kernels/gpu/weight_only_linear_kernel.cu:27, python/paddle/nn/quant/quantized_linear.py:183.
 #include <cuda.h>
 #include <cstdio>
 #include <string>
+#include <type_traits>
 
 #include "include/b200_common.cuh"
 #include "include/b200_ops.h"
@@ -33,7 +40,7 @@ constexpr uint32_t W_BYTES = BLOCK_N * 128;   // 16 KB raw box
 struct Params {
   int m, n, k;                 // tokens, output channels, reduction
   int kb_per_split;            // 64-wide k-blocks handled by one blockIdx.y
-  const float* scale;          // [n] per-channel dequantisation factors
+  const float* scale;          // [n] per-channel or [k / GS, n] group-wise dequantisation factors
   const void* bias;            // [n] in the activation dtype or nullptr
   void* out;                   // [m, n] activation dtype (splits == 1)
   int splits;                  // blockIdx.y extent = cluster size: the CTAs of one output tile
@@ -68,16 +75,19 @@ __device__ __forceinline__ void keep_regs(uint32_t (&a)[4]) {
   for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(a[i])::"memory");
 }
 
-// NTOK: token tile (MMA N).  INT4: two weights per byte (low nibble = even k).
+// NTOK: token tile (MMA N).  INT4: two weights per byte (low nibble = even k).  GS: scale group size in k (0: per-channel scales).
 //
 // Data path of one 64-wide k-block:  TMA raw box (128 channels x 128 B, shared by 2 int8 / 4 int4 k-blocks) + the activation tiles of
 // those k-blocks in one ring stage -> every MMA thread reads exactly the bytes of its own A-fragment elements (rows lane / 4 and + 8 of
 // its warp's 16 channels, k = 2 (lane % 4) .. + 1 and + 8 of each 16-wide step), converts them and issues wgmma with A in registers ->
 // D^T[64 channels, NTOK tokens] += A x_tile^T.  The dequantised weights never touch shared memory.
-template <int NTOK, int WST, bool INT4, bool BF16>
+template <int NTOK, int WST, bool INT4, bool BF16, int GS>
 __global__ void __launch_bounds__(kThreads, 1)
 wo_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_x, const Params p) {
   constexpr int KB_PER_W = INT4 ? 4 : 2;                        // k-blocks covered by one raw box
+  constexpr int KB_PER_G = GS ? GS / BLOCK_K : 1;              // k-blocks per scale group
+  constexpr int G_PER_W = GS ? KB_PER_W / KB_PER_G : 1;         // scale groups per raw box
+  static_assert(GS == 0 || (GS % BLOCK_K == 0 && KB_PER_W % KB_PER_G == 0), "weight-only gemm: a raw box holds whole scale groups");
   constexpr uint32_t X_BYTES = NTOK * BLOCK_K * 2;
   constexpr uint32_t STAGE_BYTES = W_BYTES + KB_PER_W * X_BYTES;
   static_assert(NTOK * 512 <= WST * STAGE_BYTES, "weight-only gemm: the split-K partial tile is staged in the ring");
@@ -122,12 +132,24 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
     // ================= MMA warpgroups: dequantise into the A fragment, D^T[64 channels, NTOK tokens] += A x_tile^T =================
     const int wg = warp >> 2, q = lane & 3;
     const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // channel rows r0 and r0 + 8 of the tile ((r0 + 8) & 7 == r0 & 7)
-    float acc[NTOK / 2];
+    float acc[NTOK / 2], acc_g[NTOK / 2];                      // acc_g: the current scale group (group-wise scales only)
 #pragma unroll
-    for (int i = 0; i < NTOK / 2; ++i) acc[i] = 0.f;
+    for (int i = 0; i < NTOK / 2; ++i) acc[i] = acc_g[i] = 0.f;
     for (int j = 0; j < num_box; ++j) {
       const int st = j % WST;
       const int nvalid = min(KB_PER_W, num_kb - j * KB_PER_W);
+      float gsc[G_PER_W][2];                                     // this box's group scales of rows r0 and r0 + 8
+      if constexpr (GS > 0) {
+        // boxes start on multiples of 4 k-blocks (256 k), so they hold whole groups; read the scales before the wait to hide the loads
+        const int g0 = (kb0 + j * KB_PER_W) / KB_PER_G;
+#pragma unroll
+        for (int gi = 0; gi < G_PER_W; ++gi)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int g = g0 + gi, ch = n0 + r0 + h * 8;
+            gsc[gi][h] = (g * GS < p.k && ch < p.n) ? __ldg(p.scale + (int64_t)g * p.n + ch) : 0.f;
+          }
+      }
       mbar_wait(full(st), (j / WST) & 1);
       const uint32_t sw = base + st * STAGE_BYTES;
       const uint32_t row0 = sw + r0 * 128, row1 = row0 + 8 * 128;   // 128 rows x 128 B, SWIZZLE_128B: 16-byte piece c of row r sits at piece c ^ (r & 7)
@@ -153,19 +175,41 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
             }
           }
           const uint32_t xs = sw + W_BYTES + sub * X_BYTES;
-          wgmma_fence_regs(acc);
-          wgmma_fence();
+          if constexpr (GS == 0) {
+            wgmma_fence_regs(acc);
+            wgmma_fence();
 #pragma unroll
-          for (int s = 0; s < 4; ++s) {
-            const uint64_t bdesc = make_smem_desc(xs + s * 32, 16, 1024);
-            if constexpr (NTOK == 16) wgmma_rs_n16<BF16, 0>(acc, a[s], bdesc, 1);
-            else wgmma_rs_n64<BF16, 0>(acc, a[s], bdesc, 1);
+            for (int s = 0; s < 4; ++s) {
+              const uint64_t bdesc = make_smem_desc(xs + s * 32, 16, 1024);
+              if constexpr (NTOK == 16) wgmma_rs_n16<BF16, 0>(acc, a[s], bdesc, 1);
+              else wgmma_rs_n64<BF16, 0>(acc, a[s], bdesc, 1);
+            }
+            wgmma_commit();
+            wgmma_wait<0>();                  // the fragment registers are read asynchronously: they stay untouched until the MMAs retire
+            wgmma_fence_regs(acc);
+#pragma unroll
+            for (int s = 0; s < 4; ++s) keep_regs(a[s]);
+          } else {
+            // the group's first k-block overwrites acc_g (scale-d = 0); its last one folds acc_g into acc with the group's scales
+            wgmma_fence_regs(acc_g);
+            wgmma_fence();
+#pragma unroll
+            for (int s = 0; s < 4; ++s) {
+              const uint64_t bdesc = make_smem_desc(xs + s * 32, 16, 1024);
+              const uint32_t accumulate = (s == 0 && sub % KB_PER_G == 0) ? 0u : 1u;
+              if constexpr (NTOK == 16) wgmma_rs_n16<BF16, 0>(acc_g, a[s], bdesc, accumulate);
+              else wgmma_rs_n64<BF16, 0>(acc_g, a[s], bdesc, accumulate);
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_regs(acc_g);
+#pragma unroll
+            for (int s = 0; s < 4; ++s) keep_regs(a[s]);
+            if (sub % KB_PER_G == KB_PER_G - 1) {   // nvalid is a multiple of KB_PER_G: a group never straddles boxes or splits
+#pragma unroll
+              for (int i = 0; i < NTOK / 2; ++i) acc[i] = fmaf(acc_g[i], gsc[sub / KB_PER_G][(i >> 1) & 1], acc[i]);
+            }
           }
-          wgmma_commit();
-          wgmma_wait<0>();                    // the fragment registers are read asynchronously: they stay untouched until the MMAs retire
-          wgmma_fence_regs(acc);
-#pragma unroll
-          for (int s = 0; s < 4; ++s) keep_regs(a[s]);
         }
       }
       __syncwarp();
@@ -188,7 +232,7 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
       for (int h = 0; h < 2; ++h) {
         const int ch = n0 + r0 + h * 8;
         if (ch >= p.n) continue;
-        const float sc = p.scale[ch];
+        const float sc = GS ? 1.f : p.scale[ch];              // group-wise scales are already folded into acc
         float bv = 0.f;
         if (p.bias) bv = BF16 ? __bfloat162float(((const __nv_bfloat16*)p.bias)[ch]) : __half2float(((const __half*)p.bias)[ch]);
 #pragma unroll
@@ -197,7 +241,7 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
           for (int e = 0; e < 2; ++e) {
             const int tok = tok0 + jn * 8 + 2 * q + e;
             if (tok >= p.m) continue;
-            const float y = acc[jn * 4 + h * 2 + e] * sc + bv;
+            const float y = GS ? acc[jn * 4 + h * 2 + e] + bv : acc[jn * 4 + h * 2 + e] * sc + bv;
             if constexpr (BF16) ((__nv_bfloat16*)p.out)[(int64_t)tok * p.n + ch] = __float2bfloat16_rn(y);
             else ((__half*)p.out)[(int64_t)tok * p.n + ch] = __float2half_rn(y);
           }
@@ -224,7 +268,7 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
           acc += v;
         }
         if (ch < p.n) {
-          float y = acc * p.scale[ch];
+          float y = GS ? acc : acc * p.scale[ch];
           if (p.bias) y += BF16 ? __bfloat162float(((const __nv_bfloat16*)p.bias)[ch]) : __half2float(((const __half*)p.bias)[ch]);
           if constexpr (BF16) ((__nv_bfloat16*)p.out)[(int64_t)(tok0 + tok) * p.n + ch] = __float2bfloat16_rn(y);
           else ((__half*)p.out)[(int64_t)(tok0 + tok) * p.n + ch] = __float2half_rn(y);
@@ -263,7 +307,7 @@ static bool make_w_map(CUtensorMap* out, const void* w, int n, int row_bytes) {
   return true;
 }
 
-template <int NTOK, int WST, bool INT4, bool BF16>
+template <int NTOK, int WST, bool INT4, bool BF16, int GS>
 static int launch(const WoGemmArgs& g, const CUtensorMap& mw, cudaStream_t s) {
   constexpr int KB_PER_W = INT4 ? 4 : 2;
   constexpr uint32_t SMEM = WST * (W_BYTES + KB_PER_W * NTOK * BLOCK_K * 2) + 1024 + 256;
@@ -272,7 +316,7 @@ static int launch(const WoGemmArgs& g, const CUtensorMap& mw, cudaStream_t s) {
   constexpr int kMaxSplits = 8;                 // portable cluster size
   CUtensorMap mx;
   if (!gemm::make_map(&mx, g.x, g.k, g.m, 1, g.k, 0, BLOCK_K, NTOK, g.bf16 ? kBF16 : kF16)) return 2;
-  auto kern = wo_gemm_kernel<NTOK, WST, INT4, BF16>;
+  auto kern = wo_gemm_kernel<NTOK, WST, INT4, BF16, GS>;
   static bool attr_set = false;
   static int wave_ctas[kMaxSplits + 1];         // CTAs the device holds at once when they come in clusters of `splits`
   if (!attr_set) {
@@ -307,6 +351,9 @@ static int launch(const WoGemmArgs& g, const CUtensorMap& mw, cudaStream_t s) {
     const long cost = waves * (per + 24) + (c > 1 ? 6 : 0);
     if (best < 0 || cost < best) { best = cost; splits = c; kb_per = per; }
   }
+  if constexpr (GS > 0) {                                         // the kernel folds whole groups: no split may cut one
+    if ((kb_per * BLOCK_K) % GS) { set_last_error(__FILE__, __LINE__, "weight-only gemm: split boundary inside a scale group"); return 3; }
+  }
   p.splits = splits;
   p.kb_per_split = kb_per;
   p.scale = g.scale; p.bias = g.bias; p.out = g.out;
@@ -320,23 +367,86 @@ static int launch(const WoGemmArgs& g, const CUtensorMap& mw, cudaStream_t s) {
   return 0;
 }
 
-template <bool INT4, bool BF16>
+template <bool INT4, bool BF16, int GS>
 static int dispatch_tok(const WoGemmArgs& g, const CUtensorMap& mw, cudaStream_t s) {
-  if (g.m <= 16) return launch<16, 8, INT4, BF16>(g, mw, s);      // decode: 128 KB of raw weights in flight
-  return launch<64, 4, INT4, BF16>(g, mw, s);
+  if (g.m <= 16) return launch<16, 8, INT4, BF16, GS>(g, mw, s);  // decode: 128 KB of raw weights in flight
+  return launch<64, 4, INT4, BF16, GS>(g, mw, s);
+}
+template <bool INT4, bool BF16>
+static int dispatch_group(const WoGemmArgs& g, const CUtensorMap& mw, cudaStream_t s) {
+  if (g.group_size == 64) return dispatch_tok<INT4, BF16, 64>(g, mw, s);
+  if (g.group_size == 128) return dispatch_tok<INT4, BF16, 128>(g, mw, s);
+  return dispatch_tok<INT4, BF16, 0>(g, mw, s);
+}
+
+// One-pass dequantisation for the batches that run the dense GEMM: each CTA reads a [64 channels x 64 k] tile of the quantised weight once
+// (along k), turns it around in shared memory and writes [64 k x 64 channels] of out once (along n).  out = float(q) * scale, rounded once
+// to OutT: the same value as nn/quant.py's torch expression.
+template <bool INT4, typename OutT>
+__global__ void __launch_bounds__(256)
+wo_dequant_kernel(const int8_t* __restrict__ w, const float* __restrict__ scale, OutT* __restrict__ out, int n, int k, int group_size) {
+  __shared__ float tile[64][65];                             // [k][channel], q as float (exact)
+  const int k0 = blockIdx.x * 64, n0 = blockIdx.y * 64, t = threadIdx.x;
+  if constexpr (!INT4) {
+    for (int i = t; i < 64 * 64; i += 256) {
+      const int nl = i >> 6, kl = i & 63, ch = n0 + nl, kk = k0 + kl;
+      tile[kl][nl] = (ch < n && kk < k) ? (float)w[(int64_t)ch * k + kk] : 0.f;
+    }
+  } else {
+    for (int i = t; i < 64 * 32; i += 256) {                 // byte c of a row holds k = 2c (low nibble) and 2c + 1
+      const int nl = i >> 5, bl = i & 31, ch = n0 + nl, kk = k0 + 2 * bl;
+      const uint32_t raw = (ch < n && kk < k) ? (uint32_t)(uint8_t)w[(int64_t)ch * (k / 2) + kk / 2] : 0u;
+      tile[2 * bl][nl] = (float)((int)((raw & 0xFu) ^ 8u) - 8);
+      tile[2 * bl + 1][nl] = (float)((int)(((raw >> 4) & 0xFu) ^ 8u) - 8);
+    }
+  }
+  __syncthreads();
+  for (int i = t; i < 64 * 64; i += 256) {
+    const int kl = i >> 6, nl = i & 63, ch = n0 + nl, kk = k0 + kl;
+    if (ch >= n || kk >= k) continue;
+    const float v = __fmul_rn(tile[kl][nl], scale[group_size > 0 ? (int64_t)(kk / group_size) * n + ch : ch]);
+    OutT* o = out + (int64_t)kk * n + ch;
+    if constexpr (std::is_same<OutT, float>::value) *o = v;
+    else if constexpr (std::is_same<OutT, __nv_bfloat16>::value) *o = __float2bfloat16_rn(v);
+    else *o = __float2half_rn(v);
+  }
+}
+
+template <bool INT4, typename OutT>
+static int launch_dequant(const void* w, const float* scale, void* out, int n, int k, int group_size, cudaStream_t s) {
+  const dim3 grid((k + 63) / 64, (n + 63) / 64);
+  wo_dequant_kernel<INT4, OutT><<<grid, 256, 0, s>>>((const int8_t*)w, scale, (OutT*)out, n, k, group_size);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) { set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }
+  return 0;
+}
+template <bool INT4>
+static int dispatch_dequant(const void* w, const float* scale, void* out, int n, int k, int group_size, int out_dtype, cudaStream_t s) {
+  if (out_dtype == kBF16) return launch_dequant<INT4, __nv_bfloat16>(w, scale, out, n, k, group_size, s);
+  if (out_dtype == kF16) return launch_dequant<INT4, __half>(w, scale, out, n, k, group_size, s);
+  if (out_dtype == kF32) return launch_dequant<INT4, float>(w, scale, out, n, k, group_size, s);
+  return 1;
 }
 
 }  // namespace wo
 
+int weight_dequantize(const void* w, const float* scale, void* out, int n, int k, int int4, int group_size, int out_dtype, cudaStream_t s) {
+  using namespace wo;
+  if (n <= 0 || k <= 0 || (int4 && k % 2) || (group_size > 0 && k % group_size) || (n + 63) / 64 > 65535) return 1;
+  return int4 ? dispatch_dequant<true>(w, scale, out, n, k, group_size, out_dtype, s)
+              : dispatch_dequant<false>(w, scale, out, n, k, group_size, out_dtype, s);
+}
+
 int gemm_weight_only(const WoGemmArgs& g, cudaStream_t s) {
   using namespace wo;
   if (g.k % 64 || g.n % 8 || g.m <= 0 || g.m > 64) return 1;      // larger batches: dequantise once + the bf16 GEMM (nn/quant.py)
+  if (g.group_size > 0 && ((g.group_size != 64 && g.group_size != 128) || g.k % g.group_size)) return 1;
   if ((reinterpret_cast<uintptr_t>(g.x) | reinterpret_cast<uintptr_t>(g.w) | reinterpret_cast<uintptr_t>(g.out)) & 15) return 1;
   CUtensorMap mw;
   const int row_bytes = g.int4 ? g.k / 2 : g.k;
   if (!make_w_map(&mw, g.w, g.n, row_bytes)) return 2;
-  if (g.int4) return g.bf16 ? dispatch_tok<true, true>(g, mw, s) : dispatch_tok<true, false>(g, mw, s);
-  return g.bf16 ? dispatch_tok<false, true>(g, mw, s) : dispatch_tok<false, false>(g, mw, s);
+  if (g.int4) return g.bf16 ? dispatch_group<true, true>(g, mw, s) : dispatch_group<true, false>(g, mw, s);
+  return g.bf16 ? dispatch_group<false, true>(g, mw, s) : dispatch_group<false, false>(g, mw, s);
 }
 
 }  // namespace b200

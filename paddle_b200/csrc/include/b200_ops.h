@@ -177,8 +177,12 @@ struct WoGemmArgs {
   const void* x; const void* w; const float* scale; const void* bias; void* out;
   int m, n, k;
   int int4, bf16;   // weight format; activation dtype (1 bf16, 0 fp16)
+  int group_size;   // <= 0: scale [n] per channel; 64 / 128: scale [k / group_size, n]
 };
 int gemm_weight_only(const WoGemmArgs& g, cudaStream_t s);
+// w [n, k] int8 (int4: [n, k / 2], low nibble = even k) -> out [k, n] = float(q) * scale, rounded once to out_dtype (kBF16 / kF16 / kF32).
+// scale fp32: [n] (group_size <= 0) or [k / group_size, n].
+int weight_dequantize(const void* w, const float* scale, void* out, int n, int k, int int4, int group_size, int out_dtype, cudaStream_t s);
 
 // ---- decode_attention.cu --------------------------------------------------------------------------------------
 // Single-token decode attention: q [B,H,128], k/v cache [B,Hkv,S_max,128], lens[b] valid positions; out [B,H,128].

@@ -74,7 +74,7 @@ class GPTBlock(nn.Layer):
         a = KAT.attention(qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2], None, 0.0, True, None)
         x = x + self.proj(_raw(a).reshape(b, s, h).as_subclass(Tensor))
         y = self.ln2(x)
-        y = KG.gemm(_raw(y).reshape(-1, h), self.fc1.weight, self.fc1.bias, epilogue=2).reshape(b, s, -1) if _fused_ok(y) else F.gelu(self.fc1(y))
+        y = KG.gemm(_raw(y).reshape(-1, h), self.fc1.weight, self.fc1.bias, epilogue=2).reshape(b, s, -1) if _fused_ok(y) and isinstance(self.fc1, nn.Linear) else F.gelu(self.fc1(y))
         return x + self.fc2(y if isinstance(y, Tensor) else y.as_subclass(Tensor))
 
     def forward(self, x):

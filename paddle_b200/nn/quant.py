@@ -31,31 +31,51 @@ def weight_quantize(x, algo="weight_only_int8", arch=None, group_size=-1):
     return _w(q), _w(scale.to(x.dtype if x.dtype != torch.float32 else torch.float32))
 
 
-def weight_dequantize(x, scale, algo="weight_only_int8", out_dtype="float16", group_size=-1):
-    from ..framework.dtype import convert_dtype
-
-    q = x.as_subclass(torch.Tensor)
-    if "int4" in algo:
+def _dequantize_torch(q, s, int4, dtype, group_size):
+    """The reference expression: float(q) * float(scale), rounded once to `dtype`.  q [out, in] (int4 packed [out, in / 2]) -> [in, out],
+    contiguous like the CUDA kernel's result and a Linear's weight, so both devices run the same GEMM on it."""
+    if int4:
         lo = (q << 4).to(torch.int8) >> 4
         hi = q >> 4
         q = torch.stack([lo, hi], -1).reshape(q.shape[0], -1)
     w = q.float().t()
-    s = scale.as_subclass(torch.Tensor).float()
+    s = s.float()
     if group_size and group_size > 0:
         w = (w.reshape(-1, group_size, w.shape[1]) * s.unsqueeze(1)).reshape(w.shape)
     else:
         w = w * s
-    return _w(w.to(convert_dtype(out_dtype)))
+    return w.to(dtype).contiguous()
+
+
+def weight_dequantize(x, scale, algo="weight_only_int8", out_dtype="float16", group_size=-1):
+    """x int8 [out, in] (int4: [out, in / 2]) and scale [out] or [in / group_size, out] -> [in, out] in out_dtype.  CUDA weights with a
+    bf16 / fp16 / fp32 output run one kernel (csrc/gemm_wo_sm100.cu: reads the quantised weight once, writes the result once) that gives the
+    same bits as the torch expression, which otherwise expands the weight through fp32 temporaries."""
+    from ..framework.dtype import convert_dtype
+
+    q = x.as_subclass(torch.Tensor)
+    s = scale.as_subclass(torch.Tensor)
+    dtype = convert_dtype(out_dtype)
+    int4 = "int4" in algo
+    if q.is_cuda and s.is_cuda and q.dtype == torch.int8 and q.dim() == 2 and dtype in (torch.bfloat16, torch.float16, torch.float32):
+        from .._build import ext
+
+        gs = int(group_size) if group_size and group_size > 0 else -1
+        return _w(ext().weight_dequantize(q.contiguous(), s.float().contiguous(), int4, gs, dtype))
+    return _w(_dequantize_torch(q, s, int4, dtype, group_size))
 
 
 def weight_only_linear(x, weight, bias=None, weight_scale=None, weight_dtype="int8", arch=None, group_size=-1):
-    """y = x @ dequant(weight)^T + bias.  CUDA bf16 / fp16 activations with per-channel scales run csrc/gemm_wo_sm100.cu: the int8 / int4
-    weights are streamed by TMA and expanded to 16-bit INSIDE the SM (no dequantised copy of the weight is ever written to HBM), which is
-    what makes weight-only decoding faster than the 16-bit GEMM (it is bound by weight bytes).  Grouped scales / CPU: dequantise + linear."""
+    """y = x @ dequant(weight)^T + bias.  CUDA bf16 / fp16 activations with per-channel or group-wise (group_size 64 / 128) scales run
+    csrc/gemm_wo_sm100.cu: the int8 / int4 weights are streamed by TMA and expanded to 16-bit INSIDE the SM (no dequantised copy of the
+    weight is ever written to HBM), which is what makes weight-only decoding faster than the 16-bit GEMM (it is bound by weight bytes).
+    More than 64 rows: one dequantisation kernel + the 16-bit GEMM.  Other group sizes / CPU: dequantise + linear."""
     xr = x.as_subclass(torch.Tensor)
     wr = weight.as_subclass(torch.Tensor)
-    if xr.is_cuda and xr.dtype in (torch.bfloat16, torch.float16) and weight_scale is not None and (group_size is None or group_size <= 0) \
-            and weight_dtype in ("int8", "int4") and wr.dtype == torch.int8 and xr.shape[-1] % 64 == 0 and wr.shape[0] % 8 == 0:
+    per_channel = group_size is None or group_size <= 0
+    if xr.is_cuda and xr.dtype in (torch.bfloat16, torch.float16) and weight_scale is not None and (per_channel or group_size in (64, 128)) \
+            and weight_dtype in ("int8", "int4") and wr.dtype == torch.int8 and xr.shape[-1] % (64 if per_channel else max(64, group_size)) == 0 \
+            and wr.shape[0] % 8 == 0:
         from ..framework.flags import flag
 
         if flag("FLAGS_use_fused_kernels", True):
@@ -71,7 +91,7 @@ def weight_only_linear(x, weight, bias=None, weight_scale=None, weight_dtype="in
                 return F.linear(x, w, bias)
             sc = weight_scale.as_subclass(torch.Tensor).float().contiguous()
             b = None if bias is None else bias.as_subclass(torch.Tensor).to(xr.dtype).contiguous()
-            y = ext().weight_only_gemm(x2, wr.contiguous(), sc, b, weight_dtype == "int4")
+            y = ext().weight_only_gemm(x2, wr.contiguous(), sc, b, weight_dtype == "int4", -1 if per_channel else int(group_size))
             return _w(y.reshape(*xr.shape[:-1], wr.shape[0]))
     w = weight_dequantize(weight, weight_scale, "weight_only_" + weight_dtype, x.dtype, group_size)
     from . import functional as F
