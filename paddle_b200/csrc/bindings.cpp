@@ -658,6 +658,102 @@ Tensor weight_dequantize(const Tensor& w, const Tensor& scale, bool int4, int64_
   return out;
 }
 
+// ---- weight-only MoE experts.  Failing checks use literal messages only (see weight_only_gemm).
+// expert ids of the token slots ([S] int64, -1 = dropped) -> (dest int32 [S], offsets int32 [E + 1], work int32 [1 + 2 * items]): the
+// compact plan of weight_only_gemm_experts for S rows.  Three launches (count, plan, dest), no host read.
+std::vector<Tensor> moe_wo_plan(const Tensor& idx, int64_t n_expert) {
+  check_i64(idx, "moe_wo_plan");
+  TORCH_CHECK(n_expert > 0 && n_expert <= 1024, "moe_wo_plan: 1 to 1024 experts");
+  TORCH_CHECK(idx.numel() > 0 && idx.numel() < (int64_t)1 << 30, "moe_wo_plan: bad slot count");
+  c10::cuda::CUDAGuard guard(idx.device());
+  const int m = (int)idx.numel(), ntok = b200::wo_expert_ntok(m);
+  auto i32 = idx.options().dtype(at::kInt);
+  Tensor counts = torch::zeros({n_expert}, idx.options());
+  Tensor dest = torch::empty({m}, i32), offsets = torch::empty({n_expert + 1}, i32), cursor = torch::empty({n_expert}, i32);
+  Tensor work = torch::empty({1 + 2 * (int64_t)b200::wo_expert_items(m, (int)n_expert, ntok)}, i32);
+  auto st = cur_stream();
+  b200::moe_number_count(idx.data_ptr<int64_t>(), m, counts.data_ptr<int64_t>(), (int)n_expert, st);
+  b200::moe_wo_plan(counts.data_ptr<int64_t>(), (int)n_expert, ntok, offsets.data_ptr<int>(), cursor.data_ptr<int>(), work.data_ptr<int>(), st);
+  b200::moe_dest(idx.data_ptr<int64_t>(), m, cursor.data_ptr<int>(), dest.data_ptr<int>(), st);
+  g_launches += 3; check_err();
+  return {dest, offsets, work};
+}
+
+// xp [R, K] bf16 / fp16 (routed rows grouped by expert), w int8 [E, N, K] (int4 [E, N, K/2]), scale fp32 [E, N] or [E, K / group_size, N],
+// bias [E, N] in xp's dtype or None, offsets / work from moe_wo_plan over R slots -> out [R, N]; rows past offsets[E] are left unwritten
+Tensor weight_only_gemm_experts(const Tensor& xp, const Tensor& w, const Tensor& scale, const OptT& bias, const Tensor& offsets, const Tensor& work,
+                                bool int4, int64_t group_size) {
+  TORCH_CHECK(xp.is_cuda() && xp.dim() == 2 && xp.is_contiguous() && (xp.scalar_type() == at::kBFloat16 || xp.scalar_type() == at::kHalf),
+              "weight_only_gemm_experts: xp [R, K] bf16 / fp16 contiguous");
+  TORCH_CHECK(w.is_cuda() && w.dim() == 3 && w.is_contiguous() && w.scalar_type() == at::kChar && w.size(2) == (int4 ? xp.size(1) / 2 : xp.size(1)),
+              "weight_only_gemm_experts: w int8 [E, N, K] (int4: [E, N, K/2]) contiguous");
+  const int64_t E = w.size(0), N = w.size(1), K = xp.size(1);
+  TORCH_CHECK(E > 0 && E <= 1024 && N > 0 && K < (int64_t)1 << 30 && N < (int64_t)1 << 30 && xp.size(0) > 0 && xp.size(0) < (int64_t)1 << 30,
+              "weight_only_gemm_experts: dimensions out of range");
+  if (group_size <= 0) {
+    TORCH_CHECK(scale.is_cuda() && scale.scalar_type() == at::kFloat && scale.dim() == 2 && scale.size(0) == E && scale.size(1) == N && scale.is_contiguous(),
+                "weight_only_gemm_experts: scale float32 [E, N] contiguous");
+  } else {
+    TORCH_CHECK(group_size == 64 || group_size == 128, "weight_only_gemm_experts: group_size must be -1, 64 or 128");
+    TORCH_CHECK(K % group_size == 0, "weight_only_gemm_experts: K is not a multiple of group_size");
+    TORCH_CHECK(scale.is_cuda() && scale.scalar_type() == at::kFloat && scale.dim() == 3 && scale.size(0) == E && scale.size(1) == K / group_size &&
+                scale.size(2) == N && scale.is_contiguous(), "weight_only_gemm_experts: scale float32 [E, K / group_size, N] contiguous");
+  }
+  const int m = (int)xp.size(0), ntok = b200::wo_expert_ntok(m);
+  TORCH_CHECK(offsets.is_cuda() && offsets.scalar_type() == at::kInt && offsets.is_contiguous() && offsets.numel() == E + 1,
+              "weight_only_gemm_experts: offsets int32 [E + 1] from moe_wo_plan");
+  TORCH_CHECK(work.is_cuda() && work.scalar_type() == at::kInt && work.is_contiguous() && work.numel() == 1 + 2 * (int64_t)b200::wo_expert_items(m, (int)E, ntok),
+              "weight_only_gemm_experts: work must come from moe_wo_plan over the rows of xp");
+  TORCH_CHECK(w.device() == xp.device() && scale.device() == xp.device() && offsets.device() == xp.device() && work.device() == xp.device(),
+              "weight_only_gemm_experts: all operands on one device");
+  c10::cuda::CUDAGuard guard(xp.device());
+  b200::WoExpertGemmArgs g;
+  g.m = m; g.n = (int)N; g.k = (int)K; g.experts = (int)E; g.ntok = ntok;
+  Tensor out = torch::empty({m, N}, xp.options());
+  g.x = xp.data_ptr(); g.w = w.data_ptr(); g.scale = scale.data_ptr<float>(); g.out = out.data_ptr();
+  g.offsets = offsets.data_ptr<int>(); g.work = work.data_ptr<int>();
+  g.bias = nullptr;
+  if (bias.has_value() && bias->defined()) {
+    TORCH_CHECK(bias->is_cuda() && bias->scalar_type() == xp.scalar_type() && bias->numel() == E * N && bias->is_contiguous(),
+                "weight_only_gemm_experts: bias [E, N] in xp dtype contiguous");
+    g.bias = bias->data_ptr();
+  }
+  g.int4 = int4 ? 1 : 0; g.bf16 = xp.scalar_type() == at::kBFloat16 ? 1 : 0;
+  g.group_size = group_size > 0 ? (int)group_size : 0;
+  int rc = b200::gemm_weight_only_experts(g, cur_stream());
+  g_launches += 1;
+  check_err();
+  TORCH_CHECK(rc == 0, "paddle_b200.weight_only_gemm_experts: unsupported shape (K multiple of 64, N multiple of 8, 16-byte aligned)");
+  return out;
+}
+
+// w int8 [E, N, K] (int4 [E, N, K/2]), scale fp32 [E, N] or [E, K / group_size, N] -> [E, K, N] in out_dtype; one launch for all experts,
+// every expert bit-equal to weight_dequantize of its slice
+Tensor weight_dequantize_experts(const Tensor& w, const Tensor& scale, bool int4, int64_t group_size, at::ScalarType out_dtype) {
+  TORCH_CHECK(w.is_cuda() && w.dim() == 3 && w.is_contiguous() && w.scalar_type() == at::kChar && w.numel() > 0,
+              "weight_dequantize_experts: w int8 [E, N, K] (int4: [E, N, K/2]) contiguous");
+  TORCH_CHECK(out_dtype == at::kBFloat16 || out_dtype == at::kHalf || out_dtype == at::kFloat, "weight_dequantize_experts: out_dtype bf16 / fp16 / fp32");
+  const int64_t E = w.size(0), n = w.size(1), k = int4 ? 2 * w.size(2) : w.size(2);
+  TORCH_CHECK(E <= 65535 && n < (int64_t)1 << 31 && k < (int64_t)1 << 31, "weight_dequantize_experts: dimensions too large");
+  if (group_size <= 0) {
+    TORCH_CHECK(scale.is_cuda() && scale.scalar_type() == at::kFloat && scale.dim() == 2 && scale.size(0) == E && scale.size(1) == n && scale.is_contiguous(),
+                "weight_dequantize_experts: scale float32 [E, N] contiguous");
+  } else {
+    TORCH_CHECK(k % group_size == 0, "weight_dequantize_experts: K is not a multiple of group_size");
+    TORCH_CHECK(scale.is_cuda() && scale.scalar_type() == at::kFloat && scale.dim() == 3 && scale.size(0) == E && scale.size(1) == k / group_size &&
+                scale.size(2) == n && scale.is_contiguous(), "weight_dequantize_experts: scale float32 [E, K / group_size, N] contiguous");
+  }
+  TORCH_CHECK(scale.device() == w.device(), "weight_dequantize_experts: w and scale on one device");
+  c10::cuda::CUDAGuard guard(w.device());
+  Tensor out = torch::empty({E, k, n}, w.options().dtype(out_dtype));
+  int rc = b200::weight_dequantize(w.data_ptr(), scale.data_ptr<float>(), out.data_ptr(), (int)n, (int)k, int4 ? 1 : 0, group_size > 0 ? (int)group_size : 0,
+                                   dt_code(out_dtype), cur_stream(), (int)E);
+  g_launches += 1;
+  check_err();
+  TORCH_CHECK(rc == 0, "paddle_b200.weight_dequantize_experts: unsupported shape");
+  return out;
+}
+
 // D = act(scale * A[M,K] @ B[N,K]^T + bias), A/B fp8 (e4m3 / e5m2), D half / bf16 / fp32
 // (q [M,K] fp8, qT [K,M] fp8 or undefined, inv_scale float[1]) of a 2-D bf16 / fp16 / fp32 tensor; two launches, no host sync
 std::vector<Tensor> quantize_fp8(const Tensor& x, bool e5m2, bool want_transpose) {
@@ -1337,6 +1433,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         pybind11::arg("int4") = false, pybind11::arg("group_size") = -1);
   m.def("weight_dequantize", traced("weight_dequantize", &weight_dequantize), pybind11::arg("w"), pybind11::arg("scale"), pybind11::arg("int4") = false,
         pybind11::arg("group_size") = -1, pybind11::arg("out_dtype") = at::kBFloat16);
+  m.def("moe_wo_plan", traced("moe_wo_plan", &moe_wo_plan));
+  m.def("weight_only_gemm_experts", traced("weight_only_gemm_experts", &weight_only_gemm_experts), pybind11::arg("xp"), pybind11::arg("w"),
+        pybind11::arg("scale"), pybind11::arg("bias"), pybind11::arg("offsets"), pybind11::arg("work"), pybind11::arg("int4") = false,
+        pybind11::arg("group_size") = -1);
+  m.def("weight_dequantize_experts", traced("weight_dequantize_experts", &weight_dequantize_experts), pybind11::arg("w"), pybind11::arg("scale"),
+        pybind11::arg("int4") = false, pybind11::arg("group_size") = -1, pybind11::arg("out_dtype") = at::kBFloat16);
   m.def("gemm_grouped", traced("gemm_grouped", &gemm_grouped), pybind11::arg("a"), pybind11::arg("b"), pybind11::arg("tile_expert"), pybind11::arg("b_is_nk") = false,
         pybind11::arg("out") = pybind11::none());
   m.def("gemm_grouped_wgrad", traced("gemm_grouped_wgrad", &gemm_grouped_wgrad));

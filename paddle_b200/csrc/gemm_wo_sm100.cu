@@ -279,6 +279,215 @@ wo_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant_
   }
 }
 
+// ------------------------------------------------------------------------------------------------ MoE experts
+// out[R, N] = xp[R, K] @ dequant(Wq[e])^T (+ bias[e]) where e owns the row: xp holds the routed slots grouped by expert without padding
+// (rows offsets[e] .. offsets[e + 1]).  Each blockIdx.z takes one item of a device-built work list of (expert, first row) pairs, one per
+// NTOK-row tile of an expert (moe_wo_plan); the grid's z extent is a static bound and CTAs past the real item count exit before anything
+// else.  A cluster's CTAs share blockIdx.z, so they exit together or all reach cluster_sync.  Only selected experts' weights, scales and
+// bias are ever read.  Rows of a tile past its expert's last row hold other experts' rows or TMA zero fill: they are computed (every
+// token is its own accumulator column) and masked by the epilogue and the split-K reduction.
+//
+// The mainloop is the dense kernel's (raw-box ring, dequantisation into the A fragment, group accumulator fold, cluster split-K), kept as
+// a separate kernel so the dense instantiations' instructions stay exactly as they are.
+struct ExpertParams {
+  int m, n, k;                 // rows of xp, output channels, reduction
+  int kb_per_split;
+  const float* scale;          // [E, n] or [E, k / GS, n]
+  const void* bias;            // [E, n] activation dtype or nullptr
+  void* out;                   // [m, n]
+  int splits;
+  const int* offsets;          // [E + 1] first row of every expert
+  const int* work;             // [0]: item count, then (expert, first row) pairs
+};
+
+template <int NTOK, int WST, bool INT4, bool BF16, int GS>
+__global__ void __launch_bounds__(kThreads, 1)
+wo_expert_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_x, const ExpertParams p) {
+  if ((int)blockIdx.z >= __ldg(p.work)) return;             // uniform over the cluster: every rank has the same blockIdx.z
+  constexpr int KB_PER_W = INT4 ? 4 : 2;
+  constexpr int KB_PER_G = GS ? GS / BLOCK_K : 1;
+  constexpr int G_PER_W = GS ? KB_PER_W / KB_PER_G : 1;
+  static_assert(GS == 0 || (GS % BLOCK_K == 0 && KB_PER_W % KB_PER_G == 0), "weight-only gemm: a raw box holds whole scale groups");
+  constexpr uint32_t X_BYTES = NTOK * BLOCK_K * 2;
+  constexpr uint32_t STAGE_BYTES = W_BYTES + KB_PER_W * X_BYTES;
+  static_assert(NTOK * 512 <= WST * STAGE_BYTES, "weight-only gemm: the split-K partial tile is staged in the ring");
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t bars = base + WST * STAGE_BYTES;
+  auto full = [&](int s) { return bars + 8u * s; };
+  auto empty = [&](int s) { return bars + 8u * (WST + s); };
+
+  const int expert = __ldg(p.work + 1 + 2 * blockIdx.z);
+  const int tok0 = __ldg(p.work + 2 + 2 * blockIdx.z);      // first row of this tile in xp / out
+  const int row_end = __ldg(p.offsets + expert + 1);        // rows [tok0, row_end) of the tile belong to `expert`
+  const float* scale = p.scale + (int64_t)expert * (GS ? p.k / GS : 1) * p.n;
+  const void* bias = p.bias ? (const void*)((const uint16_t*)p.bias + (int64_t)expert * p.n) : nullptr;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int n0 = blockIdx.x * BLOCK_N;
+  const int num_kb_total = (p.k + BLOCK_K - 1) / BLOCK_K;
+  const int kb0 = blockIdx.y * p.kb_per_split;
+  const int num_kb = max(0, min(p.kb_per_split, num_kb_total - kb0));
+  const int num_box = (num_kb + KB_PER_W - 1) / KB_PER_W;
+
+  if (warp == 8 && lane == 0) {
+    tma_prefetch_desc(&map_w);
+    tma_prefetch_desc(&map_x);
+    for (int s = 0; s < WST; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 8); }
+    fence_barrier_init();
+    fence_proxy_async();
+  }
+  __syncthreads();
+
+  if (warp == 8) {
+    if (lane == 0) {
+      for (int j = 0; j < num_box; ++j) {
+        const int st = j % WST;
+        const int nvalid = min(KB_PER_W, num_kb - j * KB_PER_W);
+        mbar_wait(empty(st), ((j / WST) & 1) ^ 1);
+        mbar_expect_tx(full(st), W_BYTES + nvalid * X_BYTES);
+        const uint32_t sw = base + st * STAGE_BYTES;
+        tma_load_3d(sw, &map_w, full(st), (kb0 + j * KB_PER_W) * (INT4 ? BLOCK_K / 2 : BLOCK_K), n0, expert);
+        for (int sub = 0; sub < nvalid; ++sub)
+          tma_load_3d(sw + W_BYTES + sub * X_BYTES, &map_x, full(st), (kb0 + j * KB_PER_W + sub) * BLOCK_K, tok0, 0);
+      }
+    }
+  } else {
+    const int wg = warp >> 2, q = lane & 3;
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    float acc[NTOK / 2], acc_g[NTOK / 2];
+#pragma unroll
+    for (int i = 0; i < NTOK / 2; ++i) acc[i] = acc_g[i] = 0.f;
+    for (int j = 0; j < num_box; ++j) {
+      const int st = j % WST;
+      const int nvalid = min(KB_PER_W, num_kb - j * KB_PER_W);
+      float gsc[G_PER_W][2];
+      if constexpr (GS > 0) {
+        const int g0 = (kb0 + j * KB_PER_W) / KB_PER_G;
+#pragma unroll
+        for (int gi = 0; gi < G_PER_W; ++gi)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int g = g0 + gi, ch = n0 + r0 + h * 8;
+            gsc[gi][h] = (g * GS < p.k && ch < p.n) ? __ldg(scale + (int64_t)g * p.n + ch) : 0.f;
+          }
+      }
+      mbar_wait(full(st), (j / WST) & 1);
+      const uint32_t sw = base + st * STAGE_BYTES;
+      const uint32_t row0 = sw + r0 * 128, row1 = row0 + 8 * 128;
+      const uint32_t sx = r0 & 7;
+#pragma unroll
+      for (int sub = 0; sub < KB_PER_W; ++sub) {
+        if (sub < nvalid) {
+          uint32_t a[4][4];
+#pragma unroll
+          for (int s = 0; s < 4; ++s) {
+            if constexpr (!INT4) {
+              const uint32_t off = (((uint32_t)(sub * 4 + s) ^ sx) << 4) + 2 * q;
+              a[s][0] = dequant_pair<false, BF16>(ld_shared_u16(row0 + off));
+              a[s][1] = dequant_pair<false, BF16>(ld_shared_u16(row1 + off));
+              a[s][2] = dequant_pair<false, BF16>(ld_shared_u16(row0 + off + 8));
+              a[s][3] = dequant_pair<false, BF16>(ld_shared_u16(row1 + off + 8));
+            } else {
+              const uint32_t off = (((uint32_t)(sub * 2 + (s >> 1)) ^ sx) << 4) + (s & 1) * 8 + q;
+              a[s][0] = dequant_pair<true, BF16>(ld_shared_u8(row0 + off));
+              a[s][1] = dequant_pair<true, BF16>(ld_shared_u8(row1 + off));
+              a[s][2] = dequant_pair<true, BF16>(ld_shared_u8(row0 + off + 4));
+              a[s][3] = dequant_pair<true, BF16>(ld_shared_u8(row1 + off + 4));
+            }
+          }
+          const uint32_t xs = sw + W_BYTES + sub * X_BYTES;
+          if constexpr (GS == 0) wgmma_fence_regs(acc);
+          else wgmma_fence_regs(acc_g);
+          wgmma_fence();
+#pragma unroll
+          for (int s = 0; s < 4; ++s) {
+            const uint64_t bdesc = make_smem_desc(xs + s * 32, 16, 1024);
+            const uint32_t accumulate = (GS && s == 0 && sub % KB_PER_G == 0) ? 0u : 1u;
+            if constexpr (GS == 0) {
+              if constexpr (NTOK == 16) wgmma_rs_n16<BF16, 0>(acc, a[s], bdesc, accumulate);
+              else wgmma_rs_n64<BF16, 0>(acc, a[s], bdesc, accumulate);
+            } else {
+              if constexpr (NTOK == 16) wgmma_rs_n16<BF16, 0>(acc_g, a[s], bdesc, accumulate);
+              else wgmma_rs_n64<BF16, 0>(acc_g, a[s], bdesc, accumulate);
+            }
+          }
+          wgmma_commit();
+          wgmma_wait<0>();
+          if constexpr (GS == 0) wgmma_fence_regs(acc);
+          else wgmma_fence_regs(acc_g);
+#pragma unroll
+          for (int s = 0; s < 4; ++s) keep_regs(a[s]);
+          if constexpr (GS > 0) {
+            if (sub % KB_PER_G == KB_PER_G - 1) {
+#pragma unroll
+              for (int i = 0; i < NTOK / 2; ++i) acc[i] = fmaf(acc_g[i], gsc[sub / KB_PER_G][(i >> 1) & 1], acc[i]);
+            }
+          }
+        }
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty(st));
+    }
+    if (p.splits > 1) {
+      named_bar_sync(1, 256);
+#pragma unroll
+      for (int jn = 0; jn < NTOK / 8; ++jn)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int tok = jn * 8 + 2 * q + (e & 1), chl = r0 + (e >> 1) * 8;
+          asm volatile("st.shared.f32 [%0], %1;" ::"r"(base + (uint32_t)((tok * BLOCK_N + chl) * 4)), "f"(acc[jn * 4 + e]) : "memory");
+        }
+    } else {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int ch = n0 + r0 + h * 8;
+        if (ch >= p.n) continue;
+        const float sc = GS ? 1.f : scale[ch];
+        float bv = 0.f;
+        if (bias) bv = BF16 ? __bfloat162float(((const __nv_bfloat16*)bias)[ch]) : __half2float(((const __half*)bias)[ch]);
+#pragma unroll
+        for (int jn = 0; jn < NTOK / 8; ++jn)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int tok = tok0 + jn * 8 + 2 * q + e;
+            if (tok >= row_end) continue;
+            const float y = GS ? acc[jn * 4 + h * 2 + e] + bv : acc[jn * 4 + h * 2 + e] * sc + bv;
+            if constexpr (BF16) ((__nv_bfloat16*)p.out)[(int64_t)tok * p.n + ch] = __float2bfloat16_rn(y);
+            else ((__half*)p.out)[(int64_t)tok * p.n + ch] = __float2half_rn(y);
+          }
+      }
+    }
+  }
+  if (p.splits > 1) {
+    cluster_sync();
+    if (warp >= 4 && warp < 8) {
+      uint32_t rank;
+      asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(rank));
+      const int tok_n = min(NTOK, row_end - tok0);
+      for (int c = (int)rank * 4 + (warp - 4); c < tok_n * 4; c += p.splits * 4) {
+        const int tok = c >> 2, chl = (c & 3) * 32 + lane, ch = n0 + chl;
+        float acc = 0.f;
+        const uint32_t local = base + (uint32_t)((tok * BLOCK_N + chl) * 4);
+        for (int qq = 0; qq < p.splits; ++qq) {
+          uint32_t remote;
+          float v;
+          asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(local), "r"(qq));
+          asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(remote) : "memory");
+          acc += v;
+        }
+        if (ch < p.n) {
+          float y = GS ? acc : acc * scale[ch];
+          if (bias) y += BF16 ? __bfloat162float(((const __nv_bfloat16*)bias)[ch]) : __half2float(((const __half*)bias)[ch]);
+          if constexpr (BF16) ((__nv_bfloat16*)p.out)[(int64_t)(tok0 + tok) * p.n + ch] = __float2bfloat16_rn(y);
+          else ((__half*)p.out)[(int64_t)(tok0 + tok) * p.n + ch] = __float2half_rn(y);
+        }
+      }
+    }
+    cluster_sync();
+  }
+}
+
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -307,41 +516,29 @@ static bool make_w_map(CUtensorMap* out, const void* w, int n, int row_bytes) {
   return true;
 }
 
-template <int NTOK, int WST, bool INT4, bool BF16, int GS>
-static int launch(const WoGemmArgs& g, const CUtensorMap& mw, cudaStream_t s) {
-  constexpr int KB_PER_W = INT4 ? 4 : 2;
-  constexpr uint32_t SMEM = WST * (W_BYTES + KB_PER_W * NTOK * BLOCK_K * 2) + 1024 + 256;
-  static_assert(SMEM <= 232448, "weight-only gemm: shared memory budget");
-  static_assert(8 * 2 * WST <= 256, "weight-only gemm: barrier area");
-  constexpr int kMaxSplits = 8;                 // portable cluster size
-  CUtensorMap mx;
-  if (!gemm::make_map(&mx, g.x, g.k, g.m, 1, g.k, 0, BLOCK_K, NTOK, g.bf16 ? kBF16 : kF16)) return 2;
-  auto kern = wo_gemm_kernel<NTOK, WST, INT4, BF16, GS>;
-  static bool attr_set = false;
-  static int wave_ctas[kMaxSplits + 1];         // CTAs the device holds at once when they come in clusters of `splits`
-  if (!attr_set) {
-    B200_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    for (int c = 1; c <= kMaxSplits; ++c) {
-      cudaLaunchConfig_t cfg = {};
-      cfg.gridDim = dim3(1, c, 1); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = SMEM;
-      cudaLaunchAttribute at[1];
-      at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = 1; at[0].val.clusterDim.y = c; at[0].val.clusterDim.z = 1;
-      cfg.attrs = at; cfg.numAttrs = 1;
-      int n_clusters = 0;
-      if (cudaOccupancyMaxActiveClusters(&n_clusters, kern, &cfg) != cudaSuccess) { cudaGetLastError(); n_clusters = 0; }
-      wave_ctas[c] = n_clusters * c;
-    }
-    if (wave_ctas[1] <= 0) wave_ctas[1] = sm_count();
-    attr_set = true;
-  }
-  Params p;
-  p.m = g.m; p.n = g.n; p.k = g.k;
-  const int num_kb = (g.k + BLOCK_K - 1) / BLOCK_K;
-  const int n_tiles = (g.n + BLOCK_N - 1) / BLOCK_N, t_tiles = (g.m + NTOK - 1) / NTOK;
-  // Split-K (a cluster of `splits` CTAs per output tile) when the output tiles alone leave SMs idle or the last wave ragged.  Cost in
-  // k-block units: waves x (k-blocks per CTA + fixed prologue / epilogue) + the cluster reduction.
-  const int ctas = n_tiles * t_tiles;
-  int splits = 1, kb_per = (num_kb + 3) / 4 * 4;
+// raw stacked expert weights as bytes: [experts, n rows, row_bytes], box {128 bytes, 128 rows, 1 expert}: the same shared-memory layout as
+// make_w_map, and a partial channel tile is zero filled instead of reading the next expert's rows
+static bool make_w_map_experts(CUtensorMap* out, const void* w, int experts, int n, int row_bytes) {
+  bind_primary_context();
+  EncodeTiledFn enc = get_encode();
+  if (!enc) { set_last_error(__FILE__, __LINE__, "cuTensorMapEncodeTiled unavailable"); return false; }
+  cuuint64_t dims[3] = {(cuuint64_t)row_bytes, (cuuint64_t)n, (cuuint64_t)experts};
+  cuuint64_t strides[2] = {(cuuint64_t)row_bytes, (cuuint64_t)row_bytes * n};
+  cuuint32_t box[3] = {128u, (cuuint32_t)BLOCK_N, 1u};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<void*>(w), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { set_last_error(__FILE__, __LINE__, "weight-only expert gemm: cuTensorMapEncodeTiled failed"); return false; }
+  return true;
+}
+
+constexpr int kMaxSplits = 8;                   // portable cluster size
+
+// Split-K (a cluster of `splits` CTAs per output tile) when the output tiles alone leave SMs idle or the last wave ragged.  Cost in
+// k-block units: waves x (k-blocks per CTA + fixed prologue / epilogue) + the cluster reduction.  wave_ctas[c]: CTAs the device holds at
+// once when they come in clusters of c.
+static void choose_splits(const int* wave_ctas, int num_kb, int ctas, int* splits, int* kb_per) {
+  *splits = 1; *kb_per = (num_kb + 3) / 4 * 4;
   long best = -1;
   for (int c = 1; c <= kMaxSplits; ++c) {
     if (wave_ctas[c] <= 0) continue;
@@ -349,22 +546,94 @@ static int launch(const WoGemmArgs& g, const CUtensorMap& mw, cudaStream_t s) {
     if (c > 1 && (c - 1) * per >= num_kb) continue;               // every rank of the cluster gets work
     const long waves = ((long)ctas * c + wave_ctas[c] - 1) / wave_ctas[c];
     const long cost = waves * (per + 24) + (c > 1 ? 6 : 0);
-    if (best < 0 || cost < best) { best = cost; splits = c; kb_per = per; }
+    if (best < 0 || cost < best) { best = cost; *splits = c; *kb_per = per; }
   }
+}
+
+// Once per kernel: the dynamic shared memory attribute and wave_ctas[c] for cluster sizes 1 .. kMaxSplits.
+template <typename Kern>
+static void init_kernel(Kern kern, uint32_t smem, int* wave_ctas) {
+  B200_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  for (int c = 1; c <= kMaxSplits; ++c) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(1, c, 1); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = smem;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = 1; at[0].val.clusterDim.y = c; at[0].val.clusterDim.z = 1;
+    cfg.attrs = at; cfg.numAttrs = 1;
+    int n_clusters = 0;
+    if (cudaOccupancyMaxActiveClusters(&n_clusters, kern, &cfg) != cudaSuccess) { cudaGetLastError(); n_clusters = 0; }
+    wave_ctas[c] = n_clusters * c;
+  }
+  if (wave_ctas[1] <= 0) wave_ctas[1] = sm_count();
+}
+
+template <typename Kern, typename P>
+static int launch_cluster(Kern kern, dim3 grid, uint32_t smem, cudaStream_t s, const CUtensorMap& mw, const CUtensorMap& mx, const P& p) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid; cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = smem; cfg.stream = s;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = 1; at[0].val.clusterDim.y = grid.y; at[0].val.clusterDim.z = 1;
+  cfg.attrs = at; cfg.numAttrs = 1;
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, mw, mx, p);
+  if (e != cudaSuccess) { cudaGetLastError(); set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }
+  return 0;
+}
+
+template <int NTOK, int WST, bool INT4>
+constexpr uint32_t smem_bytes() { return WST * (W_BYTES + (INT4 ? 4 : 2) * NTOK * BLOCK_K * 2) + 1024 + 256; }
+
+template <int NTOK, int WST, bool INT4, bool BF16, int GS>
+static int launch(const WoGemmArgs& g, const CUtensorMap& mw, cudaStream_t s) {
+  constexpr uint32_t SMEM = smem_bytes<NTOK, WST, INT4>();
+  static_assert(SMEM <= 232448, "weight-only gemm: shared memory budget");
+  static_assert(8 * 2 * WST <= 256, "weight-only gemm: barrier area");
+  CUtensorMap mx;
+  if (!gemm::make_map(&mx, g.x, g.k, g.m, 1, g.k, 0, BLOCK_K, NTOK, g.bf16 ? kBF16 : kF16)) return 2;
+  auto kern = wo_gemm_kernel<NTOK, WST, INT4, BF16, GS>;
+  static bool attr_set = false;
+  static int wave_ctas[kMaxSplits + 1];
+  if (!attr_set) { init_kernel(kern, SMEM, wave_ctas); attr_set = true; }
+  Params p;
+  p.m = g.m; p.n = g.n; p.k = g.k;
+  const int num_kb = (g.k + BLOCK_K - 1) / BLOCK_K;
+  const int n_tiles = (g.n + BLOCK_N - 1) / BLOCK_N, t_tiles = (g.m + NTOK - 1) / NTOK;
+  int splits, kb_per;
+  choose_splits(wave_ctas, num_kb, n_tiles * t_tiles, &splits, &kb_per);
   if constexpr (GS > 0) {                                         // the kernel folds whole groups: no split may cut one
     if ((kb_per * BLOCK_K) % GS) { set_last_error(__FILE__, __LINE__, "weight-only gemm: split boundary inside a scale group"); return 3; }
   }
   p.splits = splits;
   p.kb_per_split = kb_per;
   p.scale = g.scale; p.bias = g.bias; p.out = g.out;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(n_tiles, splits, t_tiles); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = SMEM; cfg.stream = s;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = 1; at[0].val.clusterDim.y = splits; at[0].val.clusterDim.z = 1;
-  cfg.attrs = at; cfg.numAttrs = 1;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, mw, mx, p);
-  if (e != cudaSuccess) { cudaGetLastError(); set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }
-  return 0;
+  return launch_cluster(kern, dim3(n_tiles, splits, t_tiles), SMEM, s, mw, mx, p);
+}
+
+// The expert kernel's grid: z = the static work-item bound (g.m / NTOK + min(E, g.m)), the split choice costed on that bound.
+template <int NTOK, int WST, bool INT4, bool BF16, int GS>
+static int launch_experts(const WoExpertGemmArgs& g, const CUtensorMap& mw, cudaStream_t s) {
+  constexpr uint32_t SMEM = smem_bytes<NTOK, WST, INT4>();
+  static_assert(SMEM <= 232448, "weight-only gemm: shared memory budget");
+  static_assert(8 * 2 * WST <= 256, "weight-only gemm: barrier area");
+  CUtensorMap mx;
+  if (!gemm::make_map(&mx, g.x, g.k, g.m, 1, g.k, 0, BLOCK_K, NTOK, g.bf16 ? kBF16 : kF16)) return 2;
+  auto kern = wo_expert_gemm_kernel<NTOK, WST, INT4, BF16, GS>;
+  static bool attr_set = false;
+  static int wave_ctas[kMaxSplits + 1];
+  if (!attr_set) { init_kernel(kern, SMEM, wave_ctas); attr_set = true; }
+  const int num_kb = (g.k + BLOCK_K - 1) / BLOCK_K;
+  const int n_tiles = (g.n + BLOCK_N - 1) / BLOCK_N, items = wo_expert_items(g.m, g.experts, NTOK);
+  if (items > 65535) { set_last_error(__FILE__, __LINE__, "weight-only expert gemm: too many token tiles"); return 1; }
+  int splits, kb_per;
+  choose_splits(wave_ctas, num_kb, n_tiles * items, &splits, &kb_per);
+  if constexpr (GS > 0) {
+    if ((kb_per * BLOCK_K) % GS) { set_last_error(__FILE__, __LINE__, "weight-only gemm: split boundary inside a scale group"); return 3; }
+  }
+  ExpertParams p;
+  p.m = g.m; p.n = g.n; p.k = g.k;
+  p.kb_per_split = kb_per; p.splits = splits;
+  p.scale = g.scale; p.bias = g.bias; p.out = g.out;
+  p.offsets = g.offsets; p.work = g.work;
+  return launch_cluster(kern, dim3(n_tiles, splits, items), SMEM, s, mw, mx, p);
 }
 
 template <bool INT4, bool BF16, int GS>
@@ -378,15 +647,29 @@ static int dispatch_group(const WoGemmArgs& g, const CUtensorMap& mw, cudaStream
   if (g.group_size == 128) return dispatch_tok<INT4, BF16, 128>(g, mw, s);
   return dispatch_tok<INT4, BF16, 0>(g, mw, s);
 }
+template <bool INT4, bool BF16, int GS>
+static int dispatch_experts_tok(const WoExpertGemmArgs& g, const CUtensorMap& mw, cudaStream_t s) {
+  if (g.ntok == 16) return launch_experts<16, 8, INT4, BF16, GS>(g, mw, s);
+  return launch_experts<64, 4, INT4, BF16, GS>(g, mw, s);
+}
+template <bool INT4, bool BF16>
+static int dispatch_experts(const WoExpertGemmArgs& g, const CUtensorMap& mw, cudaStream_t s) {
+  if (g.group_size == 64) return dispatch_experts_tok<INT4, BF16, 64>(g, mw, s);
+  if (g.group_size == 128) return dispatch_experts_tok<INT4, BF16, 128>(g, mw, s);
+  return dispatch_experts_tok<INT4, BF16, 0>(g, mw, s);
+}
 
 // One-pass dequantisation for the batches that run the dense GEMM: each CTA reads a [64 channels x 64 k] tile of the quantised weight once
 // (along k), turns it around in shared memory and writes [64 k x 64 channels] of out once (along n).  out = float(q) * scale, rounded once
-// to OutT: the same value as nn/quant.py's torch expression.
+// to OutT: the same value as nn/quant.py's torch expression.  blockIdx.z = expert of a stacked weight [E, n, k] -> [E, k, n].
 template <bool INT4, typename OutT>
 __global__ void __launch_bounds__(256)
 wo_dequant_kernel(const int8_t* __restrict__ w, const float* __restrict__ scale, OutT* __restrict__ out, int n, int k, int group_size) {
   __shared__ float tile[64][65];                             // [k][channel], q as float (exact)
   const int k0 = blockIdx.x * 64, n0 = blockIdx.y * 64, t = threadIdx.x;
+  w += (int64_t)blockIdx.z * n * (INT4 ? k / 2 : k);
+  scale += (int64_t)blockIdx.z * n * (group_size > 0 ? k / group_size : 1);
+  out += (int64_t)blockIdx.z * k * n;
   if constexpr (!INT4) {
     for (int i = t; i < 64 * 64; i += 256) {
       const int nl = i >> 6, kl = i & 63, ch = n0 + nl, kk = k0 + kl;
@@ -413,28 +696,40 @@ wo_dequant_kernel(const int8_t* __restrict__ w, const float* __restrict__ scale,
 }
 
 template <bool INT4, typename OutT>
-static int launch_dequant(const void* w, const float* scale, void* out, int n, int k, int group_size, cudaStream_t s) {
-  const dim3 grid((k + 63) / 64, (n + 63) / 64);
+static int launch_dequant(const void* w, const float* scale, void* out, int n, int k, int group_size, int experts, cudaStream_t s) {
+  const dim3 grid((k + 63) / 64, (n + 63) / 64, experts);
   wo_dequant_kernel<INT4, OutT><<<grid, 256, 0, s>>>((const int8_t*)w, scale, (OutT*)out, n, k, group_size);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }
   return 0;
 }
 template <bool INT4>
-static int dispatch_dequant(const void* w, const float* scale, void* out, int n, int k, int group_size, int out_dtype, cudaStream_t s) {
-  if (out_dtype == kBF16) return launch_dequant<INT4, __nv_bfloat16>(w, scale, out, n, k, group_size, s);
-  if (out_dtype == kF16) return launch_dequant<INT4, __half>(w, scale, out, n, k, group_size, s);
-  if (out_dtype == kF32) return launch_dequant<INT4, float>(w, scale, out, n, k, group_size, s);
+static int dispatch_dequant(const void* w, const float* scale, void* out, int n, int k, int group_size, int out_dtype, int experts, cudaStream_t s) {
+  if (out_dtype == kBF16) return launch_dequant<INT4, __nv_bfloat16>(w, scale, out, n, k, group_size, experts, s);
+  if (out_dtype == kF16) return launch_dequant<INT4, __half>(w, scale, out, n, k, group_size, experts, s);
+  if (out_dtype == kF32) return launch_dequant<INT4, float>(w, scale, out, n, k, group_size, experts, s);
   return 1;
 }
 
 }  // namespace wo
 
-int weight_dequantize(const void* w, const float* scale, void* out, int n, int k, int int4, int group_size, int out_dtype, cudaStream_t s) {
+int weight_dequantize(const void* w, const float* scale, void* out, int n, int k, int int4, int group_size, int out_dtype, cudaStream_t s,
+                      int experts) {
   using namespace wo;
-  if (n <= 0 || k <= 0 || (int4 && k % 2) || (group_size > 0 && k % group_size) || (n + 63) / 64 > 65535) return 1;
-  return int4 ? dispatch_dequant<true>(w, scale, out, n, k, group_size, out_dtype, s)
-              : dispatch_dequant<false>(w, scale, out, n, k, group_size, out_dtype, s);
+  if (n <= 0 || k <= 0 || experts <= 0 || experts > 65535 || (int4 && k % 2) || (group_size > 0 && k % group_size) || (n + 63) / 64 > 65535) return 1;
+  return int4 ? dispatch_dequant<true>(w, scale, out, n, k, group_size, out_dtype, experts, s)
+              : dispatch_dequant<false>(w, scale, out, n, k, group_size, out_dtype, experts, s);
+}
+
+int gemm_weight_only_experts(const WoExpertGemmArgs& g, cudaStream_t s) {
+  using namespace wo;
+  if (g.k % 64 || g.n % 8 || g.m <= 0 || g.experts <= 0 || (g.ntok != 16 && g.ntok != 64)) return 1;
+  if (g.group_size > 0 && ((g.group_size != 64 && g.group_size != 128) || g.k % g.group_size)) return 1;
+  if ((reinterpret_cast<uintptr_t>(g.x) | reinterpret_cast<uintptr_t>(g.w) | reinterpret_cast<uintptr_t>(g.out)) & 15) return 1;
+  CUtensorMap mw;
+  if (!make_w_map_experts(&mw, g.w, g.experts, g.n, g.int4 ? g.k / 2 : g.k)) return 2;
+  if (g.int4) return g.bf16 ? dispatch_experts<true, true>(g, mw, s) : dispatch_experts<true, false>(g, mw, s);
+  return g.bf16 ? dispatch_experts<false, true>(g, mw, s) : dispatch_experts<false, false>(g, mw, s);
 }
 
 int gemm_weight_only(const WoGemmArgs& g, cudaStream_t s) {

@@ -136,6 +136,42 @@ void moe_dest(const int64_t* idx, int64_t n, int* cursor, int* dest, cudaStream_
   B200_CUDA_CHECK(cudaGetLastError());
 }
 
+// Compact plan of the weight-only expert GEMM (csrc/gemm_wo_sm100.cu): segments without padding and one work item per ntok-row tile of
+// every non-empty expert; experts nobody selected get no item.  One block.
+__global__ void moe_wo_plan_kernel(const int64_t* __restrict__ counts, int n_expert, int ntok, int* __restrict__ offsets,
+                                   int* __restrict__ cursor, int* __restrict__ work) {
+  __shared__ int s_off[1025], s_item[1025];
+  if (threadIdx.x == 0) {
+    int off = 0, items = 0;
+    for (int e = 0; e < n_expert; ++e) {
+      const int c = (int)counts[e];
+      s_off[e] = off;
+      s_item[e] = items;
+      off += c;
+      items += (c + ntok - 1) / ntok;
+    }
+    s_off[n_expert] = off;
+    s_item[n_expert] = items;
+    work[0] = items;
+  }
+  __syncthreads();
+  for (int e = threadIdx.x; e < n_expert; e += blockDim.x) {
+    offsets[e] = s_off[e];
+    cursor[e] = s_off[e];
+    for (int i = s_item[e], row = s_off[e]; i < s_item[e + 1]; ++i, row += ntok) {
+      work[1 + 2 * i] = e;
+      work[2 + 2 * i] = row;
+    }
+  }
+  if (threadIdx.x == 0) offsets[n_expert] = s_off[n_expert];
+}
+
+void moe_wo_plan(const int64_t* counts, int n_expert, int ntok, int* offsets, int* cursor, int* work, cudaStream_t s) {
+  if (n_expert > 1024) { set_last_error(__FILE__, __LINE__, "moe_wo_plan: at most 1024 experts per rank"); return; }
+  moe_wo_plan_kernel<<<1, 256, 0, s>>>(counts, n_expert, ntok, offsets, cursor, work);
+  B200_CUDA_CHECK(cudaGetLastError());
+}
+
 // ------------------------------------------------------------------------------------------------ row movement
 // dst[dest[i]] = scale[i] * src[i / topk]   (one warp per slot, 16-byte vectors)
 template <typename T>

@@ -357,28 +357,82 @@ class SwitchGate(NaiveGate):
 
 # ---- expert FFN (grouped) ------------------------------------------------------------------------------------------------
 def _expert_ffn(x, counts, w1, b1, w2, b2, act):
-    """x rows sorted by local expert; counts[e] rows per expert; w1 [E, d, f(or 2f)], w2 [E, f, d]."""
-    outs, off = [], 0
+    """x rows sorted by local expert; counts[e] rows per expert; w1 [E, d, f(or 2f)], w2 [E, f, d].  w1 / w2 may be zero-argument
+    callables that produce the stack (dequantised experts): every expert's first layer runs before the second stack is made."""
     from ..kernels import activation as KA
     from ..kernels import gemm as KG
 
+    w1 = w1() if callable(w1) else w1
+    hs, off = [], 0
     for e, c in enumerate(counts):
         xe = x[off:off + c]
         off += c
         if c == 0:
-            outs.append(xe.new_zeros((0, w2.shape[-1])))
+            hs.append(None)
             continue
         h = _raw(KG.linear(xe, w1[e], None if b1 is None else b1[e]))
         if act == "swiglu":
             h = _raw(KA.swiglu(h))
         else:
             h = TF.gelu(h) if act == "gelu" else torch.relu(h)
-        outs.append(_raw(KG.linear(h, w2[e], None if b2 is None else b2[e])))
+        hs.append(h)
+    del w1
+    w2 = w2() if callable(w2) else w2
+    outs = [x.new_zeros((0, w2.shape[-1])) if h is None else _raw(KG.linear(h, w2[e], None if b2 is None else b2[e])) for e, h in enumerate(hs)]
     return torch.cat(outs, 0) if outs else x.new_zeros((0, w2.shape[-1]))
 
 
-def moe_ffn(x, gate_weight, ffn1_weight, ffn1_bias, ffn2_weight, ffn2_bias, topk=2, norm_topk_prob=True):
-    """Single-device fused MoE (all experts local). x [.., d]; ffn1 [E, d, 2f] (swiglu) ; ffn2 [E, f, d]."""
+def _moe_ffn_loop(x2, idx, val, w1, b1, w2, b2, act, n_expert):
+    """out[t] = sum_k val[t, k] * expert_{idx[t, k]}(x2[t]) with the experts run one after another over the rows sorted by expert
+    (slots with idx -1 are dropped; val None: plain sum)."""
+    flat_e = idx.reshape(-1)
+    tok = torch.arange(x2.shape[0], device=x2.device).repeat_interleave(idx.shape[-1])
+    wv = val.reshape(-1) if val is not None else torch.ones(flat_e.shape, device=x2.device)
+    keep = flat_e >= 0
+    flat_e, tok, wv = flat_e[keep], tok[keep], wv[keep]
+    order = torch.argsort(flat_e, stable=True)
+    tok = tok[order]
+    counts = torch.bincount(flat_e, minlength=n_expert).tolist()
+    y = _expert_ffn(x2[tok], counts, w1, b1, w2, b2, act)
+    w = wv[order].to(y.dtype)
+    return torch.zeros_like(x2).index_add(0, tok, y * w[:, None])
+
+
+_QUANT_METHODS = {"None": None, "weight_only_int8": False, "weight_only_int4": True}   # -> int4
+
+
+def _quantized_stack(w, scale, int4, n_expert, k, name):
+    """(q int8 [E, N, K] (int4 [E, N, K/2]), scale fp32, group_size) of a stack of weight_quantize outputs of n_expert experts with fan-in
+    k; N comes from the scale ([E, N] per-channel, [E, K / G, N] with G = 64 / 128).  Any view holding the same bytes (e.g. [E, K, N]) is
+    accepted."""
+    q, s = _raw(w), _raw(scale)
+    gs = -1
+    if s.dim() == 3 and s.shape[1] > 0 and k % s.shape[1] == 0 and k // s.shape[1] in (64, 128):
+        gs = k // s.shape[1]
+    if (s.dim() != 2 and gs < 0) or s.shape[0] != n_expert:
+        raise ValueError(f"{name}: scale of shape {tuple(s.shape)} is neither [E, N] (per-channel) nor [E, K / G, N] with E = {n_expert}, "
+                         f"K = {k} and G 64 or 128")
+    E, N = s.shape[0], s.shape[-1]
+    if q.dtype != torch.int8 or (int4 and k % 2) or q.numel() != E * N * (k // 2 if int4 else k):
+        raise ValueError(f"{name}: expected the int8 bytes of {E} experts x {N} outputs x {k} inputs{' (int4: two per byte)' if int4 else ''}, "
+                         f"got {q.dtype} of shape {tuple(q.shape)}")
+    return q.contiguous().reshape(E, N, k // 2 if int4 else k), s.float().contiguous(), gs
+
+
+def moe_ffn(x, gate_weight, ffn1_weight, ffn1_bias, ffn2_weight, ffn2_bias, topk=2, norm_topk_prob=True, ffn1_scale=None, ffn2_scale=None,
+            quant_method="None"):
+    """Single-device fused MoE (all experts local). x [.., d]; ffn1 [E, d, 2f] (swiglu) ; ffn2 [E, f, d].  quant_method
+    "weight_only_int8" / "weight_only_int4": the ffn weights hold the bytes of stacked `weight_quantize` outputs ([E, N, K], int4
+    [E, N, K/2]) and ffn*_scale their scales ([E, N] or [E, K / G, N]); they run through kernels.moe.expert_ffn_weight_only."""
+    if quant_method not in _QUANT_METHODS:
+        raise ValueError(f"quant_method must be one of {sorted(_QUANT_METHODS)}, got {quant_method!r}")
+    int4 = _QUANT_METHODS[quant_method]
+    if int4 is None and (ffn1_scale is not None or ffn2_scale is not None):
+        raise ValueError('ffn1_scale / ffn2_scale are only used with a weight-only quant_method, not "None"')
+    if int4 is None and (_raw(ffn1_weight).dtype == torch.int8 or _raw(ffn2_weight).dtype == torch.int8):
+        raise ValueError('int8 expert weights need quant_method "weight_only_int8" or "weight_only_int4" and their scales')
+    if int4 is not None and (ffn1_scale is None or ffn2_scale is None):
+        raise ValueError(f"quant_method {quant_method!r} needs ffn1_scale and ffn2_scale")
     xr = _raw(x)
     shape = xr.shape
     x2 = xr.reshape(-1, shape[-1])
@@ -387,22 +441,29 @@ def moe_ffn(x, gate_weight, ffn1_weight, ffn1_bias, ffn2_weight, ffn2_bias, topk
     val, idx = p.topk(topk, -1)
     if norm_topk_prob:
         val = val / val.sum(-1, keepdim=True)
-    E = _raw(ffn1_weight).shape[0]
     from ..kernels import moe as KM
 
+    if int4 is not None:
+        d, E = shape[-1], _raw(gate_weight).shape[-1]
+        f = _raw(ffn2_weight).numel() * (2 if int4 else 1) // (E * d)   # ffn2's fan-in, from its byte count
+        q1, s1, gs1 = _quantized_stack(ffn1_weight, ffn1_scale, int4, E, d, "ffn1")
+        q2, s2, gs2 = _quantized_stack(ffn2_weight, ffn2_scale, int4, E, f, "ffn2")
+        if s2.shape[-1] != d or gs1 != gs2 or q1.shape[1] not in (f, 2 * f):
+            raise ValueError(f"ffn1 {tuple(q1.shape)} / ffn2 {tuple(q2.shape)} quantised experts do not form [E, d = {d}, 2f or f] -> [E, f, d] "
+                             "with one scale layout")
+        act = "swiglu" if q1.shape[1] == 2 * f else "gelu"
+        b1 = None if ffn1_bias is None else _raw(ffn1_bias)
+        b2 = None if ffn2_bias is None else _raw(ffn2_bias)
+        out = KM.expert_ffn_weight_only(x2, idx, val.to(torch.float32), q1, s1, q2, s2, int4, gs1, b1, b2, act)
+        return _w(out.reshape(shape))
+    E = _raw(ffn1_weight).shape[0]
     if KM.grouped_ok(x2, _raw(ffn1_weight), _raw(ffn2_weight)) and ffn1_bias is None and ffn2_bias is None:
         act_g = "swiglu" if _raw(ffn1_weight).shape[-1] == 2 * _raw(ffn2_weight).shape[1] else "gelu"
         out = KM.expert_ffn_grouped(x2, idx, val.to(torch.float32), ffn1_weight, ffn2_weight, act_g)   # grouped tcgen05 GEMMs, routing on the device
         return _w(out.reshape(shape))
-    flat_e = idx.reshape(-1)
-    order = torch.argsort(flat_e, stable=True)
-    tok = torch.arange(x2.shape[0], device=x2.device).repeat_interleave(topk)[order]
-    counts = torch.bincount(flat_e, minlength=E).tolist()
     act = "swiglu" if _raw(ffn1_weight).shape[-1] == 2 * _raw(ffn2_weight).shape[1] else "gelu"
-    y = _expert_ffn(x2[tok], counts, _raw(ffn1_weight), None if ffn1_bias is None else _raw(ffn1_bias), _raw(ffn2_weight),
-                    None if ffn2_bias is None else _raw(ffn2_bias), act)
-    w = val.reshape(-1)[order].to(y.dtype)
-    out = torch.zeros_like(x2).index_add(0, tok, y * w[:, None])
+    out = _moe_ffn_loop(x2, idx, val, _raw(ffn1_weight), None if ffn1_bias is None else _raw(ffn1_bias), _raw(ffn2_weight),
+                        None if ffn2_bias is None else _raw(ffn2_bias), act, E)
     return _w(out.reshape(shape))
 
 
@@ -422,6 +483,51 @@ class ExpertFFN(Layer):
         return _w(_expert_ffn(_raw(x), counts, _raw(self.w1), None, _raw(self.w2), None, self.activation))
 
 
+class WeightOnlyExpertFFN(Layer):
+    """The experts of an `ExpertFFN` with weight-only int8 / int4 weights (inference).  Every expert's [in, out] weight goes through
+    nn.quant.weight_quantize: `quant_w1` int8 [E, F1, d] (int4 [E, F1, d/2]) and `quant_w2` [E, d, f] (int4 [E, d, f/2]) with fp32 scales
+    `scale_w1` / `scale_w2` ([E, N] per-channel or [E, K / group_size, N]).  They are buffers, as in WeightOnlyLinear: the layer has nothing
+    to train.  MoELayer runs it through kernels.moe.expert_ffn_weight_only."""
+
+    def __init__(self, experts, algo="weight_only_int8", group_size=-1):
+        super().__init__()
+        from ..nn import quant as Q
+
+        self.num_expert, self.activation = experts.num_expert, experts.activation
+        self.algo, self.group_size, self.int4 = algo, int(group_size), algo == "weight_only_int4"
+        for name in ("w1", "w2"):
+            w = _raw(getattr(experts, name)).detach().float()
+            qs = [Q.weight_quantize(w[e].as_subclass(Tensor), algo=algo, group_size=self.group_size) for e in range(w.shape[0])]
+            self.register_buffer("quant_" + name, torch.stack([_raw(q) for q, _ in qs]))
+            self.register_buffer("scale_" + name, torch.stack([_raw(s).float() for _, s in qs]).contiguous())
+
+    def dequantized(self, dtype):
+        """(w1 [E, d, F1], w2 [E, f, d]) in `dtype`: the 16-bit stacks this layer computes with, bit-equal to weight_dequantize per expert."""
+        from ..kernels import moe as KM
+
+        return tuple(KM.dequantize_experts(getattr(self, "quant_" + n), getattr(self, "scale_" + n), self.int4, self.group_size, dtype)
+                     for n in ("w1", "w2"))
+
+    def ffn(self, x, idx, probs):
+        """Top-k expert FFN of rows x [T, d] routed to idx [T, k] with weights probs [T, k] (kernels.moe.expert_ffn_weight_only)."""
+        from ..kernels import moe as KM
+
+        return KM.expert_ffn_weight_only(x, idx, probs, self.quant_w1, self.scale_w1, self.quant_w2, self.scale_w2, self.int4, self.group_size,
+                                         act=self.activation)
+
+    def forward(self, x, counts):
+        from ..kernels import moe as KM
+
+        xr = _raw(x)
+        deq = lambda n: (lambda: KM.dequantize_experts(getattr(self, "quant_" + n), getattr(self, "scale_" + n), self.int4,   # noqa: E731
+                                                       self.group_size, xr.dtype))
+        return _w(_expert_ffn(xr, counts, deq("w1"), None, deq("w2"), None, self.activation))
+
+    def extra_repr(self):
+        g = "per-channel" if self.group_size <= 0 else f"group_size={self.group_size}"
+        return f"num_expert={self.num_expert}, {self.algo}, {g}"
+
+
 class MoELayer(Layer):
     """Parity: python/paddle/incubate/distributed/models/moe/moe_layer.py:MoELayer.
 
@@ -438,7 +544,7 @@ class MoELayer(Layer):
         if moe_group is None:
             self.world_size = 1
         self.experts = experts
-        self.num_expert = experts.num_expert if isinstance(experts, ExpertFFN) else len(experts)
+        self.num_expert = experts.num_expert if isinstance(experts, (ExpertFFN, WeightOnlyExpertFFN)) else len(experts)
         gate = gate or {"type": "gshard", "top_k": 2}
         if isinstance(gate, dict):
             k = gate.get("top_k", 2)
@@ -464,6 +570,8 @@ class MoELayer(Layer):
         probs = torch.softmax(val.float(), -1) if not isinstance(self.gate, SwitchGate) else val.float()
         from ..kernels import moe as KM
 
+        if isinstance(self.experts, WeightOnlyExpertFFN) and self.world_size == 1:
+            return _w(self.experts.ffn(x, idx.long(), probs).reshape(shape))
         grouped = isinstance(self.experts, ExpertFFN) and KM.grouped_ok(x, _raw(self.experts.w1), _raw(self.experts.w2))
         if grouped and self.world_size == 1:
             out = KM.expert_ffn_grouped(x, idx.long(), probs, self.experts.w1, self.experts.w2, self.experts.activation)
@@ -557,7 +665,7 @@ class MoELayer(Layer):
         return KM._Combine.apply(y_back, dest_back, probs, k)
 
     def _run_experts(self, x, counts):
-        if isinstance(self.experts, ExpertFFN):
+        if isinstance(self.experts, (ExpertFFN, WeightOnlyExpertFFN)):
             return _raw(self.experts(x, counts))
         outs, off = [], 0
         for e, c in enumerate(counts):

@@ -373,10 +373,14 @@ def fused_gate_attention(query, key=None, query_weight=None, key_weight=None, va
 
 def fused_moe(x, gate_weight, ffn1_weight, ffn2_weight, ffn1_bias=None, ffn1_scale=None, ffn2_bias=None, ffn2_scale=None, quant_method="None",
               moe_topk=2, norm_topk_prob=True, group_moe=False):
-    """Token-choice top-k MoE FFN (SwiGLU experts). Parity: incubate/nn/functional/fused_moe.py."""
+    """Token-choice top-k MoE FFN (SwiGLU experts). Parity: incubate/nn/functional/fused_moe.py.  quant_method "weight_only_int8" /
+    "weight_only_int4": ffn1_weight / ffn2_weight hold the bytes of stacked weight_quantize outputs ([E, N, K], int4 [E, N, K/2]; the
+    reference's [E, K, N] view of the same bytes is accepted) and ffn1_scale / ffn2_scale their scales ([E, N] per-channel or [E, K / G, N]
+    group-wise, G = 64 / 128, any float dtype)."""
     from ....incubate.moe import moe_ffn
 
-    return moe_ffn(x, gate_weight, ffn1_weight, ffn1_bias, ffn2_weight, ffn2_bias, moe_topk, norm_topk_prob)
+    return moe_ffn(x, gate_weight, ffn1_weight, ffn1_bias, ffn2_weight, ffn2_bias, moe_topk, norm_topk_prob, ffn1_scale=ffn1_scale,
+                   ffn2_scale=ffn2_scale, quant_method=quant_method)
 
 
 __all__ = ["fused_multi_head_attention", "fused_feedforward", "fused_multi_transformer", "fused_matmul_bias", "fused_linear", "fused_linear_activation",

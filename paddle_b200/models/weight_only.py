@@ -1,17 +1,22 @@
-"""Weight-only quantised serving: `quantize_weights(model, algo, group_size)` replaces the projection layers of a decoder-only model of this
-package with `WeightOnlyLinear`, which holds int8 / int4 weights and fp32 scales and computes through `nn.quant.weight_only_linear`.
+"""Weight-only quantised serving: `quantize_weights(model, algo, group_size, experts=False)` replaces the projection layers of a decoder-only
+model of this package with `WeightOnlyLinear`, which holds int8 / int4 weights and fp32 scales and computes through
+`nn.quant.weight_only_linear`; with experts=True a Mixtral model's stacked MoE experts become `WeightOnlyExpertFFN` in the same call.
 
 The generation adapters (models/generation.py) call these layers as modules, so `generate()`, `LLMEngine` (chunked prefill, 8-bit KV
 caches, prefix caching, a quantised draft model) and `calibrate_kv_cache` serve a quantised model unchanged.  On CUDA a step with at most
 64 rows runs the in-SM dequantising GEMM (csrc/gemm_wo_sm100.cu); a larger step dequantises each weight once and runs the 16-bit GEMM.
+Quantised experts follow the same split by routed slots (tokens x top-k): up to kernels.moe.WO_MOE_MAX_SLOTS they run the grouped in-SM
+kernel over the selected experts only, above it each expert stack is dequantised in one launch for the 16-bit grouped GEMM.
 
-Quantised layers:  Llama `qkv_proj, o_proj, gate_up_proj, down_proj`;  Mixtral `qkv_proj, o_proj` (the MoE experts stay 16-bit);  GPT
-`qkv, proj, fc1, fc2`.  Embeddings, norms and the LM head stay 16-bit.  Inference only."""
+Quantised layers:  Llama `qkv_proj, o_proj, gate_up_proj, down_proj`;  Mixtral `qkv_proj, o_proj`, and with experts=True its MoE experts
+(the router stays 16-bit);  GPT `qkv, proj, fc1, fc2`.  Embeddings, norms and the LM head stay 16-bit.  Expert-parallel MoE layers cannot
+hold quantised experts.  Inference only."""
 from __future__ import annotations
 
 import torch
 
 from .. import nn
+from ..incubate.moe import ExpertFFN, WeightOnlyExpertFFN
 from ..nn import quant as Q
 from ..tensor import Tensor
 
@@ -63,14 +68,38 @@ def _targets(model):
     raise ValueError(f"quantize_weights does not know the layout of {type(model).__name__}")
 
 
-def quantize_weights(model, algo="weight_only_int8", group_size=-1):
+def _moe_layers(model):
+    """The MoELayer of every decoder layer (Mixtral), or [] for a dense model."""
+    if hasattr(model, "embed_tokens") and hasattr(model, "layers") and hasattr(list(model.layers)[0], "moe"):
+        return [layer.moe for layer in model.layers]
+    return []
+
+
+def quantize_weights(model, algo="weight_only_int8", group_size=-1, experts=False):
     """Replace the model's projection layers in place with `WeightOnlyLinear` (int8 or int4 weights, per-channel scales for group_size -1,
-    else one scale per `group_size` consecutive inputs of a channel) and return the model.  Every check runs before any layer changes."""
+    else one scale per `group_size` consecutive inputs of a channel) and return the model.  experts=True also replaces the stacked MoE
+    experts of a Mixtral model (`ExpertFFN`) with `WeightOnlyExpertFFN`.  Every check runs before any layer changes."""
     if algo not in _ALGOS:
         raise ValueError(f"algo must be one of {sorted(_ALGOS)}, got {algo!r}")
     if group_size not in (-1, 64, 128):
         raise ValueError(f"group_size must be -1 (per-channel), 64 or 128, got {group_size!r}")
     targets = _targets(model)
+    moes = _moe_layers(model) if experts else []
+    if experts and not moes:
+        raise ValueError(f"experts=True: {type(model).__name__} has no MoE experts")
+    for moe in moes:
+        if moe.world_size > 1:
+            raise ValueError("experts=True: expert-parallel MoE layers (world_size > 1) cannot hold quantized experts")
+        if isinstance(moe.experts, WeightOnlyExpertFFN):
+            raise ValueError("the model is already quantized")
+        if not isinstance(moe.experts, ExpertFFN):
+            raise ValueError(f"experts=True replaces stacked ExpertFFN experts; found {type(moe.experts).__name__}")
+        ex = moe.experts
+        for name, k in (("ffn1", int(ex.w1.shape[1])), ("ffn2", int(ex.w2.shape[1]))):
+            if group_size > 0 and k % group_size:
+                raise ValueError(f"experts {name}: fan-in {k} is not a multiple of group_size {group_size}")
+            if algo == "weight_only_int4" and k % 2:
+                raise ValueError(f"experts {name}: int4 packs two inputs per byte, fan-in {k} is odd")
     for parent, name in targets:
         layer = getattr(parent, name)
         if isinstance(layer, WeightOnlyLinear):
@@ -85,4 +114,6 @@ def quantize_weights(model, algo="weight_only_int8", group_size=-1):
     with torch.no_grad():
         for parent, name in targets:
             setattr(parent, name, WeightOnlyLinear(getattr(parent, name), algo, group_size))
+        for moe in moes:
+            moe.experts = WeightOnlyExpertFFN(moe.experts, algo, group_size)
     return model
