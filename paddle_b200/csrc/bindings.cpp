@@ -1374,6 +1374,56 @@ Tensor attention_bwd_packed(const Tensor& qkv, int64_t nh, int64_t nkv, const Te
   return dqkv;
 }
 
+// ------------------------------------------------------------------------------------------------ token sampling (csrc/sampling.cu)
+// x [rows, vocab] fp32 / fp16 / bf16 with unit column stride (any row stride); per-row parameters are contiguous CUDA vectors on x's
+// device.  Returns (ids int64 [rows], vals [rows] in x's dtype, top_vals [rows, k_out], top_ids int64 [rows, k_out]).  One launch,
+// no host read.  Failing checks use literal messages only.
+std::vector<Tensor> sample_tokens(const Tensor& x, const Tensor& temperature, const Tensor& top_k, const Tensor& top_p, const OptT& threshold,
+                                  const Tensor& seed, const Tensor& offset, bool is_prob, bool truncated, int64_t k_out) {
+  TORCH_CHECK(x.is_cuda() && x.dim() == 2 && x.stride(1) == 1 && x.size(1) > 0, "sample_tokens: x must be a CUDA [rows, vocab] matrix with unit column stride");
+  TORCH_CHECK(x.size(1) < ((int64_t)1 << 30) && x.size(0) < ((int64_t)1 << 31), "sample_tokens: too many rows or tokens");
+  TORCH_CHECK(k_out >= 0 && k_out <= b200::sample_max_top() && k_out <= x.size(1), "sample_tokens: k_out must be in [0, min(1024, vocab)]");
+  const int64_t rows = x.size(0);
+  auto vec = [&](const Tensor& t, at::ScalarType st, const char* msg) {
+    TORCH_CHECK(t.device() == x.device() && t.scalar_type() == st && t.dim() == 1 && t.size(0) == rows && t.is_contiguous(), msg);
+  };
+  vec(temperature, at::kFloat, "sample_tokens: temperature must be float32 [rows] on x's device");
+  vec(top_k, at::kInt, "sample_tokens: top_k must be int32 [rows] on x's device");
+  vec(top_p, at::kFloat, "sample_tokens: top_p must be float32 [rows] on x's device");
+  vec(seed, at::kLong, "sample_tokens: seed must be int64 [rows] on x's device");
+  vec(offset, at::kLong, "sample_tokens: offset must be int64 [rows] on x's device");
+  const bool has_thr = threshold.has_value() && threshold->defined();
+  if (has_thr) vec(*threshold, at::kFloat, "sample_tokens: threshold must be float32 [rows] on x's device");
+  c10::cuda::CUDAGuard guard(x.device());
+  Tensor ids = torch::empty({rows}, x.options().dtype(at::kLong));
+  Tensor vals = torch::empty({rows}, x.options());
+  Tensor top_vals = torch::empty({rows, k_out}, x.options());
+  Tensor top_ids = torch::empty({rows, k_out}, x.options().dtype(at::kLong));
+  b200::SampleArgs a{};
+  a.x = x.data_ptr(); a.rows = rows; a.stride = rows > 1 ? x.stride(0) : x.size(1); a.vocab = (int)x.size(1);
+  a.temperature = temperature.data_ptr<float>(); a.top_k = top_k.data_ptr<int>(); a.top_p = top_p.data_ptr<float>();
+  a.threshold = has_thr ? threshold->data_ptr<float>() : nullptr;
+  a.seed = seed.data_ptr<int64_t>(); a.offset = offset.data_ptr<int64_t>();
+  a.ids = ids.data_ptr<int64_t>(); a.vals = vals.data_ptr(); a.top_vals = top_vals.data_ptr(); a.top_ids = top_ids.data_ptr<int64_t>();
+  a.k_out = (int)k_out; a.is_prob = is_prob ? 1 : 0; a.truncated = truncated ? 1 : 0; a.dtype = dt_code(x);
+  const int rc = b200::sample_tokens(a, cur_stream());
+  g_launches += 1;
+  check_err();
+  TORCH_CHECK(rc == 0, "paddle_b200.sample_tokens: unsupported shape");
+  return {ids, vals, top_vals, top_ids};
+}
+
+// the uniforms the sampling race draws for (seed, offset), tokens 0 .. n-1 (float32 [n] on `device`)
+Tensor sampling_uniforms(int64_t seed, int64_t offset, int64_t n, const Tensor& like) {
+  TORCH_CHECK(like.is_cuda() && n >= 0 && n < ((int64_t)1 << 30), "sampling_uniforms: n in [0, 2^30) on a CUDA device");
+  c10::cuda::CUDAGuard guard(like.device());
+  Tensor out = torch::empty({n}, like.options().dtype(at::kFloat));
+  b200::sampling_uniforms(seed, offset, (int)n, out.data_ptr<float>(), cur_stream());
+  g_launches += 1;
+  check_err();
+  return out;
+}
+
 // Every kernel entry point is bound through traced(): when the tracer is on (profiler.Profiler) the call becomes a host range
 // plus a cudaEvent pair on the launching stream; when it is off the cost is one relaxed atomic load.
 template <typename R, typename... A>
@@ -1483,6 +1533,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         pybind11::arg("d_out"), pybind11::arg("scale"), pybind11::arg("causal"), pybind11::arg("colmask") = pybind11::none());
   m.def("attention_bwd_packed", traced("attention_bwd_packed", &attention_bwd_packed), pybind11::arg("qkv"), pybind11::arg("nh"), pybind11::arg("nkv"), pybind11::arg("out"),
         pybind11::arg("lse"), pybind11::arg("d_out"), pybind11::arg("scale"), pybind11::arg("causal"), pybind11::arg("seq_major") = false);
+  m.def("sample_tokens", traced("sample_tokens", &sample_tokens), pybind11::arg("x"), pybind11::arg("temperature"), pybind11::arg("top_k"),
+        pybind11::arg("top_p"), pybind11::arg("threshold"), pybind11::arg("seed"), pybind11::arg("offset"), pybind11::arg("is_prob") = false,
+        pybind11::arg("truncated") = true, pybind11::arg("k_out") = 0);
+  m.def("sampling_uniforms", traced("sampling_uniforms", &sampling_uniforms));
   m.def("launch_count", &launch_count);
   m.def("reset_launch_count", &reset_launch_count);
   m.def("add_launches", &add_launches);

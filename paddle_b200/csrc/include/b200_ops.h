@@ -357,4 +357,31 @@ struct AttnBwdArgs {
 };
 int attention_bwd(const AttnBwdArgs& a, cudaStream_t s);
 
+// Token sampling (sampling.cu): one CTA per row of x [rows, vocab] (row stride `stride` elements, unit column stride).  Per-row device
+// arrays: temperature (<= 0: greedy), top_k (int32, 0: off), top_p (1: off), threshold (optional), seed / offset (int64).  Writes ids and
+// vals (x's dtype) [rows]; with k_out > 0 (<= sample_max_top()) also the k_out largest values and their ids per row, descending.
+struct SampleArgs {
+  const void* x;
+  int64_t rows, stride;
+  int vocab;
+  const float* temperature;
+  const int* top_k;
+  const float* top_p;
+  const float* threshold;
+  const int64_t* seed;
+  const int64_t* offset;
+  int64_t* ids;
+  void* vals;
+  void* top_vals;
+  int64_t* top_ids;
+  int k_out;
+  int is_prob;     // x holds probabilities: the race uses log p, top-p uses p
+  int truncated;   // threshold mode: fall back to the smallest kept token >= threshold (else: drop tokens below it from the race)
+  int dtype;
+};
+int sample_tokens(const SampleArgs& a, cudaStream_t s);
+int sample_max_top();
+// the Philox uniforms u_0 .. u_{n-1} the race draws for (seed, offset)
+void sampling_uniforms(int64_t seed, int64_t offset, int n, float* out, cudaStream_t s);
+
 }  // namespace b200

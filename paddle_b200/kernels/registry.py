@@ -195,6 +195,11 @@ def _register_builtin(f):
     r("cross_entropy_with_softmax", G, FLOAT, "kernels.loss:softmax_cross_entropy", native="csrc/loss.cu::softmax_xent_fwd / bwd", priority=10)
     r("cross_entropy_with_softmax", A, ALL_FLOAT, "kernels.loss:softmax_cross_entropy")
     r("fused_bias_dropout_residual", G, FLOAT, "incubate.nn.functional:fused_dropout_add", native="csrc/fused_dropout.cu::bias_dropout_add_fwd")
+    # sampling
+    r("sample_tokens", G, FLOAT, "kernels.sampling:sample", native="csrc/sampling.cu::sample_kernel", priority=10)
+    r("sample_tokens", A, ALL_FLOAT, "kernels.sampling:sample_ref")
+    r("top_p_sampling", G, FLOAT, "ops.search:top_p_sampling", native="csrc/sampling.cu::sample_kernel (probabilities)", priority=10)
+    r("top_p_sampling", A, ALL_FLOAT, "ops.search:top_p_sampling")
     # MoE
     r("moe_expert_ffn", G, HALF, "kernels.moe:expert_ffn_grouped", native="csrc/moe.cu (routing), csrc/gemm_sm100.cu (grouped GEMM)")
     # fused blocks

@@ -49,7 +49,8 @@ from __future__ import annotations
 import torch
 
 from ..incubate.nn.paged_attention import block_attention, shared_prefix_pays
-from .generation import _raw, _sample, _w
+from ..kernels import sampling
+from .generation import _raw, _w
 
 
 class BlockAllocator:
@@ -160,9 +161,9 @@ class PrefixCachingAllocator(BlockAllocator):
 class Sequence:
     WAITING, RUNNING, FINISHED = "waiting", "running", "finished"
 
-    def __init__(self, seq_id, prompt, max_new_tokens, eos_token_id=None, do_sample=False, temperature=1.0, top_k=0, top_p=1.0):
+    def __init__(self, seq_id, prompt, max_new_tokens, eos_token_id=None, do_sample=False, temperature=1.0, top_k=0, top_p=1.0, seed=0):
         self.id, self.prompt, self.max_new_tokens, self.eos = seq_id, [int(t) for t in prompt], int(max_new_tokens), eos_token_id
-        self.do_sample, self.temperature, self.top_k, self.top_p = do_sample, temperature, top_k, top_p
+        self.do_sample, self.temperature, self.top_k, self.top_p, self.seed = do_sample, temperature, top_k, top_p, seed
         self.generated, self.blocks, self.cached, self.status, self.preemptions = [], [], 0, Sequence.WAITING, 0
         self.target = 0                            # tokens to prefill since admission: the sequence samples once cached reaches it
         self.draft_cached, self.spec = 0, 0        # speculative decoding: positions in the draft's cache, proposals this step
@@ -256,12 +257,20 @@ class LLMEngine:
         return dtype, quant
 
     # ---- requests ---------------------------------------------------------------------------------------------------------------
-    def add_request(self, prompt_ids, max_new_tokens=32, eos_token_id=None, do_sample=False, temperature=1.0, top_k=0, top_p=1.0):
+    def add_request(self, prompt_ids, max_new_tokens=32, eos_token_id=None, do_sample=False, temperature=1.0, top_k=0, top_p=1.0, seed=None):
+        """Queues a request and returns its id.  A sampled request draws the token at position t (= len(prompt) + tokens generated so
+        far) from Philox stream (seed, offset t), so with a `seed` its tokens depend only on its own logits: not on the requests that
+        share its steps, preemption, chunked prefill or prefix-cache hits.  Without one it gets a seed from the default CPU generator
+        here (paddle.seed makes a whole run reproducible)."""
         prompt = _raw(prompt_ids).reshape(-1).tolist() if isinstance(prompt_ids, torch.Tensor) else list(prompt_ids)
         need = (len(prompt) + max_new_tokens + self.block_size - 1) // self.block_size
         if need > self.alloc.num_blocks:
             raise ValueError(f"request needs {need} KV blocks, the pool has {self.alloc.num_blocks}")
-        s = Sequence(self._next_id, prompt, max_new_tokens, eos_token_id, do_sample, temperature, top_k, top_p)
+        if seed is None:
+            seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if do_sample else 0
+        seed = int(seed) & (2 ** 64 - 1)
+        seed = seed - 2 ** 64 if seed >= 2 ** 63 else seed               # the same 64 bits as a signed int64
+        s = Sequence(self._next_id, prompt, max_new_tokens, eos_token_id, do_sample, temperature, top_k, top_p, seed)
         self._next_id += 1
         self.waiting.append(s)
         return s.id
@@ -460,6 +469,7 @@ class LLMEngine:
         self.stats["steps"] += 1
         self.stats["decode_tokens"] += len(decode)
         self.stats["prefill_tokens"] += sum(n_new[len(decode):])
+        toks = self._sample_rows(logits, [s if s.cached + n >= s.target else None for s, n in zip(seqs, n_new)])
         out = []
         for i, (s, n) in enumerate(zip(seqs, n_new)):
             s.cached += n
@@ -469,10 +479,29 @@ class LLMEngine:
                 self.running.append(s)
             if s.cached < s.target:                # more chunks to come: nothing to sample yet
                 continue
-            tok = int(_sample(logits[i: i + 1], s.do_sample, s.temperature, s.top_k, s.top_p)[0])
+            tok = toks[i]
             out.append((s.id, tok, self._finish_token(s, tok)))
         self.stats["max_running"] = max(self.stats["max_running"], len(self.running))
         return out
+
+    def _sample_rows(self, logits, rows):
+        """The next token of every logits row [len(rows), vocab] in one sampling call: rows[i] is the sequence row i samples for, or None
+        for a greedy row (a verify row, or a prefill chunk that yields no token).  The per-row parameters go to the device as one packed
+        copy and the ids come back as one copy."""
+        n = len(rows)
+        seed, offset, temp, top_p, top_k = [0] * n, [0] * n, [0.0] * n, [1.0] * n, [0] * n
+        for i, s in enumerate(rows):
+            if s is not None and s.do_sample and s.temperature != 0.0:
+                seed[i], offset[i], temp[i] = s.seed, len(s.prompt) + len(s.generated), float(s.temperature)
+                top_k[i] = min(max(int(s.top_k or 0), 0), 2 ** 31 - 1)
+                top_p[i] = 1.0 if s.top_p is None else float(s.top_p)
+        packed = torch.cat([torch.tensor([seed, offset], dtype=torch.int64).view(torch.uint8).reshape(-1),
+                            torch.tensor([temp, top_p], dtype=torch.float32).view(torch.uint8).reshape(-1),
+                            torch.tensor(top_k, dtype=torch.int32).view(torch.uint8).reshape(-1)]).to(self.device)
+        i64 = packed[:16 * n].view(torch.int64)
+        f32 = packed[16 * n:24 * n].view(torch.float32)
+        ids = sampling.sample(logits, f32[:n], packed[24 * n:].view(torch.int32), f32[n:], i64[:n], i64[n:])[0]
+        return ids.tolist()
 
     # ---- speculative decoding -----------------------------------------------------------------------------------------------------
     def _propose(self, spec, prefill):
@@ -511,13 +540,15 @@ class LLMEngine:
         logits = self._run(self._target, seqs, n_new, enc, dec, toks, rows)      # every verify row, each prefill row's last
         self.stats["steps"] += 1
         self.stats["prefill_tokens"] += sum(n_new[len(decode):])
+        rows = [r for s in decode for r in ([s] if s.spec == 0 else [None] * (s.spec + 1))]
+        toks = self._sample_rows(logits, rows + [s if s.cached + n >= s.target else None for s, n in prefill])
         out, r = [], 0
         for s in decode:
             k = s.spec
             if k == 0:
-                emit = [int(_sample(logits[r: r + 1], s.do_sample, s.temperature, s.top_k, s.top_p)[0])]
+                emit = [toks[r]]
             else:
-                best = logits[r: r + k + 1].argmax(-1).tolist()
+                best = toks[r: r + k + 1]                   # the target's argmax at every verify row
                 a = 0
                 while a < k and prop[s][a] == best[a]:
                     a += 1
@@ -548,7 +579,7 @@ class LLMEngine:
                 self.running.append(s)
             if s.cached < s.target:
                 continue
-            tok = int(_sample(logits[i: i + 1], s.do_sample, s.temperature, s.top_k, s.top_p)[0])
+            tok = toks[i]
             out.append((s.id, tok, self._finish_token(s, tok)))
         self.stats["max_running"] = max(self.stats["max_running"], len(self.running))
         return out

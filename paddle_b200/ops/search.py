@@ -82,21 +82,51 @@ def index_sample(x, index):
     return torch.gather(T(x), 1, T(index).long())
 
 
+@_recordable(always=True)                      # a static program draws anew at every run
 def top_p_sampling(x, ps, threshold=None, topp_seed=None, seed=-1, k=0, mode="truncated", return_top=False, name=None):
-    """Nucleus sampling over the last axis. Parity: python/paddle/tensor/search.py:top_p_sampling."""
-    x, ps = T(x), T(ps)
-    probs, idx = torch.sort(x, dim=-1, descending=True)
-    cum = torch.cumsum(probs, -1)
-    keep = (cum - probs) < ps.reshape(-1, 1)
-    probs = torch.where(keep, probs, torch.zeros_like(probs))
-    probs = probs / probs.sum(-1, keepdim=True)
-    g = None
-    if seed is not None and seed >= 0:
-        g = torch.Generator(device=x.device).manual_seed(int(seed))
-    choice = torch.multinomial(raw(probs).float(), 1, generator=g)
-    ids = torch.gather(raw(idx), -1, choice)
-    scores = torch.gather(raw(x), -1, ids)
-    return wrap(scores), wrap(ids)
+    """Nucleus sampling of one token per row of probabilities x [bs, vocab].  Parity: python/paddle/tensor/search.py:top_p_sampling.
+
+    ps [bs]: each row keeps the tokens whose strictly larger tokens hold at most ps of the mass, and draws among them (kernels.sampling).
+    Seeds: topp_seed [bs] gives row b its own seed; else seed >= 0 gives every row that seed, with the row index as the Philox offset;
+    seed = -1 takes a seed from the default generator of x's device (advancing it).  threshold [bs]: a token below it is never returned
+    unless it is the top-1; mode="truncated" replaces such a draw by the smallest kept token at or above it, "non-truncated" drops the
+    tokens below it from the draw.  Returns (values [bs, 1], ids int64 [bs, 1]); with return_top=True and k > 0 also the k largest
+    probabilities and their ids [bs, k], descending.  On CUDA the whole call is one kernel launch."""
+    from ..kernels.sampling import sample
+
+    x = raw(T(x))
+    if x.dim() != 2:
+        raise ValueError(f"top_p_sampling: x must be [batch, vocab], got shape {list(x.shape)}")
+    if mode not in ("truncated", "non-truncated"):
+        raise ValueError(f"top_p_sampling: mode must be 'truncated' or 'non-truncated', got {mode!r}")
+    bs, dev = x.shape[0], x.device
+    k = int(to_int(k))
+    if return_top and not 0 < k <= min(1024, x.shape[1]):
+        raise ValueError(f"top_p_sampling: return_top needs 0 < k <= min(1024, vocab), got k={k}")
+
+    def per_row(t, dtype, what):
+        t = raw(T(t)).to(dev, dtype).reshape(-1)
+        if t.numel() == 1:
+            t = t.expand(bs)
+        if t.numel() != bs:
+            raise ValueError(f"top_p_sampling: {what} needs one value per row ({bs}), got {t.numel()}")
+        return t.contiguous()
+
+    top_p = per_row(ps, torch.float32, "ps")
+    thr = None if threshold is None else per_row(threshold, torch.float32, "threshold")
+    rows = torch.arange(bs, dtype=torch.int64, device=dev)
+    if topp_seed is not None:
+        seeds, offsets = per_row(topp_seed, torch.int64, "topp_seed"), torch.zeros_like(rows)
+    elif seed is not None and int(seed) >= 0:
+        seeds, offsets = torch.full_like(rows, int(seed)), rows
+    else:
+        seeds, offsets = torch.randint(0, 2 ** 62, (1,), dtype=torch.int64, device=dev).expand(bs).contiguous(), rows
+    ones = torch.ones(bs, dtype=torch.float32, device=dev)
+    no_k = torch.zeros(bs, dtype=torch.int32, device=dev)
+    ids, vals, top_vals, top_ids = sample(x, ones, no_k, top_p, seeds, offsets, thr, is_prob=True, truncated=mode == "truncated",
+                                          k_out=k if return_top else 0)
+    out = (wrap(vals.reshape(bs, 1)), wrap(ids.reshape(bs, 1)))
+    return out + (wrap(top_vals), wrap(top_ids)) if return_top else out
 
 
 __all__ = [n for n in list(globals()) if not n.startswith("_") and n not in ("torch", "T", "ax", "dt", "raw", "scalar_or_tensor", "to_int", "wrap", "annotations")]
