@@ -1,14 +1,19 @@
-// Flash-attention backward for sm_90a (head_dim 128, bf16/fp16), wgmma + TMA, in two kernels that share no atomics:
+// Flash-attention backward for sm_90a (head_dim 128, bf16/fp16), wgmma + TMA.
 //
+//   prep_kernel: delta[row] = dO . O, lse pre-scaled by log2(e), both per query row into a padded stats buffer the main kernel stages
+//     per tile with bulk copies; in single-pass mode it also zeroes the fp32 dQ accumulator.
 //   dkv_kernel: one CTA owns a 128-key K/V tile of one (batch, kv head) - 64 keys per MMA warpgroup - and walks the 64-row query tiles
 //     that can see it (and, under GQA, every query head of the group).  It computes the TRANSPOSED tiles S^T = K Q^T and dP^T = V dO^T
 //     (accumulator row = key), so that P^T and dS^T, packed to 16 bits, are already the register A fragments of dV += P^T dO and
-//     dK += dS^T Q: nothing is staged in shared memory and the dV / dK accumulators stay in registers across the whole loop.
-//   dq_kernel: one CTA owns 128 query rows of one (batch, head) - 64 per warpgroup - and walks the 64-key tiles it can see: S = Q K^T,
-//     dP = dO V^T (accumulator row = query), dS packed in registers is the A fragment of dQ += dS K.  Every dQ element is written once,
-//     by one thread, in a fixed order: the result is bitwise reproducible without turn-taking and dQ needs no fp32 atomics.
-//   Recomputing S and dP in the second kernel costs 2 of 7 GEMMs; in exchange no tile is transposed through shared memory and the
-//     register budget of each kernel holds its accumulators without spilling.
+//     dK += dS^T Q; the dV / dK accumulators stay in registers across the whole loop.  S^T and dP^T are committed as separate groups
+//     (the exp of P^T overlaps the dP^T MMAs) and dV is issued before dS^T is formed.
+//     With the dQ stage (the default, single-pass backward: 5 GEMMs, one main launch) dS^T also goes to shared memory, each warpgroup
+//     computes dQ = dS K for 64 of the 128 head dims over all 128 keys of the tile and adds it into the fp32 dQ with a TMA bulk
+//     reduce-add.  The additions land in arrival order, so dQ is reproducible only to rounding.
+//   dq_kernel (deterministic mode, FLAGS_cudnn_deterministic, after dkv_kernel without the dQ stage): one CTA owns 128 query rows of
+//     one (batch, head) - 64 per warpgroup - and walks the 64-key tiles it can see: S = Q K^T, dP = dO V^T (accumulator row = query),
+//     dS packed in registers is the A fragment of dQ += dS K.  Every dQ element is written once, by one thread, in a fixed order: the
+//     result is bitwise reproducible, at the price of recomputing S and dP (7 GEMMs for 5).
 // The K and Q tiles are consumed K-major (S) and MN-major (dQ, dK) from one copy by choice of descriptor.
 //
 // Parity (behaviour): flash_attn_grad (paddle/phi/kernels/gpu/flash_attn_grad_kernel.cu -> flash-attention library).
@@ -54,9 +59,9 @@ struct Params {
   int b, sq, sk, h, hk;
   float scale, scale_log2;
   int causal, causal_off;
-  const float* lse;      // [B,H,Sq] natural log
-  const float* delta;    // [B,H,Sq]
-  float* dq;             // fp32 [B,Sq,H,D]: every element is written
+  const float* stats;    // [B,H,2,sq_pad]: lse * log2(e), then delta; rows >= sq are zero
+  int sq_pad;            // sq rounded up to the 64-row query tile
+  float* dq;             // fp32 [B,Sq,H,D]
   void* dk;              // [B,Sk,Hk,D] with element strides (dkv_sb, dkv_ss, dkv_sh): may be slices of a packed dQKV tensor
   void* dv;
   int64_t dkv_sb, dkv_ss, dkv_sh;
@@ -73,23 +78,42 @@ struct Smem {
   __device__ uint32_t bar(int i) const { return base + 2 * BIG_BYTES + 4 * SMALL_BYTES + 8u * i; }
 };
 
-template <typename T, bool MASKED>
+// dkv_kernel smem (offsets from the 1024-aligned base): resident K, V; a 2-stage ring of {Q, dO, lse2 / delta}; with the dQ stage also
+// two dS^T buffers (double-buffered: one warpgroup may write the next tile's dS^T while the other still multiplies the last one) and a
+// 64 x 64 fp32 dQ staging tile per MMA warpgroup, the source of the bulk reduce-add.
+struct DkvSmem {
+  static constexpr uint32_t K = 0, V = BIG_BYTES, Q = 2 * BIG_BYTES, DO = Q + 2 * SMALL_BYTES, DS = DO + 2 * SMALL_BYTES;
+  static constexpr uint32_t DS_BYTES = 128 * 64 * 2;          // [key 128][query 64] 16-bit, 128B-swizzled
+  static constexpr uint32_t STAGE = DS + 2 * DS_BYTES;
+  static constexpr uint32_t STAGE_BYTES = 64 * 64 * 4;         // per warpgroup: two [query 64][32 fp32] 128B-swizzled boxes
+  static constexpr uint32_t STATS = STAGE + 2 * STAGE_BYTES;   // per ring stage: lse2[64], delta[64]
+  static constexpr uint32_t BARS = STATS + 2 * 512;
+  static constexpr uint32_t BYTES = BARS + 64 + 1024;
+};
+static_assert(DkvSmem::BYTES <= 227 * 1024, "dkv_kernel shared memory");
+
+// DQ = true: the single-pass backward.  Each query tile's dQ partial dS K (all 128 keys of the tile) is added into the fp32 dQ by a
+// TMA bulk reduce-add; dQ must be zero on entry.  DQ = false: dK / dV only (dq_kernel computes dQ).
+template <typename T, bool MASKED, bool DQ>
 __global__ void __launch_bounds__(kThreadsDkv, 1)
 dkv_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
-           const __grid_constant__ CUtensorMap map_do, const Params p) {
+           const __grid_constant__ CUtensorMap map_do, const __grid_constant__ CUtensorMap map_dq, const Params p) {
   constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
   constexpr int BN = 128, BQ = 64;
+  using L = DkvSmem;
   extern __shared__ uint8_t smem_raw[];
-  const Smem sm{(smem_u32(smem_raw) + 1023u) & ~1023u};
-  const uint32_t sK = sm.big(0), sV = sm.big(1);
-  auto sQ = [&](int s) { return sm.small(s); };
-  auto sDO = [&](int s) { return sm.small(2 + s); };
-  const uint32_t kv_full = sm.bar(0);
-  auto qdo_full = [&](int s) { return sm.bar(1 + s); };
-  auto qdo_empty = [&](int s) { return sm.bar(3 + s); };     // 8 warp arrivals
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  uint8_t* const base_ptr = smem_raw + (base - smem_u32(smem_raw));
+  const uint32_t sK = base + L::K, sV = base + L::V;
+  auto sQ = [&](int s) { return base + L::Q + s * SMALL_BYTES; };
+  auto sDO = [&](int s) { return base + L::DO + s * SMALL_BYTES; };
+  auto stats = [&](int s) { return reinterpret_cast<const float*>(base_ptr + L::STATS + s * 512); };
+  const uint32_t kv_full = base + L::BARS;
+  auto qdo_full = [&](int s) { return base + L::BARS + 8 * (1 + s); };
+  auto qdo_empty = [&](int s) { return base + L::BARS + 8 * (3 + s); };     // 8 warp arrivals
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_tile = blockIdx.x, kv_head = blockIdx.y, batch = blockIdx.z;
+  const int kv_head = blockIdx.x, batch = blockIdx.y, n_tile = blockIdx.z;   // key tiles slowest: under the causal mask the long ones start first
   const int n0 = n_tile * BN;
   const int group = p.h / p.hk;
   const int num_m = (p.sq + BQ - 1) / BQ;
@@ -103,6 +127,7 @@ dkv_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CU
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&map_q); tma_prefetch_desc(&map_k); tma_prefetch_desc(&map_v); tma_prefetch_desc(&map_do);
+    if constexpr (DQ) tma_prefetch_desc(&map_dq);
     mbar_init(kv_full, 1);
     for (int s = 0; s < 2; ++s) { mbar_init(qdo_full(s), 1); mbar_init(qdo_empty(s), 8); }
     fence_barrier_init();
@@ -111,7 +136,7 @@ dkv_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CU
   __syncthreads();
 
   if (warp < 4) {
-    reg_dealloc<40>();
+    reg_dealloc<24>();
     if (warp == 0 && lane == 0 && total > 0) {
       // ================= TMA producer =================
       mbar_expect_tx(kv_full, 2 * BIG_BYTES);
@@ -123,30 +148,32 @@ dkv_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CU
         const int s = it & 1;
         const int head = kv_head * group + it / tiles_per_head;
         const int m0 = (m_first + it % tiles_per_head) * BQ;
+        const float* st = p.stats + ((int64_t)batch * p.h + head) * 2 * p.sq_pad + m0;
         mbar_wait(qdo_empty(s), ((it >> 1) & 1) ^ 1);
-        mbar_expect_tx(qdo_full(s), 2 * SMALL_BYTES);
+        mbar_expect_tx(qdo_full(s), 2 * SMALL_BYTES + 512);
         tma_load_4d(sQ(s), &map_q, qdo_full(s), 0, m0, head, batch);
         tma_load_4d(sQ(s) + SMALL_HALF, &map_q, qdo_full(s), 64, m0, head, batch);
         tma_load_4d(sDO(s), &map_do, qdo_full(s), 0, m0, head, batch);
         tma_load_4d(sDO(s) + SMALL_HALF, &map_do, qdo_full(s), 64, m0, head, batch);
+        bulk_load(base + L::STATS + s * 512, st, 256, qdo_full(s));
+        bulk_load(base + L::STATS + s * 512 + 256, st + p.sq_pad, 256, qdo_full(s));
       }
+      for (int it = max(0, total - 2); it < total; ++it) mbar_wait(qdo_empty(it & 1), (it >> 1) & 1);   // the consumers' waits are unbounded
     }
   } else {
     // ================= MMA warpgroups: wg owns keys [64 wg, 64 wg + 64) of the tile; accumulator row = key, column = query =================
-    reg_alloc<232>();
+    reg_alloc<240>();
     const int wg = (warp >> 2) - 1, q = lane & 3;
     const int rl = wg * 64 + (warp & 3) * 16 + (lane >> 2);      // tile-relative key rows rl and rl + 8
-    constexpr float kLog2e = 1.4426950408889634f;
     float dv_acc[HD / 2], dk_acc[HD / 2];
 #pragma unroll
     for (int i = 0; i < HD / 2; ++i) { dv_acc[i] = 0.f; dk_acc[i] = 0.f; }
-    if (total > 0) mbar_wait(kv_full, 0);
+    if (total > 0) mbar_wait_unbounded(kv_full, 0);
     for (int it = 0; it < total; ++it) {
       const int s = it & 1;
       const int head = kv_head * group + it / tiles_per_head;
       const int m0 = (m_first + it % tiles_per_head) * BQ;
-      const int64_t stat0 = ((int64_t)batch * p.h + head) * p.sq;
-      mbar_wait(qdo_full(s), (it >> 1) & 1);
+      mbar_wait_unbounded(qdo_full(s), (it >> 1) & 1);
       float st[BQ / 2], dpt[BQ / 2];
       wgmma_fence_regs(st);
       wgmma_fence_regs(dpt);
@@ -154,16 +181,17 @@ dkv_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CU
 #pragma unroll
       for (int kb = 0; kb < 2; ++kb)
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
+        for (int k = 0; k < 4; ++k)
           wgmma_ss_n64<BF16, 0, 0>(st, make_smem_desc(sK + kb * BIG_HALF + wg * 8192 + k * 32, 16, 1024),
                                    make_smem_desc(sQ(s) + kb * SMALL_HALF + k * 32, 16, 1024), (kb | k) != 0);      // S^T = K Q^T
+      wgmma_commit();
+#pragma unroll
+      for (int kb = 0; kb < 2; ++kb)
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
           wgmma_ss_n64<BF16, 0, 0>(dpt, make_smem_desc(sV + kb * BIG_HALF + wg * 8192 + k * 32, 16, 1024),
                                    make_smem_desc(sDO(s) + kb * SMALL_HALF + k * 32, 16, 1024), (kb | k) != 0);     // dP^T = V dO^T
-        }
       wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_regs(st);
-      wgmma_fence_regs(dpt);
       int4 cm[2];
       if constexpr (MASKED) {
         const int4* cmp = p.colmask + ((int64_t)batch * p.mask_heads + (p.mask_heads > 1 ? head : 0)) * p.sk;
@@ -173,51 +201,122 @@ dkv_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CU
           cm[h] = key < p.sk ? __ldg(cmp + key) : make_int4(0, 0, 0, 0);
         }
       }
-      // P^T = exp2(S^T scale - lse[query]), dS^T = P^T (dP^T - delta[query]) scale, packed as A fragments (16-query step ks = column groups 2 ks, 2 ks + 1)
+      const float* lse2 = stats(s);        // lse[query] * log2(e)
+      const float* dlt = lse2 + BQ;        // delta[query]
+      wgmma_wait<1>();
+      wgmma_fence_regs(st);
+      // P^T = exp2(S^T scale - lse2[query]) in place of S^T, packed as the A fragments of dV += P^T dO (16-query step ks = column groups 2 ks, 2 ks + 1)
       uint32_t pa[BQ / 16][4], dsa[BQ / 16][4];
 #pragma unroll
       for (int jn = 0; jn < BQ / 8; ++jn) {
-        float pv[4], ds[4];
+        const float2 l2 = *reinterpret_cast<const float2*>(lse2 + jn * 8 + 2 * q);
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int row = m0 + jn * 8 + 2 * q + e;      // query
-          const bool row_ok = row < p.sq;
-          const float lse2 = row_ok ? __ldg(p.lse + stat0 + row) * kLog2e : 0.f;
-          const float dl = row_ok ? __ldg(p.delta + stat0 + row) : 0.f;
-          const int lim = p.causal ? min(p.sk - 1, row + p.causal_off) : p.sk - 1;   // last visible key of this query row
+          const int lim = row >= p.sq ? -1 : p.causal ? min(p.sk - 1, row + p.causal_off) : p.sk - 1;   // last visible key of this query row
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const int key = n0 + rl + h * 8;
-            float x = ex2(fmaf(st[jn * 4 + h * 2 + e], p.scale_log2, -lse2));
-            if (!row_ok || key > lim) x = 0.f;
+            float x = ex2(fmaf(st[jn * 4 + h * 2 + e], p.scale_log2, -(e ? l2.y : l2.x)));
+            if (key > lim) x = 0.f;
             if constexpr (MASKED) {
               if ((row >= cm[h].x && row < cm[h].y) || (row >= cm[h].z && row < cm[h].w)) x = 0.f;
             }
-            pv[h * 2 + e] = x;
-            ds[h * 2 + e] = x * (dpt[jn * 4 + h * 2 + e] - dl) * p.scale;
+            st[jn * 4 + h * 2 + e] = x;
           }
         }
-        pa[jn >> 1][(jn & 1) * 2 + 0] = pack2<T>(pv[0], pv[1]);
-        pa[jn >> 1][(jn & 1) * 2 + 1] = pack2<T>(pv[2], pv[3]);
-        dsa[jn >> 1][(jn & 1) * 2 + 0] = pack2<T>(ds[0], ds[1]);
-        dsa[jn >> 1][(jn & 1) * 2 + 1] = pack2<T>(ds[2], ds[3]);
+        pa[jn >> 1][(jn & 1) * 2 + 0] = pack2<T>(st[jn * 4 + 0], st[jn * 4 + 1]);
+        pa[jn >> 1][(jn & 1) * 2 + 1] = pack2<T>(st[jn * 4 + 2], st[jn * 4 + 3]);
       }
       wgmma_fence_regs(dv_acc);
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < BQ / 16; ++ks)   // B = dO tile read MN-major (N = head dim): 16 query rows = 2048 B per step, d halves SMALL_HALF apart
+        wgmma_rs_n128<BF16, 1>(dv_acc, pa[ks], make_smem_desc(sDO(s) + ks * 2048, SMALL_HALF, 1024), 1);   // dV += P^T dO
+      wgmma_commit();
+      wgmma_wait<1>();
+      wgmma_fence_regs(dpt);
+      // dS^T = P^T (dP^T - delta[query]) scale: A fragments of dK += dS^T Q and, with DQ, the tile's rows of the dS^T buffer
+      uint8_t* const ds_buf = base_ptr + L::DS + (it & 1) * L::DS_BYTES;
+#pragma unroll
+      for (int jn = 0; jn < BQ / 8; ++jn) {
+        const float2 dl = *reinterpret_cast<const float2*>(dlt + jn * 8 + 2 * q);
+        float ds[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) ds[i] = st[jn * 4 + i] * (dpt[jn * 4 + i] - ((i & 1) ? dl.y : dl.x)) * p.scale;
+        dsa[jn >> 1][(jn & 1) * 2 + 0] = pack2<T>(ds[0], ds[1]);
+        dsa[jn >> 1][(jn & 1) * 2 + 1] = pack2<T>(ds[2], ds[3]);
+        if constexpr (DQ) {        // [key][query] rows of 128 B, 16-byte chunk c of row r stored at chunk c ^ (r % 8)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int r = rl + h * 8;
+            *reinterpret_cast<uint32_t*>(ds_buf + r * 128 + ((jn ^ (r & 7)) << 4) + 4 * q) = dsa[jn >> 1][(jn & 1) * 2 + h];
+          }
+        }
+      }
       wgmma_fence_regs(dk_acc);
       wgmma_fence();
 #pragma unroll
-      for (int ks = 0; ks < BQ / 16; ++ks) {   // B = dO / Q tile read MN-major (N = head dim): 16 query rows = 2048 B per step, d halves SMALL_HALF apart
-        wgmma_rs_n128<BF16, 1>(dv_acc, pa[ks], make_smem_desc(sDO(s) + ks * 2048, SMALL_HALF, 1024), 1);   // dV += P^T dO
+      for (int ks = 0; ks < BQ / 16; ++ks)   // B = Q tile read MN-major, as dO above
         wgmma_rs_n128<BF16, 1>(dk_acc, dsa[ks], make_smem_desc(sQ(s) + ks * 2048, SMALL_HALF, 1024), 1);   // dK += dS^T Q
-      }
       wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_regs(dv_acc);
-      wgmma_fence_regs(dk_acc);
-      keep_regs(pa);
-      keep_regs(dsa);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(qdo_empty(s));
+      if constexpr (DQ) {
+        // dQ[query, 64 wg .. 64 wg + 63] = dS K over the tile's 128 keys: A = dS^T buffer read M-major (M = query), B = K half wg read
+        // N-major (N = head dim); 16 keys = 2048 B per step in both
+        fence_proxy_async();
+        named_bar_sync(1, 256);         // both warpgroups' dS^T rows are in shared memory
+        const uint32_t sDS = base + L::DS + (it & 1) * L::DS_BYTES;
+        float dq[HD / 4];
+        wgmma_fence_regs(dq);
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < BN / 16; ++ks)
+          wgmma_ss_n64<BF16, 1, 1>(dq, make_smem_desc(sDS + ks * 2048, L::DS_BYTES, 1024),
+                                   make_smem_desc(sK + wg * BIG_HALF + ks * 2048, BIG_HALF, 1024), ks != 0);
+        wgmma_commit();
+        wgmma_wait<1>();                // dV and dK are done with P^T, dS^T and the Q / dO stage
+        wgmma_fence_regs(dv_acc);
+        wgmma_fence_regs(dk_acc);
+        keep_regs(pa);
+        keep_regs(dsa);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(qdo_empty(s));
+        wgmma_wait<0>();
+        wgmma_fence_regs(dq);
+        // stage the 64 x 64 fp32 partial as two [query][32] boxes (128B-swizzled like the map) and reduce-add it into dQ
+        const bool leader = (threadIdx.x & 127) == 0;
+        if (leader) bulk_wait_group_read<0>();      // the previous tile's reduce has read the staging tile
+        named_bar_sync(2 + wg, 128);
+        uint8_t* const stage = base_ptr + L::STAGE + wg * L::STAGE_BYTES;
+#pragma unroll
+        for (int j = 0; j < HD / 16; ++j)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int r = (warp & 3) * 16 + (lane >> 2) + h * 8;      // query row of the tile
+            const int c = 2 * (j & 3) + (q >> 1);                     // 16-byte chunk of the box row
+            *reinterpret_cast<float2*>(stage + (j >> 2) * 8192 + r * 128 + ((c ^ (r & 7)) << 4) + (q & 1) * 8) =
+                make_float2(dq[j * 4 + h * 2], dq[j * 4 + h * 2 + 1]);
+          }
+        fence_proxy_async();
+        named_bar_sync(2 + wg, 128);
+        if (leader) {
+          const uint32_t src = base + L::STAGE + wg * L::STAGE_BYTES;
+          tma_reduce_add_4d(&map_dq, src, wg * 64, m0, head, batch);
+          tma_reduce_add_4d(&map_dq, src + 8192, wg * 64 + 32, m0, head, batch);
+          bulk_commit_group();
+        }
+      } else {
+        wgmma_wait<0>();
+        wgmma_fence_regs(dv_acc);
+        wgmma_fence_regs(dk_acc);
+        keep_regs(pa);
+        keep_regs(dsa);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(qdo_empty(s));
+      }
+    }
+    if constexpr (DQ) {
+      if ((threadIdx.x & 127) == 0) bulk_wait_group<0>();      // the reduces are done reading shared memory before the CTA exits
     }
     // epilogue: dV, dK rows (accumulator row = key)
 #pragma unroll
@@ -293,7 +392,6 @@ dq_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUt
     // ================= MMA warpgroups: wg owns query rows [64 wg, 64 wg + 64); accumulator row = query, column = key / head dim =================
     const int wg = warp >> 2, q = lane & 3;
     const int rl = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-    constexpr float kLog2e = 1.4426950408889634f;
     float dq_acc[HD / 2];
 #pragma unroll
     for (int i = 0; i < HD / 2; ++i) dq_acc[i] = 0.f;
@@ -304,9 +402,9 @@ dq_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUt
     for (int h = 0; h < 2; ++h) {
       const int row = m0 + rl + h * 8;
       row_ok[h] = row < p.sq;
-      const int64_t stat = ((int64_t)batch * p.h + head) * p.sq + row;
-      lse2[h] = row_ok[h] ? p.lse[stat] * kLog2e : 0.f;
-      dl[h] = row_ok[h] ? p.delta[stat] : 0.f;
+      const int64_t stat = ((int64_t)batch * p.h + head) * 2 * p.sq_pad + row;
+      lse2[h] = row_ok[h] ? p.stats[stat] : 0.f;
+      dl[h] = row_ok[h] ? p.stats[stat + p.sq_pad] : 0.f;
       lim[h] = p.causal ? min(p.sk - 1, row + p.causal_off) : p.sk - 1;
     }
     const int4* cmp = MASKED ? p.colmask + ((int64_t)batch * p.mask_heads + (p.mask_heads > 1 ? head : 0)) * p.sk : nullptr;
@@ -379,17 +477,24 @@ dq_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUt
   }
 }
 
-// delta[b,h,s] = sum_d dO[b,s,h,d] * O[b,s,h,d]   (one warp per row; O and dO share the element strides (sb, ss, sh), d contiguous)
-template <typename T>
-__global__ void delta_kernel(const T* __restrict__ o, const T* __restrict__ d_o, float* __restrict__ delta, int64_t rows, int sq, int h,
-                             int64_t sb, int64_t ss, int64_t sh) {
-  const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);   // row = (b*sq + s)*h + head
+// One warp per padded query row (b, s < sq_pad, head): stats = {lse * log2(e), delta = sum_d dO * O} (zero for s >= sq); with ZERO_DQ
+// also zeroes the row of the fp32 dQ accumulator.  O and dO share the element strides (sb, ss, sh), d contiguous.
+template <typename T, bool ZERO_DQ>
+__global__ void prep_kernel(const T* __restrict__ o, const T* __restrict__ d_o, const float* __restrict__ lse, float* __restrict__ stats,
+                            float* __restrict__ dq, int64_t rows, int sq, int sq_pad, int h, int64_t sb, int64_t ss, int64_t sh,
+                            int64_t dq_sb, int64_t dq_ss, int64_t dq_sh) {
+  const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);   // row = (b*sq_pad + s)*h + head
   if (row >= rows) return;
   const int lane = threadIdx.x & 31;
   const int64_t bs = row / h;
   const int head = (int)(row - bs * h);
-  const int64_t bb = bs / sq;
-  const int sidx = (int)(bs - bb * sq);
+  const int64_t bb = bs / sq_pad;
+  const int sidx = (int)(bs - bb * sq_pad);
+  float* st = stats + (bb * h + head) * 2 * sq_pad + sidx;
+  if (sidx >= sq) {
+    if (lane == 0) { st[0] = 0.f; st[sq_pad] = 0.f; }
+    return;
+  }
   const int64_t off = bb * sb + (int64_t)sidx * ss + (int64_t)head * sh + lane * 4;
   const uint2 a = *reinterpret_cast<const uint2*>(o + off);
   const uint2 b = *reinterpret_cast<const uint2*>(d_o + off);
@@ -400,7 +505,12 @@ __global__ void delta_kernel(const T* __restrict__ o, const T* __restrict__ d_o,
   for (int i = 0; i < 4; ++i) acc += to_f(pa[i]) * to_f(pb[i]);
 #pragma unroll
   for (int o2 = 16; o2 > 0; o2 >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o2);
-  if (lane == 0) delta[(bb * h + head) * sq + sidx] = acc;
+  if (lane == 0) {
+    st[0] = lse[(bb * h + head) * sq + sidx] * 1.4426950408889634f;
+    st[sq_pad] = acc;
+  }
+  if constexpr (ZERO_DQ)
+    *reinterpret_cast<float4*>(dq + bb * dq_sb + (int64_t)sidx * dq_ss + (int64_t)head * dq_sh + lane * 4) = make_float4(0.f, 0.f, 0.f, 0.f);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -416,33 +526,59 @@ static EncodeTiledFn get_encode() {
   }
   return fn;
 }
-static bool make_map4(CUtensorMap* out, const void* ptr, int d, int s, int h, int b, int64_t ss, int64_t sh, int64_t sb, uint32_t box_rows, int dtype) {
+static bool encode4(CUtensorMap* out, CUtensorMapDataType type, uint32_t esize, const void* ptr, int d, int s, int h, int b, int64_t ss,
+                    int64_t sh, int64_t sb, uint32_t box_d, uint32_t box_rows) {
   bind_primary_context();
   EncodeTiledFn enc = get_encode();
   if (!enc) { set_last_error(__FILE__, __LINE__, "cuTensorMapEncodeTiled unavailable"); return false; }
   cuuint64_t dims[4] = {(cuuint64_t)d, (cuuint64_t)s, (cuuint64_t)h, (cuuint64_t)b};
-  cuuint64_t strides[3] = {(cuuint64_t)ss * 2, (cuuint64_t)sh * 2, (cuuint64_t)sb * 2};
-  cuuint32_t box[4] = {64, box_rows, 1, 1};
+  cuuint64_t strides[3] = {(cuuint64_t)ss * esize, (cuuint64_t)sh * esize, (cuuint64_t)sb * esize};
+  cuuint32_t box[4] = {box_d, box_rows, 1, 1};
   cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(out, dtype == kBF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(ptr),
-                   dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = enc(out, type, 4, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_last_error(__FILE__, __LINE__, ("cuTensorMapEncodeTiled (attention bwd) failed: " + std::to_string((int)r)).c_str());
     return false;
   }
   return true;
 }
+// a 16-bit operand [B,S,H,D] in boxes of 64 d x box_rows rows
+static bool make_map4(CUtensorMap* out, const void* ptr, int d, int s, int h, int b, int64_t ss, int64_t sh, int64_t sb, uint32_t box_rows, int dtype) {
+  return encode4(out, dtype == kBF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, ptr, d, s, h, b, ss, sh, sb, 64, box_rows);
+}
+
+// deterministic: dkv_kernel without the dQ stage, then dq_kernel; otherwise the single pass (dQ zeroed by prep_kernel)
+template <typename T, bool MASKED>
+static void launch(const Params& p, bool deterministic, const CUtensorMap (&mq)[2], const CUtensorMap (&mk)[2], const CUtensorMap (&mv)[2],
+                   const CUtensorMap (&mdo)[2], const CUtensorMap& mdq, cudaStream_t s) {
+  static bool attr_set[3] = {false, false, false};
+  const dim3 grid_kv(p.hk, p.b, (p.sk + 127) / 128), grid_q((p.sq + 127) / 128, p.h, p.b);
+  auto smem = [&](auto kern, int slot, uint32_t bytes) {
+    if (!attr_set[slot]) { B200_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)); attr_set[slot] = true; }
+  };
+  if (deterministic) {
+    smem(dkv_kernel<T, MASKED, false>, 0, DkvSmem::BYTES);
+    smem(dq_kernel<T, MASKED>, 1, SMEM_BYTES);
+    dkv_kernel<T, MASKED, false><<<grid_kv, kThreadsDkv, DkvSmem::BYTES, s>>>(mq[1], mk[0], mv[0], mdo[1], mdq, p);
+    dq_kernel<T, MASKED><<<grid_q, kThreads, SMEM_BYTES, s>>>(mq[0], mk[1], mv[1], mdo[0], p);
+  } else {
+    smem(dkv_kernel<T, MASKED, true>, 2, DkvSmem::BYTES);
+    dkv_kernel<T, MASKED, true><<<grid_kv, kThreadsDkv, DkvSmem::BYTES, s>>>(mq[1], mk[0], mv[0], mdo[1], mdq, p);
+  }
+}
 }  // namespace attn_bwd
+
+int attention_bwd_stats_pad(int sq) { return (sq + 63) / 64 * 64; }
 
 int attention_bwd(const AttnBwdArgs& a, cudaStream_t s) {
   using namespace attn_bwd;
   if (!attention_fwd_supported(a.fwd)) return 1;
   const AttnArgs& f = a.fwd;
-  if (a.dq_strides[0] % 2 || a.dq_strides[1] % 2 || a.dq_strides[2] % 2 || (reinterpret_cast<uintptr_t>(a.dq) & 7)) return 1;   // float2 stores
+  if (a.dq_strides[0] % 4 || a.dq_strides[1] % 4 || a.dq_strides[2] % 4 || (reinterpret_cast<uintptr_t>(a.dq) & 15)) return 1;   // TMA / float4
   if (a.dkv_strides[0] % 2 || a.dkv_strides[1] % 2 || a.dkv_strides[2] % 2) return 1;
-  // every operand as a 128-row box map (the resident tile of a kernel) and as a 64-row box map (the streamed tile of the other kernel)
-  CUtensorMap mq[2], mk[2], mv[2], mdo[2];
+  // every operand as a 128-row box map (the resident tile of dq_kernel) and as a 64-row box map (the streamed tile of dkv_kernel)
+  CUtensorMap mq[2], mk[2], mv[2], mdo[2], mdq;
   for (int i = 0; i < 2; ++i) {
     const uint32_t rows = i ? 64 : 128;
     if (!make_map4(&mq[i], f.q, f.d, f.sq, f.h, f.b, f.q_strides[1], f.q_strides[2], f.q_strides[0], rows, f.dtype)) return 2;
@@ -450,34 +586,41 @@ int attention_bwd(const AttnBwdArgs& a, cudaStream_t s) {
     if (!make_map4(&mv[i], f.v, f.d, f.sk, f.hk, f.b, f.v_strides[1], f.v_strides[2], f.v_strides[0], rows, f.dtype)) return 2;
     if (!make_map4(&mdo[i], a.d_o, f.d, f.sq, f.h, f.b, a.o_strides[1], a.o_strides[2], a.o_strides[0], rows, f.dtype)) return 2;
   }
-  const int64_t rows = (int64_t)f.b * f.sq * f.h;
+  // the fp32 dQ accumulator over its own strides, in the reduce boxes of the single pass: 32 d (128 B) x 64 query rows
+  if (!encode4(&mdq, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, a.dq, f.d, f.sq, f.h, f.b, a.dq_strides[1], a.dq_strides[2], a.dq_strides[0], 32, 64))
+    return 2;
+  const int sq_pad = attention_bwd_stats_pad(f.sq);
+  const int64_t rows = (int64_t)f.b * sq_pad * f.h;
   const int wpb = 8;
-  if (f.dtype == kBF16)
-    delta_kernel<__nv_bfloat16><<<(unsigned)((rows + wpb - 1) / wpb), wpb * 32, 0, s>>>((const __nv_bfloat16*)f.o, (const __nv_bfloat16*)a.d_o, a.delta, rows, f.sq, f.h,
-                                                                                     a.o_strides[0], a.o_strides[1], a.o_strides[2]);
-  else
-    delta_kernel<__half><<<(unsigned)((rows + wpb - 1) / wpb), wpb * 32, 0, s>>>((const __half*)f.o, (const __half*)a.d_o, a.delta, rows, f.sq, f.h, a.o_strides[0], a.o_strides[1], a.o_strides[2]);
+  const unsigned blocks = (unsigned)((rows + wpb - 1) / wpb);
+  auto prep = [&](auto kern, auto* o) {
+    using P = std::remove_const_t<std::remove_pointer_t<decltype(o)>>;
+    kern<<<blocks, wpb * 32, 0, s>>>(o, reinterpret_cast<const P*>(a.d_o), f.lse, a.stats, a.dq, rows, f.sq, sq_pad, f.h, a.o_strides[0],
+                                     a.o_strides[1], a.o_strides[2], a.dq_strides[0], a.dq_strides[1], a.dq_strides[2]);
+  };
+  const bool det = a.deterministic;
+  if (f.dtype == kBF16) {
+    const auto* o = reinterpret_cast<const __nv_bfloat16*>(f.o);
+    det ? prep(prep_kernel<__nv_bfloat16, false>, o) : prep(prep_kernel<__nv_bfloat16, true>, o);
+  } else {
+    const auto* o = reinterpret_cast<const __half*>(f.o);
+    det ? prep(prep_kernel<__half, false>, o) : prep(prep_kernel<__half, true>, o);
+  }
   Params p;
   p.b = f.b; p.sq = f.sq; p.sk = f.sk; p.h = f.h; p.hk = f.hk;
   p.scale = f.scale; p.scale_log2 = f.scale * 1.4426950408889634f;
   p.causal = f.causal; p.causal_off = f.sk - f.sq;
   p.colmask = reinterpret_cast<const int4*>(f.colmask);
   p.mask_heads = f.mask_heads > 0 ? f.mask_heads : 1;
-  p.lse = f.lse; p.delta = a.delta; p.dq = a.dq; p.dk = a.dk; p.dv = a.dv;
+  p.stats = a.stats; p.sq_pad = sq_pad; p.dq = a.dq; p.dk = a.dk; p.dv = a.dv;
   p.dkv_sb = a.dkv_strides[0]; p.dkv_ss = a.dkv_strides[1]; p.dkv_sh = a.dkv_strides[2];
   p.dq_sb = a.dq_strides[0]; p.dq_ss = a.dq_strides[1]; p.dq_sh = a.dq_strides[2];
-  const dim3 grid_kv((f.sk + 127) / 128, f.hk, f.b), grid_q((f.sq + 127) / 128, f.h, f.b);
-  static bool attr_set[8] = {false, false, false, false, false, false, false, false};
-  auto go = [&](auto kern, int slot, dim3 grid, int threads, const CUtensorMap& q, const CUtensorMap& k, const CUtensorMap& v, const CUtensorMap& d_o) {
-    if (!attr_set[slot]) { B200_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES)); attr_set[slot] = true; }
-    kern<<<grid, threads, SMEM_BYTES, s>>>(q, k, v, d_o, p);
-  };
   if (f.dtype == kBF16) {
-    if (p.colmask) { go(dkv_kernel<__nv_bfloat16, true>, 0, grid_kv, kThreadsDkv, mq[1], mk[0], mv[0], mdo[1]); go(dq_kernel<__nv_bfloat16, true>, 1, grid_q, kThreads, mq[0], mk[1], mv[1], mdo[0]); }
-    else { go(dkv_kernel<__nv_bfloat16, false>, 2, grid_kv, kThreadsDkv, mq[1], mk[0], mv[0], mdo[1]); go(dq_kernel<__nv_bfloat16, false>, 3, grid_q, kThreads, mq[0], mk[1], mv[1], mdo[0]); }
+    if (p.colmask) launch<__nv_bfloat16, true>(p, det, mq, mk, mv, mdo, mdq, s);
+    else launch<__nv_bfloat16, false>(p, det, mq, mk, mv, mdo, mdq, s);
   } else {
-    if (p.colmask) { go(dkv_kernel<__half, true>, 4, grid_kv, kThreadsDkv, mq[1], mk[0], mv[0], mdo[1]); go(dq_kernel<__half, true>, 5, grid_q, kThreads, mq[0], mk[1], mv[1], mdo[0]); }
-    else { go(dkv_kernel<__half, false>, 6, grid_kv, kThreadsDkv, mq[1], mk[0], mv[0], mdo[1]); go(dq_kernel<__half, false>, 7, grid_q, kThreads, mq[0], mk[1], mv[1], mdo[0]); }
+    if (p.colmask) launch<__half, true>(p, det, mq, mk, mv, mdo, mdq, s);
+    else launch<__half, false>(p, det, mq, mk, mv, mdo, mdq, s);
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }

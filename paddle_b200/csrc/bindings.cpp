@@ -1321,7 +1321,7 @@ void attention_out_quant(const Tensor& x, const Tensor& y, double out_scale, con
   TORCH_CHECK(rc == 0, "paddle_b200.attention_out_quant: unsupported operands rc=", rc);
 }
 
-static bool g_deterministic = false;     // FLAGS_cudnn_deterministic (the attention backward is order-independent as it is)
+static bool g_deterministic = false;     // FLAGS_cudnn_deterministic: the attention backward takes its bitwise-reproducible two-kernel path
 
 // backward of attention_fwd: returns (dq [B,Sq,H,D], dk, dv [B,Sk,Hk,D]) in the input dtype
 std::vector<Tensor> attention_bwd(const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& out, const Tensor& lse, const Tensor& d_out,
@@ -1335,11 +1335,12 @@ std::vector<Tensor> attention_bwd(const Tensor& q, const Tensor& k, const Tensor
   Tensor dq32 = torch::empty({a.fwd.b, a.fwd.sq, a.fwd.h, a.fwd.d}, q.options().dtype(at::kFloat));
   Tensor dk = torch::empty({a.fwd.b, a.fwd.sk, a.fwd.hk, a.fwd.d}, q.options());
   Tensor dv = torch::empty_like(dk);
-  Tensor delta = torch::empty({a.fwd.b, a.fwd.h, a.fwd.sq}, q.options().dtype(at::kFloat));
-  a.d_o = d_out.data_ptr(); a.delta = delta.data_ptr<float>(); a.dq = dq32.data_ptr<float>(); a.dk = dk.data_ptr(); a.dv = dv.data_ptr();
+  Tensor stats = torch::empty({a.fwd.b, a.fwd.h, 2, b200::attention_bwd_stats_pad(a.fwd.sq)}, q.options().dtype(at::kFloat));
+  a.d_o = d_out.data_ptr(); a.stats = stats.data_ptr<float>(); a.dq = dq32.data_ptr<float>(); a.dk = dk.data_ptr(); a.dv = dv.data_ptr();
+  a.deterministic = g_deterministic;
   for (int i = 0; i < 3; ++i) { a.dkv_strides[i] = dk.stride(i); a.o_strides[i] = out.stride(i); a.dq_strides[i] = dq32.stride(i); }
   int rc = b200::attention_bwd(a, cur_stream());
-  g_launches += 2;
+  g_launches += a.deterministic ? 3 : 2;     // prep + dK/dV + dQ, or prep + single pass
   check_err();
   TORCH_CHECK(rc == 0, "paddle_b200.attention_bwd launch failed rc=", rc);
   return {dq32.to(q.scalar_type()), dk, dv};
@@ -1363,11 +1364,12 @@ Tensor attention_bwd_packed(const Tensor& qkv, int64_t nh, int64_t nkv, const Te
   Tensor dk = bs(dqkv.narrow(2, nh, nkv)), dv = bs(dqkv.narrow(2, nh + nkv, nkv));
   Tensor dq32_mem = torch::empty(out.sizes(), qkv.options().dtype(at::kFloat));     // same memory order as `out`
   Tensor dq32 = bs(dq32_mem);
-  Tensor delta = torch::empty({a.fwd.b, a.fwd.h, a.fwd.sq}, qkv.options().dtype(at::kFloat));
-  a.d_o = d_out.data_ptr(); a.delta = delta.data_ptr<float>(); a.dq = dq32_mem.data_ptr<float>(); a.dk = dk.data_ptr(); a.dv = dv.data_ptr();
+  Tensor stats = torch::empty({a.fwd.b, a.fwd.h, 2, b200::attention_bwd_stats_pad(a.fwd.sq)}, qkv.options().dtype(at::kFloat));
+  a.d_o = d_out.data_ptr(); a.stats = stats.data_ptr<float>(); a.dq = dq32_mem.data_ptr<float>(); a.dk = dk.data_ptr(); a.dv = dv.data_ptr();
+  a.deterministic = g_deterministic;
   for (int i = 0; i < 3; ++i) { a.dkv_strides[i] = dk.stride(i); a.o_strides[i] = ov.stride(i); a.dq_strides[i] = dq32.stride(i); }
   int rc = b200::attention_bwd(a, cur_stream());
-  g_launches += 2;
+  g_launches += a.deterministic ? 3 : 2;     // prep + dK/dV + dQ, or prep + single pass
   check_err();
   TORCH_CHECK(rc == 0, "paddle_b200.attention_bwd_packed launch failed rc=", rc);
   dqkv.narrow(2, 0, nh).copy_(dq32_mem);

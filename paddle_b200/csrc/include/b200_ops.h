@@ -343,17 +343,19 @@ int attention_paged_prefill_scratch_ints(int t, int b);
 int attention_paged_prefill_supported(const PagedAttnArgs& a);
 int attention_paged_prefill(const PagedAttnArgs& a, cudaStream_t s);
 // Backward (attention_bwd_sm100.cu). fwd: the forward's arguments with o (contiguous [B,Sq,H,D]) and lse filled in.
-// d_o: contiguous [B,Sq,H,D]; delta: fp32 scratch [B,H,Sq]; dq: fp32 [B,Sq,H,D], every element written; dk/dv: [B,Sk,Hk,D] views (dkv_strides).
+// d_o: contiguous [B,Sq,H,D]; dq: fp32 [B,Sq,H,D] (dq_strides); dk/dv: [B,Sk,Hk,D] views (dkv_strides).
+int attention_bwd_stats_pad(int sq);   // the padded query length of AttnBwdArgs::stats
 struct AttnBwdArgs {
   AttnArgs fwd;
   const void* d_o;
-  float* delta;
-  float* dq;
+  float* stats;             // scratch, fp32 [B,H,2,attention_bwd_stats_pad(Sq)]: lse * log2(e) and delta = rowsum(dO * O)
+  float* dq;                // fp32 accumulator, 16-byte aligned; written in full (zeroed and reduced into unless deterministic)
   void* dk;
   void* dv;
   int64_t dkv_strides[3];   // element strides (batch, seq, head) of dk and dv (16-byte aligned rows)
   int64_t o_strides[3];     // element strides (batch, seq, head) shared by the forward output `fwd.o` and d_o
-  int64_t dq_strides[3];    // element strides (batch, seq, head) of the fp32 dq accumulator
+  int64_t dq_strides[3];    // element strides (batch, seq, head) of the fp32 dq accumulator (multiples of 4)
+  bool deterministic;       // dK / dV kernel + a separate dQ kernel, bitwise reproducible; otherwise one pass, dQ bulk-reduced
 };
 int attention_bwd(const AttnBwdArgs& a, cudaStream_t s);
 

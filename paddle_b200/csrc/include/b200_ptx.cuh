@@ -46,6 +46,21 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     if (spins > 2048 && (spins & 1023) == 0 && globaltimer_ns() - t0 > 4000000000ull) __trap();
   }
 }
+// Unbounded wait, for warps that raised their register budget with setmaxnreg.inc: a trap reachable there makes ptxas allocate the
+// whole kernel at its launch budget (168 registers at 384 threads) and spill.  Such a kernel's producer waits, bounded, until the
+// consumers have released every stage, so a protocol bug still traps.
+__device__ __forceinline__ void mbar_wait_unbounded(uint32_t bar, uint32_t parity) {
+  uint32_t done = 0;
+  do {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}"
+        : "=r"(done)
+        : "r"(bar), "r"(parity)
+        : "memory");
+  } while (!done);
+}
 
 // ---------------------------------------------------------------------------------------------- fences / cluster
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
@@ -83,6 +98,11 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map
 __device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2) {
   asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
                ::"l"(map), "r"(src), "r"(c0), "r"(c1), "r"(c2) : "memory");
+}
+// tile shared -> global, element-wise added to what is there (fp32: an atomic add per element, in arrival order across CTAs)
+__device__ __forceinline__ void tma_reduce_add_4d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.reduce.async.bulk.tensor.4d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+               ::"l"(map), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
 }
 __device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // at most N of this thread's committed bulk groups still read their shared-memory source

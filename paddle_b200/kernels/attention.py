@@ -4,7 +4,8 @@
 Dispatch: the sm_90a wgmma flash kernel (csrc/attention_sm100.cu) for fp16/bf16, head_dim 128, no explicit mask and no
 dropout — it reads q/k/v in place as strided views of a packed QKV projection; everything else takes the PyTorch SDPA
 (library) path.  Backward: csrc/attention_bwd_sm100.cu (B200_ATTN_BWD=own, default) or, for comparison, a library backward
-fed with our forward's (out, logsumexp) (B200_ATTN_BWD=cudnn|flash).
+fed with our forward's (out, logsumexp) (B200_ATTN_BWD=cudnn|flash).  The own backward is a single pass that bulk-reduces dQ in
+arrival order (reproducible to rounding); FLAGS_cudnn_deterministic switches it to a bitwise-reproducible dK/dV + dQ kernel pair.
 """
 from __future__ import annotations
 
@@ -47,7 +48,7 @@ class _FlashAttn(torch.autograd.Function):
     def backward(ctx, do):
         q, k, v, out, lse = ctx.saved_tensors
         do = do.contiguous()
-        if _bwd_backend[0] == "own":   # csrc/attention_bwd_sm100.cu: wgmma dK/dV kernel + dQ kernel, no atomics
+        if _bwd_backend[0] == "own":   # csrc/attention_bwd_sm100.cu: single pass, or dK/dV + dQ kernels under FLAGS_cudnn_deterministic
             dq, dk, dv = ext().attention_bwd(q, k, v, out, lse, do, ctx.scale, ctx.causal)
             return dq, dk, dv, None, None
         if _bwd_backend[0] == "cudnn" and q.shape[2] == k.shape[2]:
