@@ -175,69 +175,88 @@ __device__ __forceinline__ void store_pair(TO* __restrict__ dst, float v0, float
 // warpgroup's whole run in `cnt`) uses slot c & 1, so it is written while the store of box c - 1 still reads the other slot.
 // Invariant: once the warpgroup has passed the named barrier of box c, slot (c + 1) & 1 is free (the elected thread waited for the
 // store of box c - 1 to finish reading it just before that barrier). In accumulate mode the old D box is TMA-loaded into its slot
-// first (box 0 of a tile during the mainloop, box c + 1 right after box c is stored) and added in fp32, rounded once, as in
-// store_pair. TMA clips the boxes at the tensor bounds, so partial tiles need no per-element tests.
+// first and added in fp32, rounded once, as in store_pair. Two loads are in flight: boxes 0 and 1 of a tile land during the mainloop,
+// box c + 2 is loaded into box c's slot as soon as the store of box c has read it. TMA clips the boxes at the tensor bounds, so
+// partial tiles need no per-element tests.
 constexpr uint32_t kStageSlotBytes = 8192;
+
+template <typename TO, int BN>
+__device__ __forceinline__ int epilogue_boxes(const Params& p, int n0) {   // boxes that start right of column n are skipped
+  constexpr int CB = 128 / sizeof(TO);
+  return min(BN / CB, (p.n - n0 + CB - 1) / CB);
+}
+
+// One epilogue box of the warpgroup's half-tile into its staging slot: bias, activation and old D (accumulate mode) in fp32, one rounding.
+// PLAIN (no bias, no activation, no accumulate: every forward and dX GEMM of the model) drops those tests from the unrolled code, which
+// is what the epilogue's time goes to; the values are computed with the same fp32 operations (acc + 0.f), so the output bits are the same.
+template <typename TO, int BN, bool PLAIN>
+__device__ __forceinline__ void write_box(const float (&acc)[BN / 2], const Params& p, uint8_t* slot, int b, int n0, int ww, int lane) {
+  constexpr int CB = 128 / sizeof(TO);
+  struct alignas(2 * sizeof(TO)) Pair { TO a, b; };
+  const int rq = lane >> 2;                               // row within the 8-row swizzle atom
+#pragma unroll
+  for (int jj = 0; jj < CB / 8; ++jj) {
+    const int j = b * (CB / 8) + jj;
+    const int col = n0 + j * 8 + (lane & 3) * 2;
+    const int valid = p.n - col;
+    float b0 = 0.f, b1 = 0.f;
+    if (!PLAIN && p.has_bias && valid > 0) {
+      if (p.in_dtype == kBF16) {
+        const __nv_bfloat16* bp = (const __nv_bfloat16*)p.bias + col;
+        b0 = __bfloat162float(bp[0]);
+        if (valid > 1) b1 = __bfloat162float(bp[1]);
+      } else {
+        const __half* bp = (const __half*)p.bias + col;
+        b0 = __half2float(bp[0]);
+        if (valid > 1) b1 = __half2float(bp[1]);
+      }
+    }
+    const uint32_t byte = (jj * 8 + (lane & 3) * 2) * sizeof(TO);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      Pair* dst = reinterpret_cast<Pair*>(slot + (ww * 16 + h * 8 + rq) * 128 + (((byte >> 4) ^ rq) << 4) + (byte & 15));
+      float v0 = acc[j * 4 + h * 2] + b0, v1 = acc[j * 4 + h * 2 + 1] + b1;
+      if (!PLAIN && p.act == 1) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
+      else if (!PLAIN && p.act == 2) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+      if (!PLAIN && p.accumulate) {
+        const Pair old = *dst;
+        v0 += to_f(old.a);
+        v1 += to_f(old.b);
+      }
+      Pair o;
+      o.a = from_f<TO>(v0);
+      o.b = from_f<TO>(v1);
+      *dst = o;
+    }
+  }
+}
 
 template <typename TO, int BN>
 __device__ __forceinline__ void epilogue_tma(const float (&acc)[BN / 2], const Params& p, const CUtensorMap* map_d, uint8_t* stg,
                                              uint32_t ld_bar, uint32_t& cnt, int m0, int n0, int zd, int ww, int lane, int bar_id) {
   constexpr int CB = 128 / sizeof(TO);                    // columns per box
   constexpr int NB = BN / CB;                             // boxes per half-tile (BN >= 64)
-  struct alignas(2 * sizeof(TO)) Pair { TO a, b; };
-  const int nbox = min(NB, (p.n - n0 + CB - 1) / CB);     // boxes that start right of column n are skipped
+  const int nbox = epilogue_boxes<TO, BN>(p, n0);
   const bool elected = ww == 0 && lane == 0;
-  const int rq = lane >> 2;                               // row within the 8-row swizzle atom
+  const bool plain = !p.has_bias && p.act == 0 && !p.accumulate;
 #pragma unroll
   for (int b = 0; b < NB; ++b) {
     if (b >= nbox) break;
     uint8_t* slot = stg + (cnt & 1) * kStageSlotBytes;
-    if (p.accumulate) mbar_wait(ld_bar + 8 * (cnt & 1), (cnt >> 1) & 1);
-#pragma unroll
-    for (int jj = 0; jj < CB / 8; ++jj) {
-      const int j = b * (CB / 8) + jj;
-      const int col = n0 + j * 8 + (lane & 3) * 2;
-      const int valid = p.n - col;
-      float b0 = 0.f, b1 = 0.f;
-      if (p.has_bias && valid > 0) {
-        if (p.in_dtype == kBF16) {
-          const __nv_bfloat16* bp = (const __nv_bfloat16*)p.bias + col;
-          b0 = __bfloat162float(bp[0]);
-          if (valid > 1) b1 = __bfloat162float(bp[1]);
-        } else {
-          const __half* bp = (const __half*)p.bias + col;
-          b0 = __half2float(bp[0]);
-          if (valid > 1) b1 = __half2float(bp[1]);
-        }
-      }
-      const uint32_t byte = (jj * 8 + (lane & 3) * 2) * sizeof(TO);
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        Pair* dst = reinterpret_cast<Pair*>(slot + (ww * 16 + h * 8 + rq) * 128 + (((byte >> 4) ^ rq) << 4) + (byte & 15));
-        float v0 = acc[j * 4 + h * 2] + b0, v1 = acc[j * 4 + h * 2 + 1] + b1;
-        if (p.act == 1) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
-        else if (p.act == 2) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-        if (p.accumulate) {
-          const Pair old = *dst;
-          v0 += to_f(old.a);
-          v1 += to_f(old.b);
-        }
-        Pair o;
-        o.a = from_f<TO>(v0);
-        o.b = from_f<TO>(v1);
-        *dst = o;
-      }
-    }
+    if (p.accumulate) mbar_wait_unbounded(ld_bar + 8 * (cnt & 1), (cnt >> 1) & 1);
+    if (plain) write_box<TO, BN, true>(acc, p, slot, b, n0, ww, lane);
+    else write_box<TO, BN, false>(acc, p, slot, b, n0, ww, lane);
     fence_proxy_async();                                  // generic-proxy writes -> the TMA store (async proxy) reads them
     if (elected) bulk_wait_group_read<0>();               // the store of box cnt - 1 is done with the other slot
     named_bar_sync(bar_id, 128);
     if (elected) {
       tma_store_3d(map_d, smem_u32(slot), n0 + b * CB, m0, zd);
       bulk_commit_group();
-      if (p.accumulate && b + 1 < nbox) {
-        const uint32_t next = (cnt + 1) & 1;
-        mbar_expect_tx(ld_bar + 8 * next, kStageSlotBytes);
-        tma_load_3d(smem_u32(stg + next * kStageSlotBytes), map_d, ld_bar + 8 * next, n0 + (b + 1) * CB, m0, zd);
+      if (p.accumulate && b + 2 < nbox) {
+        bulk_wait_group_read<0>();                        // the store of box cnt has read the slot
+        const uint32_t s = cnt & 1;
+        mbar_expect_tx(ld_bar + 8 * s, kStageSlotBytes);
+        tma_load_3d(smem_u32(slot), map_d, ld_bar + 8 * s, n0 + (b + 2) * CB, m0, zd);
       }
     }
     ++cnt;
@@ -257,6 +276,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (kStages + s); };
   auto load_bar = [&](int wg) { return bar_base + 8u * (2 * kStages + 2 * wg); };   // two slots per warpgroup (accumulate mode)
+  const uint32_t done_bar = bar_base + 8u * (2 * kStages + 4);                        // every consumer warp has finished
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_m = (p.m + BLOCK_M - 1) / BLOCK_M, num_n = (p.n + BN - 1) / BN;
@@ -270,6 +290,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
     if (p.tma_store) tma_prefetch_desc(&map_d);
     for (int s = 0; s < kStages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kConsumerWarps); }
     for (int s = 0; s < 4; ++s) mbar_init(load_bar(0) + 8u * s, 1);
+    mbar_init(done_bar, kConsumerWarps);
     fence_barrier_init();
     fence_proxy_async();
   }
@@ -348,6 +369,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
           if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
       }
+      // The consumers wait unbounded (a reachable trap would cap their registers at the launch budget), so the producer waits,
+      // bounded, until they have released every stage and finished: a protocol bug traps here instead of hanging the GPU.
+      for (int i = 0; i < kStages; ++i) {
+        mbar_wait(empty_bar(stage), phase ^ 1);
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
+      }
+      mbar_wait(done_bar, 0);
     } else if (warp == 1 && p.ag_world > 1) {
       ag_copy_role(p, lane);
     }
@@ -365,14 +393,21 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
       tile_coords(tile, bz, mb, nb);
       int za, zb, zd, kbeg, nkb;
       if (!tile_group(bz, mb, za, zb, zd, kbeg, nkb)) continue;
-      if (p.tma_store && p.accumulate && elected) {   // old D of the first epilogue box lands during the mainloop
-        const uint32_t s = boxes & 1;
+      // accumulate mode: old D of the first two epilogue boxes lands during the mainloop, box 0 into slot boxes & 1 (free since the
+      // previous tile's stores) and, after the first k-block, box 1 into the other slot once the previous tile's last store has read it
+      const int old_boxes = !(p.tma_store && p.accumulate) ? 0 : (p.out_dtype == kF32 ? epilogue_boxes<float, BN>(p, nb * BN)
+                                                                                         : epilogue_boxes<uint16_t, BN>(p, nb * BN));
+      const int old_cb = p.out_dtype == kF32 ? 32 : 64;
+      auto load_old = [&](int b) {
+        const uint32_t s = (boxes + b) & 1;
         mbar_expect_tx(load_bar(wg) + 8 * s, kStageSlotBytes);
-        tma_load_3d(smem_u32(staging[wg] + s * kStageSlotBytes), &map_d, load_bar(wg) + 8 * s, nb * BN, mb * BLOCK_M + wg * 64, zd);
-      }
+        tma_load_3d(smem_u32(staging[wg] + s * kStageSlotBytes), &map_d, load_bar(wg) + 8 * s, nb * BN + b * old_cb,
+                    mb * BLOCK_M + wg * 64, zd);
+      };
+      if (old_boxes > 0 && elected) load_old(0);
       int prev = -1;
       for (int kb = 0; kb < nkb; ++kb) {
-        mbar_wait(full_bar(stage), phase);
+        mbar_wait_unbounded(full_bar(stage), phase);
         const uint32_t sa = smem_base + stage * C::STAGE_BYTES + wg * 8192;   // 64 rows (K-major) or one {64 m, 64 k} box (MN-major)
         const uint32_t sb = smem_base + stage * C::STAGE_BYTES + A_STAGE_BYTES;
         wgmma_fence_regs(acc);
@@ -393,6 +428,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
         }
         prev = stage;
         if (++stage == kStages) { stage = 0; phase ^= 1; }
+        if (kb == 0 && old_boxes > 1 && elected) {
+          bulk_wait_group_read<0>();
+          load_old(1);
+        }
       }
       wgmma_wait<0>();
       wgmma_fence_regs(acc);
@@ -447,6 +486,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
       }
     }
     if (p.tma_store && elected) bulk_wait_group<0>();   // the staging buffer must outlive the last store's reads
+    __syncwarp();
+    if (lane == 0) mbar_arrive(done_bar);
   }
 }
 
