@@ -801,6 +801,80 @@ Tensor gemm_fp8(const Tensor& a, const Tensor& b, const OptT& bias, double scale
   return d;
 }
 
+// int8 x int8 GEMM (csrc/gemm_fp8_sm100.cu, gemm_s8_kernel): a [M,K] / [B,M,K], b [N,K] / [B,N,K] int8 contiguous, K % 16 == 0
+b200::GemmS8Args s8_args(const Tensor& a, const Tensor& b, const char* name) {
+  TORCH_CHECK(a.is_cuda() && b.is_cuda() && a.scalar_type() == at::kChar && b.scalar_type() == at::kChar, name, ": int8 CUDA operands required");
+  TORCH_CHECK(a.dim() == b.dim() && (a.dim() == 2 || a.dim() == 3) && a.is_contiguous() && b.is_contiguous() && a.size(-1) == b.size(-1)
+              && (a.dim() == 2 || a.size(0) == b.size(0)), name, ": operands must be contiguous [M,K] and [N,K] (or [B,M,K] and [B,N,K])");
+  TORCH_CHECK(a.device() == b.device(), name, ": operands on one device");
+  TORCH_CHECK(a.size(-1) % 16 == 0, name, ": K must be a multiple of 16");
+  b200::GemmS8Args g;
+  g.a = a.data_ptr(); g.b = b.data_ptr();
+  g.m = (int)a.size(-2); g.n = (int)b.size(-2); g.k = (int)a.size(-1);
+  g.lda = a.stride(-2); g.ldb = b.stride(-2);
+  g.batch = a.dim() == 3 ? (int)a.size(0) : 1;
+  g.stride_a = a.dim() == 3 ? a.stride(0) : 0;
+  g.stride_b = b.dim() == 3 ? b.stride(0) : 0;
+  return g;
+}
+
+Tensor gemm_int8(const Tensor& a, const Tensor& b) {
+  b200::GemmS8Args g = s8_args(a, b, "gemm_int8");
+  c10::cuda::CUDAGuard guard(a.device());
+  Tensor d = a.dim() == 3 ? torch::empty({a.size(0), g.m, g.n}, a.options().dtype(at::kInt)) : torch::empty({g.m, g.n}, a.options().dtype(at::kInt));
+  if (g.batch == 0 || g.m == 0 || g.n == 0) return d;
+  g.d = d.data_ptr(); g.ldd = d.stride(-2); g.stride_d = a.dim() == 3 ? d.stride(0) : 0;
+  g.out_i32 = 1; g.out_dtype = 0;
+  int rc = b200::gemm_s8(g, cur_stream());
+  g_launches += 1;
+  check_err();
+  TORCH_CHECK(rc == 0, "paddle_b200.gemm_int8 launch failed rc=", rc);
+  return d;
+}
+
+// (float(a @ b^T) * row_scale[m]) * col_scale[n] (+ bias[n]) in out_dtype; row_scale fp32 [M], col_scale fp32 [N], bias fp32 [N]
+Tensor gemm_int8_dequant(const Tensor& a, const Tensor& b, const Tensor& row_scale, const Tensor& col_scale, const OptT& bias, at::ScalarType out_dtype) {
+  TORCH_CHECK(a.dim() == 2, "gemm_int8_dequant: 2-D operands");
+  b200::GemmS8Args g = s8_args(a, b, "gemm_int8_dequant");
+  auto vec = [&](const Tensor& t, int64_t n) {
+    return t.is_cuda() && t.device() == a.device() && t.scalar_type() == at::kFloat && t.dim() == 1 && t.numel() == n && t.is_contiguous();
+  };
+  TORCH_CHECK(vec(row_scale, g.m) && vec(col_scale, g.n), "gemm_int8_dequant: row_scale / col_scale must be contiguous float32 [M] / [N]");
+  const bool has_bias = bias.has_value() && bias->defined();
+  TORCH_CHECK(!has_bias || vec(*bias, g.n), "gemm_int8_dequant: bias must be contiguous float32 [N]");
+  c10::cuda::CUDAGuard guard(a.device());
+  Tensor d = torch::empty({g.m, g.n}, a.options().dtype(out_dtype));
+  if (g.m == 0 || g.n == 0) return d;
+  g.d = d.data_ptr(); g.ldd = d.stride(0); g.stride_d = 0;
+  g.out_i32 = 0; g.out_dtype = dt_code(out_dtype);
+  g.row_scale = row_scale.data_ptr<float>(); g.col_scale = col_scale.data_ptr<float>();
+  g.bias = has_bias ? bias->data_ptr<float>() : nullptr;
+  int rc = b200::gemm_s8(g, cur_stream());
+  g_launches += 1;
+  check_err();
+  TORCH_CHECK(rc == 0, "paddle_b200.gemm_int8_dequant launch failed rc=", rc);
+  return d;
+}
+
+// per-token int8 quantisation of a contiguous [M, K] bf16 / fp16 / fp32 tensor (K % 16 == 0): (q int8 [M, K], row_scale fp32 [M]);
+// columns where mask (bool [K]) is set are left out of the scale and written as 0.  One launch.
+std::vector<Tensor> quantize_int8_rows(const Tensor& x, const OptT& mask) {
+  check_cuda_contig(x, "quantize_int8_rows: x");
+  TORCH_CHECK(x.dim() == 2 && x.size(1) % 16 == 0 && reinterpret_cast<uintptr_t>(x.data_ptr()) % 16 == 0,
+              "quantize_int8_rows: x must be a 16-byte aligned [M, K] with K a multiple of 16");
+  const bool has_mask = mask.has_value() && mask->defined();
+  TORCH_CHECK(!has_mask || (mask->is_cuda() && mask->device() == x.device() && mask->scalar_type() == at::kBool && mask->dim() == 1
+                            && mask->numel() == x.size(1) && mask->is_contiguous()), "quantize_int8_rows: mask must be a contiguous bool [K] on x's device");
+  c10::cuda::CUDAGuard guard(x.device());
+  Tensor q = torch::empty({x.size(0), x.size(1)}, x.options().dtype(at::kChar));
+  Tensor sc = torch::empty({x.size(0)}, x.options().dtype(at::kFloat));
+  b200::quantize_rows_s8(x.data_ptr(), has_mask ? reinterpret_cast<const uint8_t*>(mask->data_ptr<bool>()) : nullptr, x.size(0), x.size(1), dt_code(x),
+                         q.data_ptr<int8_t>(), sc.data_ptr<float>(), cur_stream());
+  g_launches += 1;
+  check_err();
+  return {q, sc};
+}
+
 // OCP MX quantisation of a contiguous [rows, K] tensor (rows, K multiples of 128) along K: (q e4m3 [rows, K], sf uint8 [rows / 128 * K / 128 * 512])
 std::vector<Tensor> quantize_mx(const Tensor& x) {
   TORCH_CHECK(x.is_cuda() && x.dim() == 2 && x.is_contiguous() && x.size(0) % 128 == 0 && x.size(1) % 128 == 0, "quantize_mx: contiguous [rows, K] with rows, K multiples of 128");
@@ -1500,6 +1574,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("dequantize_mx", traced("dequantize_mx", &dequantize_mx));
   m.def("gemm_fp8_mx", traced("gemm_fp8_mx", &gemm_fp8_mx), pybind11::arg("a"), pybind11::arg("sfa"), pybind11::arg("b"), pybind11::arg("sfb"), pybind11::arg("bias") = pybind11::none(),
         pybind11::arg("out_dtype") = at::kBFloat16);
+  m.def("gemm_int8", traced("gemm_int8", &gemm_int8), pybind11::arg("a"), pybind11::arg("b"));
+  m.def("gemm_int8_dequant", traced("gemm_int8_dequant", &gemm_int8_dequant), pybind11::arg("a"), pybind11::arg("b"), pybind11::arg("row_scale"),
+        pybind11::arg("col_scale"), pybind11::arg("bias") = pybind11::none(), pybind11::arg("out_dtype") = at::kFloat);
+  m.def("quantize_int8_rows", traced("quantize_int8_rows", &quantize_int8_rows), pybind11::arg("x"), pybind11::arg("mask") = pybind11::none());
   m.def("quantize_fp8", traced("quantize_fp8", &quantize_fp8), pybind11::arg("x"), pybind11::arg("e5m2") = false, pybind11::arg("want_transpose") = false);
   m.def("set_deterministic", [](bool on) { g_deterministic = on; });
   m.def("deterministic", []() { return g_deterministic; });

@@ -164,8 +164,25 @@ struct GemmFp8Args {
   int64_t stride_a, stride_b, stride_d;
 };
 int gemm_fp8_tcgen05(const GemmFp8Args& g, cudaStream_t s);
+// D[M,N] = A[M,K] * B[N,K]^T with int8 operands (K contiguous, K % 16 == 0, 16-byte aligned) and exact s32 accumulation.  out_i32: D
+// int32; else D in out_dtype (bf16 / fp16 / fp32) = (float(acc) * row_scale[m]) * col_scale[n] (+ bias[n]), each step rounded on its
+// own (fp32 row_scale [M], col_scale [N], bias [N]; batch 1 only).  Returns nonzero for an unsupported shape.
+struct GemmS8Args {
+  const void* a; const void* b; void* d;
+  const float* row_scale = nullptr; const float* col_scale = nullptr; const float* bias = nullptr;
+  int m, n, k;
+  int64_t lda, ldb, ldd;
+  int out_i32, out_dtype;
+  int batch;
+  int64_t stride_a, stride_b, stride_d;
+};
+int gemm_s8(const GemmS8Args& g, cudaStream_t s);
 // OCP MX quantisation of a contiguous [rows, k] tensor along k: q = e4m3(x / 2^e), one E8M0 byte (e + 127) per 32 elements, written in
 // the 512-byte block layout [rows / 128][k / 128][(row % 32) * 16 + ((row % 128) / 32) * 4 + (k / 32) % 4] the block-scaled MMA consumes.
+// Per-token int8 quantisation of a contiguous [rows, k] bf16 / fp16 / fp32 tensor (k % 16 == 0), in fp32 with IEEE division:
+// row_scale[r] = max(max |x[r, c]|, 1e-8) / 127 over the columns c with mask[c] == 0 (mask uint8 [k] or nullptr),
+// q[r, c] = clamp(rint(x[r, c] / row_scale[r]), -128, 127), and 0 in masked columns.  One block per row.
+void quantize_rows_s8(const void* x, const uint8_t* mask, int64_t rows, int64_t k, int dtype, int8_t* q, float* row_scale, cudaStream_t s);
 int mx_quantize(const void* x, int64_t rows, int64_t k, int dtype, void* q, uint8_t* sf, cudaStream_t s);
 int mx_dequantize(const void* q, const uint8_t* sf, int64_t rows, int64_t k, float* out, cudaStream_t s);
 // ---- quant_fp8.cu: fused per-tensor fp8 quantisation ----------------------------------------------------------

@@ -172,4 +172,43 @@ int mx_dequantize(const void* q, const uint8_t* sf, int64_t rows, int64_t k, flo
   return 0;
 }
 
+// ------------------------------------------------------------------------------------------------ per-token int8
+// One block per row, two passes over it (the second is served from L1 / L2).  The expression is the torch one of nn/quant.py
+// (llm_int8_linear), in fp32 with IEEE division and round-half-even, so both give the same bits.
+template <typename T>
+__global__ void __launch_bounds__(128) quantize_rows_s8_kernel(const T* __restrict__ x, const uint8_t* __restrict__ mask, int64_t k,
+                                                               int8_t* __restrict__ q, float* __restrict__ row_scale) {
+  __shared__ float red[33];
+  constexpr int N = Vec16<T>::N;
+  const T* xr = x + blockIdx.x * k;
+  int8_t* qr = q + blockIdx.x * k;
+  float m = 0.f;
+  for (int64_t c = threadIdx.x * N; c < k; c += blockDim.x * N) {
+    const Vec16<T> v = ld16(xr + c);
+#pragma unroll
+    for (int j = 0; j < N; ++j)
+      if (!mask || !mask[c + j]) m = fmaxf(m, fabsf(to_f(v.v[j])));
+  }
+  m = block_max(m, red);
+  const float sc = __fdiv_rn(fmaxf(m, 1e-8f), 127.f);
+  if (threadIdx.x == 0) row_scale[blockIdx.x] = sc;
+  for (int64_t c = threadIdx.x * N; c < k; c += blockDim.x * N) {
+    const Vec16<T> v = ld16(xr + c);
+    alignas(8) int8_t o[N];
+#pragma unroll
+    for (int j = 0; j < N; ++j) {
+      const float t = mask && mask[c + j] ? 0.f : rintf(__fdiv_rn(to_f(v.v[j]), sc));
+      o[j] = (int8_t)fminf(fmaxf(t, -128.f), 127.f);
+    }
+    if constexpr (N == 8) *reinterpret_cast<uint2*>(qr + c) = *reinterpret_cast<const uint2*>(o);
+    else *reinterpret_cast<uint32_t*>(qr + c) = *reinterpret_cast<const uint32_t*>(o);
+  }
+}
+
+void quantize_rows_s8(const void* x, const uint8_t* mask, int64_t rows, int64_t k, int dtype, int8_t* q, float* row_scale, cudaStream_t s) {
+  if (rows == 0) return;
+  B200_DISPATCH_DTYPE(dtype, T, (quantize_rows_s8_kernel<T><<<(unsigned)rows, 128, 0, s>>>((const T*)x, mask, k, q, row_scale)));
+  B200_CUDA_CHECK(cudaGetLastError());
+}
+
 }  // namespace b200

@@ -176,6 +176,9 @@ def _register_builtin(f):
     r("mx_gemm", G, ("float8_e4m3fn",), "kernels.gemm_fp8:mx_gemm", native="csrc/gemm_fp8_sm100.cu (MX scales applied in registers)")
     r("weight_only_linear", G, HALF, "nn.quant:weight_only_linear", native="csrc/gemm_wo_sm100.cu::wo_gemm_kernel", priority=10)
     r("weight_only_linear", A, ("*",), "nn.quant:weight_only_linear")
+    r("matmul", G, ("int8",), "ops.linalg:matmul", native="csrc/gemm_fp8_sm100.cu::gemm_s8_kernel (int8 x int8 -> int32)", priority=10)
+    r("llm_int8_linear", G, HALF, "nn.quant:llm_int8_linear", native="csrc/quant_fp8.cu::quantize_rows_s8_kernel, csrc/gemm_fp8_sm100.cu::gemm_s8_kernel", priority=10)
+    r("llm_int8_linear", A, ("*",), "nn.quant:llm_int8_linear")
     # attention
     r("flash_attn", G, HALF, "kernels.attention:attention", predicate=_hd128, native="csrc/attention_sm100.cu, csrc/attention_bwd_sm100.cu", priority=10)
     r("flash_attn", A, ("*",), "kernels.attention:attention_ref")

@@ -5,7 +5,7 @@ from .mixtral import MixtralConfig, MixtralForCausalLM, mixtral_8x7b, mixtral_ti
 from .mlp import MnistMLP  # noqa: F401,E402
 from .generation import KVCache, LlamaGenerator, generate  # noqa: F401,E402
 from .serving import BlockAllocator, LLMEngine, calibrate_kv_cache  # noqa: F401,E402
-from .weight_only import WeightOnlyLinear, quantize_weights  # noqa: F401,E402
+from .weight_only import LLMInt8Linear, WeightOnlyLinear, quantize_weights  # noqa: F401,E402
 
 
 def resnet50(**kw):

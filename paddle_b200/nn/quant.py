@@ -100,18 +100,53 @@ def weight_only_linear(x, weight, bias=None, weight_scale=None, weight_dtype="in
 
 
 def llm_int8_linear(x, weight, bias=None, weight_scale=None, threshold=6.0):
-    xr = x.as_subclass(torch.Tensor)
+    """LLM.int8(): y = x @ dequant(weight)^T + bias with int8 activations.  weight int8 [out, in] and weight_scale fp32 [out] come from
+    `weight_quantize(algo="llm.int8")`.  Outlier columns (any |x| > threshold over all rows) stay in x's dtype and are multiplied with
+    their dequantised weight rows in fp32; the other columns are quantised per token (kernels.gemm_int8.quantize_int8_rows) and run
+    through the int8 GEMM with exact integer sums, dequantised as (float(acc) * row_scale[m]) * weight_scale[n].  The two parts are
+    added in fp32, then the bias, and the result is cast once to x's dtype.
+
+    CUDA bf16 / fp16 activations (in % 16 == 0) run the sm_90a kernels.  A finite threshold reads the number of outlier columns on the
+    host once per call; threshold=float("inf") skips outlier detection entirely: two launches (quantizer, int8 GEMM) and no host read,
+    the path to use for serving."""
+    from ..kernels import gemm_int8 as G8
+
+    xr, wr = x.as_subclass(torch.Tensor), weight.as_subclass(torch.Tensor)
+    ws = weight_scale.as_subclass(torch.Tensor).float()
+    br = None if bias is None else bias.as_subclass(torch.Tensor)
+    k = xr.shape[-1]
+    x2 = xr.reshape(-1, k)
+    no_outliers = threshold == float("inf")
+    if xr.is_cuda and xr.dtype in (torch.bfloat16, torch.float16) and wr.dtype == torch.int8 and k % 16 == 0:
+        from ..framework.flags import flag
+
+        if flag("FLAGS_use_fused_kernels", True):
+            if no_outliers:
+                xq, sx = G8.quantize_int8_rows(x2)
+                y = G8.gemm_int8_dequant(xq, wr, sx, ws, br, xr.dtype)
+                return _w(y.reshape(*xr.shape[:-1], wr.shape[0]))
+            outlier = (x2.abs() > threshold).any(0)
+            xq, sx = G8.quantize_int8_rows(x2, outlier)
+            out = G8.gemm_int8_dequant(xq, wr, sx, ws, None, torch.float32)
+            idx = outlier.nonzero().flatten()                   # the one host read: the outlier count
+            if idx.numel():
+                from ..kernels.gemm import gemm
+
+                pad = (-idx.numel()) % 8                        # zero columns / rows keep the 16-byte TMA granularity
+                xo = torch.nn.functional.pad(x2[:, idx], (0, pad)).contiguous()
+                wo = torch.nn.functional.pad(_dequantize_torch(wr[:, idx], ws, False, xr.dtype, -1), (0, 0, 0, pad)).contiguous()
+                gemm(xo, wo, epilogue=4, out=out)                # out += x_outlier @ w_outlier, summed in fp32
+            if br is not None:
+                out = out + br.float()
+            return _w(out.to(xr.dtype).reshape(*xr.shape[:-1], wr.shape[0]))
+    outlier = torch.zeros(k, dtype=torch.bool, device=xr.device) if no_outliers else (x2.abs() > threshold).any(0)
+    xq, sx = G8.quantize_int8_rows(x2, outlier)
+    out = G8.matmul_exact(xq, wr.t()).float() * sx.unsqueeze(1) * ws
     w = weight_dequantize(weight, weight_scale, "weight_only_int8", x.dtype).as_subclass(torch.Tensor)
-    outlier = (xr.abs() > threshold).any(dim=tuple(range(xr.dim() - 1)))
-    x_in = xr.clone()
-    x_in[..., outlier] = 0
-    sx = x_in.abs().amax(-1, keepdim=True).clamp(min=1e-8) / 127.0
-    xq = torch.round(x_in / sx).clamp(-128, 127)
-    out = (xq.float() @ torch.round(w.float() / weight_scale.as_subclass(torch.Tensor).float()).float()) * sx.float() * weight_scale.as_subclass(torch.Tensor).float()
-    out = out + xr[..., outlier].float() @ w[outlier].float()
-    if bias is not None:
-        out = out + bias.as_subclass(torch.Tensor).float()
-    return _w(out.to(x.dtype))
+    out = out + x2[:, outlier].float() @ w[outlier].float()
+    if br is not None:
+        out = out + br.float()
+    return _w(out.to(x.dtype).reshape(*xr.shape[:-1], wr.shape[0]))
 
 
 def apply_per_channel_scale(x, scales):

@@ -11,6 +11,8 @@ def matmul(x, y, transpose_x=False, transpose_y=False, name=None):
     x, y = T(x), T(y)
     if transpose_x and x.dim() >= 2:
         x = torch.transpose(x, -1, -2)
+    if x.dtype == torch.int8 and y.dtype == torch.int8:
+        return _matmul_int8(x, y, transpose_y)
     if transpose_y and y.dim() >= 2:
         y = torch.transpose(y, -1, -2)
     from ..amp.auto_cast import _state, fp32_guard
@@ -20,6 +22,23 @@ def matmul(x, y, transpose_x=False, transpose_y=False, name=None):
         with ctx:
             return torch.matmul(x, y)
     return torch.matmul(x, y)
+
+
+def _matmul_int8(x, y, transpose_y):
+    """int8 @ int8 -> int32, exact, on every device (the reference's cuBLASLt int8 -> int32 matmul).  CUDA 2-D operands and 3-D ones with
+    one batch size run the int8 wgmma GEMM (kernels/gemm_int8.py), which takes B as [N, K]: transpose_y=True feeds y directly, otherwise
+    one int8 copy of y^T is made.  Other shapes (K % 16 != 0, broadcasting, vectors) and CPU tensors: float64 product, exact while
+    |sum| < 2^53."""
+    from ..kernels import gemm_int8 as G8
+    from ..kernels import use_fused
+
+    if use_fused(x) and y.is_cuda and x.dim() == y.dim() and x.dim() in (2, 3) and (x.dim() == 2 or x.shape[0] == y.shape[0]) \
+            and x.shape[-1] % 16 == 0 and x.shape[-1] > 0 and x.shape[-1] == y.shape[-1 if transpose_y else -2]:
+        b = y if transpose_y else torch.transpose(y, -1, -2)
+        return wrap(G8.gemm_int8(x.contiguous(), b.contiguous()))
+    if transpose_y and y.dim() >= 2:
+        y = torch.transpose(y, -1, -2)
+    return wrap(G8.matmul_exact(x, y))
 
 
 def mm(input, mat2, name=None):
