@@ -19,7 +19,6 @@
 // Parity (behaviour): flash_attn_grad (paddle/phi/kernels/gpu/flash_attn_grad_kernel.cu -> flash-attention library).
 #include <cuda.h>
 #include <cstdio>
-#include <string>
 #include <type_traits>
 
 #include "include/b200_common.cuh"
@@ -39,15 +38,6 @@ constexpr uint32_t SMALL_BYTES = 64 * 128 * 2;    // a 64-row tile, same structu
 constexpr uint32_t SMALL_HALF = SMALL_BYTES / 2;
 constexpr uint32_t SMEM_BYTES = 2 * BIG_BYTES + 4 * SMALL_BYTES + 1024 + 256;   // two resident 128-row tiles + two double-buffered 64-row tiles
 
-template <typename T> __device__ __forceinline__ uint32_t pack2(float a, float b);
-template <> __device__ __forceinline__ uint32_t pack2<__nv_bfloat16>(float a, float b) {
-  const __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<const uint32_t*>(&v);
-}
-template <> __device__ __forceinline__ uint32_t pack2<__half>(float a, float b) {
-  const __half2 v = __floats2half2_rn(a, b);
-  return *reinterpret_cast<const uint32_t*>(&v);
-}
 __device__ __forceinline__ void keep_regs(uint32_t (&a)[4][4]) {
 #pragma unroll
   for (int i = 0; i < 4; ++i)
@@ -513,57 +503,18 @@ __global__ void prep_kernel(const T* __restrict__ o, const T* __restrict__ d_o, 
     *reinterpret_cast<float4*>(dq + bb * dq_sb + (int64_t)sidx * dq_ss + (int64_t)head * dq_sh + lane * 4) = make_float4(0.f, 0.f, 0.f, 0.f);
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = (EncodeTiledFn)p;
-  }
-  return fn;
-}
-static bool encode4(CUtensorMap* out, CUtensorMapDataType type, uint32_t esize, const void* ptr, int d, int s, int h, int b, int64_t ss,
-                    int64_t sh, int64_t sb, uint32_t box_d, uint32_t box_rows) {
-  bind_primary_context();
-  EncodeTiledFn enc = get_encode();
-  if (!enc) { set_last_error(__FILE__, __LINE__, "cuTensorMapEncodeTiled unavailable"); return false; }
-  cuuint64_t dims[4] = {(cuuint64_t)d, (cuuint64_t)s, (cuuint64_t)h, (cuuint64_t)b};
-  cuuint64_t strides[3] = {(cuuint64_t)ss * esize, (cuuint64_t)sh * esize, (cuuint64_t)sb * esize};
-  cuuint32_t box[4] = {box_d, box_rows, 1, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(out, type, 4, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_last_error(__FILE__, __LINE__, ("cuTensorMapEncodeTiled (attention bwd) failed: " + std::to_string((int)r)).c_str());
-    return false;
-  }
-  return true;
-}
-// a 16-bit operand [B,S,H,D] in boxes of 64 d x box_rows rows
-static bool make_map4(CUtensorMap* out, const void* ptr, int d, int s, int h, int b, int64_t ss, int64_t sh, int64_t sb, uint32_t box_rows, int dtype) {
-  return encode4(out, dtype == kBF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, ptr, d, s, h, b, ss, sh, sb, 64, box_rows);
-}
-
 // deterministic: dkv_kernel without the dQ stage, then dq_kernel; otherwise the single pass (dQ zeroed by prep_kernel)
 template <typename T, bool MASKED>
 static void launch(const Params& p, bool deterministic, const CUtensorMap (&mq)[2], const CUtensorMap (&mk)[2], const CUtensorMap (&mv)[2],
                    const CUtensorMap (&mdo)[2], const CUtensorMap& mdq, cudaStream_t s) {
-  static bool attr_set[3] = {false, false, false};
   const dim3 grid_kv(p.hk, p.b, (p.sk + 127) / 128), grid_q((p.sq + 127) / 128, p.h, p.b);
-  auto smem = [&](auto kern, int slot, uint32_t bytes) {
-    if (!attr_set[slot]) { B200_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)); attr_set[slot] = true; }
-  };
   if (deterministic) {
-    smem(dkv_kernel<T, MASKED, false>, 0, DkvSmem::BYTES);
-    smem(dq_kernel<T, MASKED>, 1, SMEM_BYTES);
+    set_max_dynamic_smem<dkv_kernel<T, MASKED, false>>(DkvSmem::BYTES);
+    set_max_dynamic_smem<dq_kernel<T, MASKED>>(SMEM_BYTES);
     dkv_kernel<T, MASKED, false><<<grid_kv, kThreadsDkv, DkvSmem::BYTES, s>>>(mq[1], mk[0], mv[0], mdo[1], mdq, p);
     dq_kernel<T, MASKED><<<grid_q, kThreads, SMEM_BYTES, s>>>(mq[0], mk[1], mv[1], mdo[0], p);
   } else {
-    smem(dkv_kernel<T, MASKED, true>, 2, DkvSmem::BYTES);
+    set_max_dynamic_smem<dkv_kernel<T, MASKED, true>>(DkvSmem::BYTES);
     dkv_kernel<T, MASKED, true><<<grid_kv, kThreadsDkv, DkvSmem::BYTES, s>>>(mq[1], mk[0], mv[0], mdo[1], mdq, p);
   }
 }
@@ -581,14 +532,13 @@ int attention_bwd(const AttnBwdArgs& a, cudaStream_t s) {
   CUtensorMap mq[2], mk[2], mv[2], mdo[2], mdq;
   for (int i = 0; i < 2; ++i) {
     const uint32_t rows = i ? 64 : 128;
-    if (!make_map4(&mq[i], f.q, f.d, f.sq, f.h, f.b, f.q_strides[1], f.q_strides[2], f.q_strides[0], rows, f.dtype)) return 2;
-    if (!make_map4(&mk[i], f.k, f.d, f.sk, f.hk, f.b, f.k_strides[1], f.k_strides[2], f.k_strides[0], rows, f.dtype)) return 2;
-    if (!make_map4(&mv[i], f.v, f.d, f.sk, f.hk, f.b, f.v_strides[1], f.v_strides[2], f.v_strides[0], rows, f.dtype)) return 2;
-    if (!make_map4(&mdo[i], a.d_o, f.d, f.sq, f.h, f.b, a.o_strides[1], a.o_strides[2], a.o_strides[0], rows, f.dtype)) return 2;
+    if (!attn::make_map4(&mq[i], f.q, f.d, f.sq, f.h, f.b, f.q_strides[1], f.q_strides[2], f.q_strides[0], rows, f.dtype)) return 2;
+    if (!attn::make_map4(&mk[i], f.k, f.d, f.sk, f.hk, f.b, f.k_strides[1], f.k_strides[2], f.k_strides[0], rows, f.dtype)) return 2;
+    if (!attn::make_map4(&mv[i], f.v, f.d, f.sk, f.hk, f.b, f.v_strides[1], f.v_strides[2], f.v_strides[0], rows, f.dtype)) return 2;
+    if (!attn::make_map4(&mdo[i], a.d_o, f.d, f.sq, f.h, f.b, a.o_strides[1], a.o_strides[2], a.o_strides[0], rows, f.dtype)) return 2;
   }
   // the fp32 dQ accumulator over its own strides, in the reduce boxes of the single pass: 32 d (128 B) x 64 query rows
-  if (!encode4(&mdq, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, a.dq, f.d, f.sq, f.h, f.b, a.dq_strides[1], a.dq_strides[2], a.dq_strides[0], 32, 64))
-    return 2;
+  if (!attn::make_map4(&mdq, a.dq, f.d, f.sq, f.h, f.b, a.dq_strides[1], a.dq_strides[2], a.dq_strides[0], 64, kF32)) return 2;
   const int sq_pad = attention_bwd_stats_pad(f.sq);
   const int64_t rows = (int64_t)f.b * sq_pad * f.h;
   const int wpb = 8;
@@ -622,9 +572,7 @@ int attention_bwd(const AttnBwdArgs& a, cudaStream_t s) {
     if (p.colmask) launch<__half, true>(p, det, mq, mk, mv, mdo, mdq, s);
     else launch<__half, false>(p, det, mq, mk, mv, mdo, mdq, s);
   }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }
-  return 0;
+  return B200_LAUNCH_RESULT();
 }
 
 }  // namespace b200

@@ -24,7 +24,6 @@
 #include <cuda.h>
 #include <algorithm>
 #include <cstdio>
-#include <string>
 #include <type_traits>
 
 #include "include/b200_common.cuh"
@@ -42,16 +41,6 @@ constexpr int kThreadsQ8 = 384; // 8-bit paged caches: warps 8-11 convert K / V 
 constexpr uint32_t TILE_BYTES = 128 * 128 * 2;   // 32 KB: every operand tile (Q, K, V)
 constexpr uint32_t HALF_BYTES = TILE_BYTES / 2;  // one 64-wide K-block of a tile
 constexpr uint32_t SMEM_BYTES = 5 * TILE_BYTES + 1024 /*align*/ + 256 /*barriers*/;   // Q, 2x K, 2x V
-
-template <typename T> __device__ __forceinline__ uint32_t pack2(float a, float b);
-template <> __device__ __forceinline__ uint32_t pack2<__nv_bfloat16>(float a, float b) {
-  const __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<const uint32_t*>(&v);
-}
-template <> __device__ __forceinline__ uint32_t pack2<__half>(float a, float b) {
-  const __half2 v = __floats2half2_rn(a, b);
-  return *reinterpret_cast<const uint32_t*>(&v);
-}
 
 struct Params {
   int b, sq, sk, h, hk;
@@ -399,37 +388,16 @@ fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CU
 }
 
 // ---------------------------------------------------------------------------------------------- host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = (EncodeTiledFn)p;
-  }
-  return fn;
-}
-
-// 4-D map {d, s, h, b} over a strided [B,S,H,D] view (strides in elements), box {64, rows, 1, 1}, 128B swizzle
-static bool make_map4(CUtensorMap* out, const void* ptr, int d, int s, int h, int b, int64_t ss, int64_t sh, int64_t sb, uint32_t box_rows, int dtype) {
-  bind_primary_context();
-  EncodeTiledFn enc = get_encode();
-  if (!enc) { set_last_error(__FILE__, __LINE__, "cuTensorMapEncodeTiled unavailable"); return false; }
-  cuuint64_t dims[4] = {(cuuint64_t)d, (cuuint64_t)s, (cuuint64_t)h, (cuuint64_t)b};
-  cuuint64_t strides[3] = {(cuuint64_t)ss * 2, (cuuint64_t)sh * 2, (cuuint64_t)sb * 2};
-  cuuint32_t box[4] = {64, box_rows, 1, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(out, dtype == kBF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(ptr),
-                   dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_last_error(__FILE__, __LINE__, ("cuTensorMapEncodeTiled (attention) failed: " + std::to_string((int)r)).c_str());
-    return false;
-  }
-  return true;
+// 4-D map {d, s, h, b} over a strided [B,S,H,D] view (strides in elements), box {128 bytes of d, rows, 1, 1}: 64 d of the 16-bit
+// operands, 32 d of the backward's fp32 dQ accumulator (kF32)
+bool make_map4(CUtensorMap* out, const void* ptr, int d, int s, int h, int b, int64_t ss, int64_t sh, int64_t sb, uint32_t box_rows, int dtype) {
+  const uint64_t es = dtype == kF32 ? 4 : 2;
+  const uint64_t dims[4] = {(uint64_t)d, (uint64_t)s, (uint64_t)h, (uint64_t)b};
+  const uint64_t strides[3] = {(uint64_t)ss * es, (uint64_t)sh * es, (uint64_t)sb * es};
+  const uint32_t box[4] = {(uint32_t)(128 / es), box_rows, 1, 1};
+  const CUtensorMapDataType type = dtype == kBF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                                  : (dtype == kF32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
+  return encode_tensor_map(out, type, 4, ptr, dims, strides, box, "attention");
 }
 
 // Work list of the paged kernel: one (sequence, 128-row query tile) per slot, sorted by key tiles (heaviest first, ties in sequence
@@ -507,28 +475,20 @@ int attention_fwd(const AttnArgs& a, cudaStream_t s) {
   p.colmask = reinterpret_cast<const int4*>(a.colmask);
   p.mask_heads = a.mask_heads > 0 ? a.mask_heads : 1;
   dim3 grid((a.sq + BM - 1) / BM, a.h, a.b);
-  static bool attr_bf = false, attr_h = false;
-  static bool attr_bf_m = false, attr_h_m = false;
   if (a.dtype == kBF16 && !p.colmask) {
-    auto kern = fwd_kernel<__nv_bfloat16, false>;
-    if (!attr_bf) { B200_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES)); attr_bf = true; }
-    kern<<<grid, kThreads, SMEM_BYTES, s>>>(mq, mk, mv, p);
+    set_max_dynamic_smem<fwd_kernel<__nv_bfloat16, false>>(SMEM_BYTES);
+    fwd_kernel<__nv_bfloat16, false><<<grid, kThreads, SMEM_BYTES, s>>>(mq, mk, mv, p);
   } else if (a.dtype == kBF16) {
-    auto kern = fwd_kernel<__nv_bfloat16, true>;
-    if (!attr_bf_m) { B200_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES)); attr_bf_m = true; }
-    kern<<<grid, kThreads, SMEM_BYTES, s>>>(mq, mk, mv, p);
+    set_max_dynamic_smem<fwd_kernel<__nv_bfloat16, true>>(SMEM_BYTES);
+    fwd_kernel<__nv_bfloat16, true><<<grid, kThreads, SMEM_BYTES, s>>>(mq, mk, mv, p);
   } else if (!p.colmask) {
-    auto kern = fwd_kernel<__half, false>;
-    if (!attr_h) { B200_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES)); attr_h = true; }
-    kern<<<grid, kThreads, SMEM_BYTES, s>>>(mq, mk, mv, p);
+    set_max_dynamic_smem<fwd_kernel<__half, false>>(SMEM_BYTES);
+    fwd_kernel<__half, false><<<grid, kThreads, SMEM_BYTES, s>>>(mq, mk, mv, p);
   } else {
-    auto kern = fwd_kernel<__half, true>;
-    if (!attr_h_m) { B200_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES)); attr_h_m = true; }
-    kern<<<grid, kThreads, SMEM_BYTES, s>>>(mq, mk, mv, p);
+    set_max_dynamic_smem<fwd_kernel<__half, true>>(SMEM_BYTES);
+    fwd_kernel<__half, true><<<grid, kThreads, SMEM_BYTES, s>>>(mq, mk, mv, p);
   }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }
-  return 0;
+  return B200_LAUNCH_RESULT();
 }
 
 int attention_paged_prefill_slots(int t, int b) { return (t + attn::BM - 1) / attn::BM + b; }
@@ -570,20 +530,19 @@ int attention_paged_prefill(const PagedAttnArgs& a, cudaStream_t s) {
     p.k_cache = reinterpret_cast<const uint8_t*>(a.k_cache); p.v_cache = reinterpret_cast<const uint8_t*>(a.v_cache);
     p.k_dq = a.k_dq; p.v_dq = a.v_dq;
     dim3 grid(a.h, slots);
-    auto launch = [&](auto kern, bool& attr) {
-      if (!attr) { B200_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES)); attr = true; }
-      kern<<<grid, kThreadsQ8, SMEM_BYTES, s>>>(mq, mq, mq, p);
+    auto launch = [&](auto tag_t, auto tag_kv) {
+      using T = decltype(tag_t);
+      using KV = decltype(tag_kv);
+      set_max_dynamic_smem<fwd_kernel<T, false, true, KV>>(SMEM_BYTES);
+      fwd_kernel<T, false, true, KV><<<grid, kThreadsQ8, SMEM_BYTES, s>>>(mq, mq, mq, p);
     };
-    static bool attr[4] = {};
     const bool i8 = a.kv_dtype == kI8;
     if (a.dtype == kBF16) {
-      if (i8) launch(fwd_kernel<__nv_bfloat16, false, true, kv8::I8>, attr[0]); else launch(fwd_kernel<__nv_bfloat16, false, true, kv8::E4M3>, attr[1]);
+      if (i8) launch(__nv_bfloat16(), kv8::I8()); else launch(__nv_bfloat16(), kv8::E4M3());
     } else {
-      if (i8) launch(fwd_kernel<__half, false, true, kv8::I8>, attr[2]); else launch(fwd_kernel<__half, false, true, kv8::E4M3>, attr[3]);
+      if (i8) launch(__half(), kv8::I8()); else launch(__half(), kv8::E4M3());
     }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }
-    return 0;
+    return B200_LAUNCH_RESULT();
   }
   if (!make_map4(&mk, a.k_cache, a.d, a.block_size, a.hk, a.num_blocks, a.d, blk, blk * a.hk, rows, a.dtype)) return 2;
   if (!make_map4(&mv, a.v_cache, a.d, a.block_size, a.hk, a.num_blocks, a.d, blk, blk * a.hk, rows, a.dtype)) return 2;
@@ -598,19 +557,14 @@ int attention_paged_prefill(const PagedAttnArgs& a, cudaStream_t s) {
   p.work = work; p.cu_q = a.cu_q; p.n_q = a.n_q; p.past = a.past;
   p.block_tables = a.block_tables; p.max_blocks = a.max_blocks; p.block_size = a.block_size;
   dim3 grid(a.h, slots);   // every head of the heaviest tile is dispatched first
-  static bool attr_bf = false, attr_h = false;
   if (a.dtype == kBF16) {
-    auto kern = fwd_kernel<__nv_bfloat16, false, true>;
-    if (!attr_bf) { B200_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES)); attr_bf = true; }
-    kern<<<grid, kThreads, SMEM_BYTES, s>>>(mq, mk, mv, p);
+    set_max_dynamic_smem<fwd_kernel<__nv_bfloat16, false, true>>(SMEM_BYTES);
+    fwd_kernel<__nv_bfloat16, false, true><<<grid, kThreads, SMEM_BYTES, s>>>(mq, mk, mv, p);
   } else {
-    auto kern = fwd_kernel<__half, false, true>;
-    if (!attr_h) { B200_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES)); attr_h = true; }
-    kern<<<grid, kThreads, SMEM_BYTES, s>>>(mq, mk, mv, p);
+    set_max_dynamic_smem<fwd_kernel<__half, false, true>>(SMEM_BYTES);
+    fwd_kernel<__half, false, true><<<grid, kThreads, SMEM_BYTES, s>>>(mq, mk, mv, p);
   }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }
-  return 0;
+  return B200_LAUNCH_RESULT();
 }
 
 }  // namespace b200

@@ -258,16 +258,6 @@ template <> __device__ __forceinline__ void mma16816<__half>(float (&c)[4], cons
                : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-template <typename T> __device__ __forceinline__ uint32_t pack2(float lo, float hi);
-template <> __device__ __forceinline__ uint32_t pack2<__nv_bfloat16>(float lo, float hi) {
-  const __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
-  return *reinterpret_cast<const uint32_t*>(&v);
-}
-template <> __device__ __forceinline__ uint32_t pack2<__half>(float lo, float hi) {
-  const __half2 v = __floats2half2_rn(lo, hi);
-  return *reinterpret_cast<const uint32_t*>(&v);
-}
-
 // KV = T: 16-bit caches; KV = kv8::I8 / kv8::E4M3: 8-bit caches with fp32 [Hkv] dequant scales
 template <typename T, typename KV>
 __global__ void __launch_bounds__(kThreads) multi_split_kernel(const Params p) {
@@ -594,7 +584,7 @@ __global__ void __launch_bounds__(kThreads) shared_split_kernel(const Params p) 
         kv8::to_float16<KV>(raw, f);
         uint32_t w[8];
 #pragma unroll
-        for (int e = 0; e < 8; ++e) w[e] = decode_multi::pack2<T>(f[2 * e], f[2 * e + 1]);
+        for (int e = 0; e < 8; ++e) w[e] = pack2<T>(f[2 * e], f[2 * e + 1]);
         uint8_t* dst = smem + S::kKV + kv * kTile16;
         *reinterpret_cast<uint4*>(dst + decode_multi::swz(row, 2 * c)) = make_uint4(w[0], w[1], w[2], w[3]);
         *reinterpret_cast<uint4*>(dst + decode_multi::swz(row, 2 * c + 1)) = make_uint4(w[4], w[5], w[6], w[7]);
@@ -649,8 +639,8 @@ __global__ void __launch_bounds__(kThreads) shared_split_kernel(const Params p) 
       }
 #pragma unroll
       for (int kk = 0; kk < BN / 16; ++kk) {
-        const uint32_t pa[4] = {decode_multi::pack2<T>(s[2 * kk][0], s[2 * kk][1]), decode_multi::pack2<T>(s[2 * kk][2], s[2 * kk][3]),
-                                decode_multi::pack2<T>(s[2 * kk + 1][0], s[2 * kk + 1][1]), decode_multi::pack2<T>(s[2 * kk + 1][2], s[2 * kk + 1][3])};
+        const uint32_t pa[4] = {pack2<T>(s[2 * kk][0], s[2 * kk][1]), pack2<T>(s[2 * kk][2], s[2 * kk][3]),
+                                pack2<T>(s[2 * kk + 1][0], s[2 * kk + 1][1]), pack2<T>(s[2 * kk + 1][2], s[2 * kk + 1][3])};
 #pragma unroll
         for (int np = 0; np < D / 16; ++np) {
           uint32_t bf[4];
@@ -740,9 +730,7 @@ int decode_attention(const void* q, const void* k_cache, const void* v_cache, co
                                                            smax, splits, sl2, block_tables, max_blocks, block_size);
     decode_merge_kernel<__half><<<b * h, D, 0, s>>>(part_acc, part_ml, (__half*)out, splits);
   }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }
-  return 0;
+  return B200_LAUNCH_RESULT();
 }
 
 int decode_attention_paged_q8(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* out, float* part_acc, float* part_ml,
@@ -765,9 +753,7 @@ int decode_attention_paged_q8(const void* q, const void* k_cache, const void* v_
   } else {
     if (kv_dtype == kI8) launch(__half(), kv8::I8()); else launch(__half(), kv8::E4M3());
   }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }
-  return 0;
+  return B200_LAUNCH_RESULT();
 }
 
 int decode_attention_paged_multi(const PagedMultiArgs& a, cudaStream_t s) {
@@ -789,8 +775,7 @@ int decode_attention_paged_multi(const PagedMultiArgs& a, cudaStream_t s) {
     using T = decltype(tag_t);
     using KV = decltype(tag_kv);
     constexpr int smem = Smem<!std::is_same<T, KV>::value>::kBytes;
-    static bool attr = false;   // one flag per instantiation
-    if (!attr) { B200_CUDA_CHECK(cudaFuncSetAttribute(multi_split_kernel<T, KV>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); attr = true; }
+    set_max_dynamic_smem<multi_split_kernel<T, KV>>(smem);
     multi_split_kernel<T, KV><<<grid, kThreads, smem, s>>>(p);
     multi_merge_kernel<T><<<mgrid, D, 0, s>>>(p);
   };
@@ -803,9 +788,7 @@ int decode_attention_paged_multi(const PagedMultiArgs& a, cudaStream_t s) {
     else if (a.kv_dtype == kE4M3) launch(__half(), kv8::E4M3());
     else launch(__half(), __half());
   }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }
-  return 0;
+  return B200_LAUNCH_RESULT();
 }
 
 int decode_attention_paged_shared(const PagedSharedArgs& a, cudaStream_t s) {
@@ -828,8 +811,7 @@ int decode_attention_paged_shared(const PagedSharedArgs& a, cudaStream_t s) {
     using T = decltype(tag_t);
     using KV = decltype(tag_kv);
     constexpr int smem = decode_multi::Smem<!std::is_same<T, KV>::value>::kBytes;
-    static bool attr = false;   // one flag per instantiation
-    if (!attr) { B200_CUDA_CHECK(cudaFuncSetAttribute(shared_split_kernel<T, KV>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); attr = true; }
+    set_max_dynamic_smem<shared_split_kernel<T, KV>>(smem);
     shared_split_kernel<T, KV><<<grid, kThreads, smem, s>>>(p);
     shared_merge_kernel<T><<<mgrid, D, 0, s>>>(p);
   };
@@ -842,9 +824,7 @@ int decode_attention_paged_shared(const PagedSharedArgs& a, cudaStream_t s) {
     else if (a.kv_dtype == kE4M3) launch(__half(), kv8::E4M3());
     else launch(__half(), __half());
   }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }
-  return 0;
+  return B200_LAUNCH_RESULT();
 }
 
 }  // namespace b200

@@ -17,7 +17,6 @@
 #include <cuda.h>
 #include <cstdio>
 #include <cstdlib>
-#include <string>
 
 #include "include/b200_common.cuh"
 #include "include/b200_ops.h"
@@ -62,13 +61,7 @@ struct Params {
   const uint8_t* sfb;
 };
 
-__device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
 __device__ __forceinline__ float e8m0(uint32_t byte) { return __uint_as_float(byte << 23); }   // 2^(byte - 127)
-__device__ __forceinline__ uint32_t ld_shared_u8(uint32_t addr) {
-  uint32_t v;
-  asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(addr));
-  return v;
-}
 
 template <typename TO>
 __device__ __forceinline__ void store_pair(TO* __restrict__ dst, float v0, float v1, int valid) {
@@ -423,49 +416,20 @@ gemm_s8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
 }
 
 // ---------------------------------------------------------------------------------------------- host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = (EncodeTiledFn)p;
-  }
-  return fn;
-}
 // 3-D byte map {k (contiguous), rows, batch}
 static bool make_map8(CUtensorMap* out, const void* ptr, uint64_t k, uint64_t rows, uint64_t batch, uint64_t ld, uint64_t bstride, uint32_t box_rows) {
-  bind_primary_context();
-  EncodeTiledFn enc = get_encode();
-  if (!enc) { set_last_error(__FILE__, __LINE__, "cuTensorMapEncodeTiled unavailable"); return false; }
-  cuuint64_t dims[3] = {k, rows, batch};
-  cuuint64_t strides[2] = {ld, batch > 1 ? bstride : rows * ld};
-  cuuint32_t box[3] = {(cuuint32_t)BLOCK_K, box_rows, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_last_error(__FILE__, __LINE__, ("cuTensorMapEncodeTiled (fp8) failed: " + std::to_string((int)r)).c_str());
-    return false;
-  }
-  return true;
+  const uint64_t dims[3] = {k, rows, batch};
+  const uint64_t strides[2] = {ld, batch > 1 ? bstride : rows * ld};
+  const uint32_t box[3] = {(uint32_t)BLOCK_K, box_rows, 1};
+  return encode_tensor_map(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, ptr, dims, strides, box, "fp8 / int8 gemm");
 }
 // persistent launch: one CTA per SM (or per tile, when there are fewer tiles)
 template <auto Kern, typename P>
 static int start(uint32_t smem, int num_tiles, const CUtensorMap& ma, const CUtensorMap& mb, const P& p, cudaStream_t s) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    B200_CUDA_CHECK(cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    attr_set = true;
-  }
+  set_max_dynamic_smem<Kern>(smem);
   const int grid = num_tiles < sm_count() ? num_tiles : sm_count();
   Kern<<<grid, kThreads, smem, s>>>(ma, mb, p);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }
-  return 0;
+  return B200_LAUNCH_RESULT();
 }
 
 template <int BN, bool A5, bool B5, bool MX>

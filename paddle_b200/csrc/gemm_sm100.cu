@@ -18,7 +18,6 @@
 #include <cstdlib>
 #include <mutex>
 #include <unordered_map>
-#include <string>
 
 #include "include/b200_common.cuh"
 #include "include/b200_ops.h"
@@ -147,8 +146,6 @@ __device__ __forceinline__ void ag_copy_role(const Params& p, int lane) {
   if (wid == 0 && lane < p.ag_world && lane != p.ag_rank)        // peers finished reading my shard: it may be reused after exit
     spin_sys_ge(my_pad + kAgDoneSlot * kPadRanks + lane, p.ag_epoch);
 }
-
-__device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
 
 // two adjacent output columns of one row (what a thread holds per 8-column group of the accumulator fragment)
 template <typename TO>
@@ -492,21 +489,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
 }
 
 // ---------------------------------------------------------------------------------------------- host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = (EncodeTiledFn)p;
-  }
-  return fn;
-}
-
 struct MapKey {
   const void* ptr; uint64_t inner, rows, batch, ld, bstride; uint32_t box_inner, box_rows; int dtype;
   bool operator==(const MapKey& o) const {
@@ -524,8 +506,8 @@ struct MapKeyHash {
 };
 
 // 3-D map {inner (contiguous), rows, batch}; element = 2 bytes (bf16 / fp16) or 4 bytes (kF32: TMA-store maps of fp32 outputs).
-bool make_map(CUtensorMap* out, const void* ptr, uint64_t inner, uint64_t rows, uint64_t batch, uint64_t ld,
-                     uint64_t bstride, uint32_t box_inner, uint32_t box_rows, int dtype) {
+bool make_map(CUtensorMap* out, const void* ptr, uint64_t inner, uint64_t rows, uint64_t batch, uint64_t ld, uint64_t bstride,
+              uint32_t box_inner, uint32_t box_rows, int dtype) {
   static std::mutex mu;
   static std::unordered_map<MapKey, CUtensorMap, MapKeyHash> cache;
   MapKey key{ptr, inner, rows, batch, ld, bstride, box_inner, box_rows, dtype};
@@ -534,21 +516,13 @@ bool make_map(CUtensorMap* out, const void* ptr, uint64_t inner, uint64_t rows, 
     auto it = cache.find(key);
     if (it != cache.end()) { *out = it->second; return true; }
   }
-  bind_primary_context();
-  EncodeTiledFn enc = get_encode();
-  if (!enc) { set_last_error(__FILE__, __LINE__, "cuTensorMapEncodeTiled unavailable"); return false; }
-  cuuint64_t dims[3] = {inner, rows, batch};
   const uint64_t es = dtype == kF32 ? 4 : 2;
-  cuuint64_t strides[2] = {ld * es, (batch > 1 ? bstride : rows * ld) * es};
-  cuuint32_t box[3] = {box_inner, box_rows, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(out, dtype == kBF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : (dtype == kF32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16), 3,
-                   const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_last_error(__FILE__, __LINE__, ("cuTensorMapEncodeTiled failed: " + std::to_string((int)r)).c_str());
-    return false;
-  }
+  const uint64_t dims[3] = {inner, rows, batch};
+  const uint64_t strides[2] = {ld * es, (batch > 1 ? bstride : rows * ld) * es};
+  const uint32_t box[3] = {box_inner, box_rows, 1};
+  const CUtensorMapDataType type = dtype == kBF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                                  : (dtype == kF32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
+  if (!encode_tensor_map(out, type, 3, ptr, dims, strides, box, "gemm")) return false;
   std::lock_guard<std::mutex> g(mu);
   if (cache.size() > 8192) cache.clear();
   cache.emplace(key, *out);
@@ -603,22 +577,15 @@ static int launch(const GemmArgs& g, cudaStream_t s) {
     p.ag_flags = (uint32_t*)g.ag_flags;
     p.ag_epoch = g.ag_epoch;
   }
-  static bool attr_set = false;
-  auto kern = gemm_kernel<BN, BF16, A_MN, B_MN>;
-  if (!attr_set) {
-    B200_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
-    attr_set = true;
-  }
+  set_max_dynamic_smem<gemm_kernel<BN, BF16, A_MN, B_MN>>(C::SMEM_BYTES);
   const int num_tiles = ((g.m + BLOCK_M - 1) / BLOCK_M) * ((g.n + BN - 1) / BN) * (int)batch;
   // B200_GEMM_RESERVE_SMS=<n>: keep n SMs out of every persistent GEMM grid so that concurrently launched collective kernels are resident
   // unconditionally (docs/race_detection.md, "cross-rank progress"); default 0
   static const int reserve = [] { const char* e = getenv("B200_GEMM_RESERVE_SMS"); const int v = e ? atoi(e) : 0; return v < 0 ? 0 : v; }();
   const int usable = sm_count() - reserve > 0 ? sm_count() - reserve : 1;
   const int grid = num_tiles < usable ? num_tiles : usable;
-  kern<<<grid, kThreads, C::SMEM_BYTES, s>>>(ma, mb, md, p);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }
-  return 0;
+  gemm_kernel<BN, BF16, A_MN, B_MN><<<grid, kThreads, C::SMEM_BYTES, s>>>(ma, mb, md, p);
+  return B200_LAUNCH_RESULT();
 }
 
 template <int BN, bool BF16>

@@ -17,7 +17,6 @@
 // Parity: paddle/phi/kernels/gpu/weight_only_linear_kernel.cu:27, python/paddle/nn/quant/quantized_linear.py:183.
 #include <cuda.h>
 #include <cstdio>
-#include <string>
 #include <type_traits>
 
 #include "include/b200_common.cuh"
@@ -25,10 +24,6 @@
 #include "include/b200_ptx.cuh"
 
 namespace b200 {
-namespace gemm {
-bool make_map(CUtensorMap* out, const void* ptr, uint64_t inner, uint64_t rows, uint64_t batch, uint64_t ld, uint64_t bstride,
-              uint32_t box_inner, uint32_t box_rows, int dtype);
-}
 namespace wo {
 using namespace ptx;
 
@@ -46,29 +41,11 @@ struct Params {
   int splits;                  // blockIdx.y extent = cluster size: the CTAs of one output tile
 };
 
-template <bool BF16> __device__ __forceinline__ uint32_t pack2(float a, float b) {
-  if constexpr (BF16) {
-    const __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
-    return *reinterpret_cast<const uint32_t*>(&v);
-  } else {
-    const __half2 v = __floats2half2_rn(a, b);
-    return *reinterpret_cast<const uint32_t*>(&v);
-  }
-}
-__device__ __forceinline__ uint32_t ld_shared_u16(uint32_t addr) {
-  uint32_t v;
-  asm volatile("ld.shared.u16 %0, [%1];" : "=r"(v) : "r"(addr));
-  return v;
-}
-__device__ __forceinline__ uint32_t ld_shared_u8(uint32_t addr) {
-  uint32_t v;
-  asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(addr));
-  return v;
-}
 // two consecutive k of one channel -> one packed 16-bit pair in the activation dtype (|value| <= 128: exact in bf16 and fp16)
 template <bool INT4, bool BF16> __device__ __forceinline__ uint32_t dequant_pair(uint32_t raw) {
-  if constexpr (INT4) return pack2<BF16>((float)((int)((raw & 0xFu) ^ 8u) - 8), (float)((int)(((raw >> 4) & 0xFu) ^ 8u) - 8));   // low nibble = even k
-  else return pack2<BF16>((float)(int8_t)(raw & 0xFFu), (float)(int8_t)((raw >> 8) & 0xFFu));
+  using T = std::conditional_t<BF16, __nv_bfloat16, __half>;
+  if constexpr (INT4) return pack2<T>((float)((int)((raw & 0xFu) ^ 8u) - 8), (float)((int)(((raw >> 4) & 0xFu) ^ 8u) - 8));   // low nibble = even k
+  else return pack2<T>((float)(int8_t)(raw & 0xFFu), (float)(int8_t)((raw >> 8) & 0xFFu));
 }
 __device__ __forceinline__ void keep_regs(uint32_t (&a)[4]) {
 #pragma unroll
@@ -488,48 +465,21 @@ wo_expert_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_co
   }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess) fn = (EncodeTiledFn)p;
-  }
-  return fn;
-}
 // raw weights as bytes: [n rows, row_bytes], box {128 bytes, 128 rows}, SWIZZLE_128B
 static bool make_w_map(CUtensorMap* out, const void* w, int n, int row_bytes) {
-  bind_primary_context();
-  EncodeTiledFn enc = get_encode();
-  if (!enc) { set_last_error(__FILE__, __LINE__, "cuTensorMapEncodeTiled unavailable"); return false; }
-  cuuint64_t dims[2] = {(cuuint64_t)row_bytes, (cuuint64_t)n};
-  cuuint64_t strides[1] = {(cuuint64_t)row_bytes};
-  cuuint32_t box[2] = {128u, (cuuint32_t)BLOCK_N};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(w), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_last_error(__FILE__, __LINE__, ("weight-only gemm: cuTensorMapEncodeTiled failed: " + std::to_string((int)r)).c_str()); return false; }
-  return true;
+  const uint64_t dims[2] = {(uint64_t)row_bytes, (uint64_t)n};
+  const uint64_t strides[1] = {(uint64_t)row_bytes};
+  const uint32_t box[2] = {128u, (uint32_t)BLOCK_N};
+  return encode_tensor_map(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, w, dims, strides, box, "weight-only gemm");
 }
 
 // raw stacked expert weights as bytes: [experts, n rows, row_bytes], box {128 bytes, 128 rows, 1 expert}: the same shared-memory layout as
 // make_w_map, and a partial channel tile is zero filled instead of reading the next expert's rows
 static bool make_w_map_experts(CUtensorMap* out, const void* w, int experts, int n, int row_bytes) {
-  bind_primary_context();
-  EncodeTiledFn enc = get_encode();
-  if (!enc) { set_last_error(__FILE__, __LINE__, "cuTensorMapEncodeTiled unavailable"); return false; }
-  cuuint64_t dims[3] = {(cuuint64_t)row_bytes, (cuuint64_t)n, (cuuint64_t)experts};
-  cuuint64_t strides[2] = {(cuuint64_t)row_bytes, (cuuint64_t)row_bytes * n};
-  cuuint32_t box[3] = {128u, (cuuint32_t)BLOCK_N, 1u};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<void*>(w), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_last_error(__FILE__, __LINE__, "weight-only expert gemm: cuTensorMapEncodeTiled failed"); return false; }
-  return true;
+  const uint64_t dims[3] = {(uint64_t)row_bytes, (uint64_t)n, (uint64_t)experts};
+  const uint64_t strides[2] = {(uint64_t)row_bytes, (uint64_t)row_bytes * n};
+  const uint32_t box[3] = {128u, (uint32_t)BLOCK_N, 1u};
+  return encode_tensor_map(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, w, dims, strides, box, "weight-only expert gemm");
 }
 
 constexpr int kMaxSplits = 8;                   // portable cluster size
@@ -699,9 +649,7 @@ template <bool INT4, typename OutT>
 static int launch_dequant(const void* w, const float* scale, void* out, int n, int k, int group_size, int experts, cudaStream_t s) {
   const dim3 grid((k + 63) / 64, (n + 63) / 64, experts);
   wo_dequant_kernel<INT4, OutT><<<grid, 256, 0, s>>>((const int8_t*)w, scale, (OutT*)out, n, k, group_size);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }
-  return 0;
+  return B200_LAUNCH_RESULT();
 }
 template <bool INT4>
 static int dispatch_dequant(const void* w, const float* scale, void* out, int n, int k, int group_size, int out_dtype, int experts, cudaStream_t s) {

@@ -1,4 +1,4 @@
-// Common device helpers for the sm_90a kernels (no torch headers in .cu files: keeps nvcc fast).
+// Common device and launch helpers for the sm_90a kernels (no torch headers in .cu files: keeps nvcc fast).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -20,6 +20,16 @@ enum DType : int { kF32 = 0, kF16 = 1, kBF16 = 2, kI8 = 3, kE4M3 = 4 };   // kI8
 
 void set_last_error(const char* file, int line, const char* msg);
 
+// After a kernel launch: 0, or 3 with the launch error recorded (the return code of a failed launch)
+#define B200_LAUNCH_RESULT() b200::launch_result(__FILE__, __LINE__)
+
+inline int launch_result(const char* file, int line) {
+  const cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) return 0;
+  set_last_error(file, line, cudaGetErrorString(e));
+  return 3;
+}
+
 template <typename T> struct VecTraits;
 template <> struct VecTraits<float> { static constexpr int kVec = 4; };
 template <> struct VecTraits<__half> { static constexpr int kVec = 8; };
@@ -34,6 +44,19 @@ template <typename T> __device__ __forceinline__ T from_f(float v);
 template <> __device__ __forceinline__ float from_f<float>(float v) { return v; }
 template <> __device__ __forceinline__ __half from_f<__half>(float v) { return __float2half_rn(v); }
 template <> __device__ __forceinline__ __nv_bfloat16 from_f<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
+
+// two floats rounded to one packed 16-bit pair (a in the low half): an MMA A-fragment register or a 4-byte store
+template <typename T> __device__ __forceinline__ uint32_t pack2(float a, float b);
+template <> __device__ __forceinline__ uint32_t pack2<__nv_bfloat16>(float a, float b) {
+  const __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
+  return *reinterpret_cast<const uint32_t*>(&v);
+}
+template <> __device__ __forceinline__ uint32_t pack2<__half>(float a, float b) {
+  const __half2 v = __floats2half2_rn(a, b);
+  return *reinterpret_cast<const uint32_t*>(&v);
+}
+
+__device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
 
 // 16-byte vector of T
 template <typename T> struct alignas(16) Vec16 {
@@ -126,6 +149,33 @@ inline int sm_count() {
     if (n <= 0) n = 132;
   }
   return n;
+}
+
+// Tiled TMA descriptor, 128B swizzle, 256B L2 promotion, no OOB fill. Byte strides for dims 1..rank-1.
+// On failure records "<what>: cuTensorMapEncodeTiled ... (CUresult N)" via set_last_error and returns false.
+bool encode_tensor_map(CUtensorMap* out, CUtensorMapDataType type, int rank, const void* ptr, const uint64_t* dims,
+                       const uint64_t* byte_strides, const uint32_t* box, const char* what);
+
+namespace gemm {
+// 3-D map {inner (contiguous), rows, batch} of bf16 / fp16 (or kF32) elements, cached by its arguments (gemm_sm100.cu)
+bool make_map(CUtensorMap* out, const void* ptr, uint64_t inner, uint64_t rows, uint64_t batch, uint64_t ld, uint64_t bstride,
+              uint32_t box_inner, uint32_t box_rows, int dtype);
+}
+namespace attn {
+// 4-D map {d, s, h, b} over a strided [B,S,H,D] view of bf16 / fp16 (or kF32) elements, box {128 bytes of d, box_rows, 1, 1}
+// (attention_sm100.cu)
+bool make_map4(CUtensorMap* out, const void* ptr, int d, int s, int h, int b, int64_t ss, int64_t sh, int64_t sb, uint32_t box_rows,
+               int dtype);
+}
+
+// Raise the kernel's dynamic shared-memory limit before its first launch. The flag is per kernel pointer: two instantiations of one
+// kernel template with the same signature have the same type but each needs its own attribute.
+template <auto Kern> void set_max_dynamic_smem(uint32_t bytes) {
+  static bool set = false;
+  if (!set) {
+    B200_CUDA_CHECK(cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    set = true;
+  }
 }
 
 }  // namespace b200

@@ -12,6 +12,16 @@ namespace b200 {
 namespace ptx {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ uint32_t ld_shared_u8(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(addr));
+  return v;
+}
+__device__ __forceinline__ uint32_t ld_shared_u16(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.u16 %0, [%1];" : "=r"(v) : "r"(addr));
+  return v;
+}
 
 // ---------------------------------------------------------------------------------------------- mbarrier
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {

@@ -234,9 +234,7 @@ int prologue_write(const PagedKvWriteArgs& a, cudaStream_t s) {
     if (a.qkv_int32) by_kv(tag_t, int32_t()); else by_kv(tag_t, tag_t);
   };
   if (a.dtype == kBF16) by_in(__nv_bfloat16()); else by_in(__half());
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }
-  return 0;
+  return B200_LAUNCH_RESULT();
 }
 
 }  // namespace
@@ -261,9 +259,7 @@ int paged_kv_cache_write(const PagedKvWriteArgs& a, cudaStream_t s) {
   } else {
     if (a.kv_dtype == kI8) launch(__half(), kv8::I8()); else launch(__half(), kv8::E4M3());
   }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }
-  return 0;
+  return B200_LAUNCH_RESULT();
 }
 
 int attention_out_quant(const OutQuantArgs& a, cudaStream_t s) {
@@ -285,9 +281,7 @@ int attention_out_quant(const OutQuantArgs& a, cudaStream_t s) {
   } else {
     if (a.out_dtype == kI8) launch(__half(), kv8::I8()); else launch(__half(), kv8::E4M3());
   }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }
-  return 0;
+  return B200_LAUNCH_RESULT();
 }
 
 }  // namespace b200

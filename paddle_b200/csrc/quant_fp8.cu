@@ -143,9 +143,7 @@ int mx_quantize(const void* x, int64_t rows, int64_t k, int dtype, void* q, uint
   const int64_t total = rows * (k / 32);
   const unsigned blocks = (unsigned)((total + 255) / 256);
   B200_DISPATCH_DTYPE(dtype, T, { mx_quantize_kernel<T><<<blocks, 256, 0, s>>>((const T*)x, rows, k, (uint8_t*)q, sf); });
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }
-  return 0;
+  return B200_LAUNCH_RESULT();
 }
 
 __global__ void mx_dequantize_kernel(const uint8_t* __restrict__ q, const uint8_t* __restrict__ sf, int64_t rows, int64_t K, float* __restrict__ out) {
@@ -167,9 +165,7 @@ int mx_dequantize(const void* q, const uint8_t* sf, int64_t rows, int64_t k, flo
   if (rows <= 0 || k <= 0 || rows % 128 || k % 128) return 1;
   const int64_t total = rows * (k / 32);
   mx_dequantize_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>((const uint8_t*)q, sf, rows, k, out);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { set_last_error(__FILE__, __LINE__, cudaGetErrorString(e)); return 3; }
-  return 0;
+  return B200_LAUNCH_RESULT();
 }
 
 // ------------------------------------------------------------------------------------------------ per-token int8
