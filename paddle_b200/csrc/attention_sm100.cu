@@ -16,6 +16,9 @@
 // bottom-right causal limit.  A 128-key tile is assembled from {64 d, min(block_size, 64) rows} boxes, each at a 1024-byte multiple of
 // the tile, so the 128B-swizzled shared tile is byte-for-byte what one dense box would have written and the MMA code is unchanged.
 //
+// PAGED at head_dim 64 (16-bit caches): a 128-row x 64-d tile is one 128-byte swizzle span (16 KB), so Q, K and V are one "half" each:
+// S = Q K^T takes 4 k-steps, P V is one n = 64 wgmma per 16 keys, and the boxes land at the same 1024-byte placements.
+//
 // PAGED over 8-bit caches (KV = kv8::I8 / kv8::E4M3; q and o stay fp16 / bf16): a converter warpgroup (warps 8-11, 384 threads) takes
 // the TMA producer's place for K and V.  Its threads read the 8-bit rows through the block table with 16-byte loads, convert them
 // exactly to 16 bits and store them into the same swizzled K / V tiles, then fence.proxy.async and arrive on the tiles' mbarriers; keys
@@ -38,9 +41,11 @@ using namespace ptx;
 constexpr int BM = 128, BN = 128, HD = 128;
 constexpr int kThreads = 288;   // warps 0-7: two MMA / softmax warpgroups, warp 8: TMA producer
 constexpr int kThreadsQ8 = 384; // 8-bit paged caches: warps 8-11 convert K / V (warp 8 lane 0 also loads Q)
-constexpr uint32_t TILE_BYTES = 128 * 128 * 2;   // 32 KB: every operand tile (Q, K, V)
-constexpr uint32_t HALF_BYTES = TILE_BYTES / 2;  // one 64-wide K-block of a tile
-constexpr uint32_t SMEM_BYTES = 5 * TILE_BYTES + 1024 /*align*/ + 256 /*barriers*/;   // Q, 2x K, 2x V
+constexpr uint32_t TILE_BYTES = 128 * 128 * 2;   // 32 KB: every operand tile (Q, K, V) at head_dim 128
+constexpr uint32_t HALF_BYTES = 128 * 64 * 2;    // one 64-wide K-block of a tile
+// Q, 2x K, 2x V tiles of 128 rows x D
+template <int D> constexpr uint32_t kSmemBytes = 5 * (128 * D * 2) + 1024 /*align*/ + 256 /*barriers*/;
+constexpr uint32_t SMEM_BYTES = kSmemBytes<HD>;
 
 struct Params {
   int b, sq, sk, h, hk;
@@ -77,19 +82,24 @@ __device__ __forceinline__ void st_shared_zero16(uint32_t addr) {
 // MASKED: column-wise row-range mask (flashmask / varlen) compiled in; the dense instantiation carries none of its code or registers
 // PAGED: queries = new tokens of each sequence, K / V read through the block table (see the file header); always causal, never MASKED
 // KV: the cache element type; kv8::I8 / kv8::E4M3 (PAGED only) select the converter warpgroup and QuantPagedParams
-template <typename T, bool MASKED, bool PAGED = false, typename KV = T>
+// D: the head size, 128; 64 for the 16-bit PAGED instantiation
+template <typename T, bool MASKED, bool PAGED = false, typename KV = T, int D = HD>
 __global__ void __launch_bounds__(std::is_same<KV, T>::value ? kThreads : kThreadsQ8, 1)
 fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
            const std::conditional_t<PAGED, std::conditional_t<std::is_same<KV, T>::value, PagedParams, QuantPagedParams>, Params> p) {
   constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
   constexpr bool Q8 = !std::is_same<KV, T>::value;
   static_assert(!Q8 || (PAGED && !MASKED), "8-bit caches are paged only");
+  static_assert(D == HD || (D == 64 && PAGED && !Q8), "head_dim 64 is paged over 16-bit caches only");
+  constexpr int kHalves = D / 64;                            // 64-wide d chunks (128-byte swizzle spans) of a row
+  constexpr uint32_t kTile = BM * D * 2;                     // one Q, K or V tile
+  constexpr uint32_t kVBlock = kHalves * 8192;               // one 64-key block of a V tile (its d chunks 8192 B apart)
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sQ = base;
-  auto sK = [&](int s) { return base + (1 + s) * TILE_BYTES; };
-  auto sV = [&](int s) { return base + (3 + s) * TILE_BYTES; };
-  const uint32_t bars = base + 5 * TILE_BYTES;
+  auto sK = [&](int s) { return base + (1 + s) * kTile; };
+  auto sV = [&](int s) { return base + (3 + s) * kTile; };
+  const uint32_t bars = base + 5 * kTile;
   const uint32_t q_full = bars;
   auto k_full = [&](int s) { return bars + 8u * (1 + s); };
   auto v_full = [&](int s) { return bars + 8u * (3 + s); };
@@ -204,25 +214,25 @@ fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CU
         const int last_blk = __ldg(bt + (sk - 1) / bsz);            // table entries past the sequence are never read
         const int c = lane % C, half = lane / C;
         if (lane == 0) {
-          mbar_expect_tx(q_full, TILE_BYTES);
+          mbar_expect_tx(q_full, kTile);
           tma_load_4d(sQ, &map_q, q_full, 0, q0 + m0, head, 0);
-          tma_load_4d(sQ + HALF_BYTES, &map_q, q_full, 64, q0 + m0, head, 0);
+          if constexpr (kHalves == 2) tma_load_4d(sQ + HALF_BYTES, &map_q, q_full, 64, q0 + m0, head, 0);
         }
         for (int j = 0; j < n_tiles; ++j) {
           const int s = j & 1, key = j * BN + c * R;
           const uint32_t ph = ((j >> 1) & 1) ^ 1;
           // keys past the sequence come from a valid block (masked in S, zeroed in V) so every tile carries the same bytes
-          const int blk = lane < 2 * C ? (key < sk ? __ldg(bt + key / bsz) : last_blk) : 0;
+          const int blk = lane < kHalves * C ? (key < sk ? __ldg(bt + key / bsz) : last_blk) : 0;
           const int row = key % bsz;
           mbar_wait(k_empty(s), ph);
-          if (lane == 0) mbar_expect_tx(k_full(s), TILE_BYTES);
+          if (lane == 0) mbar_expect_tx(k_full(s), kTile);
           __syncwarp();
-          if (lane < 2 * C) tma_load_4d(sK(s) + half * HALF_BYTES + c * R * 128, &map_k, k_full(s), half * 64, row, kv_head, blk);
+          if (lane < kHalves * C) tma_load_4d(sK(s) + half * HALF_BYTES + c * R * 128, &map_k, k_full(s), half * 64, row, kv_head, blk);
           mbar_wait(v_empty(s), ph);
-          if (lane == 0) mbar_expect_tx(v_full(s), TILE_BYTES);
+          if (lane == 0) mbar_expect_tx(v_full(s), kTile);
           __syncwarp();
-          if (lane < 2 * C)
-            tma_load_4d(sV(s) + (c * R / 64) * HALF_BYTES + half * 8192 + (c * R % 64) * 128, &map_v, v_full(s), half * 64, row, kv_head, blk);
+          if (lane < kHalves * C)
+            tma_load_4d(sV(s) + (c * R / 64) * kVBlock + half * 8192 + (c * R % 64) * 128, &map_v, v_full(s), half * 64, row, kv_head, blk);
         }
       }
     } else if (lane == 0 && n_tiles > 0) {
@@ -252,9 +262,9 @@ fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CU
     const int rl = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's rows: rl and rl + 8
     float scale_log2 = p.scale_log2;
     if constexpr (Q8) scale_log2 *= __ldg(p.k_dq + kv_head);  // S is computed on the quantized K
-    float o_acc[HD / 2];
+    float o_acc[D / 2];
 #pragma unroll
-    for (int i = 0; i < HD / 2; ++i) o_acc[i] = 0.f;
+    for (int i = 0; i < D / 2; ++i) o_acc[i] = 0.f;
     float m_i[2] = {-INFINITY, -INFINITY}, l_i[2] = {0.f, 0.f};   // l_i: this thread's share of the row sum (reduced over the quad at the end)
     if (n_tiles > 0) mbar_wait(q_full, 0);
     for (int j = 0; j < n_tiles; ++j) {
@@ -264,7 +274,7 @@ fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CU
       wgmma_fence_regs(sv);
       wgmma_fence();
 #pragma unroll
-      for (int kb = 0; kb < 2; ++kb)
+      for (int kb = 0; kb < kHalves; ++kb)
 #pragma unroll
         for (int k = 0; k < 4; ++k)
           wgmma_ss_n128<BF16, 0, 0>(sv, make_smem_desc(sQ + kb * HALF_BYTES + wg * 8192 + k * 32, 16, 1024),
@@ -329,7 +339,7 @@ fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CU
           }
         l_i[h] = l_i[h] * alpha + sum;
 #pragma unroll
-        for (int jn = 0; jn < HD / 8; ++jn) { o_acc[jn * 4 + h * 2] *= alpha; o_acc[jn * 4 + h * 2 + 1] *= alpha; }
+        for (int jn = 0; jn < D / 8; ++jn) { o_acc[jn * 4 + h * 2] *= alpha; o_acc[jn * 4 + h * 2 + 1] *= alpha; }
       }
       // ---- P as A fragments: 16-key step ks = accumulator column groups 2 ks and 2 ks + 1 ----
       uint32_t pa[BN / 16][4];
@@ -344,9 +354,10 @@ fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CU
       if constexpr (PAGED && !Q8) {   // (the converter writes zeros past the sequence)
         if (j * BN + BN > sk) {   // V rows past the sequence hold stale cache contents (possibly NaN) and P = 0 does not cancel NaN: zero them
           const int tid = threadIdx.x & 127;
-          for (int e = (sk - j * BN) * 16 + tid; e < BN * 16; e += 128) {   // 16-byte chunks: key row e / 16, d-half (e / 8) & 1
-            const int r = e >> 4;
-            st_shared_zero16(sV(s) + (r >> 6) * HALF_BYTES + ((e >> 3) & 1) * 8192 + (r & 63) * 128 + (e & 7) * 16);
+          constexpr int kRowShift = D == 128 ? 4 : 3;           // log2 of the 16-byte chunks of a key row
+          for (int e = (sk - j * BN) * (1 << kRowShift) + tid; e < BN << kRowShift; e += 128) {   // key row e >> kRowShift, d-half (e / 8) & 1
+            const int r = e >> kRowShift;
+            st_shared_zero16(sV(s) + (r >> 6) * kVBlock + ((e >> 3) & (kHalves - 1)) * 8192 + (r & 63) * 128 + (e & 7) * 16);
           }
           fence_proxy_async();                    // generic-proxy stores before this warpgroup's wgmma reads them
           named_bar_sync(1 + wg, 128);
@@ -355,8 +366,11 @@ fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CU
       wgmma_fence_regs(o_acc);
       wgmma_fence();
 #pragma unroll
-      for (int ks = 0; ks < BN / 16; ++ks)     // V tile MN-major: 64-key block ks / 4, 16 key rows = 2048 B per step, 64-wide d chunks 8192 B apart
-        wgmma_rs_n128<BF16, 1>(o_acc, pa[ks], make_smem_desc(sV(s) + (ks >> 2) * HALF_BYTES + (ks & 3) * 2048, 8192, 1024), 1);
+      for (int ks = 0; ks < BN / 16; ++ks) {   // V tile MN-major: 64-key block ks / 4, 16 key rows = 2048 B per step, 64-wide d chunks 8192 B apart
+        const uint64_t vdesc = make_smem_desc(sV(s) + (ks >> 2) * kVBlock + (ks & 3) * 2048, 8192, 1024);
+        if constexpr (D == 128) wgmma_rs_n128<BF16, 1>(o_acc, pa[ks], vdesc, 1);
+        else wgmma_rs_n64<BF16, 1>(o_acc, pa[ks], vdesc, 1);
+      }
       wgmma_commit();
       wgmma_wait<0>();
       wgmma_fence_regs(o_acc);
@@ -379,7 +393,7 @@ fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CU
       if (row < nrows) {
         T* orow = reinterpret_cast<T*>(p.o) + (PAGED ? 0 : (int64_t)batch * p.o_sb) + (int64_t)(q0 + row) * p.o_ss + (int64_t)head * p.o_sh;
 #pragma unroll
-        for (int jn = 0; jn < HD / 8; ++jn)
+        for (int jn = 0; jn < D / 8; ++jn)
           *reinterpret_cast<uint32_t*>(orow + jn * 8 + 2 * q) = pack2<T>(o_acc[jn * 4 + h * 2] * inv, o_acc[jn * 4 + h * 2 + 1] * inv);
         if (q == 0 && p.lse) p.lse[((int64_t)(PAGED ? 0 : batch) * p.h + head) * p.sq + q0 + row] = l > 0.f ? (m_i[h] + log2f(l)) * 0.69314718055994531f : -INFINITY;
       }
@@ -495,7 +509,7 @@ int attention_paged_prefill_slots(int t, int b) { return (t + attn::BM - 1) / at
 int attention_paged_prefill_scratch_ints(int t, int b) { return 3 * attention_paged_prefill_slots(t, b) + b + 1; }
 
 int attention_paged_prefill_supported(const PagedAttnArgs& a) {
-  if (a.d != 128 || (a.dtype != kBF16 && a.dtype != kF16)) return 0;
+  if ((a.d != 128 && !(a.d == 64 && a.kv_dtype == -1)) || (a.dtype != kBF16 && a.dtype != kF16)) return 0;   // head_dim 64: 16-bit caches
   if (a.kv_dtype != -1 && ((a.kv_dtype != kI8 && a.kv_dtype != kE4M3) || !a.k_dq || !a.v_dq)) return 0;
   if (a.hk <= 0 || a.h % a.hk) return 0;
   if (a.block_size != 16 && a.block_size != 32 && a.block_size != 64 && a.block_size != 128 && a.block_size != 256) return 0;
@@ -557,12 +571,16 @@ int attention_paged_prefill(const PagedAttnArgs& a, cudaStream_t s) {
   p.work = work; p.cu_q = a.cu_q; p.n_q = a.n_q; p.past = a.past;
   p.block_tables = a.block_tables; p.max_blocks = a.max_blocks; p.block_size = a.block_size;
   dim3 grid(a.h, slots);   // every head of the heaviest tile is dispatched first
+  auto launch = [&](auto tag_t, auto tag_d) {
+    using T = decltype(tag_t);
+    constexpr int D = decltype(tag_d)::value;
+    set_max_dynamic_smem<fwd_kernel<T, false, true, T, D>>(kSmemBytes<D>);
+    fwd_kernel<T, false, true, T, D><<<grid, kThreads, kSmemBytes<D>, s>>>(mq, mk, mv, p);
+  };
   if (a.dtype == kBF16) {
-    set_max_dynamic_smem<fwd_kernel<__nv_bfloat16, false, true>>(SMEM_BYTES);
-    fwd_kernel<__nv_bfloat16, false, true><<<grid, kThreads, SMEM_BYTES, s>>>(mq, mk, mv, p);
+    if (a.d == 128) launch(__nv_bfloat16(), HeadDim<128>()); else launch(__nv_bfloat16(), HeadDim<64>());
   } else {
-    set_max_dynamic_smem<fwd_kernel<__half, false, true>>(SMEM_BYTES);
-    fwd_kernel<__half, false, true><<<grid, kThreads, SMEM_BYTES, s>>>(mq, mk, mv, p);
+    if (a.d == 128) launch(__half(), HeadDim<128>()); else launch(__half(), HeadDim<64>());
   }
   return B200_LAUNCH_RESULT();
 }

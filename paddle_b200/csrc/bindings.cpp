@@ -945,7 +945,7 @@ Tensor decode_attention(const Tensor& q, const Tensor& k_cache, const Tensor& v_
                                   pml.data_ptr<float>(), b, h, hkv, smax, d, splits, (float)scale, dt_code(q), cur_stream());
   g_launches += 2;
   check_err();
-  TORCH_CHECK(rc == 0, "paddle_b200.decode_attention: unsupported shape (head_dim 128, fp16/bf16 only) rc=", rc);
+  TORCH_CHECK(rc == 0, "paddle_b200.decode_attention: unsupported shape (head_dim 128 or 64, fp16/bf16 only) rc=", rc);
   return out;
 }
 
@@ -999,7 +999,7 @@ Tensor decode_attention_paged(const Tensor& q, const Tensor& k_cache, const Tens
                                   pml.data_ptr<float>(), b, h, hkv, mb * bs, d, splits, (float)scale, dt_code(q), cur_stream(), block_tables.data_ptr<int>(), mb, bs);
   g_launches += 2;
   check_err();
-  TORCH_CHECK(rc == 0, "paddle_b200.decode_attention_paged: unsupported shape (head_dim 128, fp16/bf16 only) rc=", rc);
+  TORCH_CHECK(rc == 0, "paddle_b200.decode_attention_paged: unsupported shape (head_dim 128 or 64, fp16/bf16 only) rc=", rc);
   return out;
 }
 
@@ -1091,8 +1091,8 @@ void attention_fwd_paged(const Tensor& q, const Tensor& k_cache, const Tensor& v
                 lse->size(1) == a.t, "attention_fwd_paged: lse must be fp32 [H, T]");
     a.lse = lse->data_ptr<float>();
   }
-  TORCH_CHECK(b200::attention_paged_prefill_supported(a), "attention_fwd_paged: unsupported operands (head_dim 128, fp16/bf16, H % Hkv == 0, "
-              "block_size in {16, 32, 64, 128, 256}, 16-byte aligned rows)");
+  TORCH_CHECK(b200::attention_paged_prefill_supported(a), "attention_fwd_paged: unsupported operands (head_dim 128, or 64 on 16-bit caches, "
+              "fp16/bf16, H % Hkv == 0, block_size in {16, 32, 64, 128, 256}, 16-byte aligned rows)");
   c10::cuda::CUDAGuard guard(q.device());
   Tensor scratch = torch::empty({b200::attention_paged_prefill_scratch_ints(a.t, a.b)}, q.options().dtype(at::kInt));
   a.scratch = scratch.data_ptr<int>();
@@ -1126,7 +1126,8 @@ void decode_attention_paged_multi(const Tensor& q, const Tensor& k_cache, const 
                 "decode_attention_paged_multi: cu_q / n_q / past must be int32 [B] on the device");
   TORCH_CHECK(out.device() == q.device() && out.scalar_type() == q.scalar_type() && out.dim() == 2 && out.size(0) == q.size(0) &&
               out.size(1) == q.size(1) * q.size(2) && out.stride(1) == 1, "decode_attention_paged_multi: out must be [T, H*D] with unit inner stride");
-  TORCH_CHECK(q.size(2) == 128 && k_cache.size(3) == 128, "decode_attention_paged_multi: head_dim must be 128");
+  TORCH_CHECK(q.size(2) == k_cache.size(3) && (q.size(2) == 128 || (q.size(2) == 64 && kv == -1)),
+              "decode_attention_paged_multi: head_dim must be 128, or 64 on 16-bit caches");
   const int64_t hkv = k_cache.size(1);
   TORCH_CHECK(hkv > 0 && q.size(1) % hkv == 0 && q.size(1) / hkv <= 64, "decode_attention_paged_multi: H must be a multiple of Hkv with H / Hkv <= 64, "
               "and n_q * (H / Hkv) <= 64 per sequence");
@@ -1140,7 +1141,7 @@ void decode_attention_paged_multi(const Tensor& q, const Tensor& k_cache, const 
   a.scale = (float)scale; a.dtype = dt_code(q);
   if (kv != -1) { a.kv_dtype = kv; a.k_dq = k_dequant_scales->data_ptr<float>(); a.v_dq = v_dequant_scales->data_ptr<float>(); }
   c10::cuda::CUDAGuard guard(q.device());
-  Tensor pacc = torch::empty({b, hkv, a.splits, 64, 128}, q.options().dtype(at::kFloat));
+  Tensor pacc = torch::empty({b, hkv, a.splits, 64, a.d}, q.options().dtype(at::kFloat));
   Tensor pml = torch::empty({b, hkv, a.splits, 64, 2}, q.options().dtype(at::kFloat));
   a.part_acc = pacc.data_ptr<float>(); a.part_ml = pml.data_ptr<float>();
   int rc = b200::decode_attention_paged_multi(a, cur_stream());

@@ -7,13 +7,13 @@
 // lens[b] = number of valid cached positions (the new token already written).  Grid = (splits, H, B): every CTA owns a
 // contiguous range of positions; thread t handles positions t, t+128, ... with a private online softmax (m, l, acc[D]);
 // the CTA combines its threads through shared memory and writes one partial (m, l, acc) per split; a second tiny kernel
-// merges the splits.  D = 128, fp16 / bf16.
+// merges the splits.  D = 128 or 64 (a template argument), fp16 / bf16.
 //
 // Paged caches (block_multihead_attention, paddle/phi/kernels/fusion/gpu/block_multi_head_attention_kernel.cu): with `block_tables`
 // [B, max_blocks] the caches are [num_blocks, Hkv, block_size, D] and position p of sequence b lives in block block_tables[b, p / block_size]
 // at row p % block_size - one table lookup per cached row, the rest of the kernel is unchanged.
 //
-// Paged int8 / fp8 e4m3 caches (decode_split_q8_kernel): the same walk over 8-bit rows, dequantized with per-KV-head scales.
+// Paged int8 / fp8 e4m3 caches (decode_split_q8_kernel, D = 128): the same walk over 8-bit rows, dequantized with per-KV-head scales.
 #include <cuda.h>
 #include <cstdio>
 #include <type_traits>
@@ -25,9 +25,10 @@
 namespace b200 {
 namespace decode {
 
-constexpr int D = 128, kThreads = 128;
+constexpr int kThreads = 128;
 
 // Combine the CTA's per-thread online-softmax partials (m, l, acc) and write this split's partial (m, l, acc * v_scale).
+template <int D>
 __device__ __forceinline__ void split_epilogue(float m, float l, const float (&acc)[D], float* red, float (*sacc)[D + 1], float* __restrict__ part_acc,
                                                float* __restrict__ part_ml, int h, int splits, float v_scale) {
   const int split = blockIdx.x, head = blockIdx.y, b = blockIdx.z, tid = threadIdx.x;
@@ -49,7 +50,7 @@ __device__ __forceinline__ void split_epilogue(float m, float l, const float (&a
     __syncthreads();
   }
   const float lg = red[0];
-  // sum the 128 per-thread accumulators: 4 rounds of 32 threads' vectors through shared memory, thread t owns output dim t
+  // sum the 128 per-thread accumulators: 4 rounds of 32 threads' vectors through shared memory, thread t < D owns output dim t
   float out = 0.f;
   for (int r = 0; r < kThreads / 32; ++r) {
     __syncthreads();
@@ -58,15 +59,16 @@ __device__ __forceinline__ void split_epilogue(float m, float l, const float (&a
       for (int i = 0; i < D; ++i) sacc[tid & 31][i] = acc[i] * f;
     }
     __syncthreads();
+    if (D < kThreads && tid >= D) continue;
 #pragma unroll 8
     for (int j = 0; j < 32; ++j) out += sacc[j][tid];
   }
   const int64_t pi = ((int64_t)b * h + head) * splits + split;
-  part_acc[pi * D + tid] = out * v_scale;
+  if (D == kThreads || tid < D) part_acc[pi * D + tid] = out * v_scale;
   if (tid == 0) { part_ml[pi * 2] = mg; part_ml[pi * 2 + 1] = lg; }
 }
 
-template <typename T>
+template <typename T, int D>
 __global__ void __launch_bounds__(kThreads) decode_split_kernel(const T* __restrict__ q, const T* __restrict__ kc, const T* __restrict__ vc,
                                                                 const int* __restrict__ lens, float* __restrict__ part_acc,
                                                                 float* __restrict__ part_ml, int h, int hkv, int smax, int splits, float scale_log2,
@@ -80,7 +82,7 @@ __global__ void __launch_bounds__(kThreads) decode_split_kernel(const T* __restr
   __shared__ float red[kThreads];
   __shared__ float sacc[32][D + 1];           // one slice of the cross-thread reduction at a time
   const int tid = threadIdx.x;
-  sq[tid] = to_f(q[((int64_t)b * h + head) * D + tid]) * scale_log2;
+  if (D == kThreads || tid < D) sq[tid] = to_f(q[((int64_t)b * h + head) * D + tid]) * scale_log2;
   __syncthreads();
   const T* kbase = kc + ((int64_t)b * hkv + kvh) * (int64_t)smax * D;
   const T* vbase = vc + ((int64_t)b * hkv + kvh) * (int64_t)smax * D;
@@ -118,7 +120,7 @@ __global__ void __launch_bounds__(kThreads) decode_split_kernel(const T* __restr
     }
     m = m_new;
   }
-  split_epilogue(m, l, acc, red, sacc, part_acc, part_ml, h, splits, 1.f);
+  split_epilogue<D>(m, l, acc, red, sacc, part_acc, part_ml, h, splits, 1.f);
 }
 
 // Paged 8-bit caches (KV = kv8::I8 / kv8::E4M3): one 16-byte load carries 16 elements.  The K dequant scale is folded into sq, the V
@@ -130,6 +132,7 @@ __global__ void __launch_bounds__(kThreads) decode_split_q8_kernel(const T* __re
                                                                    float* __restrict__ part_ml, int h, int hkv, int splits, float scale_log2,
                                                                    const float* __restrict__ k_dq, const float* __restrict__ v_dq,
                                                                    const int* __restrict__ block_tables, int max_blocks, int block_size) {
+  constexpr int D = 128;
   const int split = blockIdx.x, head = blockIdx.y, b = blockIdx.z;
   const int kvh = head / (h / hkv);
   const int len = min(lens[b], max_blocks * block_size);
@@ -178,10 +181,10 @@ __global__ void __launch_bounds__(kThreads) decode_split_q8_kernel(const T* __re
     }
     m = m_new;
   }
-  split_epilogue(m, l, acc, red, sacc, part_acc, part_ml, h, splits, __ldg(v_dq + kvh));
+  split_epilogue<D>(m, l, acc, red, sacc, part_acc, part_ml, h, splits, __ldg(v_dq + kvh));
 }
 
-template <typename T>
+template <typename T, int D>
 __global__ void __launch_bounds__(D) decode_merge_kernel(const float* __restrict__ part_acc, const float* __restrict__ part_ml, T* __restrict__ out,
                                                          int splits) {
   const int64_t bh = blockIdx.x;
@@ -209,14 +212,17 @@ __global__ void __launch_bounds__(D) decode_merge_kernel(const float* __restrict
 // < past + j + 1.  Each split writes an unnormalized partial (m, l, acc) per row; multi_merge_kernel combines them like decode_merge_kernel.
 // 8-bit caches are copied raw and converted exactly to 16 bits in shared memory; K's dequant scale joins the softmax scale and V's scales
 // the split's partial, so with power-of-two scales the result is bit-identical to the 16-bit kernel on the dequantized cache.
+// D = 128, or 64 on 16-bit caches: the same 64-row tile, with half the k-steps of S and half the output columns.
 namespace decode_multi {
 
-constexpr int D = 128, BN = 64, kRows = 64, kThreads = 128, kStages = 3;
-constexpr int kTile16 = BN * D * 2, kTile8 = BN * D;   // one K or V tile of 64 keys: 16 KB in 16 bits, 8 KB in 8 bits
+constexpr int BN = 64, kRows = 64, kThreads = 128, kStages = 3;
+// one K or V tile of 64 keys: 16 KB in 16 bits, 8 KB in 8 bits at D = 128
+template <int D> constexpr int kTile16 = BN * D * 2;
+template <int D> constexpr int kTile8 = BN * D;
 
 struct Params {
   const void* q; const void* k_cache; const void* v_cache;
-  void* out; float* part_acc; float* part_ml;
+  void* out; float* part_acc; float* part_ml;   // part_acc: [B, Hkv, splits, 64 rows, D]
   const int* block_tables; const int* cu_q; const int* n_q; const int* past;
   const float* k_dq; const float* v_dq;
   int64_t q_st, q_sh, o_st;   // element strides: q (token, head), out (token; heads are D apart)
@@ -224,15 +230,16 @@ struct Params {
   float scale_log2;
 };
 
-// shared memory: Q tile [64][128] 16-bit | K, V 16-bit tiles (kStages, or 1 for 8-bit caches) | 8-bit caches: raw K, V tiles (kStages).
-// Two tiles stay in flight while one is computed; two CTAs fit on an SM.
-template <bool Q8> struct Smem {
+// shared memory: Q tile [64][D] 16-bit | K, V 16-bit tiles (kStages, or 1 for 8-bit caches) | 8-bit caches: raw K, V tiles (kStages).
+// Two tiles stay in flight while one is computed; two CTAs fit on an SM at D = 128.
+template <bool Q8, int D> struct Smem {
   static constexpr int kKV = kRows * D * 2;
-  static constexpr int kRaw = kKV + (Q8 ? 1 : kStages) * 2 * kTile16;
-  static constexpr int kBytes = kRaw + (Q8 ? kStages * 2 * kTile8 : 0);
+  static constexpr int kRaw = kKV + (Q8 ? 1 : kStages) * 2 * kTile16<D>;
+  static constexpr int kBytes = kRaw + (Q8 ? kStages * 2 * kTile8<D> : 0);
 };
 
-// byte offset of 16-byte chunk c (0..15) of row `row` in a [rows][128] 16-bit tile; the XOR spreads 8 consecutive rows over all banks
+// byte offset of 16-byte chunk c (0 .. D / 8 - 1) of row `row` in a [rows][D] 16-bit tile; the XOR spreads 8 consecutive rows over all banks
+template <int D>
 __device__ __forceinline__ uint32_t swz(int row, int c) { return (uint32_t)(row * (D * 2) + ((c ^ (row & 7)) << 4)); }
 
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool valid) {   // !valid: zero-fill, nothing is read
@@ -258,11 +265,15 @@ template <> __device__ __forceinline__ void mma16816<__half>(float (&c)[4], cons
                : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-// KV = T: 16-bit caches; KV = kv8::I8 / kv8::E4M3: 8-bit caches with fp32 [Hkv] dequant scales
-template <typename T, typename KV>
-__global__ void __launch_bounds__(kThreads) multi_split_kernel(const Params p) {
+// The split kernel's body for head size D (inlined into multi_split_kernel and decode_verify64::multi_split_kernel).
+// KV = T: 16-bit caches; KV = kv8::I8 / kv8::E4M3: 8-bit caches with fp32 [Hkv] dequant scales (D = 128 only)
+template <typename T, typename KV, int D>
+__device__ __forceinline__ void multi_split(const Params& p) {
   constexpr bool Q8 = !std::is_same<T, KV>::value;
-  using S = Smem<Q8>;
+  static_assert(D == 128 || (D == 64 && !Q8), "head_dim 128, or 64 on 16-bit caches");
+  constexpr int kTile16 = decode_multi::kTile16<D>, kTile8 = decode_multi::kTile8<D>;
+  using S = Smem<Q8, D>;
+  constexpr int kQShift = D == 128 ? 4 : 3;                  // log2 of the 16-byte chunks of a Q row
   const int split = blockIdx.x, kvh = blockIdx.y, b = blockIdx.z;
   const int nq = p.n_q[b], g_size = p.h / p.hkv, nrows = nq * g_size;
   if (nq <= 0 || nrows > kRows) return;                      // skipped, or past the row limit (multi_merge_kernel writes NaN)
@@ -279,11 +290,11 @@ __global__ void __launch_bounds__(kThreads) multi_split_kernel(const Params p) {
   // Q tile: rows past nrows are zero
 #pragma unroll
   for (int i = 0; i < kRows * D / 8 / kThreads; ++i) {
-    const int row = i * (kThreads / 16) + (tid >> 4), c = tid & 15;
+    const int row = i * (kThreads >> kQShift) + (tid >> kQShift), c = tid & ((1 << kQShift) - 1);
     const bool ok = row < nrows;
     const T* src = reinterpret_cast<const T*>(p.q);
     if (ok) src += (int64_t)(cu + row / g_size) * p.q_st + (int64_t)(kvh * g_size + row % g_size) * p.q_sh + c * 8;
-    cp_async16(sbase + swz(row, c), src, ok);
+    cp_async16(sbase + swz<D>(row, c), src, ok);
   }
   // cached K / V rows of key tile `tile` into stage `st`; keys at or past len are zero-filled
   auto load_kv = [&](int tile, int st) {
@@ -301,7 +312,7 @@ __global__ void __launch_bounds__(kThreads) multi_split_kernel(const Params p) {
         cp_async16(dst, reinterpret_cast<const uint8_t*>(p.k_cache) + off, ok);
         cp_async16(dst + kTile8, reinterpret_cast<const uint8_t*>(p.v_cache) + off, ok);
       } else {
-        const uint32_t dst = sbase + S::kKV + st * 2 * kTile16 + swz(row, c);
+        const uint32_t dst = sbase + S::kKV + st * 2 * kTile16 + swz<D>(row, c);
         cp_async16(dst, reinterpret_cast<const T*>(p.k_cache) + off, ok);
         cp_async16(dst + kTile16, reinterpret_cast<const T*>(p.v_cache) + off, ok);
       }
@@ -333,7 +344,7 @@ __global__ void __launch_bounds__(kThreads) multi_split_kernel(const Params p) {
     cp_async_commit();
     if (t == t0 && active) {
 #pragma unroll
-      for (int kk = 0; kk < D / 16; ++kk) ldsm_x4(qf[kk], sbase + swz(warp * 16 + (lane & 15), kk * 2 + (lane >> 4)));
+      for (int kk = 0; kk < D / 16; ++kk) ldsm_x4(qf[kk], sbase + swz<D>(warp * 16 + (lane & 15), kk * 2 + (lane >> 4)));
     }
     uint32_t kv16 = sbase + S::kKV + st * 2 * kTile16;
     if constexpr (Q8) {                                      // raw 8-bit tiles -> the 16-bit tiles, exactly
@@ -348,8 +359,8 @@ __global__ void __launch_bounds__(kThreads) multi_split_kernel(const Params p) {
 #pragma unroll
         for (int e = 0; e < 8; ++e) w[e] = pack2<T>(f[2 * e], f[2 * e + 1]);
         uint8_t* dst = smem + S::kKV + kv * kTile16;
-        *reinterpret_cast<uint4*>(dst + swz(row, 2 * c)) = make_uint4(w[0], w[1], w[2], w[3]);
-        *reinterpret_cast<uint4*>(dst + swz(row, 2 * c + 1)) = make_uint4(w[4], w[5], w[6], w[7]);
+        *reinterpret_cast<uint4*>(dst + swz<D>(row, 2 * c)) = make_uint4(w[0], w[1], w[2], w[3]);
+        *reinterpret_cast<uint4*>(dst + swz<D>(row, 2 * c + 1)) = make_uint4(w[4], w[5], w[6], w[7]);
       }
       __syncthreads();
     }
@@ -363,7 +374,7 @@ __global__ void __launch_bounds__(kThreads) multi_split_kernel(const Params p) {
 #pragma unroll
         for (int np = 0; np < BN / 16; ++np) {
           uint32_t bf[4];
-          ldsm_x4(bf, kv16 + swz(np * 16 + (lane & 7) + ((lane >> 4) << 3), kk * 2 + ((lane >> 3) & 1)));
+          ldsm_x4(bf, kv16 + swz<D>(np * 16 + (lane & 7) + ((lane >> 4) << 3), kk * 2 + ((lane >> 3) & 1)));
           mma16816<T>(s[2 * np], qf[kk], bf[0], bf[1]);
           mma16816<T>(s[2 * np + 1], qf[kk], bf[2], bf[3]);
         }
@@ -408,7 +419,7 @@ __global__ void __launch_bounds__(kThreads) multi_split_kernel(const Params p) {
 #pragma unroll
         for (int np = 0; np < D / 16; ++np) {
           uint32_t bf[4];
-          ldsm_x4_t(bf, kv16 + kTile16 + swz(kk * 16 + (lane & 7) + (((lane >> 3) & 1) << 3), np * 2 + (lane >> 4)));
+          ldsm_x4_t(bf, kv16 + kTile16 + swz<D>(kk * 16 + (lane & 7) + (((lane >> 3) & 1) << 3), np * 2 + (lane >> 4)));
           mma16816<T>(acc[2 * np], pa, bf[0], bf[1]);
           mma16816<T>(acc[2 * np + 1], pa, bf[2], bf[3]);
         }
@@ -433,10 +444,13 @@ __global__ void __launch_bounds__(kThreads) multi_split_kernel(const Params p) {
   }
 }
 
+template <typename T, typename KV>
+__global__ void __launch_bounds__(kThreads) multi_split_kernel(const Params p) { multi_split<T, KV, 128>(p); }
+
 // grid (64 rows, Hkv, B), D threads: combines the splits of one query row, as decode_merge_kernel does, and writes it in place.  A
 // sequence over the row limit gets NaN rows rather than a silently partial result.
-template <typename T>
-__global__ void __launch_bounds__(D) multi_merge_kernel(const Params p) {
+template <typename T, int D>
+__device__ __forceinline__ void multi_merge(const Params& p) {
   const int r = blockIdx.x, kvh = blockIdx.y, b = blockIdx.z, tid = threadIdx.x;
   const int nq = p.n_q[b], g_size = p.h / p.hkv, nrows = nq * g_size;
   if (nq <= 0) return;
@@ -462,7 +476,24 @@ __global__ void __launch_bounds__(D) multi_merge_kernel(const Params p) {
   out[(cu + r / g_size) * p.o_st + (int64_t)(kvh * g_size + r % g_size) * D + tid] = from_f<T>(l > 0.f ? o / l : 0.f);
 }
 
+template <typename T>
+__global__ void __launch_bounds__(128) multi_merge_kernel(const Params p) { multi_merge<T, 128>(p); }
+
 }  // namespace decode_multi
+
+// Verify rows at head_dim 64 (16-bit caches): decode_multi's split and merge bodies at D = 64, in kernels of their own so that the
+// head_dim 128 kernels keep their names and code.
+namespace decode_verify64 {
+
+struct Params : decode_multi::Params {};
+
+template <typename T>
+__global__ void __launch_bounds__(decode_multi::kThreads) multi_split_kernel(const __grid_constant__ Params p) { decode_multi::multi_split<T, T, 64>(p); }
+
+template <typename T>
+__global__ void __launch_bounds__(64) multi_merge_kernel(const __grid_constant__ Params p) { decode_multi::multi_merge<T, 64>(p); }
+
+}  // namespace decode_verify64
 
 // Shared-prefix decode ("cascade" decode): single-token decode rows of sequences whose leading blocks are the same physical blocks.
 // The host turns the groups into a task list.  A prefix task packs up to 64 / G members of one group (G = H / Hkv query heads per KV
@@ -476,12 +507,10 @@ __global__ void __launch_bounds__(D) multi_merge_kernel(const Params p) {
 namespace decode_shared {
 
 using decode_multi::BN;
-using decode_multi::D;
 using decode_multi::kRows;
 using decode_multi::kStages;
 using decode_multi::kThreads;
-using decode_multi::kTile16;
-using decode_multi::kTile8;
+constexpr int D = 128, kTile16 = decode_multi::kTile16<D>, kTile8 = decode_multi::kTile8<D>;
 
 struct Params {
   const void* q; const void* k_cache; const void* v_cache;
@@ -497,7 +526,7 @@ struct Params {
 template <typename T, typename KV>
 __global__ void __launch_bounds__(kThreads) shared_split_kernel(const Params p) {
   constexpr bool Q8 = !std::is_same<T, KV>::value;
-  using S = decode_multi::Smem<Q8>;
+  using S = decode_multi::Smem<Q8, D>;
   const int* task = p.tasks + (int64_t)blockIdx.x * kSharedTaskInts;
   const int kvh = blockIdx.y;
   const int tb = task[0], m0 = task[1], cnt = task[2], lo = task[3], split = task[5], splits = task[6];
@@ -524,7 +553,7 @@ __global__ void __launch_bounds__(kThreads) shared_split_kernel(const Params p) 
     const bool ok = row < nrows;
     const T* src = reinterpret_cast<const T*>(p.q);
     if (ok) src += (int64_t)p.cu_q[p.group_seqs[m0 + row / g_size]] * p.q_st + (int64_t)(kvh * g_size + row % g_size) * p.q_sh + c * 8;
-    decode_multi::cp_async16(sbase + decode_multi::swz(row, c), src, ok);
+    decode_multi::cp_async16(sbase + decode_multi::swz<D>(row, c), src, ok);
   }
   // K / V rows of key tile `tile` (keys lo + tile * 64 ...) into stage `st`; keys at or past hi are zero-filled
   auto load_kv = [&](int tile, int st) {
@@ -542,7 +571,7 @@ __global__ void __launch_bounds__(kThreads) shared_split_kernel(const Params p) 
         decode_multi::cp_async16(dst, reinterpret_cast<const uint8_t*>(p.k_cache) + off, ok);
         decode_multi::cp_async16(dst + kTile8, reinterpret_cast<const uint8_t*>(p.v_cache) + off, ok);
       } else {
-        const uint32_t dst = sbase + S::kKV + st * 2 * kTile16 + decode_multi::swz(row, c);
+        const uint32_t dst = sbase + S::kKV + st * 2 * kTile16 + decode_multi::swz<D>(row, c);
         decode_multi::cp_async16(dst, reinterpret_cast<const T*>(p.k_cache) + off, ok);
         decode_multi::cp_async16(dst + kTile16, reinterpret_cast<const T*>(p.v_cache) + off, ok);
       }
@@ -571,7 +600,7 @@ __global__ void __launch_bounds__(kThreads) shared_split_kernel(const Params p) 
     decode_multi::cp_async_commit();
     if (t == t0 && active) {
 #pragma unroll
-      for (int kk = 0; kk < D / 16; ++kk) decode_multi::ldsm_x4(qf[kk], sbase + decode_multi::swz(warp * 16 + (lane & 15), kk * 2 + (lane >> 4)));
+      for (int kk = 0; kk < D / 16; ++kk) decode_multi::ldsm_x4(qf[kk], sbase + decode_multi::swz<D>(warp * 16 + (lane & 15), kk * 2 + (lane >> 4)));
     }
     uint32_t kv16 = sbase + S::kKV + st * 2 * kTile16;
     if constexpr (Q8) {
@@ -586,8 +615,8 @@ __global__ void __launch_bounds__(kThreads) shared_split_kernel(const Params p) 
 #pragma unroll
         for (int e = 0; e < 8; ++e) w[e] = pack2<T>(f[2 * e], f[2 * e + 1]);
         uint8_t* dst = smem + S::kKV + kv * kTile16;
-        *reinterpret_cast<uint4*>(dst + decode_multi::swz(row, 2 * c)) = make_uint4(w[0], w[1], w[2], w[3]);
-        *reinterpret_cast<uint4*>(dst + decode_multi::swz(row, 2 * c + 1)) = make_uint4(w[4], w[5], w[6], w[7]);
+        *reinterpret_cast<uint4*>(dst + decode_multi::swz<D>(row, 2 * c)) = make_uint4(w[0], w[1], w[2], w[3]);
+        *reinterpret_cast<uint4*>(dst + decode_multi::swz<D>(row, 2 * c + 1)) = make_uint4(w[4], w[5], w[6], w[7]);
       }
       __syncthreads();
     }
@@ -600,7 +629,7 @@ __global__ void __launch_bounds__(kThreads) shared_split_kernel(const Params p) 
 #pragma unroll
         for (int np = 0; np < BN / 16; ++np) {
           uint32_t bf[4];
-          decode_multi::ldsm_x4(bf, kv16 + decode_multi::swz(np * 16 + (lane & 7) + ((lane >> 4) << 3), kk * 2 + ((lane >> 3) & 1)));
+          decode_multi::ldsm_x4(bf, kv16 + decode_multi::swz<D>(np * 16 + (lane & 7) + ((lane >> 4) << 3), kk * 2 + ((lane >> 3) & 1)));
           decode_multi::mma16816<T>(s[2 * np], qf[kk], bf[0], bf[1]);
           decode_multi::mma16816<T>(s[2 * np + 1], qf[kk], bf[2], bf[3]);
         }
@@ -644,7 +673,7 @@ __global__ void __launch_bounds__(kThreads) shared_split_kernel(const Params p) 
 #pragma unroll
         for (int np = 0; np < D / 16; ++np) {
           uint32_t bf[4];
-          decode_multi::ldsm_x4_t(bf, kv16 + kTile16 + decode_multi::swz(kk * 16 + (lane & 7) + (((lane >> 3) & 1) << 3), np * 2 + (lane >> 4)));
+          decode_multi::ldsm_x4_t(bf, kv16 + kTile16 + decode_multi::swz<D>(kk * 16 + (lane & 7) + (((lane >> 3) & 1) << 3), np * 2 + (lane >> 4)));
           decode_multi::mma16816<T>(acc[2 * np], pa, bf[0], bf[1]);
           decode_multi::mma16816<T>(acc[2 * np + 1], pa, bf[2], bf[3]);
         }
@@ -717,18 +746,21 @@ int decode_attention(const void* q, const void* k_cache, const void* v_cache, co
                      int h, int hkv, int smax, int d, int splits, float scale, int dtype, cudaStream_t s, const int* block_tables, int max_blocks,
                      int block_size) {
   using namespace decode;
-  if (d != D || h % hkv || (dtype != kBF16 && dtype != kF16)) return 1;
+  if ((d != 128 && d != 64) || h % hkv || (dtype != kBF16 && dtype != kF16)) return 1;
   if (block_tables && (max_blocks <= 0 || block_size <= 0)) return 1;
   dim3 grid(splits, h, b);
   const float sl2 = scale * 1.4426950408889634f;
+  auto launch = [&](auto tag_t, auto tag_d) {
+    using T = decltype(tag_t);
+    constexpr int D = decltype(tag_d)::value;
+    decode_split_kernel<T, D><<<grid, kThreads, 0, s>>>((const T*)q, (const T*)k_cache, (const T*)v_cache, lens, part_acc, part_ml, h, hkv, smax, splits,
+                                                        sl2, block_tables, max_blocks, block_size);
+    decode_merge_kernel<T, D><<<b * h, D, 0, s>>>(part_acc, part_ml, (T*)out, splits);
+  };
   if (dtype == kBF16) {
-    decode_split_kernel<__nv_bfloat16><<<grid, kThreads, 0, s>>>((const __nv_bfloat16*)q, (const __nv_bfloat16*)k_cache, (const __nv_bfloat16*)v_cache, lens,
-                                                                   part_acc, part_ml, h, hkv, smax, splits, sl2, block_tables, max_blocks, block_size);
-    decode_merge_kernel<__nv_bfloat16><<<b * h, D, 0, s>>>(part_acc, part_ml, (__nv_bfloat16*)out, splits);
+    if (d == 128) launch(__nv_bfloat16(), HeadDim<128>()); else launch(__nv_bfloat16(), HeadDim<64>());
   } else {
-    decode_split_kernel<__half><<<grid, kThreads, 0, s>>>((const __half*)q, (const __half*)k_cache, (const __half*)v_cache, lens, part_acc, part_ml, h, hkv,
-                                                           smax, splits, sl2, block_tables, max_blocks, block_size);
-    decode_merge_kernel<__half><<<b * h, D, 0, s>>>(part_acc, part_ml, (__half*)out, splits);
+    if (d == 128) launch(__half(), HeadDim<128>()); else launch(__half(), HeadDim<64>());
   }
   return B200_LAUNCH_RESULT();
 }
@@ -737,7 +769,7 @@ int decode_attention_paged_q8(const void* q, const void* k_cache, const void* v_
                               int b, int h, int hkv, int d, int splits, float scale, int dtype, int kv_dtype, const float* k_dq, const float* v_dq,
                               const int* block_tables, int max_blocks, int block_size, cudaStream_t s) {
   using namespace decode;
-  if (d != D || h % hkv || (dtype != kBF16 && dtype != kF16) || (kv_dtype != kI8 && kv_dtype != kE4M3)) return 1;
+  if (d != 128 || h % hkv || (dtype != kBF16 && dtype != kF16) || (kv_dtype != kI8 && kv_dtype != kE4M3)) return 1;
   if (!block_tables || !k_dq || !v_dq || max_blocks <= 0 || block_size <= 0) return 1;
   dim3 grid(splits, h, b);
   const float sl2 = scale * 1.4426950408889634f;
@@ -746,7 +778,7 @@ int decode_attention_paged_q8(const void* q, const void* k_cache, const void* v_
     decode_split_q8_kernel<T, decltype(tag_kv)><<<grid, kThreads, 0, s>>>((const T*)q, (const uint8_t*)k_cache, (const uint8_t*)v_cache, lens,
                                                                           part_acc, part_ml, h, hkv, splits, sl2, k_dq, v_dq, block_tables,
                                                                           max_blocks, block_size);
-    decode_merge_kernel<T><<<b * h, D, 0, s>>>(part_acc, part_ml, (T*)out, splits);
+    decode_merge_kernel<T, 128><<<b * h, 128, 0, s>>>(part_acc, part_ml, (T*)out, splits);
   };
   if (dtype == kBF16) {
     if (kv_dtype == kI8) launch(__nv_bfloat16(), kv8::I8()); else launch(__nv_bfloat16(), kv8::E4M3());
@@ -758,7 +790,7 @@ int decode_attention_paged_q8(const void* q, const void* k_cache, const void* v_
 
 int decode_attention_paged_multi(const PagedMultiArgs& a, cudaStream_t s) {
   using namespace decode_multi;
-  if (a.d != D || a.hkv <= 0 || a.h % a.hkv || a.h / a.hkv > kRows || (a.dtype != kBF16 && a.dtype != kF16)) return 1;
+  if ((a.d != 128 && a.d != 64) || (a.d == 64 && a.kv_dtype != -1) || a.hkv <= 0 || a.h % a.hkv || a.h / a.hkv > kRows || (a.dtype != kBF16 && a.dtype != kF16)) return 1;
   if (a.kv_dtype != -1 && ((a.kv_dtype != kI8 && a.kv_dtype != kE4M3) || !a.k_dq || !a.v_dq)) return 1;
   if (a.max_blocks <= 0 || a.block_size <= 0 || a.splits < 1) return 1;
   if (a.q_st % 8 || a.q_sh % 8 || a.o_st % 8 || ((reinterpret_cast<uintptr_t>(a.q) | reinterpret_cast<uintptr_t>(a.k_cache) |
@@ -771,13 +803,26 @@ int decode_attention_paged_multi(const PagedMultiArgs& a, cudaStream_t s) {
   p.h = a.h; p.hkv = a.hkv; p.splits = a.splits; p.max_blocks = a.max_blocks; p.block_size = a.block_size;
   p.scale_log2 = a.scale * 1.4426950408889634f;
   const dim3 grid(a.splits, a.hkv, a.b), mgrid(kRows, a.hkv, a.b);
+  if (a.d == 64) {
+    auto launch64 = [&](auto tag_t) {
+      using T = decltype(tag_t);
+      constexpr int smem = Smem<false, 64>::kBytes;
+      decode_verify64::Params p64;
+      static_cast<Params&>(p64) = p;
+      set_max_dynamic_smem<decode_verify64::multi_split_kernel<T>>(smem);
+      decode_verify64::multi_split_kernel<T><<<grid, kThreads, smem, s>>>(p64);
+      decode_verify64::multi_merge_kernel<T><<<mgrid, 64, 0, s>>>(p64);
+    };
+    if (a.dtype == kBF16) launch64(__nv_bfloat16()); else launch64(__half());
+    return B200_LAUNCH_RESULT();
+  }
   auto launch = [&](auto tag_t, auto tag_kv) {
     using T = decltype(tag_t);
     using KV = decltype(tag_kv);
-    constexpr int smem = Smem<!std::is_same<T, KV>::value>::kBytes;
+    constexpr int smem = Smem<!std::is_same<T, KV>::value, 128>::kBytes;
     set_max_dynamic_smem<multi_split_kernel<T, KV>>(smem);
     multi_split_kernel<T, KV><<<grid, kThreads, smem, s>>>(p);
-    multi_merge_kernel<T><<<mgrid, D, 0, s>>>(p);
+    multi_merge_kernel<T><<<mgrid, 128, 0, s>>>(p);
   };
   if (a.dtype == kBF16) {
     if (a.kv_dtype == kI8) launch(__nv_bfloat16(), kv8::I8());
@@ -810,7 +855,7 @@ int decode_attention_paged_shared(const PagedSharedArgs& a, cudaStream_t s) {
   auto launch = [&](auto tag_t, auto tag_kv) {
     using T = decltype(tag_t);
     using KV = decltype(tag_kv);
-    constexpr int smem = decode_multi::Smem<!std::is_same<T, KV>::value>::kBytes;
+    constexpr int smem = decode_multi::Smem<!std::is_same<T, KV>::value, D>::kBytes;
     set_max_dynamic_smem<shared_split_kernel<T, KV>>(smem);
     shared_split_kernel<T, KV><<<grid, kThreads, smem, s>>>(p);
     shared_merge_kernel<T><<<mgrid, D, 0, s>>>(p);

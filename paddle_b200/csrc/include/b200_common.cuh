@@ -6,6 +6,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 namespace b200 {
 
 enum DType : int { kF32 = 0, kF16 = 1, kBF16 = 2, kI8 = 3, kE4M3 = 4 };   // kI8 / kE4M3: quantized KV caches only
@@ -167,6 +169,9 @@ namespace attn {
 bool make_map4(CUtensorMap* out, const void* ptr, int d, int s, int h, int b, int64_t ss, int64_t sh, int64_t sb, uint32_t box_rows,
                int dtype);
 }
+
+// A launcher's head size as a tag argument of its generic launch lambda.
+template <int D> using HeadDim = std::integral_constant<int, D>;
 
 // Raise the kernel's dynamic shared-memory limit before its first launch. The flag is per kernel pointer: two instantiations of one
 // kernel template with the same signature have the same type but each needs its own attribute.

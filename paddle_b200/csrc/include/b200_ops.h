@@ -221,22 +221,22 @@ int weight_dequantize(const void* w, const float* scale, void* out, int n, int k
                       int experts = 1);
 
 // ---- decode_attention.cu --------------------------------------------------------------------------------------
-// Single-token decode attention: q [B,H,128], k/v cache [B,Hkv,S_max,128], lens[b] valid positions; out [B,H,128].
-// part_acc: fp32 [B,H,splits,128] scratch, part_ml: fp32 [B,H,splits,2] scratch.
+// Single-token decode attention: q [B,H,D], k/v cache [B,Hkv,S_max,D], lens[b] valid positions; out [B,H,D]; D = 128 or 64.
+// part_acc: fp32 [B,H,splits,D] scratch, part_ml: fp32 [B,H,splits,2] scratch.
 int decode_attention_splits(int b, int h, int smax);
 int decode_attention(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* out, float* part_acc, float* part_ml, int b,
                      int h, int hkv, int smax, int d, int splits, float scale, int dtype, cudaStream_t s, const int* block_tables = nullptr,
                      int max_blocks = 0, int block_size = 0);   // block_tables: paged caches [num_blocks, Hkv, block_size, D]
-// The same over paged 8-bit caches (kv_dtype kI8 / kE4M3, q fp16 / bf16): k_dq / v_dq fp32 [Hkv] dequant scales on the device.
+// The same over paged 8-bit caches (kv_dtype kI8 / kE4M3, q fp16 / bf16, D = 128): k_dq / v_dq fp32 [Hkv] dequant scales on the device.
 int decode_attention_paged_q8(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* out, float* part_acc, float* part_ml,
                               int b, int h, int hkv, int d, int splits, float scale, int dtype, int kv_dtype, const float* k_dq, const float* v_dq,
                               const int* block_tables, int max_blocks, int block_size, cudaStream_t s);
 // Multi-token paged decode (verify rows of speculative decoding): sequence i brings n_q[i] new tokens at packed rows cu_q[i] ... over
-// past[i] cached positions (the new K / V already written); key j is visible to new token r iff j <= past[i] + r.  q: [t, h, 128] rows
-// (strides q_st, q_sh); out [t, h * 128] (row stride o_st), written only at the new tokens' rows; sequences with n_q = 0 are skipped.
-// n_q * (h / hkv) must not exceed 64: a sequence beyond that gets NaN rows.  Caches [num_blocks, hkv, block_size, 128] of q's dtype, or
-// int8 / fp8 e4m3 (kv_dtype kI8 / kE4M3) with fp32 [hkv] dequant scales.  part_acc: fp32 [b, hkv, splits, 64, 128] and part_ml: fp32
-// [b, hkv, splits, 64, 2] scratch.  No host read of the lengths.
+// past[i] cached positions (the new K / V already written); key j is visible to new token r iff j <= past[i] + r.  q: [t, h, d] rows
+// (strides q_st, q_sh); out [t, h * d] (row stride o_st), written only at the new tokens' rows; sequences with n_q = 0 are skipped.
+// n_q * (h / hkv) must not exceed 64: a sequence beyond that gets NaN rows.  Caches [num_blocks, hkv, block_size, d] of q's dtype, or
+// (d = 128 only) int8 / fp8 e4m3 (kv_dtype kI8 / kE4M3) with fp32 [hkv] dequant scales; d = 128 or 64.  part_acc: fp32
+// [b, hkv, splits, 64, d] and part_ml: fp32 [b, hkv, splits, 64, 2] scratch.  No host read of the lengths.
 struct PagedMultiArgs {
   const void* q; const void* k_cache; const void* v_cache; void* out;
   float* part_acc; float* part_ml;
@@ -339,7 +339,7 @@ int attention_fwd(const AttnArgs& a, cudaStream_t s);
 // Causal prefill over a paged KV cache: the queries are the n_q[i] new tokens of sequence i at packed rows cu_q[i] ..., its keys are the
 // past[i] + n_q[i] cached positions (the new K / V already written), read through block_tables [b, max_blocks]; key j is visible to new
 // row r iff j <= past[i] + r.  q: [t, H, D] rows (strides token, head); caches [num_blocks, Hk, block_size, D] contiguous, block_size
-// in {16, 32, 64, 128, 256}; o: [t, H, D] rows (strides token, head), written only at the new tokens' rows.  lse: fp32 [H, t] or
+// in {16, 32, 64, 128, 256}, D = 128 (D = 64 on 16-bit caches); o: [t, H, D] rows (strides token, head), written only at the new tokens' rows.  lse: fp32 [H, t] or
 // nullptr.  Sequences with n_q = 0 are skipped.  scratch: int32 [attention_paged_prefill_scratch_ints(t, b)], 8-byte aligned.
 // No host read of the lengths: the work list is built on the device.
 struct PagedAttnArgs {

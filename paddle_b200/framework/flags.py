@@ -11,7 +11,7 @@ _FLAGS = {
     "FLAGS_b200_p2p_collectives": True,    # fused compute+collective kernels over peer memory
     "FLAGS_b200_gemm_backend": "tcgen05",  # "tcgen05" | "cublas"
     "FLAGS_b200_nvls": False,              # all-reduce through NVSwitch multicast (parallel/nvls.py, multimem.ld_reduce / st); not yet run on hardware
-    "FLAGS_b200_decode_kernel": False,     # models.generation: decode steps attend through csrc/decode_attention.cu (CUDA, head_dim 128, fp16 / bf16)
+    "FLAGS_b200_decode_kernel": False,     # models.generation: decode steps attend through csrc/decode_attention.cu (CUDA, head_dim 128 or 64, fp16 / bf16)
     "FLAGS_use_cinn": False,               # pir.optimize: fuse elementwise / reduction chains into generated sm_90a kernels (paddle_b200.cinn)
     "FLAGS_enable_pir_api": False,         # static Executor: run programs through the native IR pass pipeline (paddle_b200.pir) before replay
     "FLAGS_b200_fp8_block_scaled": False,  # with FLAGS_b200_fp8_linear: OCP MX scaling (one E8M0 scale per 32 k, applied per k-block in the fp8 GEMM) instead of per-tensor

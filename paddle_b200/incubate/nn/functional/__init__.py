@@ -278,7 +278,7 @@ def masked_multihead_attention(x, cache_kv=None, bias=None, src_mask=None, cum_o
     bi = torch.arange(b, device=xr.device)
     ck[0, bi, :, lens] = k.to(ck.dtype)
     ck[1, bi, :, lens] = v.to(ck.dtype)
-    if src_mask is None and xr.is_cuda and hd == 128 and ck.dtype in (torch.bfloat16, torch.float16) and ck.is_contiguous():
+    if src_mask is None and xr.is_cuda and hd in (64, 128) and ck.dtype in (torch.bfloat16, torch.float16) and ck.is_contiguous():
         # HBM-bound split-KV decode kernel (csrc/decode_attention.cu): each cached row is read once with 16-byte loads
         from ...._build import ext
 

@@ -1,6 +1,9 @@
 """Paged (block) KV-cache attention for serving. Parity: paddle/phi/kernels/fusion/gpu/block_multi_head_attention_kernel.cu
 (python/paddle/incubate/nn/functional/block_multihead_attention.py).
 
+CUDA kernels serve head_dim 128 and, over fp16 / bf16 caches, head_dim 64 (the 1B-class models used as speculative drafts); see
+block_attention for what stays on the reference path.
+
 Quantized caches: int8 or float8_e4m3fn caches with static per-KV-head scales (fp32 [H_kv], one quant / dequant pair each for K and V).
 A new row is stored as y = (quant_max_bound * quant_scale[h]) * x in fp32; int8 rounds it (quant_round_type 0: half to even, 1: half
 away from zero) and then clamps it to [quant_min_bound, quant_max_bound]; fp8 clamps it and then rounds to nearest even.  A cached value
@@ -264,12 +267,14 @@ def _shared_prefix_groups(shared_prefix, nseq, block_size):
     return cu, seqs, plen
 
 
-def _paged_kernels_ok(qkv, kc, d, block_size, quant=None, pro=None):
+def _paged_kernels_ok(qkv, kc, d, block_size, quant=None, pro=None, shared_prefix=None):
     from ...framework.flags import flag
 
     dtype = qkv.dtype if pro is None else pro.dtype                      # the compute type: int32 qkv is dequantized to it
     cache_ok = kc.dtype == dtype or (quant is not None and kc.dtype in _KV8_DTYPES)
-    return (qkv.is_cuda and kc.is_cuda and d == 128 and dtype in (torch.float16, torch.bfloat16) and cache_ok
+    # head_dim 64 has the decode, verify and prefill kernels over 16-bit caches only: no 8-bit caches, qkv prologue or shared prefix
+    head_ok = d == 128 or (d == 64 and kc.dtype == dtype and pro is None and shared_prefix is None)
+    return (qkv.is_cuda and kc.is_cuda and head_ok and dtype in (torch.float16, torch.bfloat16) and cache_ok
             and int(block_size) in _PREFILL_BLOCK_SIZES and flag("FLAGS_use_fused_kernels", True))
 
 
@@ -289,7 +294,7 @@ def block_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_deco
     ones (a continuing chunk); it decodes when it brings exactly one token and seq_lens_encoder == 0.  A continuing chunk of 2 ..
     VERIFY_MAX tokens with now * (H / H_kv) <= 64 - the verify rows of speculative decoding - is a short chunk.
 
-    CUDA path (head_dim 128, fp16 / bf16, block_size 16 / 32 / 64 / 128 / 256): the new K / V rows of EVERY sequence are scattered into the
+    CUDA path (head_dim 128 or 64, fp16 / bf16, block_size 16 / 32 / 64 / 128 / 256): the new K / V rows of EVERY sequence are scattered into the
     paged caches with one indexed write (block and row computed on the device from the block table - no per-token Python loop); decode
     sequences attend to their cache through `decode_attention_paged` (csrc/decode_attention.cu: one table lookup per cached row, split-K
     over the positions); all prefill sequences run in ONE launch of `attention_fwd_paged` (csrc/attention_sm100.cu): causal wgmma flash
@@ -297,7 +302,8 @@ def block_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_deco
     output written in place at the tokens' rows; all short chunks run in ONE launch of `decode_attention_paged_multi`
     (csrc/decode_attention.cu: split-K over the cached positions, every query row of a KV head in one tensor-core tile, q and the output in
     place as for prefill).  The three row kinds are told apart with one host read.  Other block sizes and devices take
-    `_block_attention_ref`.
+    `_block_attention_ref`; so does head_dim 64 with an 8-bit cache, the qkv prologue / out_scale or shared_prefix (those kernels are
+    head_dim 128 only).
 
     int8 / float8_e4m3fn caches (static scales, see the module docstring): the new rows are quantized into the caches by one launch of
     `paged_kv_cache_write` (csrc/kv_cache_quant.cu), and the attention kernels read the 8-bit rows and dequantize them on the fly.
@@ -329,7 +335,7 @@ def block_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_deco
     nh = qkv.shape[1] // d - 2 * nkv
     pro = qkv_prologue_params(qkv, nh, nkv, d, qkv_out_scale, qkv_bias, rope_emb, use_neox_style, out_shift, out_smooth, out_scale, compute_dtype,
                               quant_round_type, quant_max_bound, quant_min_bound)
-    if not _paged_kernels_ok(qkv, kc, d, block_size, quant, pro):
+    if not _paged_kernels_ok(qkv, kc, d, block_size, quant, pro, shared_prefix):
         return _block_attention_ref(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_decoder, seq_lens_this_time, cu_seqlens_q, block_tables,
                                     block_size, quant=quant, shared_prefix=shared_prefix, prologue=pro)
     from ..._build import ext

@@ -9,7 +9,7 @@ The cache layout is the decode kernel's: `k`, `v` of every layer are [B, H_kv, S
 (csrc/decode_attention.cu).  Prefill runs the model's own sublayers (fused RMSNorm / packed rotary / flash attention on CUDA) and writes
 the rotated keys and the values into the cache; a decode step projects ONE token, rotates it at position `lens[b]`, appends it and attends
 to the cache - through `decode_attention` (split-K over the cached positions) when `FLAGS_b200_decode_kernel` is set and the shapes qualify
-(CUDA, head_dim 128, fp16 / bf16), otherwise through a masked softmax over the cache (any device / dtype; the default until the kernel
+(CUDA, head_dim 128 or 64, fp16 / bf16), otherwise through a masked softmax over the cache (any device / dtype; the default until the kernel
 path has been exercised end to end on hardware)."""
 from __future__ import annotations
 
@@ -58,7 +58,7 @@ def _attend_cache(q, kc, vc, lens, scale):
     """q [B, H, D] against the cache [B, H_kv, S_max, D] with `lens` valid positions (the new token already appended)."""
     from ..framework.flags import flag
 
-    if flag("FLAGS_b200_decode_kernel", False) and q.is_cuda and q.shape[-1] == 128 and q.dtype in (torch.float16, torch.bfloat16):
+    if flag("FLAGS_b200_decode_kernel", False) and q.is_cuda and q.shape[-1] in (64, 128) and q.dtype in (torch.float16, torch.bfloat16):
         from .._build import ext
 
         return ext().decode_attention(q.contiguous(), kc, vc, lens.to(torch.int32).contiguous(), float(scale))

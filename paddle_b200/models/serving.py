@@ -7,7 +7,7 @@ preempted (its blocks go back to the pool; it is re-prefilled later from prompt 
 
 Every step packs the tokens of all scheduled sequences into ONE [tokens, hidden] batch: whole prompts for the sequences being prefilled,
 one token for the sequences being decoded.  The decoder layers run on the packed batch with the model's own sublayers; attention is
-`incubate.nn.paged_attention.block_attention` - on CUDA (head_dim 128, fp16 / bf16) one indexed scatter of the new K / V rows into the
+`incubate.nn.paged_attention.block_attention` - on CUDA (head_dim 128 or 64, fp16 / bf16) one indexed scatter of the new K / V rows into the
 block pool, `decode_attention_paged` for the decode rows and one paged wgmma prefill attention (`attention_fwd_paged`) for the prefill rows.
 
 Chunked prefill (`max_prefill_chunk=N`): an admitted prompt still gets the blocks for its whole length, but is fed over successive steps,
@@ -376,8 +376,9 @@ class LLMEngine:
     def _shared_prefix_groups(self, seqs, n_new):
         """block_attention's shared_prefix argument for the plain decode rows among seqs (the first len(decode) of them, one new token and
         no speculation): rows are grouped by their first block id, a group's prefix is the longest run of leading block ids common to all
-        its members, and only groups that paged_attention.shared_prefix_pays() accepts are passed.  None when there are none."""
-        if not self.enable_prefix_caching:
+        its members, and only groups that paged_attention.shared_prefix_pays() accepts are passed.  None when there are none, and at
+        head_dim 64, which has a decode kernel but no shared-prefix one: grouped rows would take block_attention's reference path."""
+        if not self.enable_prefix_caching or self.hd == 64:
             return None
         by_first = {}
         for i, (s, n) in enumerate(zip(seqs, n_new)):
