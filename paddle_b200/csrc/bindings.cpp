@@ -930,19 +930,20 @@ Tensor gemm_fp8_mx(const Tensor& a, const Tensor& sfa, const Tensor& b, const Te
   return d;
 }
 
-// q [B,H,D], k_cache / v_cache [B,Hkv,S_max,D] contiguous, lens int32 [B] -> out [B,H,D]
-Tensor decode_attention(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& lens, double scale) {
+// q [B,H,D], k_cache / v_cache [B,Hkv,S_max,D] contiguous, lens int32 [B] -> out [B,H,D]; window > 0: the last `window` positions only
+Tensor decode_attention(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& lens, double scale, int64_t window) {
   TORCH_CHECK(q.is_cuda() && q.dim() == 3 && k_cache.dim() == 4 && v_cache.dim() == 4 && q.is_contiguous() && k_cache.is_contiguous() && v_cache.is_contiguous(),
               "decode_attention: q [B,H,D], caches [B,Hkv,S,D] contiguous");
   TORCH_CHECK(lens.scalar_type() == at::kInt && lens.is_contiguous() && lens.numel() == q.size(0), "decode_attention: lens must be int32 [B]");
   c10::cuda::CUDAGuard guard(q.device());
   const int b = (int)q.size(0), h = (int)q.size(1), d = (int)q.size(2), hkv = (int)k_cache.size(1), smax = (int)k_cache.size(2);
-  const int splits = b200::decode_attention_splits(b, h, smax);
+  const int w = window > 0 ? (int)std::min<int64_t>(window, smax) : 0;
+  const int splits = b200::decode_attention_splits(b, h, w > 0 ? w : smax);
   Tensor out = torch::empty_like(q);
   Tensor pacc = torch::empty({b, h, splits, d}, q.options().dtype(at::kFloat));
   Tensor pml = torch::empty({b, h, splits, 2}, q.options().dtype(at::kFloat));
   int rc = b200::decode_attention(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), lens.data_ptr<int>(), out.data_ptr(), pacc.data_ptr<float>(),
-                                  pml.data_ptr<float>(), b, h, hkv, smax, d, splits, (float)scale, dt_code(q), cur_stream());
+                                  pml.data_ptr<float>(), b, h, hkv, smax, d, splits, (float)scale, dt_code(q), cur_stream(), nullptr, 0, 0, w);
   g_launches += 2;
   check_err();
   TORCH_CHECK(rc == 0, "paddle_b200.decode_attention: unsupported shape (head_dim 128 or 64, fp16/bf16 only) rc=", rc);
@@ -968,9 +969,9 @@ int kv8_code(const char* op, const Tensor& q, const Tensor& k_cache, const Tenso
 }
 
 // paged KV cache: q [B,H,D], caches [num_blocks,Hkv,block_size,D], lens int32 [B] (positions valid per sequence), block_tables int32 [B,max_blocks];
-// int8 / fp8 e4m3 caches take fp32 [Hkv] k_dequant_scales / v_dequant_scales
+// int8 / fp8 e4m3 caches take fp32 [Hkv] k_dequant_scales / v_dequant_scales; window > 0: the last `window` positions only
 Tensor decode_attention_paged(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& lens, const Tensor& block_tables, double scale,
-                              const OptT& k_dequant_scales, const OptT& v_dequant_scales) {
+                              const OptT& k_dequant_scales, const OptT& v_dequant_scales, int64_t window) {
   TORCH_CHECK(q.is_cuda() && q.dim() == 3 && k_cache.dim() == 4 && v_cache.dim() == 4 && q.is_contiguous() && k_cache.is_contiguous() && v_cache.is_contiguous(),
               "decode_attention_paged: q [B,H,D], caches [num_blocks,Hkv,block_size,D] contiguous");
   TORCH_CHECK(lens.scalar_type() == at::kInt && lens.is_contiguous() && lens.numel() == q.size(0), "decode_attention_paged: lens must be int32 [B]");
@@ -978,7 +979,8 @@ Tensor decode_attention_paged(const Tensor& q, const Tensor& k_cache, const Tens
               "decode_attention_paged: block_tables must be int32 [B, max_blocks] on the device");
   c10::cuda::CUDAGuard guard(q.device());
   const int b = (int)q.size(0), h = (int)q.size(1), d = (int)q.size(2), hkv = (int)k_cache.size(1), bs = (int)k_cache.size(2), mb = (int)block_tables.size(1);
-  const int splits = b200::decode_attention_splits(b, h, mb * bs);
+  const int w = window > 0 ? (int)std::min<int64_t>(window, (int64_t)mb * bs) : 0;
+  const int splits = b200::decode_attention_splits(b, h, w > 0 ? w : mb * bs);
   Tensor out = torch::empty_like(q);
   Tensor pacc = torch::empty({b, h, splits, d}, q.options().dtype(at::kFloat));
   Tensor pml = torch::empty({b, h, splits, 2}, q.options().dtype(at::kFloat));
@@ -989,14 +991,14 @@ Tensor decode_attention_paged(const Tensor& q, const Tensor& k_cache, const Tens
     int rc = b200::decode_attention_paged_q8(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), lens.data_ptr<int>(), out.data_ptr(),
                                              pacc.data_ptr<float>(), pml.data_ptr<float>(), b, h, hkv, d, splits, (float)scale, dt_code(q), kv,
                                              k_dequant_scales->data_ptr<float>(), v_dequant_scales->data_ptr<float>(), block_tables.data_ptr<int>(),
-                                             mb, bs, cur_stream());
+                                             mb, bs, cur_stream(), w);
     g_launches += 2;
     check_err();
     TORCH_CHECK(rc == 0, "paddle_b200.decode_attention_paged: unsupported shape (head_dim 128, H % Hkv == 0) rc=", rc);
     return out;
   }
   int rc = b200::decode_attention(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), lens.data_ptr<int>(), out.data_ptr(), pacc.data_ptr<float>(),
-                                  pml.data_ptr<float>(), b, h, hkv, mb * bs, d, splits, (float)scale, dt_code(q), cur_stream(), block_tables.data_ptr<int>(), mb, bs);
+                                  pml.data_ptr<float>(), b, h, hkv, mb * bs, d, splits, (float)scale, dt_code(q), cur_stream(), block_tables.data_ptr<int>(), mb, bs, w);
   g_launches += 2;
   check_err();
   TORCH_CHECK(rc == 0, "paddle_b200.decode_attention_paged: unsupported shape (head_dim 128 or 64, fp16/bf16 only) rc=", rc);
@@ -1056,10 +1058,11 @@ std::vector<Tensor> attention_fwd(const Tensor& q, const Tensor& k, const Tensor
 // Causal prefill over the paged KV cache (new K / V already written to the caches): q [T,H,D] view of the packed qkv rows, caches
 // [num_blocks,Hkv,block_size,D], block_tables int32 [B,max_blocks], cu_q / n_q / past int32 [B] (n_q = 0: sequence skipped); writes
 // out [T,H*D] at the new tokens' rows only, and lse fp32 [H,T] at the same rows when given.  No host read of the lengths.
-// int8 / fp8 e4m3 caches take fp32 [Hkv] k_dequant_scales / v_dequant_scales.
+// int8 / fp8 e4m3 caches take fp32 [Hkv] k_dequant_scales / v_dequant_scales.  window > 0: sliding window, new row r sees keys
+// (past + r - window, past + r].
 void attention_fwd_paged(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& block_tables, const Tensor& cu_q,
                          const Tensor& n_q, const Tensor& past, double scale, const Tensor& out, const OptT& lse, const OptT& k_dequant_scales,
-                         const OptT& v_dequant_scales) {
+                         const OptT& v_dequant_scales, int64_t window) {
   TORCH_CHECK(q.is_cuda() && q.dim() == 3 && q.stride(2) == 1, "attention_fwd_paged: q must be a CUDA [T,H,D] view with unit head_dim stride");
   TORCH_CHECK(k_cache.dim() == 4 && v_cache.dim() == 4 && k_cache.is_contiguous() && v_cache.is_contiguous() && k_cache.sizes() == v_cache.sizes(),
               "attention_fwd_paged: caches must be contiguous [num_blocks,Hkv,block_size,D] of one shape");
@@ -1085,6 +1088,7 @@ void attention_fwd_paged(const Tensor& q, const Tensor& k_cache, const Tensor& v
   a.o_strides[0] = out.stride(0); a.o_strides[1] = a.d;
   a.block_tables = block_tables.data_ptr<int>(); a.cu_q = cu_q.data_ptr<int>(); a.n_q = n_q.data_ptr<int>(); a.past = past.data_ptr<int>();
   a.scale = (float)scale; a.dtype = dt_code(q);
+  a.window = window > 0 ? (int)std::min<int64_t>(window, INT32_MAX) : 0;
   if (kv != -1) { a.kv_dtype = kv; a.k_dq = k_dequant_scales->data_ptr<float>(); a.v_dq = v_dequant_scales->data_ptr<float>(); }
   if (lse.has_value() && lse->defined()) {
     TORCH_CHECK(lse->device() == q.device() && lse->scalar_type() == at::kFloat && lse->is_contiguous() && lse->dim() == 2 && lse->size(0) == a.h &&
@@ -1105,10 +1109,11 @@ void attention_fwd_paged(const Tensor& q, const Tensor& k_cache, const Tensor& v
 // Multi-token decode over the paged KV cache (the verify rows of speculative decoding; new K / V already written): q [T,H,D] view of the
 // packed qkv rows, caches [num_blocks,Hkv,block_size,D], block_tables int32 [B,max_blocks], cu_q / n_q / past int32 [B] (n_q = 0: sequence
 // skipped); writes out [T, H*D] at the new tokens' rows only.  n_q * (H / Hkv) may not exceed 64 (a sequence beyond it gets NaN rows: the
-// lengths are not read on the host).  int8 / fp8 e4m3 caches take fp32 [Hkv] k_dequant_scales / v_dequant_scales.
+// lengths are not read on the host).  int8 / fp8 e4m3 caches take fp32 [Hkv] k_dequant_scales / v_dequant_scales.  window > 0: sliding
+// window, new token r sees keys (past + r - window, past + r].
 void decode_attention_paged_multi(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& block_tables, const Tensor& cu_q,
                                   const Tensor& n_q, const Tensor& past, double scale, const Tensor& out, const OptT& k_dequant_scales,
-                                  const OptT& v_dequant_scales) {
+                                  const OptT& v_dequant_scales, int64_t window) {
   TORCH_CHECK(q.is_cuda() && q.dim() == 3 && q.stride(2) == 1, "decode_attention_paged_multi: q must be a CUDA [T,H,D] view with unit head_dim stride");
   TORCH_CHECK(q.scalar_type() == at::kHalf || q.scalar_type() == at::kBFloat16, "decode_attention_paged_multi: q must be fp16 or bf16");
   TORCH_CHECK(k_cache.dim() == 4 && v_cache.dim() == 4 && k_cache.is_contiguous() && v_cache.is_contiguous() && k_cache.sizes() == v_cache.sizes(),
@@ -1137,7 +1142,8 @@ void decode_attention_paged_multi(const Tensor& q, const Tensor& k_cache, const 
   a.q_st = q.stride(0); a.q_sh = q.stride(1); a.o_st = out.stride(0);
   a.b = (int)b; a.h = (int)q.size(1); a.hkv = (int)hkv; a.d = (int)q.size(2);
   a.max_blocks = (int)block_tables.size(1); a.block_size = (int)k_cache.size(2);
-  a.splits = b200::decode_attention_splits(a.b, a.hkv, a.max_blocks * a.block_size);
+  a.window = window > 0 ? (int)std::min<int64_t>(window, (int64_t)a.max_blocks * a.block_size) : 0;
+  a.splits = b200::decode_attention_splits(a.b, a.hkv, a.window > 0 ? a.window : a.max_blocks * a.block_size);
   a.scale = (float)scale; a.dtype = dt_code(q);
   if (kv != -1) { a.kv_dtype = kv; a.k_dq = k_dequant_scales->data_ptr<float>(); a.v_dq = v_dequant_scales->data_ptr<float>(); }
   c10::cuda::CUDAGuard guard(q.device());
@@ -1582,10 +1588,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("quantize_fp8", traced("quantize_fp8", &quantize_fp8), pybind11::arg("x"), pybind11::arg("e5m2") = false, pybind11::arg("want_transpose") = false);
   m.def("set_deterministic", [](bool on) { g_deterministic = on; });
   m.def("deterministic", []() { return g_deterministic; });
-  m.def("decode_attention", traced("decode_attention", &decode_attention));
+  m.def("decode_attention", traced("decode_attention", &decode_attention), pybind11::arg("q"), pybind11::arg("k_cache"), pybind11::arg("v_cache"),
+        pybind11::arg("lens"), pybind11::arg("scale"), pybind11::arg("window") = 0);
   m.def("decode_attention_paged", traced("decode_attention_paged", &decode_attention_paged), pybind11::arg("q"), pybind11::arg("k_cache"),
         pybind11::arg("v_cache"), pybind11::arg("lens"), pybind11::arg("block_tables"), pybind11::arg("scale"),
-        pybind11::arg("k_dequant_scales") = pybind11::none(), pybind11::arg("v_dequant_scales") = pybind11::none());
+        pybind11::arg("k_dequant_scales") = pybind11::none(), pybind11::arg("v_dequant_scales") = pybind11::none(), pybind11::arg("window") = 0);
   m.def("paged_kv_cache_write", traced("paged_kv_cache_write", &paged_kv_cache_write), pybind11::arg("qkv"), pybind11::arg("k_cache"),
         pybind11::arg("v_cache"), pybind11::arg("cu_q"), pybind11::arg("seq_lens_encoder"), pybind11::arg("seq_lens_decoder"),
         pybind11::arg("block_tables"), pybind11::arg("k_quant_scales"), pybind11::arg("v_quant_scales"), pybind11::arg("round_type") = 1,
@@ -1601,11 +1608,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("attention_fwd_paged", traced("attention_fwd_paged", &attention_fwd_paged), pybind11::arg("q"), pybind11::arg("k_cache"),
         pybind11::arg("v_cache"), pybind11::arg("block_tables"), pybind11::arg("cu_q"), pybind11::arg("n_q"), pybind11::arg("past"), pybind11::arg("scale"),
         pybind11::arg("out"), pybind11::arg("lse") = pybind11::none(), pybind11::arg("k_dequant_scales") = pybind11::none(),
-        pybind11::arg("v_dequant_scales") = pybind11::none());
+        pybind11::arg("v_dequant_scales") = pybind11::none(), pybind11::arg("window") = 0);
   m.def("decode_attention_paged_multi", traced("decode_attention_paged_multi", &decode_attention_paged_multi), pybind11::arg("q"),
         pybind11::arg("k_cache"), pybind11::arg("v_cache"), pybind11::arg("block_tables"), pybind11::arg("cu_q"), pybind11::arg("n_q"),
         pybind11::arg("past"), pybind11::arg("scale"), pybind11::arg("out"), pybind11::arg("k_dequant_scales") = pybind11::none(),
-        pybind11::arg("v_dequant_scales") = pybind11::none());
+        pybind11::arg("v_dequant_scales") = pybind11::none(), pybind11::arg("window") = 0);
   m.def("decode_attention_paged_shared", traced("decode_attention_paged_shared", &decode_attention_paged_shared), pybind11::arg("q"),
         pybind11::arg("k_cache"), pybind11::arg("v_cache"), pybind11::arg("block_tables"), pybind11::arg("cu_q"), pybind11::arg("lens"),
         pybind11::arg("cu_groups"), pybind11::arg("group_seqs"), pybind11::arg("prefix_len"), pybind11::arg("scale"), pybind11::arg("out"),

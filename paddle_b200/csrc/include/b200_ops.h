@@ -226,17 +226,19 @@ int weight_dequantize(const void* w, const float* scale, void* out, int n, int k
 int decode_attention_splits(int b, int h, int smax);
 int decode_attention(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* out, float* part_acc, float* part_ml, int b,
                      int h, int hkv, int smax, int d, int splits, float scale, int dtype, cudaStream_t s, const int* block_tables = nullptr,
-                     int max_blocks = 0, int block_size = 0);   // block_tables: paged caches [num_blocks, Hkv, block_size, D]
+                     int max_blocks = 0, int block_size = 0,    // block_tables: paged caches [num_blocks, Hkv, block_size, D]
+                     int window = 0);                           // > 0: sliding window, the last `window` positions only
 // The same over paged 8-bit caches (kv_dtype kI8 / kE4M3, q fp16 / bf16, D = 128): k_dq / v_dq fp32 [Hkv] dequant scales on the device.
 int decode_attention_paged_q8(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* out, float* part_acc, float* part_ml,
                               int b, int h, int hkv, int d, int splits, float scale, int dtype, int kv_dtype, const float* k_dq, const float* v_dq,
-                              const int* block_tables, int max_blocks, int block_size, cudaStream_t s);
+                              const int* block_tables, int max_blocks, int block_size, cudaStream_t s, int window = 0);
 // Multi-token paged decode (verify rows of speculative decoding): sequence i brings n_q[i] new tokens at packed rows cu_q[i] ... over
 // past[i] cached positions (the new K / V already written); key j is visible to new token r iff j <= past[i] + r.  q: [t, h, d] rows
 // (strides q_st, q_sh); out [t, h * d] (row stride o_st), written only at the new tokens' rows; sequences with n_q = 0 are skipped.
 // n_q * (h / hkv) must not exceed 64: a sequence beyond that gets NaN rows.  Caches [num_blocks, hkv, block_size, d] of q's dtype, or
 // (d = 128 only) int8 / fp8 e4m3 (kv_dtype kI8 / kE4M3) with fp32 [hkv] dequant scales; d = 128 or 64.  part_acc: fp32
 // [b, hkv, splits, 64, d] and part_ml: fp32 [b, hkv, splits, 64, 2] scratch.  No host read of the lengths.
+// window > 0: sliding window, key j is visible to new token r iff past[i] + r - window < j <= past[i] + r.
 struct PagedMultiArgs {
   const void* q; const void* k_cache; const void* v_cache; void* out;
   float* part_acc; float* part_ml;
@@ -248,6 +250,7 @@ struct PagedMultiArgs {
   int kv_dtype = -1;
   const float* k_dq = nullptr;
   const float* v_dq = nullptr;
+  int window = 0;
 };
 int decode_attention_paged_multi(const PagedMultiArgs& a, cudaStream_t s);
 // Shared-prefix decode over the paged KV cache: single-token decode rows (query row cu_q[b], lens[b] keys including the new one) of
@@ -341,7 +344,8 @@ int attention_fwd(const AttnArgs& a, cudaStream_t s);
 // row r iff j <= past[i] + r.  q: [t, H, D] rows (strides token, head); caches [num_blocks, Hk, block_size, D] contiguous, block_size
 // in {16, 32, 64, 128, 256}, D = 128 (D = 64 on 16-bit caches); o: [t, H, D] rows (strides token, head), written only at the new tokens' rows.  lse: fp32 [H, t] or
 // nullptr.  Sequences with n_q = 0 are skipped.  scratch: int32 [attention_paged_prefill_scratch_ints(t, b)], 8-byte aligned.
-// No host read of the lengths: the work list is built on the device.
+// No host read of the lengths: the work list is built on the device.  window > 0: sliding window, key j is visible to new row r iff
+// past[i] + r - window < j <= past[i] + r.
 struct PagedAttnArgs {
   const void* q; const void* k_cache; const void* v_cache; void* o; float* lse;
   int t, h, hk, d, b, num_blocks, block_size, max_blocks;
@@ -354,6 +358,7 @@ struct PagedAttnArgs {
   int kv_dtype = -1;
   const float* k_dq = nullptr;
   const float* v_dq = nullptr;
+  int window = 0;
 };
 int attention_paged_prefill_slots(int t, int b);
 int attention_paged_prefill_scratch_ints(int t, int b);

@@ -287,7 +287,7 @@ def block_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_deco
                     cache_k_quant_scales=None, cache_v_quant_scales=None, cache_k_dequant_scales=None, cache_v_dequant_scales=None,
                     use_dynamic_cachekv_quant=False, quant_round_type=1, quant_max_bound=127.0, quant_min_bound=-127.0, shared_prefix=None, *,
                     qkv_out_scale=None, qkv_bias=None, rope_emb=None, use_neox_style=False, out_shift=None, out_smooth=None, out_scale=-1,
-                    compute_dtype="default"):
+                    compute_dtype="default", sliding_window=None):
     """qkv: [total_tokens, (H + 2*H_kv) * D] packed over the batch; caches [num_blocks, H_kv, block_size, D].
 
     A sequence prefills when seq_lens_encoder > 0 (a fresh prompt) or when it brings more than one token on top of seq_lens_decoder cached
@@ -327,7 +327,12 @@ def block_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_deco
 
     out_scale > 0: the output is quantized to int8 (quant_max_bound 127) or float8_e4m3fn (448) by one launch of `attention_out_quant`
     after the attention: y = max_bound * out_scale * o, rounded and clamped as the cache is (quant_round_type, bounds); out_shift /
-    out_smooth (T [H * D], int8 output only) first replace o by ((o + shift) -> T) * smooth -> T."""
+    out_smooth (T [H * D], int8 output only) first replace o by ((o + shift) -> T) * smooth -> T.
+
+    sliding_window = W (an int >= 1; None: off): local attention, the query at absolute position i sees key j iff i - W < j <= i.  Decode,
+    verify and prefill rows go to the windowed kernels of csrc/attention_window.cu, which read only the window's cache rows and never read
+    the table entries of blocks wholly below it (those blocks may have been released and reused).  Not combinable with shared_prefix."""
+    sliding_window = _check_window(sliding_window, shared_prefix)
     qkv, kc, vc = _raw(qkv), _raw(key_cache), _raw(value_cache)
     nkv, d = kc.shape[1], kc.shape[3]
     quant = kv_quant_params(kc, vc, cache_k_quant_scales, cache_v_quant_scales, cache_k_dequant_scales, cache_v_dequant_scales,
@@ -337,7 +342,7 @@ def block_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_deco
                               quant_round_type, quant_max_bound, quant_min_bound)
     if not _paged_kernels_ok(qkv, kc, d, block_size, quant, pro, shared_prefix):
         return _block_attention_ref(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_decoder, seq_lens_this_time, cu_seqlens_q, block_tables,
-                                    block_size, quant=quant, shared_prefix=shared_prefix, prologue=pro)
+                                    block_size, quant=quant, shared_prefix=shared_prefix, prologue=pro, sliding_window=sliding_window)
     from ..._build import ext
 
     dev = qkv.device
@@ -351,6 +356,8 @@ def block_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_deco
     past = torch.where(enc > 0, torch.zeros_like(dec), dec)                  # prefill starts at position 0, decode continues after the cache
     i32 = lambda t: t.to(torch.int32).contiguous()                          # noqa: E731
     dq = {} if quant is None else {"k_dequant_scales": quant.k_dequant, "v_dequant_scales": quant.v_dequant}
+    if sliding_window is not None:
+        dq["window"] = sliding_window
     if pro is not None:
         # ---- the row kinds and the last new position in one host read, then the prologue and the cache write in one launch
         kinds = _row_kinds(enc, now, nh, nkv, block_size, shared_prefix, torch.where(now > 0, past + now - 1, -1).max())
@@ -410,6 +417,17 @@ def block_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_deco
     return out.as_subclass(Tensor), qkv.as_subclass(Tensor), kc.as_subclass(Tensor), vc.as_subclass(Tensor)
 
 
+def _check_window(sliding_window, shared_prefix):
+    """sliding_window as an int >= 1, or None."""
+    if sliding_window is None:
+        return None
+    if isinstance(sliding_window, bool) or not isinstance(sliding_window, int) or sliding_window < 1:
+        raise ValueError(f"block_attention: sliding_window must be an int >= 1 or None, got {sliding_window!r}")
+    if shared_prefix is not None:
+        raise ValueError("block_attention: sliding_window cannot be combined with shared_prefix")
+    return int(sliding_window)
+
+
 def _row_kinds(enc, now, nh, nkv, block_size, shared_prefix, extra=None):
     """Splits block_attention's rows into decode / verify / prefill rows with ONE host read: (is_dec, is_ver, is_pre, shared-prefix groups or
     None, any_dec, any_ver, any_pre[, int(extra)]).  Grouped rows leave is_dec; a grouped row that is not a decode row raises ValueError."""
@@ -437,12 +455,14 @@ def _row_kinds(enc, now, nh, nkv, block_size, shared_prefix, extra=None):
 def _block_attention_ref(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_decoder, seq_lens_this_time, cu_seqlens_q, block_tables, block_size,
                          cache_k_quant_scales=None, cache_v_quant_scales=None, cache_k_dequant_scales=None, cache_v_dequant_scales=None,
                          use_dynamic_cachekv_quant=False, quant_round_type=1, quant_max_bound=127.0, quant_min_bound=-127.0, quant=None,
-                         shared_prefix=None, prologue=None, **prologue_args):
+                         shared_prefix=None, prologue=None, sliding_window=None, **prologue_args):
     """qkv: [total_tokens, (H + 2*H_kv) * D] packed over the batch; caches [num_blocks, H_kv, block_size, D].  `quant`: an already
     validated KVQuant (otherwise it is built from the scale / round / bound arguments).  `shared_prefix`: as in block_attention; its whole
     contract is checked here (ValueError on a violation), and it does not change the math.  `prologue`: an already validated QKVPrologue
     (otherwise it is built from block_attention's keyword arguments qkv_out_scale, qkv_bias, rope_emb, use_neox_style, out_shift,
-    out_smooth, out_scale and compute_dtype in `prologue_args`), applied op by op in torch."""
+    out_smooth, out_scale and compute_dtype in `prologue_args`), applied op by op in torch.  `sliding_window`: as in block_attention; only
+    the cache rows of the window are read."""
+    sliding_window = _check_window(sliding_window, shared_prefix)
     qkv, kc, vc = _raw(qkv), _raw(key_cache), _raw(value_cache)
     if quant is None:
         quant = kv_quant_params(kc, vc, cache_k_quant_scales, cache_v_quant_scales, cache_k_dequant_scales, cache_v_dequant_scales,
@@ -488,17 +508,22 @@ def _block_attention_ref(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens
                 vc[blk, :, off] = quantize_kv(v[t], quant.v_quant, quant, vc.dtype)
         total = past + n
         nblk = (total + block_size - 1) // block_size
-        blks = bt[b, :nblk].long()
-        K = kc[blks].permute(1, 0, 2, 3).reshape(nkv, nblk * block_size, d)[:, :total]
-        V = vc[blks].permute(1, 0, 2, 3).reshape(nkv, nblk * block_size, d)[:, :total]
+        first = 0 if sliding_window is None else max(0, past - sliding_window + 1)   # the lowest key any new token sees
+        b0 = first // block_size
+        blks = bt[b, b0:nblk].long()
+        K = kc[blks].permute(1, 0, 2, 3).reshape(nkv, (nblk - b0) * block_size, d)[:, first - b0 * block_size:total - b0 * block_size]
+        V = vc[blks].permute(1, 0, 2, 3).reshape(nkv, (nblk - b0) * block_size, d)[:, first - b0 * block_size:total - b0 * block_size]
         if quant is not None:
             K, V = dequantize_kv(K, quant.k_dequant), dequantize_kv(V, quant.v_dequant)
         rep = nh // nkv
         K, V = K.repeat_interleave(rep, 0), V.repeat_interleave(rep, 0)
         s = torch.einsum("nhd,hsd->hns", q.float(), K.float()) / math.sqrt(d)
         qpos = torch.arange(past, total, device=qkv.device)[None, :, None]
-        kpos = torch.arange(total, device=qkv.device)[None, None, :]
-        s = s.masked_fill(kpos > qpos, float("-inf"))
+        kpos = torch.arange(first, total, device=qkv.device)[None, None, :]
+        hidden = kpos > qpos
+        if sliding_window is not None:
+            hidden = hidden | (kpos <= qpos - sliding_window)
+        s = s.masked_fill(hidden, float("-inf"))
         o = torch.einsum("hns,hsd->nhd", torch.softmax(s, -1), V.float())
         out[cu[b]:cu[b] + n] = o.reshape(n, nh * d).to(out.dtype)
     if pro is not None and pro.out_dtype is not None:

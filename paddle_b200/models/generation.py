@@ -54,14 +54,15 @@ class KVCache:
         self.v[layer][b, :, idx] = v
 
 
-def _attend_cache(q, kc, vc, lens, scale):
-    """q [B, H, D] against the cache [B, H_kv, S_max, D] with `lens` valid positions (the new token already appended)."""
+def _attend_cache(q, kc, vc, lens, scale, window=None):
+    """q [B, H, D] against the cache [B, H_kv, S_max, D] with `lens` valid positions (the new token already appended); `window`: only the
+    last `window` of them (sliding-window attention)."""
     from ..framework.flags import flag
 
     if flag("FLAGS_b200_decode_kernel", False) and q.is_cuda and q.shape[-1] in (64, 128) and q.dtype in (torch.float16, torch.bfloat16):
         from .._build import ext
 
-        return ext().decode_attention(q.contiguous(), kc, vc, lens.to(torch.int32).contiguous(), float(scale))
+        return ext().decode_attention(q.contiguous(), kc, vc, lens.to(torch.int32).contiguous(), float(scale), window or 0)
     b, h, d = q.shape
     hkv = kc.shape[1]
     smax = int(lens.max().item())
@@ -71,7 +72,10 @@ def _attend_cache(q, kc, vc, lens, scale):
         k = k.repeat_interleave(h // hkv, 1)
         v = v.repeat_interleave(h // hkv, 1)
     s = torch.einsum("bhd,bhsd->bhs", q.float(), k) * scale
-    mask = torch.arange(smax, device=q.device)[None, None, :] >= lens.long()[:, None, None]
+    pos = torch.arange(smax, device=q.device)[None, None, :]
+    mask = pos >= lens.long()[:, None, None]
+    if window is not None:
+        mask = mask | (pos < lens.long()[:, None, None] - window)
     s = s.masked_fill(mask, float("-inf"))
     return torch.einsum("bhs,bhsd->bhd", torch.softmax(s, -1), v).to(q.dtype)
 
@@ -172,6 +176,7 @@ class LlamaGenerator:
         self.nh, self.nkv, self.hd = ad.nh, ad.nkv, ad.hd
         self._rope = ad.L.rope_cache
         self._KR = ad.L.KR
+        self.window = getattr(self.cfg, "sliding_window", None)
 
     # -- one decoder layer on [B, S, hidden] with explicit positions; returns (h, k, v) with k, v [B, S, H_kv, D] (k rotated)
     def _layer(self, layer, h, cos, sin, position_ids, attend):
@@ -198,10 +203,13 @@ class LlamaGenerator:
         cos, sin = self._rope(self.cfg, _raw(h).device)
         pos = torch.arange(s, device=ids.device, dtype=torch.int64).unsqueeze(0).expand(b, s).contiguous()
 
+        mask = None if self.window is None else self.ad.L.window_mask(s, s, self.window, ids.device)
+
         def attend(q, k, v):
             rep = self.nh // self.nkv
             kk, vv = (k.repeat_interleave(rep, 2), v.repeat_interleave(rep, 2)) if rep > 1 else (k, v)
-            o = torch.nn.functional.scaled_dot_product_attention(q.transpose(1, 2), kk.transpose(1, 2), vv.transpose(1, 2), is_causal=True, scale=scale)
+            o = torch.nn.functional.scaled_dot_product_attention(q.transpose(1, 2), kk.transpose(1, 2), vv.transpose(1, 2), attn_mask=mask,
+                                                                 is_causal=mask is None, scale=scale)
             return o.transpose(1, 2)
 
         for i, layer in enumerate(self.layers):
@@ -224,7 +232,7 @@ class LlamaGenerator:
         for i, layer in enumerate(self.layers):
             def attend(q, k, v, i=i):
                 cache.append(i, k[:, 0], v[:, 0])
-                return _attend_cache(q[:, 0], cache.k[i], cache.v[i], cache.lens + 1, scale).unsqueeze(1)
+                return _attend_cache(q[:, 0], cache.k[i], cache.v[i], cache.lens + 1, scale, self.window).unsqueeze(1)
 
             h, _, _ = self._layer(layer, h, cos, sin, pos, attend)
         cache.lens += 1

@@ -45,6 +45,7 @@ class LlamaConfig:
     tie_word_embeddings: bool = False
     lean_activations: bool = True       # single-GPU: fused norm->linear / swiglu->linear nodes that do not keep the intermediate
     dtype: str = "bfloat16"
+    sliding_window: int | None = None   # local attention: position i sees keys (i - sliding_window, i]; None: full causal
 
     @property
     def head_dim(self):
@@ -57,6 +58,14 @@ def llama2_13b(**kw):
 
 def llama2_7b(**kw):
     return LlamaConfig(hidden_size=4096, intermediate_size=11008, num_hidden_layers=32, num_attention_heads=32, num_key_value_heads=32, **kw)
+
+
+def mistral_7b(**kw):
+    """Mistral-7B-v0.1: Llama layers with grouped-query attention (32 / 8 heads) and a 4096-token sliding window."""
+    base = dict(hidden_size=4096, intermediate_size=14336, num_hidden_layers=32, num_attention_heads=32, num_key_value_heads=8,
+                sliding_window=4096, max_position_embeddings=32768, rope_theta=10000.0)
+    base.update(kw)
+    return LlamaConfig(**base)
 
 
 def llama_tiny(**kw):
@@ -123,7 +132,7 @@ class LlamaAttention(nn.Layer):
         cfg = self.config
         nh, nkv, hd = self.num_heads, self.num_kv_heads, self.head_dim
         total = nh + 2 * nkv
-        if cfg.sequence_parallel and self.mp > 1 and position_ids is None and _raw(qkv).is_cuda:
+        if cfg.sequence_parallel and self.mp > 1 and position_ids is None and _raw(qkv).is_cuda and cfg.sliding_window is None:
             # sequence-parallel layout [S, B, *] is kept end to end: rotary gets explicit positions (token t = s*B + b -> s) and the
             # attention kernels address [B, S, h, d] views of the [S, B, ...] memory through their TMA strides - no transpose copies
             s, b = qkv.shape[0], qkv.shape[1]
@@ -135,11 +144,34 @@ class LlamaAttention(nn.Layer):
             qkv = qkv.transpose([1, 0, 2]).contiguous()
         b, s = qkv.shape[0], qkv.shape[1]
         qkv = KR.apply_rope_packed(qkv, cos, sin, nh + nkv, total, hd, position_ids, neox=True)
-        out = KAT.attention_packed(_raw(qkv).view(b, s, total, hd), nh, nkv, True, None)   # [B, S, nh, hd]; q/k/v read in place
+        if cfg.sliding_window is None:
+            out = KAT.attention_packed(_raw(qkv).view(b, s, total, hd), nh, nkv, True, None)   # [B, S, nh, hd]; q/k/v read in place
+        else:
+            out = _window_attention(_raw(qkv).view(b, s, total, hd), nh, nkv, cfg.sliding_window)
         out = _raw(out).reshape(b, s, nh * hd)
         if cfg.sequence_parallel and self.mp > 1:
             out = out.transpose(0, 1).contiguous()
         return self.o_proj(_w(out))
+
+
+def window_mask(sq, sk, window, device):
+    """Boolean visibility [sq, sk] of a causal sliding window, queries at the last sq of sk positions: query i sees key j iff
+    i - window < j <= i (positions counted from the first key)."""
+    qpos = torch.arange(sk - sq, sk, device=device)[:, None]
+    kpos = torch.arange(sk, device=device)[None, :]
+    return (kpos <= qpos) & (kpos > qpos - window)
+
+
+def _window_attention(x, nh, nkv, window):
+    """Causal sliding-window attention over packed x [B, S, nh + 2 nkv, D] -> [B, S, nh, D]: the wgmma column-mask kernels (forward and
+    backward) where they apply, else the reference attention with the explicit mask."""
+    b, s = x.shape[0], x.shape[1]
+    q, k, v = x[:, :, :nh], x[:, :, nh:nh + nkv], x[:, :, nh + nkv:]
+    colmask = KAT.colmask_from_window(s, s, window - 1, 0, True, x.device).expand(b, 1, s, 4)
+    out = KAT.attention_colmask(q, k, v, colmask, causal=True)
+    if out is not None:
+        return out
+    return KAT.attention(q, k, v, mask=window_mask(s, s, window, x.device)[None, None], causal=False)
 
 
 class LlamaMLP(nn.Layer):

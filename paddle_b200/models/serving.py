@@ -43,6 +43,14 @@ cached.  Each step the plain decode rows are grouped by their first block id; a 
 leading block ids, and groups that `paged_attention.shared_prefix_pays` accepts run on `decode_attention_paged_shared`, which reads that
 prefix once per tile of members.  stats gains prefix_hit_tokens.  Not covered: multi-level (tree) prefixes, grouping verify rows, parallel
 sampling (n > 1) and copy-on-write of partial blocks.
+
+Sliding-window models (`sliding_window` = W in the target's config): every block_attention call passes the window, so the windowed kernels
+read only the last W positions of each query.  After each step (so between the chunks of a chunked prefill too) block j of a sequence with
+`cached` = c positions is dead once (j + 1) * block_size <= c - W + 1: no later query of the sequence sees it.  Dead blocks go back to the
+pool and their slots in the sequence's block list stay as placeholders (RELEASED), so table indices stay positions / block_size; the
+kernels never read those table entries.  A sequence's footprint thus stops growing at about W tokens; admission still reserves the whole
+prompt.  With a draft model the caches share block ids, so a block is released only when it is dead for the draft as well (a draft
+without a window keeps every block of a greedy sequence).  stats gains released_blocks.  Not combinable with prefix caching.
 """
 from __future__ import annotations
 
@@ -51,6 +59,9 @@ import torch
 from ..incubate.nn.paged_attention import block_attention, shared_prefix_pays
 from ..kernels import sampling
 from .generation import _raw, _w
+
+
+RELEASED = -1   # a sequence's block-list slot whose block went back to the pool (below its sliding window)
 
 
 class BlockAllocator:
@@ -168,6 +179,11 @@ class Sequence:
         self.target = 0                            # tokens to prefill since admission: the sequence samples once cached reaches it
         self.draft_cached, self.spec = 0, 0        # speculative decoding: positions in the draft's cache, proposals this step
         self.keys = []                             # prefix caching: BlockKeys of the leading full blocks already keyed
+        self.released = 0                          # sliding window: blocks[:released] went back to the pool (RELEASED slots)
+
+    def owned(self):
+        """The blocks the sequence holds (released slots excluded)."""
+        return self.blocks[self.released:]
 
     def tokens(self):
         return self.prompt + self.generated
@@ -219,6 +235,12 @@ class LLMEngine:
             self.stats.update(draft_tokens=0, accepted_tokens=0)
         if self.enable_prefix_caching:
             self.stats["prefix_hit_tokens"] = 0
+        self.window = getattr(self.cfg, "sliding_window", None)
+        self._draft_window = getattr(self._draft[0].cfg, "sliding_window", None) if self._draft is not None else None
+        if self.window is not None:
+            if self.enable_prefix_caching:
+                raise ValueError("enable_prefix_caching is not supported for a model with a sliding window")
+            self.stats["released_blocks"] = 0
 
     def _draft_setup(self, draft_model, k, num_blocks):
         """(k, (adapter, key caches, value caches, no quantization)) of the draft model, or (0, None) without one."""
@@ -283,8 +305,8 @@ class LLMEngine:
         return (n_tokens + self.block_size - 1) // self.block_size
 
     def _preempt(self, s):
-        self.alloc.free(s.blocks)
-        s.blocks, s.cached, s.draft_cached, s.status, s.keys = [], 0, 0, Sequence.WAITING, []
+        self.alloc.free(s.owned())
+        s.blocks, s.cached, s.draft_cached, s.status, s.keys, s.released = [], 0, 0, Sequence.WAITING, [], 0
         s.preemptions += 1
         self.stats["preemptions"] += 1
         self.running.remove(s)
@@ -429,6 +451,7 @@ class LLMEngine:
         now_t = torch.tensor(n_new, dtype=torch.int32, device=dev)
         nh, nkv, hd = ad.nh, ad.nkv, ad.hd
         shared = self._shared_prefix_groups(seqs, n_new) if net is self._target else None
+        window = self.window if net is self._target else self._draft_window
         h = ad.embed_tokens(ids, position_ids)
         for li, layer in enumerate(ad.layers):
             qkv = ad.attn_in(layer, h, position_ids)
@@ -436,7 +459,7 @@ class LLMEngine:
             if self._observe is not None and net is self._target:
                 self._observe(li, qkv.reshape(t, (nh + 2 * nkv) * hd))
             out, _, _, _ = block_attention(qkv.reshape(t, (nh + 2 * nkv) * hd), key_cache[li], value_cache[li], enc_t, dec_t, now_t, cu, bt,
-                                           self.block_size, **kv_quant[li], shared_prefix=shared)
+                                           self.block_size, **kv_quant[li], shared_prefix=shared, sliding_window=window)
             h = ad.attn_out(layer, h, _raw(out).reshape(1, t, nh * hd))
         rows = (cu[1:].long() - 1) if rows is None else torch.tensor(rows, dtype=torch.int64, device=dev)
         return ad.logits(_raw(h)[:, rows])[0]                                          # [len(rows), vocab]
@@ -448,10 +471,26 @@ class LLMEngine:
         if fin:
             s.status = Sequence.FINISHED
             self.running.remove(s)
-            self.alloc.free(s.blocks)
-            s.blocks = []
+            self.alloc.free(s.owned())
+            s.blocks, s.released = [], 0
             self.done[s.id] = s
         return fin
+
+    def _release(self, s):
+        """Sliding window: returns s's blocks that no later query of it can see to the pool (their slots become RELEASED)."""
+        if self.window is None or s.status != Sequence.RUNNING:
+            return
+        end = s.cached - self.window + 1                         # the lowest key a query at position >= cached sees
+        if self._draft is not None and not s.do_sample:          # the draft's cache uses the same block ids
+            if self._draft_window is None:
+                return
+            end = min(end, s.draft_cached - self._draft_window + 1)
+        dead = min(max(end, 0) // self.block_size, len(s.blocks))
+        if dead > s.released:
+            self.alloc.free(s.blocks[s.released:dead])
+            self.stats["released_blocks"] += dead - s.released
+            s.blocks[s.released:dead] = [RELEASED] * (dead - s.released)
+            s.released = dead
 
     def step(self):
         """One iteration.  Returns [(request id, new token, finished)] for every sequence that produced a token."""
@@ -482,6 +521,8 @@ class LLMEngine:
                 continue
             tok = toks[i]
             out.append((s.id, tok, self._finish_token(s, tok)))
+        for s in seqs:
+            self._release(s)
         self.stats["max_running"] = max(self.stats["max_running"], len(self.running))
         return out
 
@@ -582,6 +623,8 @@ class LLMEngine:
                 continue
             tok = toks[i]
             out.append((s.id, tok, self._finish_token(s, tok)))
+        for s in seqs:
+            self._release(s)
         self.stats["max_running"] = max(self.stats["max_running"], len(self.running))
         return out
 
