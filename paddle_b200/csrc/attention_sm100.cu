@@ -25,7 +25,13 @@
 // past the sequence are written as zeros, so stale or NaN cache rows never reach the MMAs.  The K dequant scale is folded into the exp2
 // scale and the V dequant scale into the epilogue's 1 / l, so the MMA and softmax code is the 16-bit kernel's.
 //
-// The kernel bodies live in include/b200_attention_fwd.cuh, shared with the sliding-window prefill kernels of attention_window.cu.
+// PAGED with a sliding window W (window > 0, fwd_window_kernel): row i sees keys (i - W, i].  A 128-row query tile starts at key tile
+// max(0, m0 + past - W + 1) / 128 and masks each row's left edge, and the work list counts only those key tiles, so a long chunk costs
+// O(n W) instead of O(n^2).  Keys below the lowest bound of a CTA's rows are never loaded and their block-table entries never read (the
+// TMA producer fetches the window's first block in their place and the tile's V rows below the window are zeroed), so blocks wholly
+// below the window may hold NaN or belong to another sequence.
+//
+// The kernel bodies live in include/b200_attention_fwd.cuh.
 #include <cuda.h>
 #include <algorithm>
 #include <cstdio>
@@ -68,6 +74,20 @@ bool make_map4(CUtensorMap* out, const void* ptr, int d, int s, int h, int b, in
 __global__ void __launch_bounds__(1024) paged_work_kernel(const int* __restrict__ n_q, const int* __restrict__ past, int b, int slots,
                                                           int* scratch, int2* work) {
   paged_work<false>(n_q, past, b, slots, scratch, work, 0);
+}
+
+// The sliding-window paged kernels: the windowed prefill takes the larger WindowParams and the work list the window as one more
+// argument, so they are kernels of their own; the unwindowed kernels keep their smaller parameters, which their code depends on.
+template <typename T, typename KV, int D>
+__global__ void __launch_bounds__(std::is_same<KV, T>::value ? kThreads : kThreadsQ8, 1)
+fwd_window_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
+                  const WindowParams<std::conditional_t<std::is_same<KV, T>::value, PagedParams, QuantPagedParams>> p) {
+  fwd_body<T, false, true, KV, D, true>(map_q, map_k, map_v, p);
+}
+
+__global__ void __launch_bounds__(1024) paged_work_window_kernel(const int* __restrict__ n_q, const int* __restrict__ past, int b, int slots,
+                                                                 int* scratch, int2* work, int window) {
+  paged_work<true>(n_q, past, b, slots, scratch, work, window);
 }
 
 }  // namespace attn
@@ -141,9 +161,26 @@ int attention_paged_prefill(const PagedAttnArgs& a, cudaStream_t s) {
   CUtensorMap mq, mk, mv;
   // q: {d, token, head, 1} over the strided [T, H, D] view; caches: {d, row in block, kv head, block}
   if (!make_map4(&mq, a.q, a.d, a.t, a.h, 1, a.q_strides[0], a.q_strides[1], a.q_strides[0] * a.t, BM, a.dtype)) return 2;
-  int2* work = reinterpret_cast<int2*>(a.scratch);
   if (a.kv_dtype != -1) {   // 8-bit caches: no tensor maps over them (the converter warpgroup reads them)
-    QuantPagedParams p = {};
+    mk = mv = mq;
+  } else {
+    if (!make_map4(&mk, a.k_cache, a.d, a.block_size, a.hk, a.num_blocks, a.d, blk, blk * a.hk, rows, a.dtype)) return 2;
+    if (!make_map4(&mv, a.v_cache, a.d, a.block_size, a.hk, a.num_blocks, a.d, blk, blk * a.hk, rows, a.dtype)) return 2;
+  }
+  int2* work = reinterpret_cast<int2*>(a.scratch);
+  int* keys = a.scratch + 2 * slots;
+  if (a.window > 0) paged_work_window_kernel<<<1, 1024, 0, s>>>(a.n_q, a.past, a.b, slots, keys, work, a.window);
+  else paged_work_kernel<<<1, 1024, 0, s>>>(a.n_q, a.past, a.b, slots, keys, work);
+  dim3 grid(a.h, slots);   // every head of the heaviest tile is dispatched first
+  auto launch = [&](auto tag_t, auto tag_kv, auto tag_d) {
+    using T = decltype(tag_t);
+    using KV = decltype(tag_kv);
+    constexpr int D = decltype(tag_d)::value;
+    constexpr bool Q8 = !std::is_same<T, KV>::value;
+    constexpr int threads = Q8 ? kThreadsQ8 : kThreads;
+    constexpr uint32_t smem = kSmemBytes<D>;
+    using P = std::conditional_t<Q8, QuantPagedParams, PagedParams>;
+    WindowParams<P> p = {};
     p.b = a.b; p.sq = a.t; p.sk = 0; p.h = a.h; p.hk = a.hk;
     p.scale_log2 = a.scale * 1.4426950408889634f;
     p.causal = 1; p.causal_off = 0;
@@ -152,49 +189,29 @@ int attention_paged_prefill(const PagedAttnArgs& a, cudaStream_t s) {
     p.colmask = nullptr; p.mask_heads = 1;
     p.work = work; p.cu_q = a.cu_q; p.n_q = a.n_q; p.past = a.past;
     p.block_tables = a.block_tables; p.max_blocks = a.max_blocks; p.block_size = a.block_size;
-    p.k_cache = reinterpret_cast<const uint8_t*>(a.k_cache); p.v_cache = reinterpret_cast<const uint8_t*>(a.v_cache);
-    p.k_dq = a.k_dq; p.v_dq = a.v_dq;
-    if (a.window > 0) return attention_paged_prefill_window(mq, p, a, slots, s);
-    paged_work_kernel<<<1, 1024, 0, s>>>(a.n_q, a.past, a.b, slots, a.scratch + 2 * slots, work);
-    dim3 grid(a.h, slots);
-    auto launch = [&](auto tag_t, auto tag_kv) {
-      using T = decltype(tag_t);
-      using KV = decltype(tag_kv);
-      set_max_dynamic_smem<fwd_kernel<T, false, true, KV>>(SMEM_BYTES);
-      fwd_kernel<T, false, true, KV><<<grid, kThreadsQ8, SMEM_BYTES, s>>>(mq, mq, mq, p);
-    };
-    const bool i8 = a.kv_dtype == kI8;
-    if (a.dtype == kBF16) {
-      if (i8) launch(__nv_bfloat16(), kv8::I8()); else launch(__nv_bfloat16(), kv8::E4M3());
-    } else {
-      if (i8) launch(__half(), kv8::I8()); else launch(__half(), kv8::E4M3());
+    if constexpr (Q8) {
+      p.k_cache = reinterpret_cast<const uint8_t*>(a.k_cache); p.v_cache = reinterpret_cast<const uint8_t*>(a.v_cache);
+      p.k_dq = a.k_dq; p.v_dq = a.v_dq;
     }
-    return B200_LAUNCH_RESULT();
-  }
-  if (!make_map4(&mk, a.k_cache, a.d, a.block_size, a.hk, a.num_blocks, a.d, blk, blk * a.hk, rows, a.dtype)) return 2;
-  if (!make_map4(&mv, a.v_cache, a.d, a.block_size, a.hk, a.num_blocks, a.d, blk, blk * a.hk, rows, a.dtype)) return 2;
-  PagedParams p = {};
-  p.b = a.b; p.sq = a.t; p.sk = 0; p.h = a.h; p.hk = a.hk;
-  p.scale_log2 = a.scale * 1.4426950408889634f;
-  p.causal = 1; p.causal_off = 0;
-  p.o = a.o; p.lse = a.lse;
-  p.o_sb = 0; p.o_ss = a.o_strides[0]; p.o_sh = a.o_strides[1];
-  p.colmask = nullptr; p.mask_heads = 1;
-  p.work = work; p.cu_q = a.cu_q; p.n_q = a.n_q; p.past = a.past;
-  p.block_tables = a.block_tables; p.max_blocks = a.max_blocks; p.block_size = a.block_size;
-  if (a.window > 0) return attention_paged_prefill_window(mq, mk, mv, p, a, slots, s);
-  paged_work_kernel<<<1, 1024, 0, s>>>(a.n_q, a.past, a.b, slots, a.scratch + 2 * slots, work);
-  dim3 grid(a.h, slots);   // every head of the heaviest tile is dispatched first
-  auto launch = [&](auto tag_t, auto tag_d) {
-    using T = decltype(tag_t);
-    constexpr int D = decltype(tag_d)::value;
-    set_max_dynamic_smem<fwd_kernel<T, false, true, T, D>>(kSmemBytes<D>);
-    fwd_kernel<T, false, true, T, D><<<grid, kThreads, kSmemBytes<D>, s>>>(mq, mk, mv, p);
+    p.window = a.window;
+    if (a.window > 0) {
+      set_max_dynamic_smem<fwd_window_kernel<T, KV, D>>(smem);
+      fwd_window_kernel<T, KV, D><<<grid, threads, smem, s>>>(mq, mk, mv, p);
+    } else {
+      set_max_dynamic_smem<fwd_kernel<T, false, true, KV, D>>(smem);
+      fwd_kernel<T, false, true, KV, D><<<grid, threads, smem, s>>>(mq, mk, mv, static_cast<const P&>(p));
+    }
   };
   if (a.dtype == kBF16) {
-    if (a.d == 128) launch(__nv_bfloat16(), HeadDim<128>()); else launch(__nv_bfloat16(), HeadDim<64>());
+    if (a.d == 64) launch(__nv_bfloat16(), __nv_bfloat16(), HeadDim<64>());
+    else if (a.kv_dtype == kI8) launch(__nv_bfloat16(), kv8::I8(), HeadDim<128>());
+    else if (a.kv_dtype == kE4M3) launch(__nv_bfloat16(), kv8::E4M3(), HeadDim<128>());
+    else launch(__nv_bfloat16(), __nv_bfloat16(), HeadDim<128>());
   } else {
-    if (a.d == 128) launch(__half(), HeadDim<128>()); else launch(__half(), HeadDim<64>());
+    if (a.d == 64) launch(__half(), __half(), HeadDim<64>());
+    else if (a.kv_dtype == kI8) launch(__half(), kv8::I8(), HeadDim<128>());
+    else if (a.kv_dtype == kE4M3) launch(__half(), kv8::E4M3(), HeadDim<128>());
+    else launch(__half(), __half(), HeadDim<128>());
   }
   return B200_LAUNCH_RESULT();
 }

@@ -968,15 +968,37 @@ int kv8_code(const char* op, const Tensor& q, const Tensor& k_cache, const Tenso
   return st == at::kChar ? kKvI8 : kKvE4M3;
 }
 
+// The operands the paged attention bindings share, checked with messages that name `op`: q a CUDA [T,H,D] view with unit head_dim
+// stride, caches contiguous [num_blocks,Hkv,block_size,D] of one shape on q's device (8-bit with their dequant scales, or of q's dtype),
+// block_tables int32 [B, max_blocks > 0] on the device, the per-sequence vectors `seq` (named `seq_names` in messages) int32 [B] on the
+// device, and out (when given) [T, H*D] of q's dtype with unit inner stride.  Returns the 8-bit cache code (kv8_code).
+int check_paged_operands(const char* op, const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& block_tables,
+                         const OptT& k_dq, const OptT& v_dq, std::initializer_list<const Tensor*> seq, const char* seq_names, const Tensor* out) {
+  TORCH_CHECK(q.is_cuda() && q.dim() == 3 && q.stride(2) == 1, op, ": q must be a CUDA [T,H,D] view with unit head_dim stride");
+  TORCH_CHECK(k_cache.dim() == 4 && v_cache.dim() == 4 && k_cache.is_contiguous() && v_cache.is_contiguous() && k_cache.sizes() == v_cache.sizes(),
+              op, ": caches must be contiguous [num_blocks,Hkv,block_size,D] of one shape");
+  TORCH_CHECK(k_cache.device() == q.device() && v_cache.device() == q.device(), op, ": q and caches must be on one device");
+  const int kv = kv8_code(op, q, k_cache, v_cache, k_dq, v_dq);
+  if (kv == -1)
+    TORCH_CHECK(k_cache.scalar_type() == q.scalar_type() && v_cache.scalar_type() == q.scalar_type(), op, ": q and caches must share a dtype");
+  TORCH_CHECK(block_tables.device() == q.device() && block_tables.scalar_type() == at::kInt && block_tables.is_contiguous() && block_tables.dim() == 2
+              && block_tables.size(1) > 0, op, ": block_tables must be int32 [B, max_blocks] on the device");
+  for (const Tensor* t : seq)
+    TORCH_CHECK(t->device() == q.device() && t->scalar_type() == at::kInt && t->is_contiguous() && t->numel() == block_tables.size(0), op, ": ",
+                seq_names, " must be int32 [B] on the device");
+  if (out)
+    TORCH_CHECK(out->device() == q.device() && out->scalar_type() == q.scalar_type() && out->dim() == 2 && out->size(0) == q.size(0) &&
+                out->size(1) == q.size(1) * q.size(2) && out->stride(1) == 1, op, ": out must be [T, H*D] with unit inner stride");
+  return kv;
+}
+
 // paged KV cache: q [B,H,D], caches [num_blocks,Hkv,block_size,D], lens int32 [B] (positions valid per sequence), block_tables int32 [B,max_blocks];
 // int8 / fp8 e4m3 caches take fp32 [Hkv] k_dequant_scales / v_dequant_scales; window > 0: the last `window` positions only
 Tensor decode_attention_paged(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& lens, const Tensor& block_tables, double scale,
                               const OptT& k_dequant_scales, const OptT& v_dequant_scales, int64_t window) {
-  TORCH_CHECK(q.is_cuda() && q.dim() == 3 && k_cache.dim() == 4 && v_cache.dim() == 4 && q.is_contiguous() && k_cache.is_contiguous() && v_cache.is_contiguous(),
-              "decode_attention_paged: q [B,H,D], caches [num_blocks,Hkv,block_size,D] contiguous");
-  TORCH_CHECK(lens.scalar_type() == at::kInt && lens.is_contiguous() && lens.numel() == q.size(0), "decode_attention_paged: lens must be int32 [B]");
-  TORCH_CHECK(block_tables.is_cuda() && block_tables.scalar_type() == at::kInt && block_tables.is_contiguous() && block_tables.dim() == 2 && block_tables.size(0) == q.size(0),
-              "decode_attention_paged: block_tables must be int32 [B, max_blocks] on the device");
+  const char* op = "decode_attention_paged";
+  const int kv = check_paged_operands(op, q, k_cache, v_cache, block_tables, k_dequant_scales, v_dequant_scales, {&lens}, "lens", nullptr);
+  TORCH_CHECK(q.is_contiguous() && block_tables.size(0) == q.size(0), op, ": q must be contiguous [B,H,D] with one block table row per sequence");
   c10::cuda::CUDAGuard guard(q.device());
   const int b = (int)q.size(0), h = (int)q.size(1), d = (int)q.size(2), hkv = (int)k_cache.size(1), bs = (int)k_cache.size(2), mb = (int)block_tables.size(1);
   const int w = window > 0 ? (int)std::min<int64_t>(window, (int64_t)mb * bs) : 0;
@@ -984,10 +1006,7 @@ Tensor decode_attention_paged(const Tensor& q, const Tensor& k_cache, const Tens
   Tensor out = torch::empty_like(q);
   Tensor pacc = torch::empty({b, h, splits, d}, q.options().dtype(at::kFloat));
   Tensor pml = torch::empty({b, h, splits, 2}, q.options().dtype(at::kFloat));
-  const int kv = kv8_code("decode_attention_paged", q, k_cache, v_cache, k_dequant_scales, v_dequant_scales);
   if (kv != -1) {
-    TORCH_CHECK(k_cache.device() == q.device() && v_cache.device() == q.device() && k_cache.sizes() == v_cache.sizes(),
-                "decode_attention_paged: caches must be of one shape on the device of q");
     int rc = b200::decode_attention_paged_q8(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), lens.data_ptr<int>(), out.data_ptr(),
                                              pacc.data_ptr<float>(), pml.data_ptr<float>(), b, h, hkv, d, splits, (float)scale, dt_code(q), kv,
                                              k_dequant_scales->data_ptr<float>(), v_dequant_scales->data_ptr<float>(), block_tables.data_ptr<int>(),
@@ -1063,21 +1082,9 @@ std::vector<Tensor> attention_fwd(const Tensor& q, const Tensor& k, const Tensor
 void attention_fwd_paged(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& block_tables, const Tensor& cu_q,
                          const Tensor& n_q, const Tensor& past, double scale, const Tensor& out, const OptT& lse, const OptT& k_dequant_scales,
                          const OptT& v_dequant_scales, int64_t window) {
-  TORCH_CHECK(q.is_cuda() && q.dim() == 3 && q.stride(2) == 1, "attention_fwd_paged: q must be a CUDA [T,H,D] view with unit head_dim stride");
-  TORCH_CHECK(k_cache.dim() == 4 && v_cache.dim() == 4 && k_cache.is_contiguous() && v_cache.is_contiguous() && k_cache.sizes() == v_cache.sizes(),
-              "attention_fwd_paged: caches must be contiguous [num_blocks,Hkv,block_size,D] of one shape");
-  TORCH_CHECK(k_cache.device() == q.device() && v_cache.device() == q.device(), "attention_fwd_paged: q and caches must be on one device");
-  const int kv = kv8_code("attention_fwd_paged", q, k_cache, v_cache, k_dequant_scales, v_dequant_scales);
-  if (kv == -1)
-    TORCH_CHECK(k_cache.scalar_type() == q.scalar_type() && v_cache.scalar_type() == q.scalar_type(), "attention_fwd_paged: q and caches must share a dtype");
-  TORCH_CHECK(block_tables.device() == q.device() && block_tables.scalar_type() == at::kInt && block_tables.is_contiguous() && block_tables.dim() == 2,
-              "attention_fwd_paged: block_tables must be int32 [B, max_blocks] on the device");
+  const int kv = check_paged_operands("attention_fwd_paged", q, k_cache, v_cache, block_tables, k_dequant_scales, v_dequant_scales,
+                                      {&cu_q, &n_q, &past}, "cu_q / n_q / past", &out);
   const int64_t b = block_tables.size(0);
-  for (const Tensor* t : {&cu_q, &n_q, &past})
-    TORCH_CHECK(t->device() == q.device() && t->scalar_type() == at::kInt && t->is_contiguous() && t->numel() == b,
-                "attention_fwd_paged: cu_q / n_q / past must be int32 [B] on the device");
-  TORCH_CHECK(out.device() == q.device() && out.scalar_type() == q.scalar_type() && out.dim() == 2 && out.size(0) == q.size(0) &&
-              out.size(1) == q.size(1) * q.size(2) && out.stride(1) == 1, "attention_fwd_paged: out must be [T, H*D] with unit inner stride");
   b200::PagedAttnArgs a;
   a.q = q.data_ptr(); a.k_cache = k_cache.data_ptr(); a.v_cache = v_cache.data_ptr(); a.o = out.data_ptr(); a.lse = nullptr;
   a.t = (int)q.size(0); a.h = (int)q.size(1); a.d = (int)q.size(2);
@@ -1114,23 +1121,10 @@ void attention_fwd_paged(const Tensor& q, const Tensor& k_cache, const Tensor& v
 void decode_attention_paged_multi(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& block_tables, const Tensor& cu_q,
                                   const Tensor& n_q, const Tensor& past, double scale, const Tensor& out, const OptT& k_dequant_scales,
                                   const OptT& v_dequant_scales, int64_t window) {
-  TORCH_CHECK(q.is_cuda() && q.dim() == 3 && q.stride(2) == 1, "decode_attention_paged_multi: q must be a CUDA [T,H,D] view with unit head_dim stride");
   TORCH_CHECK(q.scalar_type() == at::kHalf || q.scalar_type() == at::kBFloat16, "decode_attention_paged_multi: q must be fp16 or bf16");
-  TORCH_CHECK(k_cache.dim() == 4 && v_cache.dim() == 4 && k_cache.is_contiguous() && v_cache.is_contiguous() && k_cache.sizes() == v_cache.sizes(),
-              "decode_attention_paged_multi: caches must be contiguous [num_blocks,Hkv,block_size,D] of one shape");
-  TORCH_CHECK(k_cache.device() == q.device() && v_cache.device() == q.device(), "decode_attention_paged_multi: q and caches must be on one device");
-  const int kv = kv8_code("decode_attention_paged_multi", q, k_cache, v_cache, k_dequant_scales, v_dequant_scales);
-  if (kv == -1)
-    TORCH_CHECK(k_cache.scalar_type() == q.scalar_type() && v_cache.scalar_type() == q.scalar_type(),
-                "decode_attention_paged_multi: q and caches must share a dtype");
-  TORCH_CHECK(block_tables.device() == q.device() && block_tables.scalar_type() == at::kInt && block_tables.is_contiguous() && block_tables.dim() == 2
-              && block_tables.size(1) > 0, "decode_attention_paged_multi: block_tables must be int32 [B, max_blocks] on the device");
+  const int kv = check_paged_operands("decode_attention_paged_multi", q, k_cache, v_cache, block_tables, k_dequant_scales, v_dequant_scales,
+                                      {&cu_q, &n_q, &past}, "cu_q / n_q / past", &out);
   const int64_t b = block_tables.size(0);
-  for (const Tensor* t : {&cu_q, &n_q, &past})
-    TORCH_CHECK(t->device() == q.device() && t->scalar_type() == at::kInt && t->is_contiguous() && t->numel() == b,
-                "decode_attention_paged_multi: cu_q / n_q / past must be int32 [B] on the device");
-  TORCH_CHECK(out.device() == q.device() && out.scalar_type() == q.scalar_type() && out.dim() == 2 && out.size(0) == q.size(0) &&
-              out.size(1) == q.size(1) * q.size(2) && out.stride(1) == 1, "decode_attention_paged_multi: out must be [T, H*D] with unit inner stride");
   TORCH_CHECK(q.size(2) == k_cache.size(3) && (q.size(2) == 128 || (q.size(2) == 64 && kv == -1)),
               "decode_attention_paged_multi: head_dim must be 128, or 64 on 16-bit caches");
   const int64_t hkv = k_cache.size(1);
@@ -1166,24 +1160,12 @@ void decode_attention_paged_shared(const Tensor& q, const Tensor& k_cache, const
                                    const Tensor& lens, const Tensor& cu_groups, const Tensor& group_seqs, const Tensor& prefix_len, double scale,
                                    const Tensor& out, const OptT& k_dequant_scales, const OptT& v_dequant_scales) {
   const char* fn = "decode_attention_paged_shared";
-  TORCH_CHECK(q.is_cuda() && q.dim() == 3 && q.stride(2) == 1, fn, ": q must be a CUDA [T,H,D] view with unit head_dim stride");
   TORCH_CHECK(q.scalar_type() == at::kHalf || q.scalar_type() == at::kBFloat16, fn, ": q must be fp16 or bf16");
-  TORCH_CHECK(k_cache.dim() == 4 && v_cache.dim() == 4 && k_cache.is_contiguous() && v_cache.is_contiguous() && k_cache.sizes() == v_cache.sizes(),
-              fn, ": caches must be contiguous [num_blocks,Hkv,block_size,D] of one shape");
-  TORCH_CHECK(k_cache.device() == q.device() && v_cache.device() == q.device(), fn, ": q and caches must be on one device");
-  const int kv = kv8_code(fn, q, k_cache, v_cache, k_dequant_scales, v_dequant_scales);
-  if (kv == -1)
-    TORCH_CHECK(k_cache.scalar_type() == q.scalar_type() && v_cache.scalar_type() == q.scalar_type(), fn, ": q and caches must share a dtype");
-  TORCH_CHECK(block_tables.device() == q.device() && block_tables.scalar_type() == at::kInt && block_tables.is_contiguous() && block_tables.dim() == 2
-              && block_tables.size(1) > 0, fn, ": block_tables must be int32 [B, max_blocks] on the device");
+  const int kv = check_paged_operands(fn, q, k_cache, v_cache, block_tables, k_dequant_scales, v_dequant_scales, {&cu_q, &lens}, "cu_q / lens", &out);
   const int64_t b = block_tables.size(0);
-  for (const Tensor* t : {&cu_q, &lens})
-    TORCH_CHECK(t->device() == q.device() && t->scalar_type() == at::kInt && t->is_contiguous() && t->numel() == b, fn, ": cu_q / lens must be int32 [B] on the device");
   for (const Tensor* t : {&cu_groups, &group_seqs, &prefix_len})
     TORCH_CHECK(t->device().is_cpu() && t->scalar_type() == at::kInt && t->is_contiguous() && t->dim() == 1, fn,
                 ": cu_groups / group_seqs / prefix_len must be int32 1-D tensors on the host");
-  TORCH_CHECK(out.device() == q.device() && out.scalar_type() == q.scalar_type() && out.dim() == 2 && out.size(0) == q.size(0) &&
-              out.size(1) == q.size(1) * q.size(2) && out.stride(1) == 1, fn, ": out must be [T, H*D] with unit inner stride");
   TORCH_CHECK(q.size(2) == 128 && k_cache.size(3) == 128, fn, ": head_dim must be 128");
   const int64_t hkv = k_cache.size(1), h = q.size(1), bs = k_cache.size(2), max_blocks = block_tables.size(1);
   TORCH_CHECK(hkv > 0 && h % hkv == 0 && h / hkv <= 64, fn, ": H must be a multiple of Hkv with H / Hkv <= 64");

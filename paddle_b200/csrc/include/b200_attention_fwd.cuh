@@ -1,6 +1,9 @@
 // Bodies of the flash-attention forward kernel and of the paged prefill's work-list kernel (see attention_sm100.cu for the algorithms).
-// attention_sm100.cu instantiates them in fwd_kernel and paged_work_kernel; attention_window.cu instantiates the sliding-window (WINDOW)
-// paged versions in kernels of its own.
+// attention_sm100.cu instantiates them in fwd_kernel and paged_work_kernel, and the sliding-window (WINDOW) paged versions in
+// fwd_window_kernel and paged_work_window_kernel.
+//
+// Sliding window W (WINDOW): the query at absolute position i sees key j iff i - W < j <= i.  Keys below the lowest bound of a CTA's
+// rows are never loaded and their block-table entries never read, so blocks wholly below the window may hold anything.
 #pragma once
 #include <cuda.h>
 #include <type_traits>
@@ -460,11 +463,5 @@ __device__ __forceinline__ void paged_work(const int* __restrict__ n_q, const in
 }
 
 }  // namespace attn
-
-// The sliding-window paged prefill (attention_window.cu), called by attention_paged_prefill with its tensor maps and parameters built:
-// launches the windowed work list into a.scratch and the windowed kernel over 16-bit caches, or over 8-bit caches (map_q only).
-int attention_paged_prefill_window(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv, const attn::PagedParams& p,
-                                   const PagedAttnArgs& a, int slots, cudaStream_t s);
-int attention_paged_prefill_window(const CUtensorMap& mq, const attn::QuantPagedParams& p, const PagedAttnArgs& a, int slots, cudaStream_t s);
 
 }  // namespace b200

@@ -1,9 +1,13 @@
-// Bodies of the paged decode and verify attention kernels (see decode_attention.cu for the algorithms).  Each body is a
-// __device__ __forceinline__ template with a compile-time WINDOW flag: decode_attention.cu instantiates WINDOW = false in its kernels,
-// attention_window.cu instantiates WINDOW = true for sliding-window attention in kernels of its own.
+// Bodies of the paged decode, verify and shared-prefix attention kernels (see decode_attention.cu for the algorithms).  Each body is a
+// __device__ __forceinline__ template with a compile-time WINDOW flag, instantiated by the kernels of decode_attention.cu.
 //
-// Sliding window W (WINDOW = true): the query at absolute position i sees key j iff i - W < j <= i.  Keys below the lowest bound of a
-// CTA's rows are never loaded and their block-table entries never read, so blocks wholly below the window may hold anything.
+// Sliding window W (WINDOW = true): the query at absolute position i sees key j iff i - W < j <= i (W keys including itself), the mask
+// of models trained with a local window (Mistral, Phi-3) and a way to bound a sequence's KV memory.  Only the key range and the left
+// edge of the mask change:
+// - decode: a split covers positions [max(0, len - W), len), so a call touches min(len, W) rows per query;
+// - verify: the splits cover the key tiles from the one holding past - W + 1, and row r of token j masks keys below past + j - W + 1.
+// Keys below the lowest bound of a CTA's rows are never loaded and their block-table entries never read, so blocks wholly below the
+// window may hold NaN or belong to another sequence.
 #pragma once
 #include <cuda.h>
 #include <type_traits>
@@ -233,6 +237,7 @@ struct Params {
   int64_t q_st, q_sh, o_st;   // element strides: q (token, head), out (token; heads are D apart)
   int h, hkv, splits, max_blocks, block_size;
   float scale_log2;
+  int window;                 // > 0: sliding window (read by the WINDOW kernels only)
 };
 
 // shared memory: Q tile [64][D] 16-bit | K, V 16-bit tiles (kStages, or 1 for 8-bit caches) | 8-bit caches: raw K, V tiles (kStages).
@@ -270,38 +275,83 @@ template <> __device__ __forceinline__ void mma16816<__half>(float (&c)[4], cons
                : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-// The split kernel's body for head size D (inlined into multi_split_kernel, decode_verify64::multi_split_kernel and the windowed verify
-// kernels).  KV = T: 16-bit caches; KV = kv8::I8 / kv8::E4M3: 8-bit caches with fp32 [Hkv] dequant scales (D = 128 only).
+// The split kernel's body for head size D, inlined into the verify kernels (multi_split_kernel) and, with SHARED, into the
+// shared-prefix kernel (decode_shared::shared_split_kernel, P = decode_shared::Params).  KV = T: 16-bit caches; KV = kv8::I8 /
+// kv8::E4M3: 8-bit caches with fp32 [Hkv] dequant scales (D = 128 only).  The two kinds differ only in
+// - the key range [lo, hi): verify rows see the keys of their own sequence below past + n_q, in absolute 64-key tiles; a shared task
+//   sees the keys [lo, hi) of its task, in tiles from lo;
+// - where Q row r comes from: token r / G of the sequence, or member r / G of the group;
+// - the mask: bottom-right causal per token (and, with WINDOW, the window's left edge), or none below hi;
+// - where the partials go: the split's 64 rows of the sequence, or the task's rows (an empty task split writes an empty partial).
 // WINDOW: the splits cover the key tiles from the one holding past - window + 1 (the first token's lowest key); keys below it are
 // zero-filled without reading their table entries, and row r of token j also masks the keys below past + j - window + 1.
-template <typename T, typename KV, int D, bool WINDOW = false>
-__device__ __forceinline__ void multi_split(const Params& p, int window = 0) {
+template <typename T, typename KV, int D, bool WINDOW = false, bool SHARED = false, typename P>
+__device__ __forceinline__ void multi_split(const P& p, int window = 0) {
   constexpr bool Q8 = !std::is_same<T, KV>::value;
   static_assert(D == 128 || (D == 64 && !Q8), "head_dim 128, or 64 on 16-bit caches");
+  static_assert(!SHARED || (D == 128 && !WINDOW), "shared-prefix decode is head_dim 128 and unwindowed");
   constexpr int kTile16 = decode_multi::kTile16<D>, kTile8 = decode_multi::kTile8<D>;
   using S = Smem<Q8, D>;
   constexpr int kQShift = D == 128 ? 4 : 3;                  // log2 of the 16-byte chunks of a Q row
-  const int split = blockIdx.x, kvh = blockIdx.y, b = blockIdx.z;
-  const int nq = p.n_q[b], g_size = p.h / p.hkv, nrows = nq * g_size;
-  if (nq <= 0 || nrows > kRows) return;                      // skipped, or past the row limit (multi_merge_kernel writes NaN)
-  const int past = p.past[b];
-  const int len = min(past + nq, p.max_blocks * p.block_size);
-  int t0, t1, lo = 0;                                        // lo: the lowest key any row sees
-  if constexpr (WINDOW) {
-    lo = max(0, past - window + 1);
-    const int first = lo / BN, ntiles = (len + BN - 1) / BN, per = (ntiles - first + p.splits - 1) / p.splits;
-    t0 = first + split * per;
-    t1 = min(ntiles, t0 + per);
-  } else {
-    const int ntiles = (len + BN - 1) / BN, per = (ntiles + p.splits - 1) / p.splits;
+  extern __shared__ __align__(128) uint8_t smem[];
+  // The prologue of each kind, in the order its kernel has always computed it (the order of the loads shapes ptxas's schedule).
+  // keys at or past hi are never loaded: verify rows' len, or the end of a shared task's keys.  lo: a shared task's first key, or with
+  // WINDOW the lowest key any verify row sees
+  int split, kvh, b = 0, g_size, nrows, t0, t1, hi, lo = 0, past = 0, cu = 0, m0 = 0, tid, warp, lane;
+  int64_t pbase = 0;
+  uint32_t sbase;
+  const int* bt;
+  if constexpr (SHARED) {
+    const int* task = p.tasks + (int64_t)blockIdx.x * kSharedTaskInts;
+    kvh = blockIdx.y;
+    const int tb = task[0];
+    m0 = task[1];
+    const int cnt = task[2];
+    lo = task[3];
+    split = task[5];
+    const int splits = task[6];
+    g_size = p.h / p.hkv;
+    nrows = cnt * g_size;
+    const int cap = p.max_blocks * p.block_size, len_tb = p.lens[tb];
+    // prefix: keys below prefix_len, never past the reference member's cached ones (a bad group is NaN-ed by the merge); suffix: up to len
+    hi = task[4] >= 0 ? min(min(task[4], len_tb - 1), cap) : min(len_tb, cap);
+    const int ntiles = hi > lo ? (hi - lo + BN - 1) / BN : 0, per = (ntiles + splits - 1) / splits;
     t0 = split * per;
     t1 = min(ntiles, t0 + per);
+    pbase = (int64_t)kvh * p.rows + task[7];
+    tid = threadIdx.x; warp = tid >> 5; lane = tid & 31;
+    if (t0 >= t1) {                                          // no keys: an empty partial (the merge skips it)
+      for (int r = tid; r < nrows; r += kThreads) { p.part_ml[(pbase + r) * 2] = -INFINITY; p.part_ml[(pbase + r) * 2 + 1] = 0.f; }
+      return;
+    }
+    sbase = (uint32_t)__cvta_generic_to_shared(smem);
+    bt = p.block_tables + (int64_t)tb * p.max_blocks;
+  } else {
+    split = blockIdx.x;
+    kvh = blockIdx.y;
+    b = blockIdx.z;
+    const int nq = p.n_q[b];
+    g_size = p.h / p.hkv;
+    nrows = nq * g_size;
+    if (nq <= 0 || nrows > kRows) return;                    // skipped, or past the row limit (multi_merge_kernel writes NaN)
+    past = p.past[b];
+    hi = min(past + nq, p.max_blocks * p.block_size);
+    if constexpr (WINDOW) {
+      lo = max(0, past - window + 1);
+      const int first = lo / BN, ntiles = (hi + BN - 1) / BN, per = (ntiles - first + p.splits - 1) / p.splits;
+      t0 = first + split * per;
+      t1 = min(ntiles, t0 + per);
+    } else {
+      const int ntiles = (hi + BN - 1) / BN, per = (ntiles + p.splits - 1) / p.splits;
+      t0 = split * per;
+      t1 = min(ntiles, t0 + per);
+    }
+    sbase = (uint32_t)__cvta_generic_to_shared(smem);
+    tid = threadIdx.x; warp = tid >> 5; lane = tid & 31;
+    bt = p.block_tables + (int64_t)b * p.max_blocks;
+    cu = p.cu_q[b];
   }
-  extern __shared__ __align__(128) uint8_t smem[];
-  const uint32_t sbase = (uint32_t)__cvta_generic_to_shared(smem);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int* bt = p.block_tables + (int64_t)b * p.max_blocks;
-  const int cu = p.cu_q[b];
+  const int key0 = SHARED ? lo : 0;                          // the first key of tile 0
 
   // Q tile: rows past nrows are zero
 #pragma unroll
@@ -309,18 +359,23 @@ __device__ __forceinline__ void multi_split(const Params& p, int window = 0) {
     const int row = i * (kThreads >> kQShift) + (tid >> kQShift), c = tid & ((1 << kQShift) - 1);
     const bool ok = row < nrows;
     const T* src = reinterpret_cast<const T*>(p.q);
-    if (ok) src += (int64_t)(cu + row / g_size) * p.q_st + (int64_t)(kvh * g_size + row % g_size) * p.q_sh + c * 8;
+    if (ok) {
+      int token;
+      if constexpr (SHARED) token = p.cu_q[p.group_seqs[m0 + row / g_size]];
+      else token = cu + row / g_size;
+      src += (int64_t)token * p.q_st + (int64_t)(kvh * g_size + row % g_size) * p.q_sh + c * 8;
+    }
     cp_async16(sbase + swz<D>(row, c), src, ok);
   }
-  // cached K / V rows of key tile `tile` into stage `st`; keys at or past len (and below lo) are zero-filled
+  // cached K / V rows of key tile `tile` into stage `st`; keys at or past hi (and below lo with WINDOW) are zero-filled
   auto load_kv = [&](int tile, int st) {
     constexpr int kEl = Q8 ? 16 : 8;                         // elements per 16-byte chunk
     constexpr int kChunks = D / kEl;
 #pragma unroll
     for (int i = 0; i < BN * kChunks / kThreads; ++i) {
       const int row = i * (kThreads / kChunks) + tid / kChunks, c = tid % kChunks;
-      const int pos = tile * BN + row;
-      const bool ok = WINDOW ? pos < len && pos >= lo : pos < len;
+      const int pos = key0 + tile * BN + row;
+      const bool ok = WINDOW ? pos < hi && pos >= lo : pos < hi;
       int64_t off = 0;
       if (ok) off = (((int64_t)bt[pos / p.block_size] * p.hkv + kvh) * p.block_size + pos % p.block_size) * D + c * kEl;
       if constexpr (Q8) {
@@ -334,7 +389,7 @@ __device__ __forceinline__ void multi_split(const Params& p, int window = 0) {
       }
     }
   };
-  if (t0 < t1) load_kv(t0, 0);
+  if (SHARED || t0 < t1) load_kv(t0, 0);                     // (a shared task with no tile has returned)
   cp_async_commit();
   if (t0 + 1 < t1) load_kv(t0 + 1, 1);
   cp_async_commit();
@@ -343,9 +398,11 @@ __device__ __forceinline__ void multi_split(const Params& p, int window = 0) {
   if constexpr (Q8) { qk_scale *= __ldg(p.k_dq + kvh); v_scale = __ldg(p.v_dq + kvh); }
   const bool active = warp * 16 < nrows;
   const int r_lo = warp * 16 + (lane >> 2);                  // this lane's two rows: r_lo and r_lo + 8
-  int limit[2];                                              // keys < limit are visible to the row
+  int limit[2];                                              // verify: keys < limit are visible to the row
+  if constexpr (!SHARED) {
 #pragma unroll
-  for (int hh = 0; hh < 2; ++hh) limit[hh] = min(len, past + (r_lo + hh * 8) / g_size + 1);
+    for (int hh = 0; hh < 2; ++hh) limit[hh] = min(hi, past + (r_lo + hh * 8) / g_size + 1);
+  }
   int lower[2] = {0, 0};                                     // ... and keys >= lower (WINDOW)
   if constexpr (WINDOW) {
 #pragma unroll
@@ -408,9 +465,10 @@ __device__ __forceinline__ void multi_split(const Params& p, int window = 0) {
         for (int n = 0; n < BN / 8; ++n)
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
-            const int key = t * BN + n * 8 + 2 * (lane & 3) + e;
+            const int key = key0 + t * BN + n * 8 + 2 * (lane & 3) + e;
             float& v = s[n][hh * 2 + e];
-            v = key < limit[hh] && (!WINDOW || key >= lower[hh]) ? v * qk_scale : -INFINITY;
+            const bool visible = SHARED ? key < hi : key < limit[hh] && (!WINDOW || key >= lower[hh]);   // SHARED: every key below hi
+            v = visible ? v * qk_scale : -INFINITY;
             mx = fmaxf(mx, v);
           }
         mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
@@ -449,8 +507,8 @@ __device__ __forceinline__ void multi_split(const Params& p, int window = 0) {
   }
   cp_async_wait<0>();
   if (!active) return;
-  // this split's partial for the warp's rows (an empty split writes m = -inf, l = 0, acc = 0)
-  const int64_t pbase = (((int64_t)b * p.hkv + kvh) * p.splits + split) * kRows;
+  // this split's partial for the warp's rows (an empty verify split writes m = -inf, l = 0, acc = 0)
+  if constexpr (!SHARED) pbase = (((int64_t)b * p.hkv + kvh) * p.splits + split) * kRows;
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
     float lq = l[hh];
@@ -495,15 +553,4 @@ __device__ __forceinline__ void multi_merge(const Params& p) {
 }
 
 }  // namespace decode_multi
-
-// The sliding-window launchers (attention_window.cu), called by decode_attention, decode_attention_paged_q8 and
-// decode_attention_paged_multi once they have checked their arguments.
-int decode_attention_window(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* out, float* part_acc, float* part_ml,
-                            int b, int h, int hkv, int smax, int d, int splits, float scale, int dtype, cudaStream_t s, const int* block_tables,
-                            int max_blocks, int block_size, int window);
-int decode_attention_paged_q8_window(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* out, float* part_acc,
-                                     float* part_ml, int b, int h, int hkv, int splits, float scale, int dtype, int kv_dtype, const float* k_dq,
-                                     const float* v_dq, const int* block_tables, int max_blocks, int block_size, int window, cudaStream_t s);
-int decode_attention_paged_multi_window(const decode_multi::Params& p, const PagedMultiArgs& a, cudaStream_t s);
-
 }  // namespace b200

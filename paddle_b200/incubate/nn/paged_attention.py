@@ -330,7 +330,7 @@ def block_attention(qkv, key_cache, value_cache, seq_lens_encoder, seq_lens_deco
     out_smooth (T [H * D], int8 output only) first replace o by ((o + shift) -> T) * smooth -> T.
 
     sliding_window = W (an int >= 1; None: off): local attention, the query at absolute position i sees key j iff i - W < j <= i.  Decode,
-    verify and prefill rows go to the windowed kernels of csrc/attention_window.cu, which read only the window's cache rows and never read
+    verify and prefill rows go to the windowed instantiations of the paged kernels, which read only the window's cache rows and never read
     the table entries of blocks wholly below it (those blocks may have been released and reused).  Not combinable with shared_prefix."""
     sliding_window = _check_window(sliding_window, shared_prefix)
     qkv, kc, vc = _raw(qkv), _raw(key_cache), _raw(value_cache)

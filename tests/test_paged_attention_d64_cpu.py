@@ -1,8 +1,7 @@
 """The head_dim 64 attention kernels, read from the built objects with `cuobjdump -sass`: no d 64 instantiation touches local memory,
-and every head_dim 128 instantiation in attention_sm100.cu and decode_attention.cu compiles to the instructions it compiled to before
-the head size became a template argument (tests/golden/attention_d128_sass.json: SHA-256 of each kernel's instructions, keyed by its
-demangled name with the trailing head-size template argument removed; the verify kernels keep their names and have head_dim 64
-instantiations of their own in decode_verify64)."""
+and every unwindowed head_dim 128 instantiation in attention_sm100.cu and decode_attention.cu compiles to the instructions it compiled
+to before the head size became a template argument (tests/golden/attention_d128_sass.json: SHA-256 of each kernel's instructions, keyed
+by its demangled name with the trailing head-size template argument, and the verify kernels' WINDOW = false after it, removed)."""
 import hashlib
 import json
 import os
@@ -19,7 +18,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden", "attention_d128_sass.json")
 pytestmark = pytest.mark.skipif(shutil.which("cuobjdump") is None or shutil.which("cu++filt") is None
                                 or not all(os.path.exists(o) for o in OBJS), reason="cuobjdump, cu++filt or the built objects are missing")
 
-HEAD = re.compile(r", \(int\)(64|128)>\(")   # the head size as the last template argument of a kernel
+HEAD = re.compile(r", \(int\)(64|128)(, \(bool\)0)?>\(")   # the head size as the last template argument of a kernel, or before WINDOW = false
 
 
 def sass_functions(objs=OBJS):
@@ -36,19 +35,23 @@ def sass_functions(objs=OBJS):
 
 
 def head_size(name):
-    if "::decode_verify64::" in name:                          # the head_dim 64 verify kernels
-        return 64
     m = HEAD.search(name)
     return int(m.group(1)) if m else None
 
 
+def windowed(name):
+    """A sliding-window kernel (their instructions are checked by test_paged_attention_sass_cpu.py)."""
+    return "_window_kernel" in name or ", (bool)1>(" in name
+
+
 def d128_digests(funcs):
-    """SHA-256 of every kernel that is not a head_dim 64 instantiation, keyed by its name without the head-size argument."""
-    return {HEAD.sub(">(", n): hashlib.sha256("\n".join(ins).encode()).hexdigest() for n, ins in funcs.items() if head_size(n) != 64}
+    """SHA-256 of every unwindowed kernel that is not a head_dim 64 instantiation, keyed by its name without the head-size argument."""
+    return {HEAD.sub(">(", n): hashlib.sha256("\n".join(ins).encode()).hexdigest() for n, ins in funcs.items()
+            if head_size(n) != 64 and not windowed(n)}
 
 
-def test_d64_kernels_use_no_local_memory():
-    d64 = {n: ins for n, ins in sass_functions().items() if head_size(n) == 64}
+def test_unwindowed_d64_kernels_use_no_local_memory():
+    d64 = {n: ins for n, ins in sass_functions().items() if head_size(n) == 64 and not windowed(n)}
     # decode split / merge, verify split / merge, paged prefill: bf16 and fp16 each
     kinds = ("decode_split_kernel", "decode_merge_kernel", "multi_split_kernel", "multi_merge_kernel", "fwd_kernel")
     assert sorted(sum(k + "<" in n for n in d64) for k in kinds) == [2] * len(kinds), sorted(d64)
@@ -56,7 +59,7 @@ def test_d64_kernels_use_no_local_memory():
         assert not any(re.search(r"\b(LDL|STL)\b", i) for i in ins), n
 
 
-def test_d128_kernels_compile_as_before():
+def test_unwindowed_d128_kernels_compile_as_before():
     with open(GOLDEN) as f:
         golden = json.load(f)
     assert d128_digests(sass_functions()) == golden

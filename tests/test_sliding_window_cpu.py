@@ -1,6 +1,6 @@
 """Sliding-window attention without a GPU: block_attention's reference under a window against dense masked attention, the argument checks,
 LlamaForCausalLM with a window against an explicit-mask forward, LLMEngine's block release against generate(), and the windowed kernels
-in the built attention_window object (no local memory, pipelined wgmma)."""
+in the built attention objects (no local memory, pipelined wgmma)."""
 import math
 import os
 import re
@@ -15,7 +15,7 @@ from paddle_b200 import models
 from paddle_b200.incubate.nn.paged_attention import _block_attention_ref, block_attention
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-WINDOW_OBJ = os.path.join(ROOT, "paddle_b200", "_build_cache", "attention_window.cuda.o")
+WINDOW_OBJS = [os.path.join(ROOT, "paddle_b200", "_build_cache", f) for f in ("attention_sm100.cuda.o", "decode_attention.cuda.o")]
 
 
 def _dense(q, k, v, window):
@@ -228,18 +228,31 @@ def test_engine_window_rejects_prefix_caching():
         models.LLMEngine(m, num_blocks=8, block_size=4, enable_prefix_caching=True)
 
 
-@pytest.mark.skipif(shutil.which("cuobjdump") is None or not os.path.exists(WINDOW_OBJ), reason="cuobjdump or the built object is missing")
-def test_window_kernels_use_no_local_memory_and_keep_wgmma_pipelined():
-    sass = subprocess.run(["cuobjdump", "-sass", WINDOW_OBJ], capture_output=True, text=True, check=True).stdout
+@pytest.mark.skipif(shutil.which("cuobjdump") is None or not all(os.path.exists(o) for o in WINDOW_OBJS),
+                    reason="cuobjdump or the built objects are missing")
+def test_windowed_launches_use_no_local_memory_and_keep_wgmma_pipelined():
     funcs = {}
-    for f in re.split(r"\n\s*Function : ", sass)[1:]:
-        name, body = f.split("\n", 1)
-        funcs[name.strip()] = body
-    kinds = {"decode_split_window_kernel": 4, "decode_split_q8_window_kernel": 4, "decode_merge_window_kernel": 4,
-             "multi_split_window_kernel": 8, "multi_merge_window_kernel": 4, "paged_work_window_kernel": 1, "fwd_window_kernel": 8}
-    for k, n in kinds.items():
-        assert sum(k in name for name in funcs) == n, (k, sorted(funcs))
+    for obj in WINDOW_OBJS:
+        sass = subprocess.run(["cuobjdump", "-sass", obj], capture_output=True, text=True, check=True).stdout
+        for f in re.split(r"\n\s*Function : ", sass)[1:]:
+            name, body = f.split("\n", 1)
+            funcs[name.strip()] = body
+    # the kernels a windowed call launches, by mangled name: windowed verify splits carry WINDOW = true (Lb1E) after the head size, and
+    # windowed decode and verify merge their splits with the unwindowed merge kernels
+    kinds = {"decode_split_window_kernel": lambda n: "decode_split_window_kernel" in n,
+             "decode_split_q8_window_kernel": lambda n: "decode_split_q8_window_kernel" in n,
+             "decode_merge_kernel": lambda n: "decode_merge_kernel" in n,
+             "multi_split_kernel (WINDOW)": lambda n: "multi_split_kernel" in n and re.search(r"Li(64|128)ELb1E", n) is not None,
+             "multi_merge_kernel": lambda n: "multi_merge_kernel" in n,
+             "paged_work_window_kernel": lambda n: "paged_work_window_kernel" in n,
+             "fwd_window_kernel": lambda n: "fwd_window_kernel" in n}
+    counts = {"decode_split_window_kernel": 4, "decode_split_q8_window_kernel": 4, "decode_merge_kernel": 4, "multi_split_kernel (WINDOW)": 8,
+              "multi_merge_kernel": 4, "paged_work_window_kernel": 1, "fwd_window_kernel": 8}
+    for k, n in counts.items():
+        assert sum(kinds[k](name) for name in funcs) == n, (k, sorted(funcs))
     for name, body in funcs.items():
+        if not any(is_kind(name) for is_kind in kinds.values()):
+            continue
         assert not re.search(r"\b(LDL|STL)\b", body), name
         if "fwd_window_kernel" in name:
             mma = len(re.findall(r"\bHGMMA\.", body))

@@ -176,12 +176,13 @@ def test_engine_verify_logits_match_plain_decode():
     assert checked >= 2
 
 
-def test_multi_decode_kernels_use_no_local_memory():
+def test_verify_kernels_of_every_head_size_and_window_use_no_local_memory():
     obj = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "paddle_b200", "_build_cache", "decode_attention.cuda.o")
     sass = subprocess.run(["cuobjdump", "-sass", obj], capture_output=True, text=True, check=True).stdout
     funcs = re.split(r"\n\s*Function : ", sass)[1:]
     multi = [f for f in funcs if "decode_multi" in f.split("\n", 1)[0]]
-    assert len(multi) == 8                                        # split kernels (2 dtypes x 16-bit / int8 / fp8) and 2 merge kernels
+    # split kernels (2 dtypes x (16-bit / int8 / fp8 at head_dim 128, 16-bit at 64) x unwindowed / windowed) and 4 merge kernels
+    assert len(multi) == 20
     for f in multi:
         name = f.split("\n", 1)[0]
         assert not re.search(r"\b(LDL|STL)\b", f), name
