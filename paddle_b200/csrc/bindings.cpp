@@ -604,61 +604,90 @@ Tensor moe_rows_dot(const Tensor& src, const Tensor& dest, const Tensor& g, int6
   return dw;
 }
 
+// ---- weight-only GEMM and dequantisation.  Failing checks use literal messages only: with this extension's host toolchain a failing
+// TORCH_CHECK that formats an integer aborts instead of raising.  experts: every weight operand carries a leading [E].
+
+// w int8 [N, K] (int4 packed [N, K/2]) contiguous and non-empty on a CUDA device, and its scales fp32 [N] per channel (group_size <= 0)
+// or [K / group_size, N], contiguous on w's device.  Messages name `op`.  Returns K.
+int64_t check_wo_weight(const char* op, const Tensor& w, const Tensor& scale, bool int4, int64_t group_size, bool experts) {
+  const char* lead = experts ? "E, " : "";
+  TORCH_CHECK(w.is_cuda() && w.dim() == (experts ? 3 : 2) && w.is_contiguous() && w.scalar_type() == at::kChar && w.numel() > 0,
+              op, ": w int8 [", lead, "N, K] (int4: [", lead, "N, K/2]) contiguous");
+  const int64_t n = w.size(-2), k = int4 ? 2 * w.size(-1) : w.size(-1);
+  const bool scale_ok = scale.scalar_type() == at::kFloat && scale.is_contiguous();
+  if (group_size <= 0) {
+    TORCH_CHECK(scale_ok && (experts ? scale.dim() == 2 && scale.size(0) == w.size(0) && scale.size(1) == n : scale.numel() == n),
+                op, ": scale float32 [", lead, "N] contiguous");
+  } else {
+    TORCH_CHECK(k % group_size == 0, op, ": K is not a multiple of group_size");
+    TORCH_CHECK(scale_ok && scale.dim() == (experts ? 3 : 2) && (!experts || scale.size(0) == w.size(0)) && scale.size(-2) == k / group_size &&
+                scale.size(-1) == n, op, ": scale float32 [", lead, "K / group_size, N] contiguous");
+  }
+  TORCH_CHECK(scale.device() == w.device(), op, ": w and scale on one device");
+  return k;
+}
+
+// The operands of weight_only_gemm and weight_only_gemm_experts: x [M, K] bf16 / fp16 contiguous on a CUDA device, w and scale as in
+// check_wo_weight with group_size -1, 64 or 128, bias [N] in x's dtype or None, every operand on x's device, and E, N, K, M in range.
+void check_wo_operands(const char* op, const Tensor& x, const Tensor& w, const Tensor& scale, const OptT& bias, bool int4, int64_t group_size,
+                       bool experts) {
+  const char* lead = experts ? "E, " : "";
+  TORCH_CHECK(x.is_cuda() && x.dim() == 2 && x.is_contiguous() && (x.scalar_type() == at::kBFloat16 || x.scalar_type() == at::kHalf),
+              op, ": x [M, K] bf16 / fp16 contiguous");
+  TORCH_CHECK(group_size <= 0 || group_size == 64 || group_size == 128, op, ": group_size must be -1, 64 or 128");
+  const int64_t K = check_wo_weight(op, w, scale, int4, group_size, experts), N = w.size(-2), E = experts ? w.size(0) : 1;
+  TORCH_CHECK(x.size(1) == K, op, ": x [M, K] and w [", lead, "N, K] (int4: [", lead, "N, K/2]) disagree on K");
+  TORCH_CHECK(E <= 1024 && K < (int64_t)1 << 30 && N < (int64_t)1 << 30 && x.size(0) > 0 && x.size(0) < (int64_t)1 << 30, op, ": dimensions out of range");
+  if (bias.has_value() && bias->defined())
+    TORCH_CHECK(bias->is_cuda() && bias->scalar_type() == x.scalar_type() && bias->numel() == E * N && bias->is_contiguous(),
+                op, ": bias [", lead, "N] contiguous CUDA tensor in x dtype");
+  TORCH_CHECK(w.device() == x.device() && (!bias.has_value() || !bias->defined() || bias->device() == x.device()), op, ": all operands on one device");
+}
+
+// the arguments of gemm_weight_only for checked operands; the expert binding adds its plan
+b200::WoGemmArgs wo_gemm_args(const Tensor& x, const Tensor& w, const Tensor& scale, const OptT& bias, const Tensor& out, bool int4, int64_t group_size) {
+  b200::WoGemmArgs g;
+  g.m = (int)x.size(0); g.k = (int)x.size(1); g.n = (int)w.size(-2);
+  g.x = x.data_ptr(); g.w = w.data_ptr(); g.scale = scale.data_ptr<float>(); g.out = out.data_ptr();
+  g.bias = bias.has_value() && bias->defined() ? bias->data_ptr() : nullptr;
+  g.int4 = int4 ? 1 : 0; g.bf16 = x.scalar_type() == at::kBFloat16 ? 1 : 0;
+  g.group_size = group_size > 0 ? (int)group_size : 0;
+  return g;
+}
+
 // x [M, K] bf16 / fp16, w int8 [N, K] (or int4 packed [N, K/2]), scale float [N] (group_size <= 0) or [K / group_size, N] (64 / 128),
 // bias [N] or None -> [M, N]
 Tensor weight_only_gemm(const Tensor& x, const Tensor& w, const Tensor& scale, const OptT& bias, bool int4, int64_t group_size) {
-  TORCH_CHECK(x.is_cuda() && x.dim() == 2 && x.is_contiguous() && (x.scalar_type() == at::kBFloat16 || x.scalar_type() == at::kHalf), "weight_only_gemm: x [M, K] bf16 / fp16 contiguous");
-  TORCH_CHECK(w.is_cuda() && w.dim() == 2 && w.is_contiguous() && w.scalar_type() == at::kChar && w.size(1) == (int4 ? x.size(1) / 2 : x.size(1)), "weight_only_gemm: w int8 [N, K] (int4: [N, K/2])");
-  if (group_size <= 0) {
-    TORCH_CHECK(scale.is_cuda() && scale.scalar_type() == at::kFloat && scale.numel() == w.size(0) && scale.is_contiguous(), "weight_only_gemm: scale float32 [N]");
-  } else {
-    // literal messages: with this extension's host toolchain a failing TORCH_CHECK that formats an integer aborts instead of raising
-    TORCH_CHECK(group_size == 64 || group_size == 128, "weight_only_gemm: group_size must be -1, 64 or 128");
-    TORCH_CHECK(x.size(1) % group_size == 0, "weight_only_gemm: K is not a multiple of group_size");
-    TORCH_CHECK(scale.is_cuda() && scale.scalar_type() == at::kFloat && scale.dim() == 2 && scale.size(0) == x.size(1) / group_size && scale.size(1) == w.size(0) && scale.is_contiguous(),
-                "weight_only_gemm: scale float32 [K / group_size, N] contiguous");
-  }
+  check_wo_operands("weight_only_gemm", x, w, scale, bias, int4, group_size, false);
   c10::cuda::CUDAGuard guard(x.device());
-  b200::WoGemmArgs g;
-  g.m = (int)x.size(0); g.k = (int)x.size(1); g.n = (int)w.size(0);
-  Tensor out = torch::empty({g.m, g.n}, x.options());
-  g.x = x.data_ptr(); g.w = w.data_ptr(); g.scale = scale.data_ptr<float>(); g.out = out.data_ptr();
-  g.bias = nullptr;
-  if (bias.has_value() && bias->defined()) { TORCH_CHECK(bias->scalar_type() == x.scalar_type() && bias->numel() == g.n && bias->is_contiguous(), "weight_only_gemm: bias [N] in x dtype"); g.bias = bias->data_ptr(); }
-  g.int4 = int4 ? 1 : 0; g.bf16 = x.scalar_type() == at::kBFloat16 ? 1 : 0;
-  g.group_size = group_size > 0 ? (int)group_size : 0;
-  int rc = b200::gemm_weight_only(g, cur_stream());
+  Tensor out = torch::empty({x.size(0), w.size(0)}, x.options());
+  int rc = b200::gemm_weight_only(wo_gemm_args(x, w, scale, bias, out, int4, group_size), cur_stream());
   g_launches += 1;
   check_err();
   TORCH_CHECK(rc == 0, "paddle_b200.weight_only_gemm: unsupported shape (K multiple of 64, N multiple of 8, M <= 64, 16-byte aligned)");
   return out;
 }
 
-// w int8 [N, K] (int4 packed [N, K/2]), scale float [N] or [K / group_size, N] -> [K, N] in out_dtype (bf16 / fp16 / fp32); one launch
-Tensor weight_dequantize(const Tensor& w, const Tensor& scale, bool int4, int64_t group_size, at::ScalarType out_dtype) {
-  TORCH_CHECK(w.is_cuda() && w.dim() == 2 && w.is_contiguous() && w.scalar_type() == at::kChar && w.numel() > 0, "weight_dequantize: w int8 [N, K] (int4: [N, K/2]) contiguous");
-  TORCH_CHECK(out_dtype == at::kBFloat16 || out_dtype == at::kHalf || out_dtype == at::kFloat, "weight_dequantize: out_dtype bf16 / fp16 / fp32");
-  const int64_t n = w.size(0), k = int4 ? 2 * w.size(1) : w.size(1);
-  TORCH_CHECK(n < (int64_t)1 << 31 && k < (int64_t)1 << 31, "weight_dequantize: dimensions too large");
-  if (group_size <= 0) {
-    TORCH_CHECK(scale.is_cuda() && scale.scalar_type() == at::kFloat && scale.numel() == n && scale.is_contiguous(), "weight_dequantize: scale float32 [N]");
-  } else {
-    TORCH_CHECK(k % group_size == 0, "weight_dequantize: K is not a multiple of group_size");
-    TORCH_CHECK(scale.is_cuda() && scale.scalar_type() == at::kFloat && scale.dim() == 2 && scale.size(0) == k / group_size && scale.size(1) == n && scale.is_contiguous(),
-                "weight_dequantize: scale float32 [K / group_size, N] contiguous");
-  }
-  TORCH_CHECK(scale.device() == w.device(), "weight_dequantize: w and scale on one device");
+// w int8 [(E,) N, K] (int4 packed [(E,) N, K/2]), scale float [(E,) N] or [(E,) K / group_size, N] -> [(E,) K, N] in out_dtype (bf16 / fp16 /
+// fp32); one launch for all experts, every expert bit-equal to weight_dequantize of its slice
+Tensor dequantize_wo(const char* op, const Tensor& w, const Tensor& scale, bool int4, int64_t group_size, at::ScalarType out_dtype, bool experts) {
+  TORCH_CHECK(out_dtype == at::kBFloat16 || out_dtype == at::kHalf || out_dtype == at::kFloat, op, ": out_dtype bf16 / fp16 / fp32");
+  const int64_t k = check_wo_weight(op, w, scale, int4, group_size, experts), n = w.size(-2), E = experts ? w.size(0) : 1;
+  TORCH_CHECK(E <= 65535 && n < (int64_t)1 << 31 && k < (int64_t)1 << 31, op, ": dimensions too large");
   c10::cuda::CUDAGuard guard(w.device());
-  Tensor out = torch::empty({k, n}, w.options().dtype(out_dtype));
+  Tensor out = experts ? torch::empty({E, k, n}, w.options().dtype(out_dtype)) : torch::empty({k, n}, w.options().dtype(out_dtype));
   int rc = b200::weight_dequantize(w.data_ptr(), scale.data_ptr<float>(), out.data_ptr(), (int)n, (int)k, int4 ? 1 : 0, group_size > 0 ? (int)group_size : 0,
-                                   dt_code(out_dtype), cur_stream());
+                                   dt_code(out_dtype), cur_stream(), (int)E);
   g_launches += 1;
   check_err();
-  TORCH_CHECK(rc == 0, "paddle_b200.weight_dequantize: unsupported shape");
+  TORCH_CHECK(rc == 0, "paddle_b200.", op, ": unsupported shape");
   return out;
 }
+Tensor weight_dequantize(const Tensor& w, const Tensor& scale, bool int4, int64_t group_size, at::ScalarType out_dtype) {
+  return dequantize_wo("weight_dequantize", w, scale, int4, group_size, out_dtype, false);
+}
 
-// ---- weight-only MoE experts.  Failing checks use literal messages only (see weight_only_gemm).
+// ---- weight-only MoE experts.  Failing checks use literal messages only, as above.
 // expert ids of the token slots ([S] int64, -1 = dropped) -> (dest int32 [S], offsets int32 [E + 1], work int32 [1 + 2 * items]): the
 // compact plan of weight_only_gemm_experts for S rows.  Three launches (count, plan, dest), no host read.
 std::vector<Tensor> moe_wo_plan(const Tensor& idx, int64_t n_expert) {
@@ -683,75 +712,29 @@ std::vector<Tensor> moe_wo_plan(const Tensor& idx, int64_t n_expert) {
 // bias [E, N] in xp's dtype or None, offsets / work from moe_wo_plan over R slots -> out [R, N]; rows past offsets[E] are left unwritten
 Tensor weight_only_gemm_experts(const Tensor& xp, const Tensor& w, const Tensor& scale, const OptT& bias, const Tensor& offsets, const Tensor& work,
                                 bool int4, int64_t group_size) {
-  TORCH_CHECK(xp.is_cuda() && xp.dim() == 2 && xp.is_contiguous() && (xp.scalar_type() == at::kBFloat16 || xp.scalar_type() == at::kHalf),
-              "weight_only_gemm_experts: xp [R, K] bf16 / fp16 contiguous");
-  TORCH_CHECK(w.is_cuda() && w.dim() == 3 && w.is_contiguous() && w.scalar_type() == at::kChar && w.size(2) == (int4 ? xp.size(1) / 2 : xp.size(1)),
-              "weight_only_gemm_experts: w int8 [E, N, K] (int4: [E, N, K/2]) contiguous");
-  const int64_t E = w.size(0), N = w.size(1), K = xp.size(1);
-  TORCH_CHECK(E > 0 && E <= 1024 && N > 0 && K < (int64_t)1 << 30 && N < (int64_t)1 << 30 && xp.size(0) > 0 && xp.size(0) < (int64_t)1 << 30,
-              "weight_only_gemm_experts: dimensions out of range");
-  if (group_size <= 0) {
-    TORCH_CHECK(scale.is_cuda() && scale.scalar_type() == at::kFloat && scale.dim() == 2 && scale.size(0) == E && scale.size(1) == N && scale.is_contiguous(),
-                "weight_only_gemm_experts: scale float32 [E, N] contiguous");
-  } else {
-    TORCH_CHECK(group_size == 64 || group_size == 128, "weight_only_gemm_experts: group_size must be -1, 64 or 128");
-    TORCH_CHECK(K % group_size == 0, "weight_only_gemm_experts: K is not a multiple of group_size");
-    TORCH_CHECK(scale.is_cuda() && scale.scalar_type() == at::kFloat && scale.dim() == 3 && scale.size(0) == E && scale.size(1) == K / group_size &&
-                scale.size(2) == N && scale.is_contiguous(), "weight_only_gemm_experts: scale float32 [E, K / group_size, N] contiguous");
-  }
-  const int m = (int)xp.size(0), ntok = b200::wo_expert_ntok(m);
+  const char* op = "weight_only_gemm_experts";
+  check_wo_operands(op, xp, w, scale, bias, int4, group_size, true);
+  const int64_t E = w.size(0);
+  const int m = (int)xp.size(0);
   TORCH_CHECK(offsets.is_cuda() && offsets.scalar_type() == at::kInt && offsets.is_contiguous() && offsets.numel() == E + 1,
-              "weight_only_gemm_experts: offsets int32 [E + 1] from moe_wo_plan");
-  TORCH_CHECK(work.is_cuda() && work.scalar_type() == at::kInt && work.is_contiguous() && work.numel() == 1 + 2 * (int64_t)b200::wo_expert_items(m, (int)E, ntok),
-              "weight_only_gemm_experts: work must come from moe_wo_plan over the rows of xp");
-  TORCH_CHECK(w.device() == xp.device() && scale.device() == xp.device() && offsets.device() == xp.device() && work.device() == xp.device(),
-              "weight_only_gemm_experts: all operands on one device");
+              op, ": offsets int32 [E + 1] from moe_wo_plan");
+  TORCH_CHECK(work.is_cuda() && work.scalar_type() == at::kInt && work.is_contiguous() &&
+              work.numel() == 1 + 2 * (int64_t)b200::wo_expert_items(m, (int)E, b200::wo_expert_ntok(m)),
+              op, ": work must come from moe_wo_plan over the rows of xp");
+  TORCH_CHECK(offsets.device() == xp.device() && work.device() == xp.device(), op, ": all operands on one device");
   c10::cuda::CUDAGuard guard(xp.device());
-  b200::WoExpertGemmArgs g;
-  g.m = m; g.n = (int)N; g.k = (int)K; g.experts = (int)E; g.ntok = ntok;
-  Tensor out = torch::empty({m, N}, xp.options());
-  g.x = xp.data_ptr(); g.w = w.data_ptr(); g.scale = scale.data_ptr<float>(); g.out = out.data_ptr();
-  g.offsets = offsets.data_ptr<int>(); g.work = work.data_ptr<int>();
-  g.bias = nullptr;
-  if (bias.has_value() && bias->defined()) {
-    TORCH_CHECK(bias->is_cuda() && bias->scalar_type() == xp.scalar_type() && bias->numel() == E * N && bias->is_contiguous(),
-                "weight_only_gemm_experts: bias [E, N] in xp dtype contiguous");
-    g.bias = bias->data_ptr();
-  }
-  g.int4 = int4 ? 1 : 0; g.bf16 = xp.scalar_type() == at::kBFloat16 ? 1 : 0;
-  g.group_size = group_size > 0 ? (int)group_size : 0;
-  int rc = b200::gemm_weight_only_experts(g, cur_stream());
+  Tensor out = torch::empty({m, w.size(1)}, xp.options());
+  b200::WoGemmArgs g = wo_gemm_args(xp, w, scale, bias, out, int4, group_size);
+  g.experts = (int)E; g.offsets = offsets.data_ptr<int>(); g.work = work.data_ptr<int>();
+  int rc = b200::gemm_weight_only(g, cur_stream());
   g_launches += 1;
   check_err();
   TORCH_CHECK(rc == 0, "paddle_b200.weight_only_gemm_experts: unsupported shape (K multiple of 64, N multiple of 8, 16-byte aligned)");
   return out;
 }
 
-// w int8 [E, N, K] (int4 [E, N, K/2]), scale fp32 [E, N] or [E, K / group_size, N] -> [E, K, N] in out_dtype; one launch for all experts,
-// every expert bit-equal to weight_dequantize of its slice
 Tensor weight_dequantize_experts(const Tensor& w, const Tensor& scale, bool int4, int64_t group_size, at::ScalarType out_dtype) {
-  TORCH_CHECK(w.is_cuda() && w.dim() == 3 && w.is_contiguous() && w.scalar_type() == at::kChar && w.numel() > 0,
-              "weight_dequantize_experts: w int8 [E, N, K] (int4: [E, N, K/2]) contiguous");
-  TORCH_CHECK(out_dtype == at::kBFloat16 || out_dtype == at::kHalf || out_dtype == at::kFloat, "weight_dequantize_experts: out_dtype bf16 / fp16 / fp32");
-  const int64_t E = w.size(0), n = w.size(1), k = int4 ? 2 * w.size(2) : w.size(2);
-  TORCH_CHECK(E <= 65535 && n < (int64_t)1 << 31 && k < (int64_t)1 << 31, "weight_dequantize_experts: dimensions too large");
-  if (group_size <= 0) {
-    TORCH_CHECK(scale.is_cuda() && scale.scalar_type() == at::kFloat && scale.dim() == 2 && scale.size(0) == E && scale.size(1) == n && scale.is_contiguous(),
-                "weight_dequantize_experts: scale float32 [E, N] contiguous");
-  } else {
-    TORCH_CHECK(k % group_size == 0, "weight_dequantize_experts: K is not a multiple of group_size");
-    TORCH_CHECK(scale.is_cuda() && scale.scalar_type() == at::kFloat && scale.dim() == 3 && scale.size(0) == E && scale.size(1) == k / group_size &&
-                scale.size(2) == n && scale.is_contiguous(), "weight_dequantize_experts: scale float32 [E, K / group_size, N] contiguous");
-  }
-  TORCH_CHECK(scale.device() == w.device(), "weight_dequantize_experts: w and scale on one device");
-  c10::cuda::CUDAGuard guard(w.device());
-  Tensor out = torch::empty({E, k, n}, w.options().dtype(out_dtype));
-  int rc = b200::weight_dequantize(w.data_ptr(), scale.data_ptr<float>(), out.data_ptr(), (int)n, (int)k, int4 ? 1 : 0, group_size > 0 ? (int)group_size : 0,
-                                   dt_code(out_dtype), cur_stream(), (int)E);
-  g_launches += 1;
-  check_err();
-  TORCH_CHECK(rc == 0, "paddle_b200.weight_dequantize_experts: unsupported shape");
-  return out;
+  return dequantize_wo("weight_dequantize_experts", w, scale, int4, group_size, out_dtype, true);
 }
 
 // D = act(scale * A[M,K] @ B[N,K]^T + bias), A/B fp8 (e4m3 / e5m2), D half / bf16 / fp32

@@ -96,7 +96,7 @@ void moe_prune_gate(const int64_t* idx, int64_t n, int64_t* remaining, int64_t* 
 void moe_plan(const int64_t* counts, int n_expert, int n_tiles, int* seg_start, int* cursor, int* tile_expert, int* k0, int* kb, cudaStream_t s);
 void moe_dest(const int64_t* idx, int64_t n, int* cursor, int* dest, cudaStream_t s);
 // compact plan of the weight-only expert GEMM: offsets[E + 1] (no padding), cursor[e] = offsets[e], and the work list of
-// gemm_weight_only_experts for ntok-row tiles (work[0] = item count, then (expert, first row) pairs)
+// gemm_weight_only for ntok-row tiles (work[0] = item count, then (expert, first row) pairs)
 void moe_wo_plan(const int64_t* counts, int n_expert, int ntok, int* offsets, int* cursor, int* work, cudaStream_t s);
 void moe_rows_scatter(const void* src, const int* dest, const float* scale, int64_t n_slots, int topk, int d, void* dst, int dtype, cudaStream_t s);
 void moe_rows_combine(const void* src, const int* dest, const float* w, int64_t n_tok, int topk, int d, void* out, int dtype, cudaStream_t s);
@@ -193,27 +193,23 @@ void fp8_cast_transpose(const void* x, int64_t m, int64_t k, int dtype, const fl
 
 // ---- gemm_wo_sm100.cu: weight-only quantised GEMM (dequantisation inside the SM) ---------------------------------
 // out[m, n] = x[m, k] @ dequant(w)[n, k]^T * scale[n] (+ bias[n]).  w: int8 [n, k] or packed int4 [n, k / 2] (low nibble = even k).
+// MoE experts (work != nullptr): out[m, n] = x[m, k] @ dequant(w[e])^T (+ bias[e]) for the rows offsets[e] .. offsets[e + 1] of every
+// expert e.  w: int8 [experts, n, k] or int4 [experts, n, k / 2]; scale fp32 [experts, n] or [experts, k / group_size, n]; bias
+// [experts, n] or nullptr.  work (device int32): [0] = item count, then one (expert, first row) pair per wo_expert_ntok(m)-row tile of an
+// expert (moe_wo_plan); the launch reserves wo_expert_items(m, experts, wo_expert_ntok(m)) items.
 struct WoGemmArgs {
   const void* x; const void* w; const float* scale; const void* bias; void* out;
   int m, n, k;
   int int4, bf16;   // weight format; activation dtype (1 bf16, 0 fp16)
   int group_size;   // <= 0: scale [n] per channel; 64 / 128: scale [k / group_size, n]
+  int experts = 0;
+  const int* offsets = nullptr;   // [experts + 1] first row of every expert
+  const int* work = nullptr;
 };
 int gemm_weight_only(const WoGemmArgs& g, cudaStream_t s);
-// MoE experts: out[m, n] = x[m, k] @ dequant(w[e])^T (+ bias[e]) for the rows offsets[e] .. offsets[e + 1] of every expert e.
-// w: int8 [experts, n, k] or int4 [experts, n, k / 2]; scale fp32 [experts, n] or [experts, k / group_size, n]; bias [experts, n] or nullptr.
-// work (device int32): [0] = item count, then one (expert, first row) pair per ntok-row tile of an expert (moe_wo_plan); the launch
-// reserves wo_expert_items(m, experts, ntok) items.
-struct WoExpertGemmArgs {
-  const void* x; const void* w; const float* scale; const void* bias; void* out;
-  const int* offsets; const int* work;
-  int m, n, k, experts, ntok;
-  int int4, bf16, group_size;
-};
-int gemm_weight_only_experts(const WoExpertGemmArgs& g, cudaStream_t s);
 // static bound of the work items of m rows over `experts` experts in ntok-row tiles: every non-empty expert adds at most one partial tile
 inline int wo_expert_items(int m, int experts, int ntok) { return m / ntok + (experts < m ? experts : m); }
-// token tile of m routed rows: 16 for decode batches, else 64
+// token tile of the weight-only GEMM over m rows (dense or routed): 16 for decode batches, else 64
 inline int wo_expert_ntok(int64_t m) { return m <= 16 ? 16 : 64; }
 // w [n, k] int8 (int4: [n, k / 2], low nibble = even k) -> out [k, n] = float(q) * scale, rounded once to out_dtype (kBF16 / kF16 / kF32).
 // scale fp32: [n] (group_size <= 0) or [k / group_size, n].  experts > 1: stacked w [experts, n, k], scale [experts, ...] -> [experts, k, n].

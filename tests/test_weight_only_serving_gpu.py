@@ -1,12 +1,7 @@
 """Group-wise weight-only GEMM (csrc/gemm_wo_sm100.cu, group_size 64 / 128) against an fp64 product of the dequantised weight, the
-one-pass dequantisation kernel bit for bit against the torch expression, the per-channel instantiations' unchanged SASS, and LLMEngine
-serving an int4-g128 Llama: decode steps on the in-SM kernel, larger steps on dequantise + GEMM (needs a GPU)."""
+one-pass dequantisation kernel bit for bit against the torch expression, the bindings' operand checks, and LLMEngine serving an
+int4-g128 Llama: decode steps on the in-SM kernel, larger steps on dequantise + GEMM (needs a GPU)."""
 import copy
-import hashlib
-import json
-import os
-import re
-import subprocess
 
 import pytest
 import torch
@@ -18,7 +13,6 @@ from test_paged_prefill_gpu import rel_err
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 # k = 1408: 22 k-blocks (ragged int4 raw boxes, uneven split ranks); 5120: many ring phases; 11008 x 256: few channel tiles, cluster split-K.
 # n = 1000: a partial channel tile.
 SHAPES = [(1408, 1000), (1408, 1536), (5120, 1000), (5120, 1536), (11008, 256)]
@@ -87,35 +81,38 @@ def test_binding_checks_the_scale_for_each_mode():
         C.weight_dequantize(w[:, :192].contiguous(), torch.ones(1, 64, device="cuda"), False, 128, torch.bfloat16)
 
 
-def _sass_functions():
-    obj = os.path.join(ROOT, "paddle_b200", "_build_cache", "gemm_wo_sm100.cuda.o")
-    sass = subprocess.run(["cuobjdump", "-sass", obj], capture_output=True, text=True, check=True).stdout
-    out = {}
-    for f in re.split(r"\n\s*Function : ", sass)[1:]:
-        name, body = f.split("\n", 1)
-        out[name.strip()] = [re.sub(r"/\*[0-9a-f]{4}\*/", "", ln).strip() for ln in body.split("\n") if re.search(r"/\*[0-9a-f]{4}\*/", ln)]
-    return out
+def _expert_operands(dev):
+    """A 2-expert weight_only_gemm_experts call on `dev`: xp, w, scale, bias, offsets, work (the plan of 4 routed rows)."""
+    C = _build.ext()
+    _, offsets, work = C.moe_wo_plan(torch.tensor([0, 1, 1, 0], device=dev), 2)
+    return (torch.randn(4, 256, device=dev, dtype=torch.bfloat16), torch.zeros(2, 64, 256, device=dev, dtype=torch.int8),
+            torch.ones(2, 64, device=dev), torch.zeros(2, 64, device=dev, dtype=torch.bfloat16), offsets, work)
 
 
-def test_wo_kernels_sass():
-    funcs = _sass_functions()
-    per_channel, grouped = {}, []
-    for name, ins in funcs.items():
-        mt = re.search(r"wo_gemm_kernelI((?:L[ib]\d+E)+)E", name)
-        if mt is None:
-            continue
-        ntok, wst, int4, bf16, gs = (int(v) for v in re.findall(r"L[ib](\d+)E", mt.group(1)))
-        if gs == 0:
-            per_channel[f"NTOK={ntok},WST={wst},INT4={int4},BF16={bf16}"] = hashlib.sha256("\n".join(ins).encode()).hexdigest()
-        else:
-            grouped.append(name)
-    assert len(grouped) == 2 * 2 * 2 * 2                             # token tile x int8 / int4 x bf16 / fp16 x group 64 / 128
-    for name, ins in funcs.items():
-        if "wo_gemm_kernel" in name or "wo_dequant_kernel" in name:
-            assert not any(re.search(r"\b(LDL|STL)\b", i) for i in ins), name
-    # the per-channel instantiations compile to the instructions they compiled to before group-wise scales were added
-    with open(os.path.join(ROOT, "tests", "golden", "wo_gemm_per_channel_sass.json")) as f:
-        assert per_channel == json.load(f)
+def test_bindings_reject_a_cpu_bias():
+    C = _build.ext()
+    x = torch.randn(4, 256, device="cuda", dtype=torch.bfloat16)
+    w = torch.zeros(64, 256, device="cuda", dtype=torch.int8)
+    with pytest.raises(RuntimeError, match="bias"):
+        C.weight_only_gemm(x, w, torch.ones(64, device="cuda"), torch.zeros(64, dtype=torch.bfloat16), False, -1)
+    xp, w3, s3, b3, offsets, work = _expert_operands("cuda")
+    with pytest.raises(RuntimeError, match="bias"):
+        C.weight_only_gemm_experts(xp, w3, s3, b3.cpu(), offsets, work, False, -1)
+
+
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two GPUs")
+def test_bindings_reject_operands_on_another_device():
+    C = _build.ext()
+    x = torch.randn(4, 256, device="cuda:0", dtype=torch.bfloat16)
+    w = torch.zeros(64, 256, device="cuda:0", dtype=torch.int8)
+    sc, b = torch.ones(64, device="cuda:0"), torch.zeros(64, device="cuda:0", dtype=torch.bfloat16)
+    for args in ((w, sc, b.to("cuda:1")), (w, sc.to("cuda:1"), b), (w.to("cuda:1"), sc.to("cuda:1"), b)):
+        with pytest.raises(RuntimeError, match="one device"):
+            C.weight_only_gemm(x, *args, False, -1)
+    xp, w3, s3, b3, offsets, work = _expert_operands("cuda:0")
+    for args in ((w3, s3, b3.to("cuda:1")), (w3, s3.to("cuda:1"), b3)):
+        with pytest.raises(RuntimeError, match="one device"):
+            C.weight_only_gemm_experts(xp, *args, offsets, work, False, -1)
 
 
 def _llama_pair():
