@@ -10,6 +10,9 @@ namespace b200 {
 static constexpr int kCEThreads = 512;
 
 __device__ __forceinline__ void online_combine(float& m, float& s, float m2, float s2) {
+  // A part whose max is -inf holds no mass.  Skip it: for a vector of masked (-inf) logits, s2 = exp(-inf - -inf) = NaN,
+  // and NaN * exp(-inf - m) would turn a finite running sum into NaN.
+  if (m2 == -INFINITY) return;
   const float nm = fmaxf(m, m2);
   if (nm == -INFINITY) { s = 0.f; m = nm; return; }
   s = s * __expf(m - nm) + s2 * __expf(m2 - nm);

@@ -90,8 +90,8 @@ def test_linear_autograd_matches_fp32():
     assert rel_err(b.grad, bf.grad) < 1e-2
 
 
-@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float32])
-@pytest.mark.parametrize("cols", [512, 5120, 4096, 8192])
+@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float32, torch.float16])
+@pytest.mark.parametrize("cols", [512, 5120, 4096, 8192, 1000, 2056])
 def test_rms_norm(dtype, cols):
     torch.manual_seed(0)
     x = torch.randn(300, cols, device="cuda", dtype=dtype, requires_grad=True)
@@ -102,7 +102,7 @@ def test_rms_norm(dtype, cols):
     xf, wf = x.detach().float().requires_grad_(True), w.detach().float().requires_grad_(True)
     yr = xf * torch.rsqrt(xf.pow(2).mean(-1, keepdim=True) + 1e-6) * wf
     yr.backward(dy.float())
-    tol = 1e-2 if dtype == torch.bfloat16 else 1e-4
+    tol = {torch.bfloat16: 1e-2, torch.float16: 2e-3, torch.float32: 1e-4}[dtype]
     assert rel_err(y, yr) < tol
     assert rel_err(x.grad, xf.grad) < tol
     assert rel_err(w.grad, wf.grad) < tol * 2
@@ -119,7 +119,7 @@ def test_rms_norm_residual():
     assert rel_err(y, hh * torch.rsqrt(hh.pow(2).mean(-1, keepdim=True) + 1e-6) * w.float()) < 1e-2
 
 
-@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float32])
+@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float32, torch.float16])
 def test_layer_norm(dtype):
     torch.manual_seed(0)
     cols = 1024
@@ -132,7 +132,7 @@ def test_layer_norm(dtype):
     xf, wf, bf = (t.detach().float().requires_grad_(True) for t in (x, w, b))
     yr = torch.nn.functional.layer_norm(xf, (cols,), wf, bf, 1e-5)
     yr.backward(dy.float())
-    tol = 1e-2 if dtype == torch.bfloat16 else 1e-4
+    tol = {torch.bfloat16: 1e-2, torch.float16: 2e-3, torch.float32: 1e-4}[dtype]
     assert rel_err(y, yr) < tol and rel_err(x.grad, xf.grad) < tol
     assert rel_err(w.grad, wf.grad) < 2 * tol and rel_err(b.grad, bf.grad) < 2 * tol
 
@@ -172,11 +172,12 @@ def test_rope(neox):
     assert rel_err(x.grad, xf.grad) < 1e-2
 
 
+@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16, torch.float32])
 @pytest.mark.parametrize("vocab", [32000, 1000, 50257])
-def test_softmax_ce(vocab):
+def test_softmax_ce(vocab, dtype):
     torch.manual_seed(0)
     n = 257
-    lg = (torch.randn(n, vocab, device="cuda") * 3).to(torch.bfloat16).requires_grad_(True)
+    lg = (torch.randn(n, vocab, device="cuda") * 3).to(dtype).requires_grad_(True)
     lab = torch.randint(0, vocab, (n,), device="cuda")
     lab[5] = -100
     loss = KL.softmax_cross_entropy(lg, lab, -100)
