@@ -1,4 +1,4 @@
-// Flash-attention backward for sm_90a (head_dim 128, bf16/fp16), wgmma + TMA.
+// Flash-attention backward for sm_90a (head_dim 128, and 64 in attention_d64_sm100.cu; bf16/fp16), wgmma + TMA.
 //
 //   prep_kernel: delta[row] = dO . O, lse pre-scaled by log2(e), both per query row into a padded stats buffer the main kernel stages
 //     per tile with bulk copies; in single-pass mode it also zeroes the fp32 dQ accumulator.
@@ -16,563 +16,21 @@
 //     result is bitwise reproducible, at the price of recomputing S and dP (7 GEMMs for 5).
 // The K and Q tiles are consumed K-major (S) and MN-major (dQ, dK) from one copy by choice of descriptor.
 //
+// The kernel bodies and the launcher live in include/b200_attention_bwd.cuh.
+//
 // Parity (behaviour): flash_attn_grad (paddle/phi/kernels/gpu/flash_attn_grad_kernel.cu -> flash-attention library).
 #include <cuda.h>
-#include <cstdio>
-#include <type_traits>
 
-#include "include/b200_common.cuh"
+#include "include/b200_attention_bwd.cuh"
 #include "include/b200_ops.h"
-#include "include/b200_ptx.cuh"
 
 namespace b200 {
-namespace attn_bwd {
-using namespace ptx;
-
-constexpr int HD = 128;
-constexpr int kThreads = 288;      // dq_kernel: warps 0-7 two MMA warpgroups, warp 8 TMA producer
-constexpr int kThreadsDkv = 384;   // dkv_kernel: warpgroup 0 = producer (warp 0) giving its registers to the MMA warpgroups 1 and 2
-constexpr uint32_t BIG_BYTES = 128 * 128 * 2;     // a 128-row tile: two 64-wide d halves [half][row][128 B swizzled]
-constexpr uint32_t BIG_HALF = BIG_BYTES / 2;
-constexpr uint32_t SMALL_BYTES = 64 * 128 * 2;    // a 64-row tile, same structure
-constexpr uint32_t SMALL_HALF = SMALL_BYTES / 2;
-constexpr uint32_t SMEM_BYTES = 2 * BIG_BYTES + 4 * SMALL_BYTES + 1024 + 256;   // two resident 128-row tiles + two double-buffered 64-row tiles
-
-__device__ __forceinline__ void keep_regs(uint32_t (&a)[4][4]) {
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) asm volatile("" : "+r"(a[i][j])::"memory");
-}
-
-struct Params {
-  int b, sq, sk, h, hk;
-  float scale, scale_log2;
-  int causal, causal_off;
-  const float* stats;    // [B,H,2,sq_pad]: lse * log2(e), then delta; rows >= sq are zero
-  int sq_pad;            // sq rounded up to the 64-row query tile
-  float* dq;             // fp32 [B,Sq,H,D]
-  void* dk;              // [B,Sk,Hk,D] with element strides (dkv_sb, dkv_ss, dkv_sh): may be slices of a packed dQKV tensor
-  void* dv;
-  int64_t dkv_sb, dkv_ss, dkv_sh;
-  int64_t dq_sb, dq_ss, dq_sh;   // element strides of the fp32 dQ [B,Sq,H,D] (may be laid out seq-major)
-  const int4* colmask;   // [b, mask_heads, sk] hidden row ranges per key column (see AttnArgs::colmask); nullptr: none
-  int mask_heads;
-};
-
-// resident tile (128 rows) in slot 0 / 1, streamed tiles (64 rows): operand a in slots [0, 2), operand b in slots [2, 4)
-struct Smem {
-  uint32_t base;
-  __device__ uint32_t big(int i) const { return base + i * BIG_BYTES; }
-  __device__ uint32_t small(int i) const { return base + 2 * BIG_BYTES + i * SMALL_BYTES; }
-  __device__ uint32_t bar(int i) const { return base + 2 * BIG_BYTES + 4 * SMALL_BYTES + 8u * i; }
-};
-
-// dkv_kernel smem (offsets from the 1024-aligned base): resident K, V; a 2-stage ring of {Q, dO, lse2 / delta}; with the dQ stage also
-// two dS^T buffers (double-buffered: one warpgroup may write the next tile's dS^T while the other still multiplies the last one) and a
-// 64 x 64 fp32 dQ staging tile per MMA warpgroup, the source of the bulk reduce-add.
-struct DkvSmem {
-  static constexpr uint32_t K = 0, V = BIG_BYTES, Q = 2 * BIG_BYTES, DO = Q + 2 * SMALL_BYTES, DS = DO + 2 * SMALL_BYTES;
-  static constexpr uint32_t DS_BYTES = 128 * 64 * 2;          // [key 128][query 64] 16-bit, 128B-swizzled
-  static constexpr uint32_t STAGE = DS + 2 * DS_BYTES;
-  static constexpr uint32_t STAGE_BYTES = 64 * 64 * 4;         // per warpgroup: two [query 64][32 fp32] 128B-swizzled boxes
-  static constexpr uint32_t STATS = STAGE + 2 * STAGE_BYTES;   // per ring stage: lse2[64], delta[64]
-  static constexpr uint32_t BARS = STATS + 2 * 512;
-  static constexpr uint32_t BYTES = BARS + 64 + 1024;
-};
-static_assert(DkvSmem::BYTES <= 227 * 1024, "dkv_kernel shared memory");
-
-// DQ = true: the single-pass backward.  Each query tile's dQ partial dS K (all 128 keys of the tile) is added into the fp32 dQ by a
-// TMA bulk reduce-add; dQ must be zero on entry.  DQ = false: dK / dV only (dq_kernel computes dQ).
-template <typename T, bool MASKED, bool DQ>
-__global__ void __launch_bounds__(kThreadsDkv, 1)
-dkv_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
-           const __grid_constant__ CUtensorMap map_do, const __grid_constant__ CUtensorMap map_dq, const Params p) {
-  constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
-  constexpr int BN = 128, BQ = 64;
-  using L = DkvSmem;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* const base_ptr = smem_raw + (base - smem_u32(smem_raw));
-  const uint32_t sK = base + L::K, sV = base + L::V;
-  auto sQ = [&](int s) { return base + L::Q + s * SMALL_BYTES; };
-  auto sDO = [&](int s) { return base + L::DO + s * SMALL_BYTES; };
-  auto stats = [&](int s) { return reinterpret_cast<const float*>(base_ptr + L::STATS + s * 512); };
-  const uint32_t kv_full = base + L::BARS;
-  auto qdo_full = [&](int s) { return base + L::BARS + 8 * (1 + s); };
-  auto qdo_empty = [&](int s) { return base + L::BARS + 8 * (3 + s); };     // 8 warp arrivals
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int kv_head = blockIdx.x, batch = blockIdx.y, n_tile = blockIdx.z;   // key tiles slowest: under the causal mask the long ones start first
-  const int n0 = n_tile * BN;
-  const int group = p.h / p.hk;
-  const int num_m = (p.sq + BQ - 1) / BQ;
-  int m_first = 0;
-  if (p.causal) {                       // first query row that can see key n0 + BN - 1 or an earlier one of the tile: i >= n0 - causal_off
-    const int r0 = max(0, n0 - p.causal_off);
-    m_first = min(num_m, r0 / BQ);
-  }
-  const int tiles_per_head = num_m - m_first;
-  const int total = tiles_per_head * group;    // iteration it -> (query head = kv_head*group + it / tiles_per_head, m tile = m_first + it % tiles_per_head)
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&map_q); tma_prefetch_desc(&map_k); tma_prefetch_desc(&map_v); tma_prefetch_desc(&map_do);
-    if constexpr (DQ) tma_prefetch_desc(&map_dq);
-    mbar_init(kv_full, 1);
-    for (int s = 0; s < 2; ++s) { mbar_init(qdo_full(s), 1); mbar_init(qdo_empty(s), 8); }
-    fence_barrier_init();
-    fence_proxy_async();
-  }
-  __syncthreads();
-
-  if (warp < 4) {
-    reg_dealloc<24>();
-    if (warp == 0 && lane == 0 && total > 0) {
-      // ================= TMA producer =================
-      mbar_expect_tx(kv_full, 2 * BIG_BYTES);
-      tma_load_4d(sK, &map_k, kv_full, 0, n0, kv_head, batch);
-      tma_load_4d(sK + BIG_HALF, &map_k, kv_full, 64, n0, kv_head, batch);
-      tma_load_4d(sV, &map_v, kv_full, 0, n0, kv_head, batch);
-      tma_load_4d(sV + BIG_HALF, &map_v, kv_full, 64, n0, kv_head, batch);
-      for (int it = 0; it < total; ++it) {
-        const int s = it & 1;
-        const int head = kv_head * group + it / tiles_per_head;
-        const int m0 = (m_first + it % tiles_per_head) * BQ;
-        const float* st = p.stats + ((int64_t)batch * p.h + head) * 2 * p.sq_pad + m0;
-        mbar_wait(qdo_empty(s), ((it >> 1) & 1) ^ 1);
-        mbar_expect_tx(qdo_full(s), 2 * SMALL_BYTES + 512);
-        tma_load_4d(sQ(s), &map_q, qdo_full(s), 0, m0, head, batch);
-        tma_load_4d(sQ(s) + SMALL_HALF, &map_q, qdo_full(s), 64, m0, head, batch);
-        tma_load_4d(sDO(s), &map_do, qdo_full(s), 0, m0, head, batch);
-        tma_load_4d(sDO(s) + SMALL_HALF, &map_do, qdo_full(s), 64, m0, head, batch);
-        bulk_load(base + L::STATS + s * 512, st, 256, qdo_full(s));
-        bulk_load(base + L::STATS + s * 512 + 256, st + p.sq_pad, 256, qdo_full(s));
-      }
-      for (int it = max(0, total - 2); it < total; ++it) mbar_wait(qdo_empty(it & 1), (it >> 1) & 1);   // the consumers' waits are unbounded
-    }
-  } else {
-    // ================= MMA warpgroups: wg owns keys [64 wg, 64 wg + 64) of the tile; accumulator row = key, column = query =================
-    reg_alloc<240>();
-    const int wg = (warp >> 2) - 1, q = lane & 3;
-    const int rl = wg * 64 + (warp & 3) * 16 + (lane >> 2);      // tile-relative key rows rl and rl + 8
-    float dv_acc[HD / 2], dk_acc[HD / 2];
-#pragma unroll
-    for (int i = 0; i < HD / 2; ++i) { dv_acc[i] = 0.f; dk_acc[i] = 0.f; }
-    if (total > 0) mbar_wait_unbounded(kv_full, 0);
-    for (int it = 0; it < total; ++it) {
-      const int s = it & 1;
-      const int head = kv_head * group + it / tiles_per_head;
-      const int m0 = (m_first + it % tiles_per_head) * BQ;
-      mbar_wait_unbounded(qdo_full(s), (it >> 1) & 1);
-      float st[BQ / 2], dpt[BQ / 2];
-      wgmma_fence_regs(st);
-      wgmma_fence_regs(dpt);
-      wgmma_fence();
-#pragma unroll
-      for (int kb = 0; kb < 2; ++kb)
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          wgmma_ss_n64<BF16, 0, 0>(st, make_smem_desc(sK + kb * BIG_HALF + wg * 8192 + k * 32, 16, 1024),
-                                   make_smem_desc(sQ(s) + kb * SMALL_HALF + k * 32, 16, 1024), (kb | k) != 0);      // S^T = K Q^T
-      wgmma_commit();
-#pragma unroll
-      for (int kb = 0; kb < 2; ++kb)
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          wgmma_ss_n64<BF16, 0, 0>(dpt, make_smem_desc(sV + kb * BIG_HALF + wg * 8192 + k * 32, 16, 1024),
-                                   make_smem_desc(sDO(s) + kb * SMALL_HALF + k * 32, 16, 1024), (kb | k) != 0);     // dP^T = V dO^T
-      wgmma_commit();
-      int4 cm[2];
-      if constexpr (MASKED) {
-        const int4* cmp = p.colmask + ((int64_t)batch * p.mask_heads + (p.mask_heads > 1 ? head : 0)) * p.sk;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int key = n0 + rl + h * 8;
-          cm[h] = key < p.sk ? __ldg(cmp + key) : make_int4(0, 0, 0, 0);
-        }
-      }
-      const float* lse2 = stats(s);        // lse[query] * log2(e)
-      const float* dlt = lse2 + BQ;        // delta[query]
-      wgmma_wait<1>();
-      wgmma_fence_regs(st);
-      // P^T = exp2(S^T scale - lse2[query]) in place of S^T, packed as the A fragments of dV += P^T dO (16-query step ks = column groups 2 ks, 2 ks + 1)
-      uint32_t pa[BQ / 16][4], dsa[BQ / 16][4];
-#pragma unroll
-      for (int jn = 0; jn < BQ / 8; ++jn) {
-        const float2 l2 = *reinterpret_cast<const float2*>(lse2 + jn * 8 + 2 * q);
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int row = m0 + jn * 8 + 2 * q + e;      // query
-          const int lim = row >= p.sq ? -1 : p.causal ? min(p.sk - 1, row + p.causal_off) : p.sk - 1;   // last visible key of this query row
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int key = n0 + rl + h * 8;
-            float x = ex2(fmaf(st[jn * 4 + h * 2 + e], p.scale_log2, -(e ? l2.y : l2.x)));
-            if (key > lim) x = 0.f;
-            if constexpr (MASKED) {
-              if ((row >= cm[h].x && row < cm[h].y) || (row >= cm[h].z && row < cm[h].w)) x = 0.f;
-            }
-            st[jn * 4 + h * 2 + e] = x;
-          }
-        }
-        pa[jn >> 1][(jn & 1) * 2 + 0] = pack2<T>(st[jn * 4 + 0], st[jn * 4 + 1]);
-        pa[jn >> 1][(jn & 1) * 2 + 1] = pack2<T>(st[jn * 4 + 2], st[jn * 4 + 3]);
-      }
-      wgmma_fence_regs(dv_acc);
-      wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < BQ / 16; ++ks)   // B = dO tile read MN-major (N = head dim): 16 query rows = 2048 B per step, d halves SMALL_HALF apart
-        wgmma_rs_n128<BF16, 1>(dv_acc, pa[ks], make_smem_desc(sDO(s) + ks * 2048, SMALL_HALF, 1024), 1);   // dV += P^T dO
-      wgmma_commit();
-      wgmma_wait<1>();
-      wgmma_fence_regs(dpt);
-      // dS^T = P^T (dP^T - delta[query]) scale: A fragments of dK += dS^T Q and, with DQ, the tile's rows of the dS^T buffer
-      uint8_t* const ds_buf = base_ptr + L::DS + (it & 1) * L::DS_BYTES;
-#pragma unroll
-      for (int jn = 0; jn < BQ / 8; ++jn) {
-        const float2 dl = *reinterpret_cast<const float2*>(dlt + jn * 8 + 2 * q);
-        float ds[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) ds[i] = st[jn * 4 + i] * (dpt[jn * 4 + i] - ((i & 1) ? dl.y : dl.x)) * p.scale;
-        dsa[jn >> 1][(jn & 1) * 2 + 0] = pack2<T>(ds[0], ds[1]);
-        dsa[jn >> 1][(jn & 1) * 2 + 1] = pack2<T>(ds[2], ds[3]);
-        if constexpr (DQ) {        // [key][query] rows of 128 B, 16-byte chunk c of row r stored at chunk c ^ (r % 8)
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int r = rl + h * 8;
-            *reinterpret_cast<uint32_t*>(ds_buf + r * 128 + ((jn ^ (r & 7)) << 4) + 4 * q) = dsa[jn >> 1][(jn & 1) * 2 + h];
-          }
-        }
-      }
-      wgmma_fence_regs(dk_acc);
-      wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < BQ / 16; ++ks)   // B = Q tile read MN-major, as dO above
-        wgmma_rs_n128<BF16, 1>(dk_acc, dsa[ks], make_smem_desc(sQ(s) + ks * 2048, SMALL_HALF, 1024), 1);   // dK += dS^T Q
-      wgmma_commit();
-      if constexpr (DQ) {
-        // dQ[query, 64 wg .. 64 wg + 63] = dS K over the tile's 128 keys: A = dS^T buffer read M-major (M = query), B = K half wg read
-        // N-major (N = head dim); 16 keys = 2048 B per step in both
-        fence_proxy_async();
-        named_bar_sync(1, 256);         // both warpgroups' dS^T rows are in shared memory
-        const uint32_t sDS = base + L::DS + (it & 1) * L::DS_BYTES;
-        float dq[HD / 4];
-        wgmma_fence_regs(dq);
-        wgmma_fence();
-#pragma unroll
-        for (int ks = 0; ks < BN / 16; ++ks)
-          wgmma_ss_n64<BF16, 1, 1>(dq, make_smem_desc(sDS + ks * 2048, L::DS_BYTES, 1024),
-                                   make_smem_desc(sK + wg * BIG_HALF + ks * 2048, BIG_HALF, 1024), ks != 0);
-        wgmma_commit();
-        wgmma_wait<1>();                // dV and dK are done with P^T, dS^T and the Q / dO stage
-        wgmma_fence_regs(dv_acc);
-        wgmma_fence_regs(dk_acc);
-        keep_regs(pa);
-        keep_regs(dsa);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(qdo_empty(s));
-        wgmma_wait<0>();
-        wgmma_fence_regs(dq);
-        // stage the 64 x 64 fp32 partial as two [query][32] boxes (128B-swizzled like the map) and reduce-add it into dQ
-        const bool leader = (threadIdx.x & 127) == 0;
-        if (leader) bulk_wait_group_read<0>();      // the previous tile's reduce has read the staging tile
-        named_bar_sync(2 + wg, 128);
-        uint8_t* const stage = base_ptr + L::STAGE + wg * L::STAGE_BYTES;
-#pragma unroll
-        for (int j = 0; j < HD / 16; ++j)
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int r = (warp & 3) * 16 + (lane >> 2) + h * 8;      // query row of the tile
-            const int c = 2 * (j & 3) + (q >> 1);                     // 16-byte chunk of the box row
-            *reinterpret_cast<float2*>(stage + (j >> 2) * 8192 + r * 128 + ((c ^ (r & 7)) << 4) + (q & 1) * 8) =
-                make_float2(dq[j * 4 + h * 2], dq[j * 4 + h * 2 + 1]);
-          }
-        fence_proxy_async();
-        named_bar_sync(2 + wg, 128);
-        if (leader) {
-          const uint32_t src = base + L::STAGE + wg * L::STAGE_BYTES;
-          tma_reduce_add_4d(&map_dq, src, wg * 64, m0, head, batch);
-          tma_reduce_add_4d(&map_dq, src + 8192, wg * 64 + 32, m0, head, batch);
-          bulk_commit_group();
-        }
-      } else {
-        wgmma_wait<0>();
-        wgmma_fence_regs(dv_acc);
-        wgmma_fence_regs(dk_acc);
-        keep_regs(pa);
-        keep_regs(dsa);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(qdo_empty(s));
-      }
-    }
-    if constexpr (DQ) {
-      if ((threadIdx.x & 127) == 0) bulk_wait_group<0>();      // the reduces are done reading shared memory before the CTA exits
-    }
-    // epilogue: dV, dK rows (accumulator row = key)
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int key = n0 + rl + h * 8;
-      if (key >= p.sk) continue;
-      const int64_t kv_off = (int64_t)batch * p.dkv_sb + (int64_t)key * p.dkv_ss + (int64_t)kv_head * p.dkv_sh;
-      T* dv_row = reinterpret_cast<T*>(p.dv) + kv_off;
-      T* dk_row = reinterpret_cast<T*>(p.dk) + kv_off;
-#pragma unroll
-      for (int jn = 0; jn < HD / 8; ++jn) {
-        *reinterpret_cast<uint32_t*>(dv_row + jn * 8 + 2 * q) = pack2<T>(dv_acc[jn * 4 + h * 2], dv_acc[jn * 4 + h * 2 + 1]);
-        *reinterpret_cast<uint32_t*>(dk_row + jn * 8 + 2 * q) = pack2<T>(dk_acc[jn * 4 + h * 2], dk_acc[jn * 4 + h * 2 + 1]);
-      }
-    }
-  }
-}
-
-template <typename T, bool MASKED>
-__global__ void __launch_bounds__(kThreads, 1)
-dq_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
-          const __grid_constant__ CUtensorMap map_do, const Params p) {
-  constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
-  constexpr int BM = 128, BK = 64;
-  extern __shared__ uint8_t smem_raw[];
-  const Smem sm{(smem_u32(smem_raw) + 1023u) & ~1023u};
-  const uint32_t sQ = sm.big(0), sDO = sm.big(1);
-  auto sK = [&](int s) { return sm.small(s); };
-  auto sV = [&](int s) { return sm.small(2 + s); };
-  const uint32_t qdo_full = sm.bar(0);
-  auto kv_full = [&](int s) { return sm.bar(1 + s); };
-  auto kv_empty = [&](int s) { return sm.bar(3 + s); };     // 8 warp arrivals
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m_tile = (int)gridDim.x - 1 - (int)blockIdx.x;   // long (late) rows first under the causal mask
-  const int head = blockIdx.y, batch = blockIdx.z;
-  const int kv_head = head / (p.h / p.hk);
-  const int m0 = m_tile * BM;
-  int n_tiles = (p.sk + BK - 1) / BK;
-  if (p.causal) {
-    const int last_key = min(p.sk - 1, m0 + BM - 1 + p.causal_off);
-    n_tiles = last_key < 0 ? 0 : min(n_tiles, last_key / BK + 1);
-  }
-
-  if (warp == 8 && lane == 0) {
-    tma_prefetch_desc(&map_q); tma_prefetch_desc(&map_k); tma_prefetch_desc(&map_v); tma_prefetch_desc(&map_do);
-    mbar_init(qdo_full, 1);
-    for (int s = 0; s < 2; ++s) { mbar_init(kv_full(s), 1); mbar_init(kv_empty(s), 8); }
-    fence_barrier_init();
-    fence_proxy_async();
-  }
-  __syncthreads();
-
-  if (warp == 8) {
-    if (lane == 0 && n_tiles > 0) {
-      // ================= TMA producer =================
-      mbar_expect_tx(qdo_full, 2 * BIG_BYTES);
-      tma_load_4d(sQ, &map_q, qdo_full, 0, m0, head, batch);
-      tma_load_4d(sQ + BIG_HALF, &map_q, qdo_full, 64, m0, head, batch);
-      tma_load_4d(sDO, &map_do, qdo_full, 0, m0, head, batch);
-      tma_load_4d(sDO + BIG_HALF, &map_do, qdo_full, 64, m0, head, batch);
-      for (int j = 0; j < n_tiles; ++j) {
-        const int s = j & 1, n0 = j * BK;
-        mbar_wait(kv_empty(s), ((j >> 1) & 1) ^ 1);
-        mbar_expect_tx(kv_full(s), 2 * SMALL_BYTES);
-        tma_load_4d(sK(s), &map_k, kv_full(s), 0, n0, kv_head, batch);
-        tma_load_4d(sK(s) + SMALL_HALF, &map_k, kv_full(s), 64, n0, kv_head, batch);
-        tma_load_4d(sV(s), &map_v, kv_full(s), 0, n0, kv_head, batch);
-        tma_load_4d(sV(s) + SMALL_HALF, &map_v, kv_full(s), 64, n0, kv_head, batch);
-      }
-    }
-  } else {
-    // ================= MMA warpgroups: wg owns query rows [64 wg, 64 wg + 64); accumulator row = query, column = key / head dim =================
-    const int wg = warp >> 2, q = lane & 3;
-    const int rl = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-    float dq_acc[HD / 2];
-#pragma unroll
-    for (int i = 0; i < HD / 2; ++i) dq_acc[i] = 0.f;
-    float lse2[2], dl[2];
-    int lim[2];
-    bool row_ok[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = m0 + rl + h * 8;
-      row_ok[h] = row < p.sq;
-      const int64_t stat = ((int64_t)batch * p.h + head) * 2 * p.sq_pad + row;
-      lse2[h] = row_ok[h] ? p.stats[stat] : 0.f;
-      dl[h] = row_ok[h] ? p.stats[stat + p.sq_pad] : 0.f;
-      lim[h] = p.causal ? min(p.sk - 1, row + p.causal_off) : p.sk - 1;
-    }
-    const int4* cmp = MASKED ? p.colmask + ((int64_t)batch * p.mask_heads + (p.mask_heads > 1 ? head : 0)) * p.sk : nullptr;
-    (void)cmp;
-    if (n_tiles > 0) mbar_wait(qdo_full, 0);
-    for (int j = 0; j < n_tiles; ++j) {
-      const int s = j & 1, n0 = j * BK;
-      mbar_wait(kv_full(s), (j >> 1) & 1);
-      float sv[BK / 2], dpv[BK / 2];
-      wgmma_fence_regs(sv);
-      wgmma_fence_regs(dpv);
-      wgmma_fence();
-#pragma unroll
-      for (int kb = 0; kb < 2; ++kb)
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          wgmma_ss_n64<BF16, 0, 0>(sv, make_smem_desc(sQ + kb * BIG_HALF + wg * 8192 + k * 32, 16, 1024),
-                                   make_smem_desc(sK(s) + kb * SMALL_HALF + k * 32, 16, 1024), (kb | k) != 0);      // S = Q K^T
-          wgmma_ss_n64<BF16, 0, 0>(dpv, make_smem_desc(sDO + kb * BIG_HALF + wg * 8192 + k * 32, 16, 1024),
-                                   make_smem_desc(sV(s) + kb * SMALL_HALF + k * 32, 16, 1024), (kb | k) != 0);      // dP = dO V^T
-        }
-      wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_regs(sv);
-      wgmma_fence_regs(dpv);
-      uint32_t dsa[BK / 16][4];
-#pragma unroll
-      for (int jn = 0; jn < BK / 8; ++jn) {
-        float ds[4];
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int key = n0 + jn * 8 + 2 * q + e;
-          int4 m = make_int4(0, 0, 0, 0);
-          if constexpr (MASKED) { if (key < p.sk) m = __ldg(cmp + key); }
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int row = m0 + rl + h * 8;
-            float x = ex2(fmaf(sv[jn * 4 + h * 2 + e], p.scale_log2, -lse2[h]));
-            if (!row_ok[h] || key > lim[h]) x = 0.f;
-            if constexpr (MASKED) {
-              if ((row >= m.x && row < m.y) || (row >= m.z && row < m.w)) x = 0.f;
-            }
-            ds[h * 2 + e] = x * (dpv[jn * 4 + h * 2 + e] - dl[h]) * p.scale;
-          }
-        }
-        dsa[jn >> 1][(jn & 1) * 2 + 0] = pack2<T>(ds[0], ds[1]);
-        dsa[jn >> 1][(jn & 1) * 2 + 1] = pack2<T>(ds[2], ds[3]);
-      }
-      wgmma_fence_regs(dq_acc);
-      wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < BK / 16; ++ks)     // B = K tile read MN-major (N = head dim): 16 key rows = 2048 B per step
-        wgmma_rs_n128<BF16, 1>(dq_acc, dsa[ks], make_smem_desc(sK(s) + ks * 2048, SMALL_HALF, 1024), 1);   // dQ += dS K
-      wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_regs(dq_acc);
-      keep_regs(dsa);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(kv_empty(s));
-    }
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = m0 + rl + h * 8;
-      if (!row_ok[h]) continue;
-      float* dst = p.dq + (int64_t)batch * p.dq_sb + (int64_t)row * p.dq_ss + (int64_t)head * p.dq_sh;
-#pragma unroll
-      for (int jn = 0; jn < HD / 8; ++jn)
-        *reinterpret_cast<float2*>(dst + jn * 8 + 2 * q) = make_float2(dq_acc[jn * 4 + h * 2], dq_acc[jn * 4 + h * 2 + 1]);
-    }
-  }
-}
-
-// One warp per padded query row (b, s < sq_pad, head): stats = {lse * log2(e), delta = sum_d dO * O} (zero for s >= sq); with ZERO_DQ
-// also zeroes the row of the fp32 dQ accumulator.  O and dO share the element strides (sb, ss, sh), d contiguous.
-template <typename T, bool ZERO_DQ>
-__global__ void prep_kernel(const T* __restrict__ o, const T* __restrict__ d_o, const float* __restrict__ lse, float* __restrict__ stats,
-                            float* __restrict__ dq, int64_t rows, int sq, int sq_pad, int h, int64_t sb, int64_t ss, int64_t sh,
-                            int64_t dq_sb, int64_t dq_ss, int64_t dq_sh) {
-  const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);   // row = (b*sq_pad + s)*h + head
-  if (row >= rows) return;
-  const int lane = threadIdx.x & 31;
-  const int64_t bs = row / h;
-  const int head = (int)(row - bs * h);
-  const int64_t bb = bs / sq_pad;
-  const int sidx = (int)(bs - bb * sq_pad);
-  float* st = stats + (bb * h + head) * 2 * sq_pad + sidx;
-  if (sidx >= sq) {
-    if (lane == 0) { st[0] = 0.f; st[sq_pad] = 0.f; }
-    return;
-  }
-  const int64_t off = bb * sb + (int64_t)sidx * ss + (int64_t)head * sh + lane * 4;
-  const uint2 a = *reinterpret_cast<const uint2*>(o + off);
-  const uint2 b = *reinterpret_cast<const uint2*>(d_o + off);
-  const T* pa = reinterpret_cast<const T*>(&a);
-  const T* pb = reinterpret_cast<const T*>(&b);
-  float acc = 0.f;
-#pragma unroll
-  for (int i = 0; i < 4; ++i) acc += to_f(pa[i]) * to_f(pb[i]);
-#pragma unroll
-  for (int o2 = 16; o2 > 0; o2 >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o2);
-  if (lane == 0) {
-    st[0] = lse[(bb * h + head) * sq + sidx] * 1.4426950408889634f;
-    st[sq_pad] = acc;
-  }
-  if constexpr (ZERO_DQ)
-    *reinterpret_cast<float4*>(dq + bb * dq_sb + (int64_t)sidx * dq_ss + (int64_t)head * dq_sh + lane * 4) = make_float4(0.f, 0.f, 0.f, 0.f);
-}
-
-// deterministic: dkv_kernel without the dQ stage, then dq_kernel; otherwise the single pass (dQ zeroed by prep_kernel)
-template <typename T, bool MASKED>
-static void launch(const Params& p, bool deterministic, const CUtensorMap (&mq)[2], const CUtensorMap (&mk)[2], const CUtensorMap (&mv)[2],
-                   const CUtensorMap (&mdo)[2], const CUtensorMap& mdq, cudaStream_t s) {
-  const dim3 grid_kv(p.hk, p.b, (p.sk + 127) / 128), grid_q((p.sq + 127) / 128, p.h, p.b);
-  if (deterministic) {
-    set_max_dynamic_smem<dkv_kernel<T, MASKED, false>>(DkvSmem::BYTES);
-    set_max_dynamic_smem<dq_kernel<T, MASKED>>(SMEM_BYTES);
-    dkv_kernel<T, MASKED, false><<<grid_kv, kThreadsDkv, DkvSmem::BYTES, s>>>(mq[1], mk[0], mv[0], mdo[1], mdq, p);
-    dq_kernel<T, MASKED><<<grid_q, kThreads, SMEM_BYTES, s>>>(mq[0], mk[1], mv[1], mdo[0], p);
-  } else {
-    set_max_dynamic_smem<dkv_kernel<T, MASKED, true>>(DkvSmem::BYTES);
-    dkv_kernel<T, MASKED, true><<<grid_kv, kThreadsDkv, DkvSmem::BYTES, s>>>(mq[1], mk[0], mv[0], mdo[1], mdq, p);
-  }
-}
-}  // namespace attn_bwd
 
 int attention_bwd_stats_pad(int sq) { return (sq + 63) / 64 * 64; }
 
 int attention_bwd(const AttnBwdArgs& a, cudaStream_t s) {
-  using namespace attn_bwd;
   if (!attention_fwd_supported(a.fwd)) return 1;
-  const AttnArgs& f = a.fwd;
-  if (a.dq_strides[0] % 4 || a.dq_strides[1] % 4 || a.dq_strides[2] % 4 || (reinterpret_cast<uintptr_t>(a.dq) & 15)) return 1;   // TMA / float4
-  if (a.dkv_strides[0] % 2 || a.dkv_strides[1] % 2 || a.dkv_strides[2] % 2) return 1;
-  // every operand as a 128-row box map (the resident tile of dq_kernel) and as a 64-row box map (the streamed tile of dkv_kernel)
-  CUtensorMap mq[2], mk[2], mv[2], mdo[2], mdq;
-  for (int i = 0; i < 2; ++i) {
-    const uint32_t rows = i ? 64 : 128;
-    if (!attn::make_map4(&mq[i], f.q, f.d, f.sq, f.h, f.b, f.q_strides[1], f.q_strides[2], f.q_strides[0], rows, f.dtype)) return 2;
-    if (!attn::make_map4(&mk[i], f.k, f.d, f.sk, f.hk, f.b, f.k_strides[1], f.k_strides[2], f.k_strides[0], rows, f.dtype)) return 2;
-    if (!attn::make_map4(&mv[i], f.v, f.d, f.sk, f.hk, f.b, f.v_strides[1], f.v_strides[2], f.v_strides[0], rows, f.dtype)) return 2;
-    if (!attn::make_map4(&mdo[i], a.d_o, f.d, f.sq, f.h, f.b, a.o_strides[1], a.o_strides[2], a.o_strides[0], rows, f.dtype)) return 2;
-  }
-  // the fp32 dQ accumulator over its own strides, in the reduce boxes of the single pass: 32 d (128 B) x 64 query rows
-  if (!attn::make_map4(&mdq, a.dq, f.d, f.sq, f.h, f.b, a.dq_strides[1], a.dq_strides[2], a.dq_strides[0], 64, kF32)) return 2;
-  const int sq_pad = attention_bwd_stats_pad(f.sq);
-  const int64_t rows = (int64_t)f.b * sq_pad * f.h;
-  const int wpb = 8;
-  const unsigned blocks = (unsigned)((rows + wpb - 1) / wpb);
-  auto prep = [&](auto kern, auto* o) {
-    using P = std::remove_const_t<std::remove_pointer_t<decltype(o)>>;
-    kern<<<blocks, wpb * 32, 0, s>>>(o, reinterpret_cast<const P*>(a.d_o), f.lse, a.stats, a.dq, rows, f.sq, sq_pad, f.h, a.o_strides[0],
-                                     a.o_strides[1], a.o_strides[2], a.dq_strides[0], a.dq_strides[1], a.dq_strides[2]);
-  };
-  const bool det = a.deterministic;
-  if (f.dtype == kBF16) {
-    const auto* o = reinterpret_cast<const __nv_bfloat16*>(f.o);
-    det ? prep(prep_kernel<__nv_bfloat16, false>, o) : prep(prep_kernel<__nv_bfloat16, true>, o);
-  } else {
-    const auto* o = reinterpret_cast<const __half*>(f.o);
-    det ? prep(prep_kernel<__half, false>, o) : prep(prep_kernel<__half, true>, o);
-  }
-  Params p;
-  p.b = f.b; p.sq = f.sq; p.sk = f.sk; p.h = f.h; p.hk = f.hk;
-  p.scale = f.scale; p.scale_log2 = f.scale * 1.4426950408889634f;
-  p.causal = f.causal; p.causal_off = f.sk - f.sq;
-  p.colmask = reinterpret_cast<const int4*>(f.colmask);
-  p.mask_heads = f.mask_heads > 0 ? f.mask_heads : 1;
-  p.stats = a.stats; p.sq_pad = sq_pad; p.dq = a.dq; p.dk = a.dk; p.dv = a.dv;
-  p.dkv_sb = a.dkv_strides[0]; p.dkv_ss = a.dkv_strides[1]; p.dkv_sh = a.dkv_strides[2];
-  p.dq_sb = a.dq_strides[0]; p.dq_ss = a.dq_strides[1]; p.dq_sh = a.dq_strides[2];
-  if (f.dtype == kBF16) {
-    if (p.colmask) launch<__nv_bfloat16, true>(p, det, mq, mk, mv, mdo, mdq, s);
-    else launch<__nv_bfloat16, false>(p, det, mq, mk, mv, mdo, mdq, s);
-  } else {
-    if (p.colmask) launch<__half, true>(p, det, mq, mk, mv, mdo, mdq, s);
-    else launch<__half, false>(p, det, mq, mk, mv, mdo, mdq, s);
-  }
-  return B200_LAUNCH_RESULT();
+  return a.fwd.d == 64 ? attention_bwd_d64(a, s) : attn_bwd::run<attn_bwd::HD>(a, s);
 }
 
 }  // namespace b200

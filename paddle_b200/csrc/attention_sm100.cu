@@ -1,7 +1,7 @@
-// Flash-attention forward for sm_90a (head_dim 128, bf16/fp16): S = Q K^T and O += P V run on wgmma tensor cores, K/V tiles streamed
-// by TMA (4-D maps straight over the strided [B,S,H,D] views of a packed QKV tensor, so no q/k/v split copies), online softmax on the
-// accumulator fragment in registers, and P never leaves registers: the S fragment of a thread IS the A-operand fragment of the P V MMA
-// once packed to 16 bits.  Hand-written PTX; no CUTLASS, no library attention.
+// Flash-attention forward for sm_90a (head_dim 128, and 64 in attention_d64_sm100.cu; bf16/fp16): S = Q K^T and O += P V run on
+// wgmma tensor cores, K/V tiles streamed by TMA (4-D maps straight over the strided [B,S,H,D] views of a packed QKV tensor, so no
+// q/k/v split copies), online softmax on the accumulator fragment in registers, and P never leaves registers: the S fragment of a
+// thread IS the A-operand fragment of the P V MMA once packed to 16 bits.  Hand-written PTX; no CUTLASS, no library attention.
 //
 // Parity (behaviour): paddle.nn.functional.flash_attention / scaled_dot_product_attention
 // (python/paddle/nn/functional/flash_attention.py -> phi flash_attn kernels calling the flash-attention library).
@@ -31,6 +31,9 @@
 // TMA producer fetches the window's first block in their place and the tile's V rows below the window are zeroed), so blocks wholly
 // below the window may hold NaN or belong to another sequence.
 //
+// Dense at head_dim 64 (training, attention_d64_sm100.cu): the same CTA and tiles with every operand tile one 64-wide d chunk, so the
+// producer issues one box for Q and K and two for V per tile.
+//
 // The kernel bodies live in include/b200_attention_fwd.cuh.
 #include <cuda.h>
 #include <algorithm>
@@ -46,17 +49,6 @@
 namespace b200 {
 namespace attn {
 using namespace ptx;
-
-// MASKED: column-wise row-range mask (flashmask / varlen) compiled in; the dense instantiation carries none of its code or registers
-// PAGED: queries = new tokens of each sequence, K / V read through the block table (see the file header); always causal, never MASKED
-// KV: the cache element type; kv8::I8 / kv8::E4M3 (PAGED only) select the converter warpgroup and QuantPagedParams
-// D: the head size, 128; 64 for the 16-bit PAGED instantiation
-template <typename T, bool MASKED, bool PAGED = false, typename KV = T, int D = HD>
-__global__ void __launch_bounds__(std::is_same<KV, T>::value ? kThreads : kThreadsQ8, 1)
-fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
-           const std::conditional_t<PAGED, std::conditional_t<std::is_same<KV, T>::value, PagedParams, QuantPagedParams>, Params> p) {
-  fwd_body<T, MASKED, PAGED, KV, D, false>(map_q, map_k, map_v, p);
-}
 
 // ---------------------------------------------------------------------------------------------- host side
 // 4-D map {d, s, h, b} over a strided [B,S,H,D] view (strides in elements), box {128 bytes of d, rows, 1, 1}: 64 d of the 16-bit
@@ -93,7 +85,7 @@ __global__ void __launch_bounds__(1024) paged_work_window_kernel(const int* __re
 }  // namespace attn
 
 int attention_fwd_supported(const AttnArgs& a) {
-  if (a.d != 128 || (a.dtype != kBF16 && a.dtype != kF16)) return 0;
+  if ((a.d != 128 && a.d != 64) || (a.dtype != kBF16 && a.dtype != kF16)) return 0;
   if (a.h % a.hk) return 0;
   const int64_t* st[3] = {a.q_strides, a.k_strides, a.v_strides};
   for (auto s : st)
@@ -105,36 +97,8 @@ int attention_fwd_supported(const AttnArgs& a) {
 }
 
 int attention_fwd(const AttnArgs& a, cudaStream_t s) {
-  using namespace attn;
   if (!attention_fwd_supported(a)) return 1;
-  CUtensorMap mq, mk, mv;
-  // strides arrays are (batch, seq, head)
-  if (!make_map4(&mq, a.q, a.d, a.sq, a.h, a.b, a.q_strides[1], a.q_strides[2], a.q_strides[0], BM, a.dtype)) return 2;
-  if (!make_map4(&mk, a.k, a.d, a.sk, a.hk, a.b, a.k_strides[1], a.k_strides[2], a.k_strides[0], BN, a.dtype)) return 2;
-  if (!make_map4(&mv, a.v, a.d, a.sk, a.hk, a.b, a.v_strides[1], a.v_strides[2], a.v_strides[0], 64, a.dtype)) return 2;
-  Params p;
-  p.b = a.b; p.sq = a.sq; p.sk = a.sk; p.h = a.h; p.hk = a.hk;
-  p.scale_log2 = a.scale * 1.4426950408889634f;
-  p.causal = a.causal; p.causal_off = a.sk - a.sq;
-  p.o = a.o; p.lse = a.lse;
-  p.o_sb = a.o_strides[0]; p.o_ss = a.o_strides[1]; p.o_sh = a.o_strides[2];
-  p.colmask = reinterpret_cast<const int4*>(a.colmask);
-  p.mask_heads = a.mask_heads > 0 ? a.mask_heads : 1;
-  dim3 grid((a.sq + BM - 1) / BM, a.h, a.b);
-  if (a.dtype == kBF16 && !p.colmask) {
-    set_max_dynamic_smem<fwd_kernel<__nv_bfloat16, false>>(SMEM_BYTES);
-    fwd_kernel<__nv_bfloat16, false><<<grid, kThreads, SMEM_BYTES, s>>>(mq, mk, mv, p);
-  } else if (a.dtype == kBF16) {
-    set_max_dynamic_smem<fwd_kernel<__nv_bfloat16, true>>(SMEM_BYTES);
-    fwd_kernel<__nv_bfloat16, true><<<grid, kThreads, SMEM_BYTES, s>>>(mq, mk, mv, p);
-  } else if (!p.colmask) {
-    set_max_dynamic_smem<fwd_kernel<__half, false>>(SMEM_BYTES);
-    fwd_kernel<__half, false><<<grid, kThreads, SMEM_BYTES, s>>>(mq, mk, mv, p);
-  } else {
-    set_max_dynamic_smem<fwd_kernel<__half, true>>(SMEM_BYTES);
-    fwd_kernel<__half, true><<<grid, kThreads, SMEM_BYTES, s>>>(mq, mk, mv, p);
-  }
-  return B200_LAUNCH_RESULT();
+  return a.d == 64 ? attention_fwd_d64(a, s) : attn::fwd_dense<attn::HD>(a, s);
 }
 
 int attention_paged_prefill_slots(int t, int b) { return (t + attn::BM - 1) / attn::BM + b; }

@@ -65,7 +65,7 @@ __device__ __forceinline__ void fwd_body(const CUtensorMap& map_q, const CUtenso
   constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
   constexpr bool Q8 = !std::is_same<KV, T>::value;
   static_assert(!Q8 || (PAGED && !MASKED), "8-bit caches are paged only");
-  static_assert(D == HD || (D == 64 && PAGED && !Q8), "head_dim 64 is paged over 16-bit caches only");
+  static_assert(D == HD || (D == 64 && !Q8), "head_dim 64 reads 16-bit K / V only");
   static_assert(!WINDOW || (PAGED && !MASKED), "sliding windows are paged only");
   constexpr int kHalves = D / 64;                            // 64-wide d chunks (128-byte swizzle spans) of a row
   constexpr uint32_t kTile = BM * D * 2;                     // one Q, K or V tile
@@ -221,23 +221,24 @@ __device__ __forceinline__ void fwd_body(const CUtensorMap& map_q, const CUtenso
       }
     } else if (lane == 0 && n_tiles > 0) {
       // ================= TMA producer =================
-      mbar_expect_tx(q_full, TILE_BYTES);
+      // one box per 64-wide d chunk: two per Q / K tile and four per V tile at D = 128, one and two at D = 64
+      mbar_expect_tx(q_full, kTile);
       tma_load_4d(sQ, &map_q, q_full, 0, m0, head, batch);
-      tma_load_4d(sQ + HALF_BYTES, &map_q, q_full, 64, m0, head, batch);
+      if constexpr (kHalves == 2) tma_load_4d(sQ + HALF_BYTES, &map_q, q_full, 64, m0, head, batch);
       for (int j = 0; j < n_tiles; ++j) {
         const int s = j & 1, n0 = j * BN;
         const uint32_t ph = ((j >> 1) & 1) ^ 1;
         mbar_wait(k_empty(s), ph);
-        mbar_expect_tx(k_full(s), TILE_BYTES);
+        mbar_expect_tx(k_full(s), kTile);
         tma_load_4d(sK(s), &map_k, k_full(s), 0, n0, kv_head, batch);               // box {64 d, 128 keys}: K-major B operand
-        tma_load_4d(sK(s) + HALF_BYTES, &map_k, k_full(s), 64, n0, kv_head, batch);
+        if constexpr (kHalves == 2) tma_load_4d(sK(s) + HALF_BYTES, &map_k, k_full(s), 64, n0, kv_head, batch);
         mbar_wait(v_empty(s), ph);
-        mbar_expect_tx(v_full(s), TILE_BYTES);
+        mbar_expect_tx(v_full(s), kTile);
 #pragma unroll
         for (int kb = 0; kb < 2; ++kb)                                              // box {64 d, 64 keys}: MN-major B operand
 #pragma unroll
-          for (int i = 0; i < 2; ++i)
-            tma_load_4d(sV(s) + kb * HALF_BYTES + i * 8192, &map_v, v_full(s), i * 64, n0 + kb * 64, kv_head, batch);
+          for (int i = 0; i < kHalves; ++i)
+            tma_load_4d(sV(s) + kb * kVBlock + i * 8192, &map_v, v_full(s), i * 64, n0 + kb * 64, kv_head, batch);
       }
     }
   } else {
@@ -408,6 +409,49 @@ __device__ __forceinline__ void fwd_body(const CUtensorMap& map_q, const CUtenso
       }
     }
   }
+}
+
+// MASKED: column-wise row-range mask (flashmask / varlen) compiled in; the dense instantiation carries none of its code or registers
+// PAGED: queries = new tokens of each sequence, K / V read through the block table (see attention_sm100.cu); always causal, never MASKED
+// KV: the cache element type; kv8::I8 / kv8::E4M3 (PAGED only) select the converter warpgroup and QuantPagedParams
+// D: the head size, 128 or 64 (64: 16-bit K / V).  attention_sm100.cu instantiates D = 128 and the paged D = 64 kernels,
+// attention_d64_sm100.cu the dense D = 64 ones.
+template <typename T, bool MASKED, bool PAGED = false, typename KV = T, int D = HD>
+__global__ void __launch_bounds__(std::is_same<KV, T>::value ? kThreads : kThreadsQ8, 1)
+fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
+           const std::conditional_t<PAGED, std::conditional_t<std::is_same<KV, T>::value, PagedParams, QuantPagedParams>, Params> p) {
+  fwd_body<T, MASKED, PAGED, KV, D, false>(map_q, map_k, map_v, p);
+}
+
+// The dense forward at head size D over the strided [B,S,H,D] views of AttnArgs (checked by attention_fwd_supported).
+template <int D>
+int fwd_dense(const AttnArgs& a, cudaStream_t s) {
+  CUtensorMap mq, mk, mv;
+  // strides arrays are (batch, seq, head)
+  if (!make_map4(&mq, a.q, a.d, a.sq, a.h, a.b, a.q_strides[1], a.q_strides[2], a.q_strides[0], BM, a.dtype)) return 2;
+  if (!make_map4(&mk, a.k, a.d, a.sk, a.hk, a.b, a.k_strides[1], a.k_strides[2], a.k_strides[0], BN, a.dtype)) return 2;
+  if (!make_map4(&mv, a.v, a.d, a.sk, a.hk, a.b, a.v_strides[1], a.v_strides[2], a.v_strides[0], 64, a.dtype)) return 2;
+  Params p;
+  p.b = a.b; p.sq = a.sq; p.sk = a.sk; p.h = a.h; p.hk = a.hk;
+  p.scale_log2 = a.scale * 1.4426950408889634f;
+  p.causal = a.causal; p.causal_off = a.sk - a.sq;
+  p.o = a.o; p.lse = a.lse;
+  p.o_sb = a.o_strides[0]; p.o_ss = a.o_strides[1]; p.o_sh = a.o_strides[2];
+  p.colmask = reinterpret_cast<const int4*>(a.colmask);
+  p.mask_heads = a.mask_heads > 0 ? a.mask_heads : 1;
+  const dim3 grid((a.sq + BM - 1) / BM, a.h, a.b);
+  constexpr uint32_t smem = kSmemBytes<D>;
+  auto launch = [&](auto tag_t, auto tag_masked) {
+    using T = decltype(tag_t);
+    constexpr bool MASKED = decltype(tag_masked)::value;
+    set_max_dynamic_smem<fwd_kernel<T, MASKED, false, T, D>>(smem);
+    fwd_kernel<T, MASKED, false, T, D><<<grid, kThreads, smem, s>>>(mq, mk, mv, p);
+  };
+  if (a.dtype == kBF16 && !p.colmask) launch(__nv_bfloat16(), std::false_type());
+  else if (a.dtype == kBF16) launch(__nv_bfloat16(), std::true_type());
+  else if (!p.colmask) launch(__half(), std::false_type());
+  else launch(__half(), std::true_type());
+  return B200_LAUNCH_RESULT();
 }
 
 // A paged instantiation's parameters with a sliding window: key j is visible to query i iff i - window < j <= i (window >= 1).

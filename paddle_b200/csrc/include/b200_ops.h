@@ -318,7 +318,7 @@ struct OutQuantArgs {
 int attention_out_quant(const OutQuantArgs& a, cudaStream_t s);
 
 // ---- attention_sm100.cu ---------------------------------------------------------------------------------------
-// Flash-attention forward (head_dim 128, fp16/bf16). q [B,Sq,H,D], k/v [B,Sk,Hk,D], o [B,Sq,H,D] as strided views (element
+// Flash-attention forward (head_dim 128 or 64, fp16/bf16). q [B,Sq,H,D], k/v [B,Sk,Hk,D], o [B,Sq,H,D] as strided views (element
 // strides given as {batch, seq, head}; the head_dim stride must be 1). lse: fp32 [B,H,Sq] (natural log) or nullptr.
 struct AttnArgs {
   const void* q; const void* k; const void* v; void* o; float* lse;
@@ -335,6 +335,7 @@ struct AttnArgs {
 };
 int attention_fwd_supported(const AttnArgs& a);
 int attention_fwd(const AttnArgs& a, cudaStream_t s);
+int attention_fwd_d64(const AttnArgs& a, cudaStream_t s);   // head_dim 64 (attention_d64_sm100.cu), called by attention_fwd
 // Causal prefill over a paged KV cache: the queries are the n_q[i] new tokens of sequence i at packed rows cu_q[i] ..., its keys are the
 // past[i] + n_q[i] cached positions (the new K / V already written), read through block_tables [b, max_blocks]; key j is visible to new
 // row r iff j <= past[i] + r.  q: [t, H, D] rows (strides token, head); caches [num_blocks, Hk, block_size, D] contiguous, block_size
@@ -376,6 +377,7 @@ struct AttnBwdArgs {
   bool deterministic;       // dK / dV kernel + a separate dQ kernel, bitwise reproducible; otherwise one pass, dQ bulk-reduced
 };
 int attention_bwd(const AttnBwdArgs& a, cudaStream_t s);
+int attention_bwd_d64(const AttnBwdArgs& a, cudaStream_t s);   // head_dim 64 (attention_d64_sm100.cu), called by attention_bwd
 
 // Token sampling (sampling.cu): one CTA per row of x [rows, vocab] (row stride `stride` elements, unit column stride).  Per-row device
 // arrays: temperature (<= 0: greedy), top_k (int32, 0: off), top_p (1: off), threshold (optional), seed / offset (int64).  Writes ids and

@@ -1,9 +1,10 @@
 """Attention entry point ([B,S,H,D] layout). Parity: paddle flash_attention / scaled_dot_product_attention
 (python/paddle/nn/functional/flash_attention.py).
 
-Dispatch: the sm_90a wgmma flash kernel (csrc/attention_sm100.cu) for fp16/bf16, head_dim 128, no explicit mask and no
-dropout — it reads q/k/v in place as strided views of a packed QKV projection; everything else takes the PyTorch SDPA
-(library) path.  Backward: csrc/attention_bwd_sm100.cu (B200_ATTN_BWD=own, default) or, for comparison, a library backward
+Dispatch: the sm_90a wgmma flash kernels for fp16/bf16, head_dim 128 (csrc/attention_sm100.cu) or 64
+(csrc/attention_d64_sm100.cu), no explicit mask and no dropout — they read q/k/v in place as strided views of a packed QKV
+projection, and a column-wise row-range mask (attention_colmask) runs on the same kernels.  Other head sizes, dense masks and
+dropout take the PyTorch SDPA (library) path.  Backward: csrc/attention_bwd_sm100.cu (B200_ATTN_BWD=own, default) or, for comparison, a library backward
 fed with our forward's (out, logsumexp) (B200_ATTN_BWD=cudnn|flash).  The own backward is a single pass that bulk-reduces dQ in
 arrival order (reproducible to rounding); FLAGS_cudnn_deterministic switches it to a bitwise-reproducible dK/dV + dQ kernel pair.
 """
@@ -189,7 +190,7 @@ def attention_packed(qkv, nh, nkv, causal=True, scale=None, seq_major=False):
 def fused_ok(q, k, v, mask, dropout_p, causal):
     if not (use_fused(q) and flag("FLAGS_b200_flash_attention", True)) or mask is not None or dropout_p != 0.0:
         return False
-    if q.dtype not in (torch.float16, torch.bfloat16) or q.dim() != 4 or q.shape[-1] != 128:
+    if q.dtype not in (torch.float16, torch.bfloat16) or q.dim() != 4 or q.shape[-1] not in (64, 128):
         return False
     if causal and q.shape[1] != k.shape[1]:
         return False

@@ -68,6 +68,14 @@ def mistral_7b(**kw):
     return LlamaConfig(**base)
 
 
+def tinyllama_1b(**kw):
+    """TinyLlama-1.1B: 22 Llama layers of hidden 2048 with grouped-query attention (32 / 4 heads of 64)."""
+    base = dict(vocab_size=32000, hidden_size=2048, intermediate_size=5632, num_hidden_layers=22, num_attention_heads=32,
+                num_key_value_heads=4, max_position_embeddings=2048)
+    base.update(kw)
+    return LlamaConfig(**base)
+
+
 def llama_tiny(**kw):
     base = dict(vocab_size=512, hidden_size=128, intermediate_size=256, num_hidden_layers=2, num_attention_heads=4, num_key_value_heads=4,
                 max_position_embeddings=128)
