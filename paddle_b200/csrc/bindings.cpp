@@ -1,5 +1,6 @@
 // pybind11 bindings: at::Tensor <-> plain-C launch API (include/b200_ops.h). The only TU that includes torch headers.
 #include <ATen/cuda/CUDAContext.h>
+#include <ATen/cuda/CUDAGeneratorImpl.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
 
@@ -1040,8 +1041,47 @@ static void set_colmask(b200::AttnArgs& a, const OptT& colmask) {
   a.mask_heads = (int)m.size(1);
 }
 
-std::vector<Tensor> attention_fwd(const Tensor& q, const Tensor& k, const Tensor& v, double scale, bool causal, bool out_seq_major, const OptT& colmask) {
+// Attention dropout's generator state.  fixed_seed_offset (int64 [2] = (seed, offset), on the host or the device) is used as given;
+// otherwise the call takes B*H offsets of torch's default CUDA generator as a PhiloxCudaState, which the kernel resolves on the device,
+// so a call captured in a CUDA graph reads the graph's seed and offset slots at every replay and draws a fresh mask each time.
+static b200::AttnDropoutArgs dropout_args(double p, const OptT& fixed_seed_offset, const Tensor& seed_offset, int64_t planes, c10::Device dev) {
+  b200::AttnDropoutArgs d;
+  d.p = p;
+  d.seed_offset = seed_offset.data_ptr<int64_t>();
+  if (fixed_seed_offset.has_value() && fixed_seed_offset->defined()) {
+    const Tensor& f = *fixed_seed_offset;
+    TORCH_CHECK(f.scalar_type() == at::kLong && f.numel() == 2 && f.is_contiguous(), "attention: fixed_seed_offset must be int64 [2] (seed, offset)");
+    if (f.is_cuda()) {
+      TORCH_CHECK(f.device() == dev, "attention: fixed_seed_offset is on another device");
+      d.seed_ptr = f.data_ptr<int64_t>(); d.offset_ptr = d.seed_ptr + 1;
+    } else {
+      d.seed = (uint64_t)f.data_ptr<int64_t>()[0]; d.offset = (uint64_t)f.data_ptr<int64_t>()[1];
+    }
+    return d;
+  }
+  auto* gen = at::get_generator_or_default<at::CUDAGeneratorImpl>(std::nullopt, at::cuda::detail::getDefaultCUDAGenerator(dev.index()));
+  at::PhiloxCudaState st;
+  {
+    std::lock_guard<std::mutex> lock(gen->mutex_);
+    st = gen->philox_cuda_state((uint64_t)planes);
+  }
+  if (st.captured_) {
+    d.seed_ptr = st.seed_.ptr; d.offset_ptr = st.offset_.ptr; d.offset_add = (int64_t)st.offset_intragraph_;
+  } else {
+    d.seed = st.seed_.val; d.offset = st.offset_.val;
+  }
+  return d;
+}
+
+static void check_dropout(double p, const char* what) {
+  TORCH_CHECK(p >= 0.0 && p < 1.0, what, ": dropout_p must be in [0, 1)");
+}
+
+// dropout_p > 0: attention dropout (csrc/attention_dropout_sm100.cu); also returns the int64 [2] (seed, offset) the mask was drawn with
+std::vector<Tensor> attention_fwd(const Tensor& q, const Tensor& k, const Tensor& v, double scale, bool causal, bool out_seq_major, const OptT& colmask,
+                                  double dropout_p, const OptT& fixed_seed_offset) {
   c10::cuda::CUDAGuard guard(q.device());
+  check_dropout(dropout_p, "attention_fwd");
   b200::AttnArgs a;
   TORCH_CHECK(fill_attn(a, q, k, v, scale, causal), "paddle_b200.attention_fwd: unsupported operands");
   set_colmask(a, colmask);
@@ -1050,6 +1090,15 @@ std::vector<Tensor> attention_fwd(const Tensor& q, const Tensor& k, const Tensor
   if (out_seq_major) { a.o_strides[0] = (int64_t)a.h * a.d; a.o_strides[1] = (int64_t)a.b * a.h * a.d; a.o_strides[2] = a.d; }
   Tensor lse = torch::empty({a.b, a.h, a.sq}, q.options().dtype(at::kFloat));
   a.o = out.data_ptr(); a.lse = lse.data_ptr<float>();
+  if (dropout_p > 0.0) {
+    Tensor seed_offset = torch::empty({2}, q.options().dtype(at::kLong));
+    const b200::AttnDropoutArgs d = dropout_args(dropout_p, fixed_seed_offset, seed_offset, (int64_t)a.b * a.h, q.device());
+    int rc = b200::attention_fwd_dropout(a, d, cur_stream());
+    g_launches += 1;
+    check_err();
+    TORCH_CHECK(rc == 0, "paddle_b200.attention_fwd (dropout) launch failed rc=", rc);
+    return {out, lse, seed_offset};
+  }
   int rc = b200::attention_fwd(a, cur_stream());
   g_launches += 1;
   check_err();
@@ -1369,10 +1418,22 @@ void attention_out_quant(const Tensor& x, const Tensor& y, double out_scale, con
 
 static bool g_deterministic = false;     // FLAGS_cudnn_deterministic: the attention backward takes its bitwise-reproducible two-kernel path
 
+// The backward's launch: dropout_p > 0 takes the mask of seed_offset, the (seed, offset) pair the forward returned.
+static int launch_bwd(const b200::AttnBwdArgs& a, double dropout_p, const OptT& seed_offset, const char* what) {
+  if (dropout_p == 0.0) return b200::attention_bwd(a, cur_stream());
+  TORCH_CHECK(seed_offset.has_value() && seed_offset->defined() && seed_offset->is_cuda() && seed_offset->scalar_type() == at::kLong &&
+              seed_offset->numel() == 2, what, ": dropout needs the forward's seed_offset (int64 [2] on the device)");
+  b200::AttnDropoutArgs d;
+  d.p = dropout_p;
+  d.seed_offset = seed_offset->data_ptr<int64_t>();
+  return b200::attention_bwd_dropout(a, d, cur_stream());
+}
+
 // backward of attention_fwd: returns (dq [B,Sq,H,D], dk, dv [B,Sk,Hk,D]) in the input dtype
 std::vector<Tensor> attention_bwd(const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& out, const Tensor& lse, const Tensor& d_out,
-                                  double scale, bool causal, const OptT& colmask) {
+                                  double scale, bool causal, const OptT& colmask, double dropout_p, const OptT& seed_offset) {
   c10::cuda::CUDAGuard guard(q.device());
+  check_dropout(dropout_p, "attention_bwd");
   b200::AttnBwdArgs a;
   TORCH_CHECK(fill_attn(a.fwd, q, k, v, scale, causal), "paddle_b200.attention_bwd: unsupported operands");
   set_colmask(a.fwd, colmask);
@@ -1385,7 +1446,7 @@ std::vector<Tensor> attention_bwd(const Tensor& q, const Tensor& k, const Tensor
   a.d_o = d_out.data_ptr(); a.stats = stats.data_ptr<float>(); a.dq = dq32.data_ptr<float>(); a.dk = dk.data_ptr(); a.dv = dv.data_ptr();
   a.deterministic = g_deterministic;
   for (int i = 0; i < 3; ++i) { a.dkv_strides[i] = dk.stride(i); a.o_strides[i] = out.stride(i); a.dq_strides[i] = dq32.stride(i); }
-  int rc = b200::attention_bwd(a, cur_stream());
+  int rc = launch_bwd(a, dropout_p, seed_offset, "attention_bwd");
   g_launches += a.deterministic ? 3 : 2;     // prep + dK/dV + dQ, or prep + single pass
   check_err();
   TORCH_CHECK(rc == 0, "paddle_b200.attention_bwd launch failed rc=", rc);
@@ -1395,8 +1456,9 @@ std::vector<Tensor> attention_bwd(const Tensor& q, const Tensor& k, const Tensor
 // packed variant: qkv [B,S,nh+2*nkv,D] (q heads | k heads | v heads); returns d(qkv) of the same shape, written in place by
 // the kernel (dk/dv slices) plus one cast-copy of the fp32 dq accumulator - no slice-backward zero fills / adds
 Tensor attention_bwd_packed(const Tensor& qkv, int64_t nh, int64_t nkv, const Tensor& out, const Tensor& lse, const Tensor& d_out, double scale,
-                            bool causal, bool seq_major) {
+                            bool causal, bool seq_major, double dropout_p, const OptT& seed_offset) {
   c10::cuda::CUDAGuard guard(qkv.device());
+  check_dropout(dropout_p, "attention_bwd_packed");
   TORCH_CHECK(qkv.dim() == 4 && qkv.is_contiguous() && qkv.size(2) == nh + 2 * nkv, "attention_bwd_packed: qkv layout");
   // seq_major: qkv / out / d_out memory is [S,B,*,D]; the kernels see [B,S,*,D] views of it (strides only, no copies)
   auto bs = [&](const Tensor& t) { return seq_major ? t.transpose(0, 1) : t; };
@@ -1414,7 +1476,7 @@ Tensor attention_bwd_packed(const Tensor& qkv, int64_t nh, int64_t nkv, const Te
   a.d_o = d_out.data_ptr(); a.stats = stats.data_ptr<float>(); a.dq = dq32_mem.data_ptr<float>(); a.dk = dk.data_ptr(); a.dv = dv.data_ptr();
   a.deterministic = g_deterministic;
   for (int i = 0; i < 3; ++i) { a.dkv_strides[i] = dk.stride(i); a.o_strides[i] = ov.stride(i); a.dq_strides[i] = dq32.stride(i); }
-  int rc = b200::attention_bwd(a, cur_stream());
+  int rc = launch_bwd(a, dropout_p, seed_offset, "attention_bwd_packed");
   g_launches += a.deterministic ? 3 : 2;     // prep + dK/dV + dQ, or prep + single pass
   check_err();
   TORCH_CHECK(rc == 0, "paddle_b200.attention_bwd_packed launch failed rc=", rc);
@@ -1569,7 +1631,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         pybind11::arg("max_bound") = 127.0, pybind11::arg("min_bound") = -127.0);
   m.def("attention_supported", &attention_supported);
   m.def("attention_fwd", traced("attention_fwd", &attention_fwd), pybind11::arg("q"), pybind11::arg("k"), pybind11::arg("v"), pybind11::arg("scale"), pybind11::arg("causal"),
-        pybind11::arg("out_seq_major") = false, pybind11::arg("colmask") = pybind11::none());
+        pybind11::arg("out_seq_major") = false, pybind11::arg("colmask") = pybind11::none(), pybind11::arg("dropout_p") = 0.0,
+        pybind11::arg("seed_offset") = pybind11::none());
   m.def("attention_fwd_paged", traced("attention_fwd_paged", &attention_fwd_paged), pybind11::arg("q"), pybind11::arg("k_cache"),
         pybind11::arg("v_cache"), pybind11::arg("block_tables"), pybind11::arg("cu_q"), pybind11::arg("n_q"), pybind11::arg("past"), pybind11::arg("scale"),
         pybind11::arg("out"), pybind11::arg("lse") = pybind11::none(), pybind11::arg("k_dequant_scales") = pybind11::none(),
@@ -1583,9 +1646,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         pybind11::arg("cu_groups"), pybind11::arg("group_seqs"), pybind11::arg("prefix_len"), pybind11::arg("scale"), pybind11::arg("out"),
         pybind11::arg("k_dequant_scales") = pybind11::none(), pybind11::arg("v_dequant_scales") = pybind11::none());
   m.def("attention_bwd", traced("attention_bwd", &attention_bwd), pybind11::arg("q"), pybind11::arg("k"), pybind11::arg("v"), pybind11::arg("out"), pybind11::arg("lse"),
-        pybind11::arg("d_out"), pybind11::arg("scale"), pybind11::arg("causal"), pybind11::arg("colmask") = pybind11::none());
+        pybind11::arg("d_out"), pybind11::arg("scale"), pybind11::arg("causal"), pybind11::arg("colmask") = pybind11::none(),
+        pybind11::arg("dropout_p") = 0.0, pybind11::arg("seed_offset") = pybind11::none());
   m.def("attention_bwd_packed", traced("attention_bwd_packed", &attention_bwd_packed), pybind11::arg("qkv"), pybind11::arg("nh"), pybind11::arg("nkv"), pybind11::arg("out"),
-        pybind11::arg("lse"), pybind11::arg("d_out"), pybind11::arg("scale"), pybind11::arg("causal"), pybind11::arg("seq_major") = false);
+        pybind11::arg("lse"), pybind11::arg("d_out"), pybind11::arg("scale"), pybind11::arg("causal"), pybind11::arg("seq_major") = false,
+        pybind11::arg("dropout_p") = 0.0, pybind11::arg("seed_offset") = pybind11::none());
   m.def("sample_tokens", traced("sample_tokens", &sample_tokens), pybind11::arg("x"), pybind11::arg("temperature"), pybind11::arg("top_k"),
         pybind11::arg("top_p"), pybind11::arg("threshold"), pybind11::arg("seed"), pybind11::arg("offset"), pybind11::arg("is_prob") = false,
         pybind11::arg("truncated") = true, pybind11::arg("k_out") = 0);

@@ -12,6 +12,7 @@
 
 #include "b200_common.cuh"
 #include "b200_ops.h"
+#include "b200_philox.cuh"
 #include "b200_ptx.cuh"
 
 namespace b200 {
@@ -75,9 +76,11 @@ static_assert(DkvSmem<HD>::BYTES <= 227 * 1024, "dkv_kernel shared memory");
 
 // DQ = true: the single-pass backward.  Each query tile's dQ partial dS K (all 128 keys of the tile) is added into the fp32 dQ by a
 // TMA bulk reduce-add; dQ must be zero on entry.  DQ = false: dK / dV only (dq_kernel computes dQ).
-template <typename T, bool MASKED, bool DQ, int D>
+// DROPOUT (P = dropout::DropoutParams<Params>): with Zs = Z / (1 - p) for the keep mask Z of p.seed_offset, dV += (Zs P)^T dO and
+// dS = P (Zs dP - delta) scale (dP = dO V^T is the gradient of the dropped probabilities; delta = rowsum(dO O) on the dropped O).
+template <typename T, bool MASKED, bool DQ, int D, bool DROPOUT = false, typename P = Params>
 __device__ __forceinline__ void dkv_body(const CUtensorMap& map_q, const CUtensorMap& map_k, const CUtensorMap& map_v,
-                                         const CUtensorMap& map_do, const CUtensorMap& map_dq, const Params p) {
+                                         const CUtensorMap& map_do, const CUtensorMap& map_dq, const P p) {
   static_assert(D == HD || D == 64, "head_dim 128 or 64");
   constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
   constexpr int BN = 128, BQ = 64;
@@ -150,6 +153,18 @@ __device__ __forceinline__ void dkv_body(const CUtensorMap& map_q, const CUtenso
     float dv_acc[D / 2], dk_acc[D / 2];
 #pragma unroll
     for (int i = 0; i < D / 2; ++i) { dv_acc[i] = 0.f; dk_acc[i] = 0.f; }
+    // DROPOUT: this lane's keys n0 + rl (+ 8) have parity kpar; it draws the calls of the queries of parity kpar and trades the bits its
+    // partner (lane ^ 4, keys of the other parity) needs for the calls of the other parity (see b200_philox.cuh)
+    uint32_t dk0 = 0, dk1 = 0, dkc = 0;
+    int64_t doff = 0;
+    const int kpar = (lane >> 2) & 1;
+    if constexpr (DROPOUT) {
+      const uint64_t seed = (uint64_t)__ldg(p.seed_offset);
+      doff = __ldg(p.seed_offset + 1);
+      dk0 = (uint32_t)seed; dk1 = (uint32_t)(seed >> 32);
+      dkc = dropout::key_counter(n0 + rl);
+    }
+    (void)kpar;
     if (total > 0) mbar_wait_unbounded(kv_full, 0);
     for (int it = 0; it < total; ++it) {
       const int s = it & 1;
@@ -174,6 +189,19 @@ __device__ __forceinline__ void dkv_body(const CUtensorMap& map_q, const CUtenso
           wgmma_ss_n64<BF16, 0, 0>(dpt, make_smem_desc(sV + kb * BIG_HALF + wg * 8192 + k * 32, 16, 1024),
                                    make_smem_desc(sDO(s) + kb * SMALL_HALF + k * 32, 16, 1024), (kb | k) != 0);     // dP^T = V dO^T
       wgmma_commit();
+      // DROPOUT, while S^T and dP^T are in flight: z0 / z1 hold the calls of the even / odd queries 2 q (+ 1) of column groups
+      // 2 cc, 2 cc + 1 at bits 8 cc .., shifted so that the element (query 8 jn + 2 q + e, key rl + 8 h) is bit 8 (jn >> 1) + 4 (jn & 1) + 2 h
+      uint32_t z0 = 0, z1 = 0;
+      if constexpr (DROPOUT) {
+        uint32_t c2, c3, own = 0;
+        dropout::plane_counter(doff, batch, p.h, head, c2, c3);
+#pragma unroll 1
+        for (int cc = 0; cc < BQ / 16; ++cc)   // one call's temporaries live at a time
+          own |= dropout::keep_bits(dropout::row_counter(m0 + 16 * cc + 2 * q + kpar), dkc, dk0, dk1, c2, c3, p.keep) << (8 * cc);
+        const uint32_t other = __shfl_xor_sync(0xffffffffu, own, 4);
+        z0 = (kpar ? other : own) >> kpar;
+        z1 = (kpar ? own : other) >> kpar;
+      }
       int4 cm[2];
       if constexpr (MASKED) {
         const int4* cmp = p.colmask + ((int64_t)batch * p.mask_heads + (p.mask_heads > 1 ? head : 0)) * p.sk;
@@ -207,8 +235,19 @@ __device__ __forceinline__ void dkv_body(const CUtensorMap& map_q, const CUtenso
             st[jn * 4 + h * 2 + e] = x;
           }
         }
-        pa[jn >> 1][(jn & 1) * 2 + 0] = pack2<T>(st[jn * 4 + 0], st[jn * 4 + 1]);
-        pa[jn >> 1][(jn & 1) * 2 + 1] = pack2<T>(st[jn * 4 + 2], st[jn * 4 + 3]);
+        if constexpr (DROPOUT) {   // st keeps the undropped P^T for dS^T; dV takes Zs P^T
+          float zp[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const int bit = 8 * (jn >> 1) + 4 * (jn & 1) + 2 * (i >> 1);
+            zp[i] = (((i & 1) ? z1 : z0) >> bit) & 1u ? st[jn * 4 + i] * p.rscale : 0.f;
+          }
+          pa[jn >> 1][(jn & 1) * 2 + 0] = pack2<T>(zp[0], zp[1]);
+          pa[jn >> 1][(jn & 1) * 2 + 1] = pack2<T>(zp[2], zp[3]);
+        } else {
+          pa[jn >> 1][(jn & 1) * 2 + 0] = pack2<T>(st[jn * 4 + 0], st[jn * 4 + 1]);
+          pa[jn >> 1][(jn & 1) * 2 + 1] = pack2<T>(st[jn * 4 + 2], st[jn * 4 + 3]);
+        }
       }
       wgmma_fence_regs(dv_acc);
       wgmma_fence();
@@ -228,7 +267,14 @@ __device__ __forceinline__ void dkv_body(const CUtensorMap& map_q, const CUtenso
         const float2 dl = *reinterpret_cast<const float2*>(dlt + jn * 8 + 2 * q);
         float ds[4];
 #pragma unroll
-        for (int i = 0; i < 4; ++i) ds[i] = st[jn * 4 + i] * (dpt[jn * 4 + i] - ((i & 1) ? dl.y : dl.x)) * p.scale;
+        for (int i = 0; i < 4; ++i) {
+          float dp = dpt[jn * 4 + i];
+          if constexpr (DROPOUT) {
+            const int bit = 8 * (jn >> 1) + 4 * (jn & 1) + 2 * (i >> 1);
+            dp = (((i & 1) ? z1 : z0) >> bit) & 1u ? dp * p.rscale : 0.f;
+          }
+          ds[i] = st[jn * 4 + i] * (dp - ((i & 1) ? dl.y : dl.x)) * p.scale;
+        }
         dsa[jn >> 1][(jn & 1) * 2 + 0] = pack2<T>(ds[0], ds[1]);
         dsa[jn >> 1][(jn & 1) * 2 + 1] = pack2<T>(ds[2], ds[3]);
         if constexpr (DQ) {        // [key][query] rows of 128 B, 16-byte chunk c of row r stored at chunk c ^ (r % 8)
@@ -331,9 +377,10 @@ __device__ __forceinline__ void dkv_body(const CUtensorMap& map_q, const CUtenso
   }
 }
 
-template <typename T, bool MASKED, int D>
+// DROPOUT: as in dkv_body, with the forward's call layout (row = query)
+template <typename T, bool MASKED, int D, bool DROPOUT = false, typename P = Params>
 __device__ __forceinline__ void dq_body(const CUtensorMap& map_q, const CUtensorMap& map_k, const CUtensorMap& map_v,
-                                        const CUtensorMap& map_do, const Params p) {
+                                        const CUtensorMap& map_do, const P p) {
   static_assert(D == HD || D == 64, "head_dim 128 or 64");
   constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
   constexpr int BM = 128, BK = 64;
@@ -406,6 +453,29 @@ __device__ __forceinline__ void dq_body(const CUtensorMap& map_q, const CUtensor
     }
     const int4* cmp = MASKED ? p.colmask + ((int64_t)batch * p.mask_heads + (p.mask_heads > 1 ? head : 0)) * p.sk : nullptr;
     (void)cmp;
+    uint32_t dk0 = 0, dk1 = 0, dc2 = 0, dc3 = 0, drc = 0;
+    if constexpr (DROPOUT) {
+      const uint64_t seed = (uint64_t)__ldg(p.seed_offset);
+      dk0 = (uint32_t)seed; dk1 = (uint32_t)(seed >> 32);
+      dropout::plane_counter(__ldg(p.seed_offset + 1), batch, p.h, head, dc2, dc3);
+      drc = dropout::row_counter(m0 + rl);
+    }
+    // DROPOUT: the keep bits of key tile jt, bit 8 (jn >> 1) + 4 h + 2 (jn & 1) + e as in the forward; tile j + 1's are drawn while the
+    // dQ MMAs of tile j are in flight, where S and dP are dead
+    auto draw = [&](int jt) {
+      uint32_t bits = 0;
+      if constexpr (DROPOUT) {
+#pragma unroll 1
+        for (int kk = 0; kk < BK / 16; ++kk)   // one call's temporaries live at a time
+          bits |= dropout::keep_bits(drc, dropout::key_counter(jt * BK + 16 * kk + 2 * q), dk0, dk1, dc2, dc3, p.keep) << (8 * kk);
+      }
+      return bits;
+    };
+    uint32_t keep = 0;
+    if constexpr (DROPOUT) {
+      if (n_tiles > 0) keep = draw(0);
+    }
+    (void)draw;
     if (n_tiles > 0) mbar_wait(qdo_full, 0);
     for (int j = 0; j < n_tiles; ++j) {
       const int s = j & 1, n0 = j * BK;
@@ -444,7 +514,9 @@ __device__ __forceinline__ void dq_body(const CUtensorMap& map_q, const CUtensor
             if constexpr (MASKED) {
               if ((row >= m.x && row < m.y) || (row >= m.z && row < m.w)) x = 0.f;
             }
-            ds[h * 2 + e] = x * (dpv[jn * 4 + h * 2 + e] - dl[h]) * p.scale;
+            float dp = dpv[jn * 4 + h * 2 + e];
+            if constexpr (DROPOUT) dp = (keep >> (8 * (jn >> 1) + 4 * h + 2 * (jn & 1) + e)) & 1u ? dp * p.rscale : 0.f;
+            ds[h * 2 + e] = x * (dp - dl[h]) * p.scale;
           }
         }
         dsa[jn >> 1][(jn & 1) * 2 + 0] = pack2<T>(ds[0], ds[1]);
@@ -459,6 +531,9 @@ __device__ __forceinline__ void dq_body(const CUtensorMap& map_q, const CUtensor
         else wgmma_rs_n64<BF16, 1>(dq_acc, dsa[ks], desc, 1);
       }
       wgmma_commit();
+      if constexpr (DROPOUT) {
+        if (j + 1 < n_tiles) keep = draw(j + 1);
+      }
       wgmma_wait<0>();
       wgmma_fence_regs(dq_acc);
       keep_regs(dsa);
@@ -595,9 +670,10 @@ void launch(const Params& p, bool deterministic, const CUtensorMap (&mq)[2], con
   }
 }
 
-// The backward at head size D (the operands checked by attention_bwd).
-template <int D>
-int run(const AttnBwdArgs& a, cudaStream_t s) {
+// The backward at head size D (the operands checked by attention_bwd): builds the tensor maps, launches the stats kernel and calls
+// launch(T(), std::bool_constant<MASKED>(), params, deterministic, maps...) for the main kernels of the operands' type and mask.
+template <int D, typename Launch>
+int run_with(const AttnBwdArgs& a, cudaStream_t s, Launch&& launch) {
   const AttnArgs& f = a.fwd;
   if (a.dq_strides[0] % 4 || a.dq_strides[1] % 4 || a.dq_strides[2] % 4 || (reinterpret_cast<uintptr_t>(a.dq) & 15)) return 1;   // TMA / float4
   if (a.dkv_strides[0] % 2 || a.dkv_strides[1] % 2 || a.dkv_strides[2] % 2) return 1;
@@ -639,13 +715,21 @@ int run(const AttnBwdArgs& a, cudaStream_t s) {
   p.dkv_sb = a.dkv_strides[0]; p.dkv_ss = a.dkv_strides[1]; p.dkv_sh = a.dkv_strides[2];
   p.dq_sb = a.dq_strides[0]; p.dq_ss = a.dq_strides[1]; p.dq_sh = a.dq_strides[2];
   if (f.dtype == kBF16) {
-    if (p.colmask) launch<D, __nv_bfloat16, true>(p, det, mq, mk, mv, mdo, mdq, s);
-    else launch<D, __nv_bfloat16, false>(p, det, mq, mk, mv, mdo, mdq, s);
+    if (p.colmask) launch(__nv_bfloat16(), std::true_type(), p, det, mq, mk, mv, mdo, mdq);
+    else launch(__nv_bfloat16(), std::false_type(), p, det, mq, mk, mv, mdo, mdq);
   } else {
-    if (p.colmask) launch<D, __half, true>(p, det, mq, mk, mv, mdo, mdq, s);
-    else launch<D, __half, false>(p, det, mq, mk, mv, mdo, mdq, s);
+    if (p.colmask) launch(__half(), std::true_type(), p, det, mq, mk, mv, mdo, mdq);
+    else launch(__half(), std::false_type(), p, det, mq, mk, mv, mdo, mdq);
   }
   return B200_LAUNCH_RESULT();
+}
+
+template <int D>
+int run(const AttnBwdArgs& a, cudaStream_t s) {
+  return run_with<D>(a, s, [&](auto tag_t, auto tag_masked, const Params& p, bool det, const CUtensorMap (&mq)[2], const CUtensorMap (&mk)[2],
+                               const CUtensorMap (&mv)[2], const CUtensorMap (&mdo)[2], const CUtensorMap& mdq) {
+    launch<D, decltype(tag_t), decltype(tag_masked)::value>(p, det, mq, mk, mv, mdo, mdq, s);
+  });
 }
 
 }  // namespace attn_bwd

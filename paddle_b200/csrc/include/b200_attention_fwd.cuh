@@ -11,6 +11,7 @@
 #include "b200_common.cuh"
 #include "b200_kv8.cuh"
 #include "b200_ops.h"
+#include "b200_philox.cuh"
 #include "b200_ptx.cuh"
 
 namespace b200 {
@@ -24,6 +25,7 @@ constexpr uint32_t TILE_BYTES = 128 * 128 * 2;   // 32 KB: every operand tile (Q
 constexpr uint32_t HALF_BYTES = 128 * 64 * 2;    // one 64-wide K-block of a tile
 // Q, 2x K, 2x V tiles of 128 rows x D
 template <int D> constexpr uint32_t kSmemBytes = 5 * (128 * D * 2) + 1024 /*align*/ + 256 /*barriers*/;
+constexpr uint32_t kDropoutSmemBytes = 128 + kThreads * 8;   // DROPOUT: one 64-bit keep mask per thread past the barriers' 128 bytes
 constexpr uint32_t SMEM_BYTES = kSmemBytes<HD>;
 
 struct Params {
@@ -60,13 +62,15 @@ __device__ __forceinline__ void st_shared_zero16(uint32_t addr) {
 
 // MASKED, PAGED, KV, D: see fwd_kernel in attention_sm100.cu.
 // WINDOW (PAGED only, P = WindowParams<...>): sliding window p.window, see fwd_body's key range below
-template <typename T, bool MASKED, bool PAGED, typename KV, int D, bool WINDOW, typename P>
+// DROPOUT (dense only, P = dropout::DropoutParams<Params>): attention dropout, see attention_dropout_sm100.cu
+template <typename T, bool MASKED, bool PAGED, typename KV, int D, bool WINDOW, bool DROPOUT = false, typename P>
 __device__ __forceinline__ void fwd_body(const CUtensorMap& map_q, const CUtensorMap& map_k, const CUtensorMap& map_v, const P p) {
   constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
   constexpr bool Q8 = !std::is_same<KV, T>::value;
   static_assert(!Q8 || (PAGED && !MASKED), "8-bit caches are paged only");
   static_assert(D == HD || (D == 64 && !Q8), "head_dim 64 reads 16-bit K / V only");
   static_assert(!WINDOW || (PAGED && !MASKED), "sliding windows are paged only");
+  static_assert(!DROPOUT || !PAGED, "dropout is dense (training) only");
   constexpr int kHalves = D / 64;                            // 64-wide d chunks (128-byte swizzle spans) of a row
   constexpr uint32_t kTile = BM * D * 2;                     // one Q, K or V tile
   constexpr uint32_t kVBlock = kHalves * 8192;               // one 64-key block of a V tile (its d chunks 8192 B apart)
@@ -251,6 +255,41 @@ __device__ __forceinline__ void fwd_body(const CUtensorMap& map_q, const CUtenso
 #pragma unroll
     for (int i = 0; i < D / 2; ++i) o_acc[i] = 0.f;
     float m_i[2] = {-INFINITY, -INFINITY}, l_i[2] = {0.f, 0.f};   // l_i: this thread's share of the row sum (reduced over the quad at the end)
+    // DROPOUT: the keep bits of key tile jt (see b200_philox.cuh); rows rl and rl + 8 share every call, and call kk covers key column
+    // groups 2 kk, 2 kk + 1: bit 8 kk + 4 h + 2 (jn & 1) + e.  Tile j + 1's bits are drawn while the P V MMAs of tile j are in flight,
+    // where S is dead, and the key and counter words are rebuilt on each draw: held across the loop (or drawn under the S MMAs) they
+    // would make the D = 128 kernel spill.
+    auto draw = [&](int jt) {
+      uint64_t bits = 0;
+      if constexpr (DROPOUT) {
+        const uint64_t seed = p.seed_ptr ? (uint64_t)__ldg(p.seed_ptr) : p.seed;
+        const int64_t offset = p.seed_ptr ? __ldg(p.offset_ptr) + p.offset_add : (int64_t)p.offset;
+        uint32_t c2, c3;
+        dropout::plane_counter(offset, batch, p.h, head, c2, c3);
+        const uint32_t rc = dropout::row_counter(m0 + rl);
+        uint32_t lo = 0, hi = 0;   // word h: the bits of row rl + 8 h, call kk at bits 4 kk + 2 (jn & 1) + e
+#pragma unroll 1
+        for (int kk = 0; kk < BN / 16; ++kk) {   // one call's temporaries live at a time
+          const uint32_t b = dropout::keep_bits(rc, dropout::key_counter(jt * BN + 16 * kk + 2 * q), (uint32_t)seed, (uint32_t)(seed >> 32), c2, c3,
+                                                p.keep);
+          lo |= (b & 15u) << (4 * kk);
+          hi |= (b >> 4) << (4 * kk);
+        }
+        bits = ((uint64_t)hi << 32) | lo;
+      }
+      return bits;
+    };
+    // the bits wait in shared memory past the barriers (kDropoutSmemBytes more), not in registers, while S and O fill the register file
+    uint64_t* const keep_slot = reinterpret_cast<uint64_t*>(smem_raw + (bars + 128 - smem_u32(smem_raw))) + threadIdx.x;
+    (void)keep_slot;
+    if constexpr (DROPOUT) {
+      if ((blockIdx.x | blockIdx.y | blockIdx.z | threadIdx.x) == 0) {   // the pair this launch used, for the backward
+        p.seed_offset[0] = p.seed_ptr ? __ldg(p.seed_ptr) : (int64_t)p.seed;
+        p.seed_offset[1] = p.seed_ptr ? __ldg(p.offset_ptr) + p.offset_add : (int64_t)p.offset;
+      }
+      if (j0 < n_tiles) *keep_slot = draw(j0);
+    }
+    (void)draw;
     if (n_tiles > 0) mbar_wait(q_full, 0);
     for (int j = j0; j < n_tiles; ++j) {
       const int s = (j - j0) & 1, ph = ((j - j0) >> 1) & 1;
@@ -338,6 +377,15 @@ __device__ __forceinline__ void fwd_body(const CUtensorMap& map_q, const CUtenso
         l_i[h] = l_i[h] * alpha + sum;
 #pragma unroll
         for (int jn = 0; jn < D / 8; ++jn) { o_acc[jn * 4 + h * 2] *= alpha; o_acc[jn * 4 + h * 2 + 1] *= alpha; }
+        if constexpr (DROPOUT) {   // after the row sum: l and lse stay those of the undropped softmax
+          const uint32_t keep = reinterpret_cast<const uint32_t*>(keep_slot)[h];   // bits of row h in word h (see draw)
+#pragma unroll
+          for (int jn = 0; jn < BN / 8; ++jn)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              if (!((keep >> (4 * (jn >> 1) + 2 * (jn & 1) + e)) & 1u)) sv[jn * 4 + h * 2 + e] = 0.f;
+            }
+        }
       }
       // ---- P as A fragments: 16-key step ks = accumulator column groups 2 ks and 2 ks + 1 ----
       uint32_t pa[BN / 16][4];
@@ -382,6 +430,9 @@ __device__ __forceinline__ void fwd_body(const CUtensorMap& map_q, const CUtenso
         else wgmma_rs_n64<BF16, 1>(o_acc, pa[ks], vdesc, 1);
       }
       wgmma_commit();
+      if constexpr (DROPOUT) {
+        if (j + 1 < n_tiles) *keep_slot = draw(j + 1);
+      }
       wgmma_wait<0>();
       wgmma_fence_regs(o_acc);
 #pragma unroll
@@ -399,6 +450,7 @@ __device__ __forceinline__ void fwd_body(const CUtensorMap& map_q, const CUtenso
       l += __shfl_xor_sync(0xffffffffu, l, 2);
       float inv = l > 0.f ? 1.f / l : 0.f;
       if constexpr (Q8) inv *= __ldg(p.v_dq + kv_head);   // O is accumulated on the quantized V
+      if constexpr (DROPOUT) inv *= p.rscale;             // 1 / (1 - p): kept entries of P enter P V unscaled
       const int row = m0 + rl + h * 8;
       if (row < nrows) {
         T* orow = reinterpret_cast<T*>(p.o) + (PAGED ? 0 : (int64_t)batch * p.o_sb) + (int64_t)(q0 + row) * p.o_ss + (int64_t)head * p.o_sh;
@@ -423,9 +475,10 @@ fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CU
   fwd_body<T, MASKED, PAGED, KV, D, false>(map_q, map_k, map_v, p);
 }
 
-// The dense forward at head size D over the strided [B,S,H,D] views of AttnArgs (checked by attention_fwd_supported).
-template <int D>
-int fwd_dense(const AttnArgs& a, cudaStream_t s) {
+// The dense forward at head size D over the strided [B,S,H,D] views of AttnArgs (checked by attention_fwd_supported): builds the
+// tensor maps and parameters and calls launch(T(), std::bool_constant<MASKED>(), maps, params, grid, smem) for the operands' type and mask.
+template <int D, typename Launch>
+int fwd_dense_with(const AttnArgs& a, cudaStream_t s, Launch&& launch) {
   CUtensorMap mq, mk, mv;
   // strides arrays are (batch, seq, head)
   if (!make_map4(&mq, a.q, a.d, a.sq, a.h, a.b, a.q_strides[1], a.q_strides[2], a.q_strides[0], BM, a.dtype)) return 2;
@@ -441,17 +494,22 @@ int fwd_dense(const AttnArgs& a, cudaStream_t s) {
   p.mask_heads = a.mask_heads > 0 ? a.mask_heads : 1;
   const dim3 grid((a.sq + BM - 1) / BM, a.h, a.b);
   constexpr uint32_t smem = kSmemBytes<D>;
-  auto launch = [&](auto tag_t, auto tag_masked) {
+  if (a.dtype == kBF16 && !p.colmask) launch(__nv_bfloat16(), std::false_type(), mq, mk, mv, p, grid, smem);
+  else if (a.dtype == kBF16) launch(__nv_bfloat16(), std::true_type(), mq, mk, mv, p, grid, smem);
+  else if (!p.colmask) launch(__half(), std::false_type(), mq, mk, mv, p, grid, smem);
+  else launch(__half(), std::true_type(), mq, mk, mv, p, grid, smem);
+  return B200_LAUNCH_RESULT();
+}
+
+template <int D>
+int fwd_dense(const AttnArgs& a, cudaStream_t s) {
+  return fwd_dense_with<D>(a, s, [&](auto tag_t, auto tag_masked, const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv,
+                                     const Params& p, dim3 grid, uint32_t smem) {
     using T = decltype(tag_t);
     constexpr bool MASKED = decltype(tag_masked)::value;
     set_max_dynamic_smem<fwd_kernel<T, MASKED, false, T, D>>(smem);
     fwd_kernel<T, MASKED, false, T, D><<<grid, kThreads, smem, s>>>(mq, mk, mv, p);
-  };
-  if (a.dtype == kBF16 && !p.colmask) launch(__nv_bfloat16(), std::false_type());
-  else if (a.dtype == kBF16) launch(__nv_bfloat16(), std::true_type());
-  else if (!p.colmask) launch(__half(), std::false_type());
-  else launch(__half(), std::true_type());
-  return B200_LAUNCH_RESULT();
+  });
 }
 
 // A paged instantiation's parameters with a sliding window: key j is visible to query i iff i - window < j <= i (window >= 1).

@@ -378,6 +378,21 @@ struct AttnBwdArgs {
 };
 int attention_bwd(const AttnBwdArgs& a, cudaStream_t s);
 int attention_bwd_d64(const AttnBwdArgs& a, cudaStream_t s);   // head_dim 64 (attention_d64_sm100.cu), called by attention_bwd
+// Attention dropout (attention_dropout_sm100.cu): the dense / column-masked forward and backward above with the probabilities dropped
+// at rate p (0 < p < 1) and the kept ones scaled by 1 / (1 - p).  The mask is a pure function of (seed, offset, batch, head, query, key)
+// (include/b200_philox.cuh); a call uses the generator offsets offset .. offset + B H - 1.  The forward resolves (seed, offset) on the
+// device (seed_ptr != nullptr: *seed_ptr and *offset_ptr + offset_add, a CUDA-graph-safe generator state; otherwise seed and offset)
+// and writes them to seed_offset; the backward reads its mask from seed_offset alone.
+struct AttnDropoutArgs {
+  double p;
+  int64_t* seed_offset;                 // int64 [2] on the device
+  const int64_t* seed_ptr = nullptr;    // forward only
+  const int64_t* offset_ptr = nullptr;
+  int64_t offset_add = 0;
+  uint64_t seed = 0, offset = 0;
+};
+int attention_fwd_dropout(const AttnArgs& a, const AttnDropoutArgs& d, cudaStream_t s);
+int attention_bwd_dropout(const AttnBwdArgs& a, const AttnDropoutArgs& d, cudaStream_t s);
 
 // Token sampling (sampling.cu): one CTA per row of x [rows, vocab] (row stride `stride` elements, unit column stride).  Per-row device
 // arrays: temperature (<= 0: greedy), top_k (int32, 0: off), top_p (1: off), threshold (optional), seed / offset (int64).  Writes ids and

@@ -21,6 +21,7 @@
 
 #include "include/b200_common.cuh"
 #include "include/b200_ops.h"
+#include "include/b200_philox.cuh"
 
 namespace b200 {
 namespace {
@@ -42,17 +43,6 @@ struct SampleSmem {
   int top_idx[kMaxTop];
   int warp_cnt[32];
 };
-
-__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
-#pragma unroll
-  for (int r = 0; r < 10; ++r) {
-    if (r) { k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
-    const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
-    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
-    c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
-  }
-  return c;
-}
 
 __device__ __forceinline__ uint4 philox_quad(int64_t seed, int64_t offset, uint32_t quad) {
   return philox4x32_10(make_uint4(quad, 0u, (uint32_t)offset, (uint32_t)((uint64_t)offset >> 32)), (uint32_t)seed,

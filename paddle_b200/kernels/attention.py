@@ -2,9 +2,11 @@
 (python/paddle/nn/functional/flash_attention.py).
 
 Dispatch: the sm_90a wgmma flash kernels for fp16/bf16, head_dim 128 (csrc/attention_sm100.cu) or 64
-(csrc/attention_d64_sm100.cu), no explicit mask and no dropout — they read q/k/v in place as strided views of a packed QKV
-projection, and a column-wise row-range mask (attention_colmask) runs on the same kernels.  Other head sizes, dense masks and
-dropout take the PyTorch SDPA (library) path.  Backward: csrc/attention_bwd_sm100.cu (B200_ATTN_BWD=own, default) or, for comparison, a library backward
+(csrc/attention_d64_sm100.cu), no explicit mask — they read q/k/v in place as strided views of a packed QKV
+projection, and a column-wise row-range mask (attention_colmask) runs on the same kernels.  Attention dropout (0 < p < 1) runs on
+their dropout instantiations (csrc/attention_dropout_sm100.cu): the mask is a pure function of (seed, offset, batch, head, query,
+key) (dropout_keep_mask is its torch twin), drawn from torch's CUDA generator or a given `seed_offset` (int64 [2]), and the backward
+regenerates it from the pair the forward used.  Other head sizes, dense masks and dropout >= 1 take the PyTorch SDPA (library) path.  Backward: csrc/attention_bwd_sm100.cu (B200_ATTN_BWD=own, default) or, for comparison, a library backward
 fed with our forward's (out, logsumexp) (B200_ATTN_BWD=cudnn|flash).  The own backward is a single pass that bulk-reduces dQ in
 arrival order (reproducible to rounding); FLAGS_cudnn_deterministic switches it to a bitwise-reproducible dK/dV + dQ kernel pair.
 """
@@ -37,21 +39,75 @@ def attention_ref(q, k, v, mask=None, dropout_p=0.0, causal=False, scale=None):
 _bwd_backend = [__import__("os").environ.get("B200_ATTN_BWD", "own")]   # own | cudnn | flash
 
 
+_U32 = 0xFFFFFFFF
+
+
+def dropout_keep(p):
+    """The kernels' 16-bit keep threshold: an element is kept iff its draw is below round((1 - p) * 2^16)."""
+    return int(round((1.0 - float(p)) * 65536.0))
+
+
+def dropout_keep_mask(seed, offset, b, h, sq, sk, p=0.1, device=None):
+    """The attention dropout mask of the kernels, bool [b, h, sq, sk] (True: kept), for a call with generator (seed, offset).
+
+    Element (b, h, i, j) is kept iff its 16-bit Philox4x32-10 draw is below dropout_keep(p) (csrc/include/b200_philox.cuh): key
+    (seed lo, seed hi), counter (kc, rc, (offset + b H + h) lo, hi) with rc = 8 (i >> 4) + (i & 7), kc = 4 (j >> 4) + ((j & 7) >> 1),
+    half (j & 1) of output word 2 ((i >> 3) & 1) + ((j >> 3) & 1).  Computed on the CPU with int64 torch ops."""
+    from .sampling import philox4x32_10
+
+    seed, offset = int(seed) & 0xFFFFFFFFFFFFFFFF, int(offset)
+    i = torch.arange(sq, dtype=torch.int64)
+    j = torch.arange(sk, dtype=torch.int64)
+    rc = ((i >> 4) << 3) | (i & 7)                                         # [sq]
+    kc = ((j >> 4) << 2) | ((j & 7) >> 1)                                  # [sk]
+    plane = offset + torch.arange(b * h, dtype=torch.int64)                # [b h]
+    nr, nk = int(rc.max()) + 1 if sq else 0, int(kc.max()) + 1 if sk else 0
+    P, R, C = torch.meshgrid(torch.arange(b * h), torch.arange(nr), torch.arange(nk), indexing="ij")
+    words = torch.stack(philox4x32_10(seed & _U32, (seed >> 32) & _U32, C, R, plane[P] & _U32, (plane[P] >> 32) & _U32), -1).reshape(-1)
+    word = 2 * ((i >> 3) & 1).reshape(-1, 1) + ((j >> 3) & 1).reshape(1, -1)                      # [sq, sk]
+    at = ((torch.arange(b * h).reshape(-1, 1, 1) * nr + rc.reshape(1, -1, 1)) * nk + kc.reshape(1, 1, -1)) * 4 + word
+    draw = (words[at] >> (16 * (j & 1))) & 0xFFFF
+    keep = (draw < dropout_keep(p)).reshape(b, h, sq, sk)
+    return keep.to(device) if device is not None else keep
+
+
+def _seed_offset_arg(seed_offset):
+    """fixed seed_offset (paddle's fixed_seed_offset: int64 [2] = (seed, offset)) as a tensor the kernels read, or None."""
+    if seed_offset is None:
+        return None
+    t = raw(seed_offset)
+    if not isinstance(t, torch.Tensor):
+        t = torch.tensor([int(x) for x in t], dtype=torch.int64)
+    return t.to(torch.int64).reshape(2).contiguous()
+
+
+def _dropout_ok(dropout_p):
+    return 0.0 <= float(dropout_p) < 1.0
+
+
 class _FlashAttn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, q, k, v, scale, causal):
-        out, lse = ext().attention_fwd(q, k, v, scale, causal)
-        ctx.save_for_backward(q, k, v, out, lse)
-        ctx.scale, ctx.causal = scale, causal
-        return out
+    def forward(ctx, q, k, v, scale, causal, dropout_p=0.0, seed_offset=None):
+        res = ext().attention_fwd(q, k, v, scale, causal, False, None, dropout_p, seed_offset)
+        out, lse = res[0], res[1]
+        so = res[2] if dropout_p > 0.0 else None
+        ctx.save_for_backward(q, k, v, out, lse, so)
+        ctx.scale, ctx.causal, ctx.dropout_p = scale, causal, dropout_p
+        ctx.seed_offset = so
+        if so is not None:
+            ctx.mark_non_differentiable(so)
+        return out, so
 
     @staticmethod
-    def backward(ctx, do):
-        q, k, v, out, lse = ctx.saved_tensors
+    def backward(ctx, do, _dso=None):
+        q, k, v, out, lse, so = ctx.saved_tensors
         do = do.contiguous()
+        if ctx.dropout_p > 0.0:
+            dq, dk, dv = ext().attention_bwd(q, k, v, out, lse, do, ctx.scale, ctx.causal, None, ctx.dropout_p, so)
+            return dq, dk, dv, None, None, None, None
         if _bwd_backend[0] == "own":   # csrc/attention_bwd_sm100.cu: single pass, or dK/dV + dQ kernels under FLAGS_cudnn_deterministic
             dq, dk, dv = ext().attention_bwd(q, k, v, out, lse, do, ctx.scale, ctx.causal)
-            return dq, dk, dv, None, None
+            return dq, dk, dv, None, None, None, None
         if _bwd_backend[0] == "cudnn" and q.shape[2] == k.shape[2]:
             # Hopper-tuned library backward fed with OUR forward's (out, logsumexp); [B,S,H,D] tensors enter as [B,H,S,D] views
             try:
@@ -59,14 +115,14 @@ class _FlashAttn(torch.autograd.Function):
                 dq, dk, dv = torch.ops.aten._scaled_dot_product_cudnn_attention_backward(
                     do.transpose(1, 2), q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2), out.transpose(1, 2), lse.unsqueeze(-1), z, z,
                     None, None, None, q.shape[1], k.shape[1], 0.0, ctx.causal, scale=ctx.scale)
-                return dq.transpose(1, 2), dk.transpose(1, 2), dv.transpose(1, 2), None, None
+                return dq.transpose(1, 2), dk.transpose(1, 2), dv.transpose(1, 2), None, None, None, None
             except Exception:  # noqa: BLE001  (op unavailable / shape unsupported: use the flash backward from here on)
                 _bwd_backend[0] = "flash"
         empty = torch.empty(0, dtype=torch.int64, device=q.device)
         rng = torch.zeros(2, dtype=torch.int64, device=q.device)
         dq, dk, dv = torch.ops.aten._flash_attention_backward(do, q, k, v, out, lse, None, None, q.shape[1], k.shape[1], 0.0, ctx.causal,
                                                                rng, empty, scale=ctx.scale)
-        return dq, dk, dv, None, None
+        return dq, dk, dv, None, None, None, None
 
 
 class _FlashAttnColMask(torch.autograd.Function):
@@ -76,17 +132,24 @@ class _FlashAttnColMask(torch.autograd.Function):
     attention_bwd_sm100.cu) with the mask test added to their score-tile loops."""
 
     @staticmethod
-    def forward(ctx, q, k, v, colmask, scale, causal):
-        out, lse = ext().attention_fwd(q, k, v, scale, causal, False, colmask)
-        ctx.save_for_backward(q, k, v, out, lse, colmask)
-        ctx.scale, ctx.causal = scale, causal
-        return out
+    def forward(ctx, q, k, v, colmask, scale, causal, dropout_p=0.0, seed_offset=None):
+        res = ext().attention_fwd(q, k, v, scale, causal, False, colmask, dropout_p, seed_offset)
+        out, lse = res[0], res[1]
+        so = res[2] if dropout_p > 0.0 else None
+        ctx.save_for_backward(q, k, v, out, lse, colmask, so)
+        ctx.scale, ctx.causal, ctx.dropout_p = scale, causal, dropout_p
+        if so is not None:
+            ctx.mark_non_differentiable(so)
+        return out, so
 
     @staticmethod
-    def backward(ctx, do):
-        q, k, v, out, lse, colmask = ctx.saved_tensors
-        dq, dk, dv = ext().attention_bwd(q, k, v, out, lse, do.contiguous(), ctx.scale, ctx.causal, colmask)
-        return dq, dk, dv, None, None, None
+    def backward(ctx, do, _dso=None):
+        q, k, v, out, lse, colmask, so = ctx.saved_tensors
+        if ctx.dropout_p > 0.0:
+            dq, dk, dv = ext().attention_bwd(q, k, v, out, lse, do.contiguous(), ctx.scale, ctx.causal, colmask, ctx.dropout_p, so)
+        else:
+            dq, dk, dv = ext().attention_bwd(q, k, v, out, lse, do.contiguous(), ctx.scale, ctx.causal, colmask)
+        return dq, dk, dv, None, None, None, None, None
 
 
 _INT_MAX = 2 ** 31 - 1
@@ -135,13 +198,17 @@ def colmask_from_window(sq, sk, left, right, causal, device):
     return torch.stack([lts, lte, uts, ute], -1).reshape(1, 1, sk, 4).contiguous()
 
 
-def attention_colmask(q, k, v, colmask, causal=False, scale=None):
-    """[B,S,H,D] attention under a column-wise row-range mask on the own wgmma kernels; None if the operands do not qualify."""
+def attention_colmask(q, k, v, colmask, causal=False, scale=None, dropout_p=0.0, seed_offset=None, return_seed_offset=False):
+    """[B,S,H,D] attention under a column-wise row-range mask on the own wgmma kernels; None if the operands do not qualify.
+    dropout_p > 0: attention dropout (mask of `seed_offset`, or of torch's CUDA generator); with return_seed_offset the result is
+    (out, the int64 [2] (seed, offset) of the mask)."""
     q, k, v = raw(q), raw(k), raw(v)
-    if not fused_ok(q, k, v, None, 0.0, causal):
+    if not fused_ok(q, k, v, None, dropout_p, causal):
         return None
     sc = float(scale) if scale is not None else 1.0 / math.sqrt(q.shape[-1])
-    return wrap(_FlashAttnColMask.apply(q, k, v, raw(colmask).to(torch.int32).contiguous(), sc, bool(causal)))
+    out, so = _FlashAttnColMask.apply(q, k, v, raw(colmask).to(torch.int32).contiguous(), sc, bool(causal), float(dropout_p),
+                                      _seed_offset_arg(seed_offset))
+    return (wrap(out), so) if return_seed_offset else wrap(out)
 
 
 def colmask_to_dense(colmask, sq):
@@ -159,36 +226,47 @@ class _FlashAttnPacked(torch.autograd.Function):
     autograd never builds zero-filled slice gradients and the sequence-parallel layout needs no transpose copies."""
 
     @staticmethod
-    def forward(ctx, qkv, nh, nkv, scale, causal, seq_major):
+    def forward(ctx, qkv, nh, nkv, scale, causal, seq_major, dropout_p=0.0, seed_offset=None):
         x = qkv.transpose(0, 1) if seq_major else qkv
         q, k, v = x[:, :, :nh], x[:, :, nh:nh + nkv], x[:, :, nh + nkv:]
-        out, lse = ext().attention_fwd(q, k, v, scale, causal, seq_major)    # out: same memory order as qkv
-        ctx.save_for_backward(qkv, out, lse)
-        ctx.cfg = (nh, nkv, scale, causal, seq_major)
-        return out
+        res = ext().attention_fwd(q, k, v, scale, causal, seq_major, None, dropout_p, seed_offset)    # out: same memory order as qkv
+        out, lse = res[0], res[1]
+        so = res[2] if dropout_p > 0.0 else None
+        ctx.save_for_backward(qkv, out, lse, so)
+        ctx.cfg = (nh, nkv, scale, causal, seq_major, dropout_p)
+        if so is not None:
+            ctx.mark_non_differentiable(so)
+        return out, so
 
     @staticmethod
-    def backward(ctx, do):
-        qkv, out, lse = ctx.saved_tensors
-        nh, nkv, scale, causal, seq_major = ctx.cfg
-        return ext().attention_bwd_packed(qkv, nh, nkv, out, lse, do.contiguous(), scale, causal, seq_major), None, None, None, None, None
+    def backward(ctx, do, _dso=None):
+        qkv, out, lse, so = ctx.saved_tensors
+        nh, nkv, scale, causal, seq_major, dropout_p = ctx.cfg
+        if dropout_p > 0.0:
+            dqkv = ext().attention_bwd_packed(qkv, nh, nkv, out, lse, do.contiguous(), scale, causal, seq_major, dropout_p, so)
+        else:
+            dqkv = ext().attention_bwd_packed(qkv, nh, nkv, out, lse, do.contiguous(), scale, causal, seq_major)
+        return dqkv, None, None, None, None, None, None, None
 
 
-def attention_packed(qkv, nh, nkv, causal=True, scale=None, seq_major=False):
+def attention_packed(qkv, nh, nkv, causal=True, scale=None, seq_major=False, dropout_p=0.0, seed_offset=None, return_seed_offset=False):
     """qkv: [B,S,nh+2*nkv,D] contiguous (q heads | k heads | v heads), or [S,B,...] with seq_major=True (the layout of
-    sequence-parallel layers). Returns [B,S,nh,D] (resp. [S,B,nh,D])."""
+    sequence-parallel layers). Returns [B,S,nh,D] (resp. [S,B,nh,D]).  dropout_p, seed_offset, return_seed_offset: as `attention`."""
     x = raw(qkv)
     xb = x.transpose(0, 1) if seq_major else x
     q, k, v = xb[:, :, :nh], xb[:, :, nh:nh + nkv], xb[:, :, nh + nkv:]
-    if _bwd_backend[0] == "own" and x.is_contiguous() and fused_ok(q, k, v, None, 0.0, causal):
+    if _bwd_backend[0] == "own" and x.is_contiguous() and fused_ok(q, k, v, None, dropout_p, causal):
         sc = float(scale) if scale is not None else 1.0 / math.sqrt(x.shape[-1])
-        return wrap(_FlashAttnPacked.apply(x, int(nh), int(nkv), sc, bool(causal), bool(seq_major)))
-    out = attention(q, k, v, None, 0.0, causal, scale)
+        out, so = _FlashAttnPacked.apply(x, int(nh), int(nkv), sc, bool(causal), bool(seq_major), float(dropout_p), _seed_offset_arg(seed_offset))
+        return (wrap(out), so) if return_seed_offset else wrap(out)
+    if return_seed_offset:
+        raise ValueError("attention_packed: return_seed_offset needs the own kernels (fp16/bf16, head_dim 64 or 128, 0 <= dropout_p < 1)")
+    out = attention(q, k, v, None, dropout_p, causal, scale)
     return wrap(raw(out).transpose(0, 1).contiguous()) if seq_major else out
 
 
 def fused_ok(q, k, v, mask, dropout_p, causal):
-    if not (use_fused(q) and flag("FLAGS_b200_flash_attention", True)) or mask is not None or dropout_p != 0.0:
+    if not (use_fused(q) and flag("FLAGS_b200_flash_attention", True)) or mask is not None or not _dropout_ok(dropout_p):
         return False
     if q.dtype not in (torch.float16, torch.bfloat16) or q.dim() != 4 or q.shape[-1] not in (64, 128):
         return False
@@ -198,11 +276,17 @@ def fused_ok(q, k, v, mask, dropout_p, causal):
 
 
 @recordable
-def attention(q, k, v, mask=None, dropout_p=0.0, causal=False, scale=None):
+def attention(q, k, v, mask=None, dropout_p=0.0, causal=False, scale=None, seed_offset=None, return_seed_offset=False):
+    """[B,S,H,D] attention.  0 < dropout_p < 1 on the own kernels drops attention probabilities with the mask of `seed_offset` (int64 [2]
+    (seed, offset), used as given) or of torch's CUDA generator; return_seed_offset=True returns (out, the pair the mask was drawn
+    with), which replays the mask through `seed_offset` and `dropout_keep_mask`."""
     q, k, v, mask = raw(q), raw(k), raw(v), raw(mask)
     if fused_ok(q, k, v, mask, dropout_p, causal):
         sc = float(scale) if scale is not None else 1.0 / math.sqrt(q.shape[-1])
-        return wrap(_FlashAttn.apply(q, k, v, sc, bool(causal)))
+        out, so = _FlashAttn.apply(q, k, v, sc, bool(causal), float(dropout_p), _seed_offset_arg(seed_offset))
+        return (wrap(out), so) if return_seed_offset else wrap(out)
+    if return_seed_offset:
+        raise ValueError("attention: return_seed_offset needs the own kernels (fp16/bf16, head_dim 64 or 128, no dense mask, 0 <= dropout_p < 1)")
     if causal and mask is not None:
         sq, sk = q.shape[1], k.shape[1]
         cm = torch.ones(sq, sk, dtype=torch.bool, device=q.device).tril(sk - sq)

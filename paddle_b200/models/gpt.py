@@ -29,6 +29,7 @@ class GPTConfig:
     initializer_range: float = 0.02
     recompute: bool = False
     dropout: float = 0.0
+    attention_dropout: float = 0.0   # attention-probability dropout in training (the flash kernels' dropout instantiations)
 
     @property
     def head_dim(self):
@@ -71,7 +72,7 @@ class GPTBlock(nn.Layer):
         cfg = self.cfg
         b, s, h = x.shape
         qkv = _raw(self.qkv(self.ln1(x))).view(b, s, 3, cfg.num_attention_heads, cfg.head_dim)
-        a = KAT.attention(qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2], None, 0.0, True, None)
+        a = KAT.attention(qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2], None, cfg.attention_dropout if self.training else 0.0, True, None)
         x = x + self.proj(_raw(a).reshape(b, s, h).as_subclass(Tensor))
         y = self.ln2(x)
         y = KG.gemm(_raw(y).reshape(-1, h), self.fc1.weight, self.fc1.bias, epilogue=2).reshape(b, s, -1) if _fused_ok(y) and isinstance(self.fc1, nn.Linear) else F.gelu(self.fc1(y))

@@ -23,7 +23,7 @@ def flash_attention(query, key, value, dropout=0.0, causal=False, return_softmax
                     rng_name="", training=True, name=None):
     from ...kernels import attention as K
 
-    out = K.attention(T(query), T(key), T(value), None, dropout if training else 0.0, causal, None)
+    out = K.attention(T(query), T(key), T(value), None, dropout if training else 0.0, causal, None, seed_offset=fixed_seed_offset)
     return out, None
 
 
@@ -33,7 +33,7 @@ def flash_attn_qkvpacked(qkv, dropout=0.0, causal=False, return_softmax=False, f
     g = qkv.size(2) - 2
     b, s, _, hk, d = qkv.size()
     q = qkv[:, :, :g].reshape(b, s, g * hk, d)
-    return flash_attention(q, qkv[:, :, g], qkv[:, :, g + 1], dropout, causal, return_softmax, training=training)
+    return flash_attention(q, qkv[:, :, g], qkv[:, :, g + 1], dropout, causal, return_softmax, fixed_seed_offset=fixed_seed_offset, training=training)
 
 
 def flash_attn_unpadded(query, key, value, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, scale,
@@ -43,20 +43,21 @@ def flash_attn_unpadded(query, key, value, cu_seqlens_q, cu_seqlens_k, max_seqle
     from ...kernels import attention as K
 
     q, k, v = T(query), T(key), T(value)
-    if q.is_cuda and (dropout == 0.0 or not training) and q.dim() == 3:
+    p = dropout if training else 0.0
+    if q.is_cuda and q.dim() == 3:
         # packed batch as ONE sequence under a document mask: no host read of cu_seqlens, no per-sequence launches.
         # (causal: the diagonal of every sequence is the global diagonal when q and k are packed alike - self attention)
         same = cu_seqlens_q is cu_seqlens_k or (raw(cu_seqlens_q).shape == raw(cu_seqlens_k).shape and q.size(0) == k.size(0))
         if same or not causal:
             cm = K.colmask_from_cu_seqlens(cu_seqlens_q, cu_seqlens_k, k.size(0))
-            out = K.attention_colmask(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), cm, causal and same, scale)
+            out = K.attention_colmask(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), cm, causal and same, scale, p, fixed_seed_offset)
             if out is not None:
                 return out.squeeze(0), None
     cq, ck = raw(cu_seqlens_q).tolist(), raw(cu_seqlens_k).tolist()
     outs = []
     for i in range(len(cq) - 1):
         qi, ki, vi = q[cq[i]:cq[i + 1]], k[ck[i]:ck[i + 1]], v[ck[i]:ck[i + 1]]
-        outs.append(K.attention(qi.unsqueeze(0), ki.unsqueeze(0), vi.unsqueeze(0), None, dropout if training else 0.0, causal, scale).squeeze(0))
+        outs.append(K.attention(qi.unsqueeze(0), ki.unsqueeze(0), vi.unsqueeze(0), None, p, causal, scale).squeeze(0))
     return torch.cat(outs, 0), None
 
 
@@ -67,7 +68,8 @@ def flash_attn_varlen_qkvpacked(qkv, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, m
     g = qkv.size(1) - 2
     t, _, hk, d = qkv.size()
     q = qkv[:, :g].reshape(t, g * hk, d)
-    return flash_attn_unpadded(q, qkv[:, g], qkv[:, g + 1], cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, scale, dropout, causal, training=training)
+    return flash_attn_unpadded(q, qkv[:, g], qkv[:, g + 1], cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, scale, dropout, causal,
+                               fixed_seed_offset=fixed_seed_offset, training=training)
 
 
 def flashmask_attention(query, key, value, startend_row_indices=None, dropout=0.0, causal=False, window_size=None,
@@ -76,14 +78,16 @@ def flashmask_attention(query, key, value, startend_row_indices=None, dropout=0.
     """Column-wise sparse mask attention. Parity: flash_attention.py:flashmask_attention.
 
     startend_row_indices: [B, Hm, S_k, {1,2,4}] int32; for key column j, rows in [LTS, LTE) (lower triangle) and
-    [UTS, UTE) (upper) are masked.
+    [UTS, UTE) (upper) are masked.  Dropout in training runs on the own kernels; fixed_seed_offset (int64 [2]) fixes its mask, and
+    return_seed_offset=True returns [out, seed_offset], the pair that reproduces it.
     """
     from ...kernels import attention as K
 
     q, k, v = T(query), T(key), T(value)
     sq, sk = q.size(1), k.size(1)
     mask = None
-    if q.is_cuda and (dropout == 0.0 or not training) and (startend_row_indices is not None or window_size is not None):
+    p = dropout if training else 0.0
+    if q.is_cuda and (startend_row_indices is not None or window_size is not None):
         if startend_row_indices is not None:
             cm = K.colmask_from_startend(startend_row_indices, causal, sq)
         else:
@@ -91,9 +95,15 @@ def flashmask_attention(query, key, value, startend_row_indices=None, dropout=0.
             cm = K.colmask_from_window(sq, sk, int(w[0]), int(w[1]), causal, q.device)
         if cm.shape[0] == 1 and q.size(0) > 1:
             cm = cm.expand(q.size(0), -1, -1, -1).contiguous()
-        out = K.attention_colmask(q, k, v, cm, causal, None)
-        if out is not None:
-            return out
+        res = K.attention_colmask(q, k, v, cm, causal, None, p, fixed_seed_offset, return_seed_offset=True)
+        if res is not None:
+            return [res[0], res[1]] if return_seed_offset else res[0]
+    elif startend_row_indices is None and window_size is None:
+        res = K.attention(q, k, v, None, p, causal, None, seed_offset=fixed_seed_offset, return_seed_offset=return_seed_offset and K.fused_ok(
+            raw(q), raw(k), raw(v), None, p, causal))
+        if return_seed_offset:
+            return [res[0], res[1]] if isinstance(res, tuple) else [res, None]
+        return res
     if startend_row_indices is not None:
         idx = raw(startend_row_indices).long()
         rows = torch.arange(sq, device=q.device).reshape(1, 1, sq, 1)
@@ -120,8 +130,8 @@ def flashmask_attention(query, key, value, startend_row_indices=None, dropout=0.
         j = torch.arange(sk, device=q.device).unsqueeze(0)
         mask = (j >= i - w[0]) & ((j <= i + w[1]) if not causal else (j <= i))
         mask = mask.reshape(1, 1, sq, sk)
-    out = K.attention(q, k, v, mask, dropout if training else 0.0, causal and mask is None, None)
-    return out
+    out = K.attention(q, k, v, mask, p, causal and mask is None, None)
+    return [out, None] if return_seed_offset else out
 
 
 def calc_reduced_attention_scores(query, key, softmax_lse, name=None):
