@@ -30,6 +30,7 @@ int attention_bwd_stats_pad(int sq) { return (sq + 63) / 64 * 64; }
 
 int attention_bwd(const AttnBwdArgs& a, cudaStream_t s) {
   if (!attention_fwd_supported(a.fwd)) return 1;
+  if (a.fwd.colmask && a.fwd.mask_tiles) return attention_bwd_flashmask(a, nullptr, s);
   return a.fwd.d == 64 ? attention_bwd_d64(a, s) : attn_bwd::run<attn_bwd::HD>(a, s);
 }
 

@@ -24,21 +24,7 @@
 #include "include/b200_philox.cuh"
 
 namespace b200 {
-namespace {
-
-template <typename P>
-dropout::DropoutParams<P> with_dropout(const P& base, const AttnDropoutArgs& d) {
-  dropout::DropoutParams<P> p{};
-  static_cast<P&>(p) = base;
-  p.keep = (uint32_t)std::lrint((1.0 - d.p) * 65536.0);
-  p.rscale = (float)(1.0 / (1.0 - d.p));
-  p.seed_offset = d.seed_offset;
-  p.seed_ptr = d.seed_ptr; p.offset_ptr = d.offset_ptr; p.offset_add = d.offset_add;
-  p.seed = d.seed; p.offset = d.offset;
-  return p;
-}
-
-}  // namespace
+using dropout::with_dropout;
 
 namespace attn {
 
@@ -104,11 +90,13 @@ int run_dropout(const AttnBwdArgs& a, const AttnDropoutArgs& d, cudaStream_t s) 
 
 int attention_fwd_dropout(const AttnArgs& a, const AttnDropoutArgs& d, cudaStream_t s) {
   if (!attention_fwd_supported(a) || !(d.p > 0.0 && d.p < 1.0) || !d.seed_offset) return 1;
+  if (a.colmask && a.mask_tiles) return attention_fwd_flashmask(a, &d, s);
   return a.d == 64 ? attn::fwd_dense_dropout<64>(a, d, s) : attn::fwd_dense_dropout<attn::HD>(a, d, s);
 }
 
 int attention_bwd_dropout(const AttnBwdArgs& a, const AttnDropoutArgs& d, cudaStream_t s) {
   if (!attention_fwd_supported(a.fwd) || !(d.p > 0.0 && d.p < 1.0) || !d.seed_offset) return 1;
+  if (a.fwd.colmask && a.fwd.mask_tiles) return attention_bwd_flashmask(a, &d, s);
   return a.fwd.d == 64 ? attn_bwd::run_dropout<64>(a, d, s) : attn_bwd::run_dropout<attn_bwd::HD>(a, d, s);
 }
 

@@ -98,6 +98,7 @@ int attention_fwd_supported(const AttnArgs& a) {
 
 int attention_fwd(const AttnArgs& a, cudaStream_t s) {
   if (!attention_fwd_supported(a)) return 1;
+  if (a.colmask && a.mask_tiles) return attention_fwd_flashmask(a, nullptr, s);
   return a.d == 64 ? attention_fwd_d64(a, s) : attn::fwd_dense<attn::HD>(a, s);
 }
 

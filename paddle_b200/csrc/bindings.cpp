@@ -1032,13 +1032,20 @@ bool attention_supported(const Tensor& q, const Tensor& k, const Tensor& v) {
 }
 
 // q [B,Sq,H,D], k/v [B,Sk,Hk,D] (strided views allowed) -> (out [B,Sq,H,D] contiguous, lse fp32 [B,H,Sq])
-static void set_colmask(b200::AttnArgs& a, const OptT& colmask) {
-  if (!(colmask.has_value() && colmask->defined())) return;
+// mask_skip: the call takes the kernels that skip the tiles the mask hides (csrc/attention_flashmask_sm100.cu); the returned scratch holds
+// their tile summary, built on the device by a small kernel the call launches first.  That kernel is not counted in the launch count,
+// which counts attention kernels alike for both kinds of masked call.  Otherwise the masked kernels test every element.
+static Tensor set_colmask(b200::AttnArgs& a, const OptT& colmask, bool mask_skip) {
+  if (!(colmask.has_value() && colmask->defined())) return Tensor();
   const Tensor& m = *colmask;
   TORCH_CHECK(m.is_cuda() && m.scalar_type() == at::kInt && m.is_contiguous() && m.dim() == 4 && m.size(0) == a.b && m.size(2) == a.sk && m.size(3) == 4 &&
               (m.size(1) == 1 || m.size(1) == a.h), "attention: colmask must be int32 [B, 1|H, Sk, 4] (lt_start, lt_end, ut_start, ut_end)");
   a.colmask = m.data_ptr<int>();
   a.mask_heads = (int)m.size(1);
+  if (!mask_skip) return Tensor();
+  Tensor scratch = torch::empty({b200::attention_mask_tiles_ints(a.b, a.mask_heads, a.sq, a.sk)}, m.options());
+  a.mask_tiles = scratch.data_ptr<int>();
+  return scratch;
 }
 
 // Attention dropout's generator state.  fixed_seed_offset (int64 [2] = (seed, offset), on the host or the device) is used as given;
@@ -1079,12 +1086,12 @@ static void check_dropout(double p, const char* what) {
 
 // dropout_p > 0: attention dropout (csrc/attention_dropout_sm100.cu); also returns the int64 [2] (seed, offset) the mask was drawn with
 std::vector<Tensor> attention_fwd(const Tensor& q, const Tensor& k, const Tensor& v, double scale, bool causal, bool out_seq_major, const OptT& colmask,
-                                  double dropout_p, const OptT& fixed_seed_offset) {
+                                  double dropout_p, const OptT& fixed_seed_offset, bool mask_skip) {
   c10::cuda::CUDAGuard guard(q.device());
   check_dropout(dropout_p, "attention_fwd");
   b200::AttnArgs a;
   TORCH_CHECK(fill_attn(a, q, k, v, scale, causal), "paddle_b200.attention_fwd: unsupported operands");
-  set_colmask(a, colmask);
+  const Tensor tiles = set_colmask(a, colmask, mask_skip);
   // out_seq_major: the output is laid out [Sq,B,H,D] (sequence-parallel layers consume it without a transpose copy)
   Tensor out = out_seq_major ? torch::empty({a.sq, a.b, a.h, a.d}, q.options()) : torch::empty({a.b, a.sq, a.h, a.d}, q.options());
   if (out_seq_major) { a.o_strides[0] = (int64_t)a.h * a.d; a.o_strides[1] = (int64_t)a.b * a.h * a.d; a.o_strides[2] = a.d; }
@@ -1431,12 +1438,12 @@ static int launch_bwd(const b200::AttnBwdArgs& a, double dropout_p, const OptT& 
 
 // backward of attention_fwd: returns (dq [B,Sq,H,D], dk, dv [B,Sk,Hk,D]) in the input dtype
 std::vector<Tensor> attention_bwd(const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& out, const Tensor& lse, const Tensor& d_out,
-                                  double scale, bool causal, const OptT& colmask, double dropout_p, const OptT& seed_offset) {
+                                  double scale, bool causal, const OptT& colmask, double dropout_p, const OptT& seed_offset, bool mask_skip) {
   c10::cuda::CUDAGuard guard(q.device());
   check_dropout(dropout_p, "attention_bwd");
   b200::AttnBwdArgs a;
   TORCH_CHECK(fill_attn(a.fwd, q, k, v, scale, causal), "paddle_b200.attention_bwd: unsupported operands");
-  set_colmask(a.fwd, colmask);
+  const Tensor tiles = set_colmask(a.fwd, colmask, mask_skip);
   TORCH_CHECK(out.is_contiguous() && d_out.is_contiguous() && lse.is_contiguous() && lse.scalar_type() == at::kFloat, "attention_bwd: out / d_out / lse layout");
   a.fwd.o = out.data_ptr(); a.fwd.lse = lse.data_ptr<float>();
   Tensor dq32 = torch::empty({a.fwd.b, a.fwd.sq, a.fwd.h, a.fwd.d}, q.options().dtype(at::kFloat));
@@ -1454,9 +1461,10 @@ std::vector<Tensor> attention_bwd(const Tensor& q, const Tensor& k, const Tensor
 }
 
 // packed variant: qkv [B,S,nh+2*nkv,D] (q heads | k heads | v heads); returns d(qkv) of the same shape, written in place by
-// the kernel (dk/dv slices) plus one cast-copy of the fp32 dq accumulator - no slice-backward zero fills / adds
+// the kernel (dk/dv slices) plus one cast-copy of the fp32 dq accumulator - no slice-backward zero fills / adds.  colmask: as attention_bwd,
+// over the [B,S] view
 Tensor attention_bwd_packed(const Tensor& qkv, int64_t nh, int64_t nkv, const Tensor& out, const Tensor& lse, const Tensor& d_out, double scale,
-                            bool causal, bool seq_major, double dropout_p, const OptT& seed_offset) {
+                            bool causal, bool seq_major, double dropout_p, const OptT& seed_offset, const OptT& colmask, bool mask_skip) {
   c10::cuda::CUDAGuard guard(qkv.device());
   check_dropout(dropout_p, "attention_bwd_packed");
   TORCH_CHECK(qkv.dim() == 4 && qkv.is_contiguous() && qkv.size(2) == nh + 2 * nkv, "attention_bwd_packed: qkv layout");
@@ -1465,6 +1473,7 @@ Tensor attention_bwd_packed(const Tensor& qkv, int64_t nh, int64_t nkv, const Te
   Tensor q = bs(qkv.narrow(2, 0, nh)), k = bs(qkv.narrow(2, nh, nkv)), v = bs(qkv.narrow(2, nh + nkv, nkv));
   b200::AttnBwdArgs a;
   TORCH_CHECK(fill_attn(a.fwd, q, k, v, scale, causal), "paddle_b200.attention_bwd_packed: unsupported operands");
+  const Tensor tiles = set_colmask(a.fwd, colmask, mask_skip);
   TORCH_CHECK(out.is_contiguous() && d_out.is_contiguous() && lse.is_contiguous() && out.sizes() == d_out.sizes(), "attention_bwd_packed: out / d_out / lse layout");
   Tensor ov = bs(out);
   a.fwd.o = out.data_ptr(); a.fwd.lse = lse.data_ptr<float>();
@@ -1632,7 +1641,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("attention_supported", &attention_supported);
   m.def("attention_fwd", traced("attention_fwd", &attention_fwd), pybind11::arg("q"), pybind11::arg("k"), pybind11::arg("v"), pybind11::arg("scale"), pybind11::arg("causal"),
         pybind11::arg("out_seq_major") = false, pybind11::arg("colmask") = pybind11::none(), pybind11::arg("dropout_p") = 0.0,
-        pybind11::arg("seed_offset") = pybind11::none());
+        pybind11::arg("seed_offset") = pybind11::none(), pybind11::arg("mask_skip") = true);
   m.def("attention_fwd_paged", traced("attention_fwd_paged", &attention_fwd_paged), pybind11::arg("q"), pybind11::arg("k_cache"),
         pybind11::arg("v_cache"), pybind11::arg("block_tables"), pybind11::arg("cu_q"), pybind11::arg("n_q"), pybind11::arg("past"), pybind11::arg("scale"),
         pybind11::arg("out"), pybind11::arg("lse") = pybind11::none(), pybind11::arg("k_dequant_scales") = pybind11::none(),
@@ -1647,10 +1656,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         pybind11::arg("k_dequant_scales") = pybind11::none(), pybind11::arg("v_dequant_scales") = pybind11::none());
   m.def("attention_bwd", traced("attention_bwd", &attention_bwd), pybind11::arg("q"), pybind11::arg("k"), pybind11::arg("v"), pybind11::arg("out"), pybind11::arg("lse"),
         pybind11::arg("d_out"), pybind11::arg("scale"), pybind11::arg("causal"), pybind11::arg("colmask") = pybind11::none(),
-        pybind11::arg("dropout_p") = 0.0, pybind11::arg("seed_offset") = pybind11::none());
+        pybind11::arg("dropout_p") = 0.0, pybind11::arg("seed_offset") = pybind11::none(), pybind11::arg("mask_skip") = true);
   m.def("attention_bwd_packed", traced("attention_bwd_packed", &attention_bwd_packed), pybind11::arg("qkv"), pybind11::arg("nh"), pybind11::arg("nkv"), pybind11::arg("out"),
         pybind11::arg("lse"), pybind11::arg("d_out"), pybind11::arg("scale"), pybind11::arg("causal"), pybind11::arg("seq_major") = false,
-        pybind11::arg("dropout_p") = 0.0, pybind11::arg("seed_offset") = pybind11::none());
+        pybind11::arg("dropout_p") = 0.0, pybind11::arg("seed_offset") = pybind11::none(), pybind11::arg("colmask") = pybind11::none(),
+        pybind11::arg("mask_skip") = true);
   m.def("sample_tokens", traced("sample_tokens", &sample_tokens), pybind11::arg("x"), pybind11::arg("temperature"), pybind11::arg("top_k"),
         pybind11::arg("top_p"), pybind11::arg("threshold"), pybind11::arg("seed"), pybind11::arg("offset"), pybind11::arg("is_prob") = false,
         pybind11::arg("truncated") = true, pybind11::arg("k_out") = 0);

@@ -11,6 +11,7 @@
 #include <type_traits>
 
 #include "b200_common.cuh"
+#include "b200_mask_tiles.cuh"
 #include "b200_ops.h"
 #include "b200_philox.cuh"
 #include "b200_ptx.cuh"
@@ -78,10 +79,13 @@ static_assert(DkvSmem<HD>::BYTES <= 227 * 1024, "dkv_kernel shared memory");
 // TMA bulk reduce-add; dQ must be zero on entry.  DQ = false: dK / dV only (dq_kernel computes dQ).
 // DROPOUT (P = dropout::DropoutParams<Params>): with Zs = Z / (1 - p) for the keep mask Z of p.seed_offset, dV += (Zs P)^T dO and
 // dS = P (Zs dP - delta) scale (dP = dO V^T is the gradient of the dropped probabilities; delta = rowsum(dO O) on the dropped O).
-template <typename T, bool MASKED, bool DQ, int D, bool DROPOUT = false, typename P = Params>
+// SKIP (MASKED only, P = mask_skip::SkipParams<...>): walk only the (query head, 64-row query tile) pairs the column mask does not hide
+// from the CTA's key tile (b200_mask_tiles.cuh); the producer publishes each pair beside its stage.
+template <typename T, bool MASKED, bool DQ, int D, bool DROPOUT = false, bool SKIP = false, typename P = Params>
 __device__ __forceinline__ void dkv_body(const CUtensorMap& map_q, const CUtensorMap& map_k, const CUtensorMap& map_v,
                                          const CUtensorMap& map_do, const CUtensorMap& map_dq, const P p) {
   static_assert(D == HD || D == 64, "head_dim 128 or 64");
+  static_assert(!SKIP || MASKED, "tile skipping needs a column mask");
   constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
   constexpr int BN = 128, BQ = 64;
   constexpr int kHalves = D / 64;
@@ -96,6 +100,10 @@ __device__ __forceinline__ void dkv_body(const CUtensorMap& map_q, const CUtenso
   const uint32_t kv_full = base + L::BARS;
   auto qdo_full = [&](int s) { return base + L::BARS + 8 * (1 + s); };
   auto qdo_empty = [&](int s) { return base + L::BARS + 8 * (3 + s); };     // 8 warp arrivals
+  // SKIP: stage s's pair {query head << 20 | query tile (-1: end of the list), open}: one word, from which the D = 128 dropout kernel
+  // recomputes head and m0 where it needs them instead of holding both
+  auto slot = [&](int s) { return base + L::BARS + 40 + 8 * s; };
+  (void)slot;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int kv_head = blockIdx.x, batch = blockIdx.y, n_tile = blockIdx.z;   // key tiles slowest: under the causal mask the long ones start first
@@ -122,7 +130,46 @@ __device__ __forceinline__ void dkv_body(const CUtensorMap& map_q, const CUtenso
 
   if (warp < 4) {
     reg_dealloc<24>();
-    if (warp == 0 && lane == 0 && total > 0) {
+    if constexpr (SKIP) {
+      if (warp == 0 && lane == 0) {
+        // ================= TMA producer over the pairs the column mask does not hide =================
+        // (one lane in 24 registers: the classes of the pairs come precomputed with the tile summary)
+        if (total > 0) {   // (the consumers wait for K / V only then)
+          mbar_expect_tx(kv_full, 2 * L::BIG);
+          tma_load_4d(sK, &map_k, kv_full, 0, n0, kv_head, batch);
+          if constexpr (kHalves == 2) tma_load_4d(sK + BIG_HALF, &map_k, kv_full, 64, n0, kv_head, batch);
+          tma_load_4d(sV, &map_v, kv_full, 0, n0, kv_head, batch);
+          if constexpr (kHalves == 2) tma_load_4d(sV + BIG_HALF, &map_v, kv_full, 64, n0, kv_head, batch);
+        }
+        int cnt = 0;
+        for (int it = 0; it < total; ++it) {
+          const int head = kv_head * group + it / tiles_per_head;
+          const int mt = m_first + it % tiles_per_head, m0 = mt * BQ;
+          const int cls = __ldg(p.classes + ((batch * p.mask_heads + (p.mask_heads > 1 ? head : 0)) * p.n_ktiles + n_tile) * num_m + mt);
+          if (cls == mask_skip::kHidden) continue;
+          const int s = cnt & 1;
+          const float* st = p.stats + ((int64_t)batch * p.h + head) * 2 * p.sq_pad + m0;
+          mbar_wait(qdo_empty(s), ((cnt >> 1) & 1) ^ 1);
+          mask_skip::st_slot(slot(s), head << 20 | mt);
+          mask_skip::st_slot(slot(s) + 4, cls == mask_skip::kOpen);
+          mbar_expect_tx(qdo_full(s), 2 * L::SMALL + 512);
+          tma_load_4d(sQ(s), &map_q, qdo_full(s), 0, m0, head, batch);
+          if constexpr (kHalves == 2) tma_load_4d(sQ(s) + SMALL_HALF, &map_q, qdo_full(s), 64, m0, head, batch);
+          tma_load_4d(sDO(s), &map_do, qdo_full(s), 0, m0, head, batch);
+          if constexpr (kHalves == 2) tma_load_4d(sDO(s) + SMALL_HALF, &map_do, qdo_full(s), 64, m0, head, batch);
+          bulk_load(base + L::STATS + s * 512, st, 256, qdo_full(s));
+          bulk_load(base + L::STATS + s * 512 + 256, st + p.sq_pad, 256, qdo_full(s));
+          ++cnt;
+        }
+        {   // end of the list: the consumers' loop has no other bound (it would cost the D = 128 dropout kernel a register)
+          const int s = cnt & 1;
+          mbar_wait(qdo_empty(s), ((cnt >> 1) & 1) ^ 1);
+          mask_skip::st_slot(slot(s), -1);
+          mbar_arrive(qdo_full(s));
+        }
+        for (int it = max(0, cnt - 2); it < cnt; ++it) mbar_wait(qdo_empty(it & 1), (it >> 1) & 1);   // the consumers' waits are unbounded
+      }
+    } else if (warp == 0 && lane == 0 && total > 0) {
       // ================= TMA producer: one box per 64-wide d chunk =================
       mbar_expect_tx(kv_full, 2 * L::BIG);
       tma_load_4d(sK, &map_k, kv_full, 0, n0, kv_head, batch);
@@ -166,11 +213,19 @@ __device__ __forceinline__ void dkv_body(const CUtensorMap& map_q, const CUtenso
     }
     (void)kpar;
     if (total > 0) mbar_wait_unbounded(kv_full, 0);
-    for (int it = 0; it < total; ++it) {
+    for (int it = 0; SKIP || it < total; ++it) {   // SKIP: it counts the pairs processed, head and m0 come from the producer
       const int s = it & 1;
-      const int head = kv_head * group + it / tiles_per_head;
-      const int m0 = (m_first + it % tiles_per_head) * BQ;
-      mbar_wait_unbounded(qdo_full(s), (it >> 1) & 1);
+      int head, m0;
+      if constexpr (SKIP) {
+        mbar_wait_unbounded(qdo_full(s), (it >> 1) & 1);
+        const int w = mask_skip::ld_slot(slot(s));
+        if (w < 0) break;
+        head = w >> 20; m0 = (w & 0xfffff) * BQ;
+      } else {
+        head = kv_head * group + it / tiles_per_head;
+        m0 = (m_first + it % tiles_per_head) * BQ;
+        mbar_wait_unbounded(qdo_full(s), (it >> 1) & 1);
+      }
       float st[BQ / 2], dpt[BQ / 2];
       wgmma_fence_regs(st);
       wgmma_fence_regs(dpt);
@@ -205,10 +260,11 @@ __device__ __forceinline__ void dkv_body(const CUtensorMap& map_q, const CUtenso
       int4 cm[2];
       if constexpr (MASKED) {
         const int4* cmp = p.colmask + ((int64_t)batch * p.mask_heads + (p.mask_heads > 1 ? head : 0)) * p.sk;
+        const bool open = SKIP && (mask_skip::ld_slot(slot(s) + 4) & 1);   // SKIP: an open pair tests against an empty mask
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int key = n0 + rl + h * 8;
-          cm[h] = key < p.sk ? __ldg(cmp + key) : make_int4(0, 0, 0, 0);
+          cm[h] = key < p.sk && !open ? __ldg(cmp + key) : make_int4(0, 0, 0, 0);
         }
       }
       const float* lse2 = stats(s);        // lse[query] * log2(e)
@@ -378,7 +434,8 @@ __device__ __forceinline__ void dkv_body(const CUtensorMap& map_q, const CUtenso
 }
 
 // DROPOUT: as in dkv_body, with the forward's call layout (row = query)
-template <typename T, bool MASKED, int D, bool DROPOUT = false, typename P = Params>
+// SKIP: walk only the 64-key tiles the column mask does not hide from the CTA's 128 rows (classified by their 128-key summary tile)
+template <typename T, bool MASKED, int D, bool DROPOUT = false, bool SKIP = false, typename P = Params>
 __device__ __forceinline__ void dq_body(const CUtensorMap& map_q, const CUtensorMap& map_k, const CUtensorMap& map_v,
                                         const CUtensorMap& map_do, const P p) {
   static_assert(D == HD || D == 64, "head_dim 128 or 64");
@@ -393,6 +450,8 @@ __device__ __forceinline__ void dq_body(const CUtensorMap& map_q, const CUtensor
   const uint32_t qdo_full = sm.bar(0);
   auto kv_full = [&](int s) { return sm.bar(1 + s); };
   auto kv_empty = [&](int s) { return sm.bar(3 + s); };     // 8 warp arrivals
+  auto slot = [&](int s) { return sm.bar(6 + s); };         // SKIP: stage s's key tile, 2 j + open (-1: end of the list)
+  (void)slot;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_tile = (int)gridDim.x - 1 - (int)blockIdx.x;   // long (late) rows first under the causal mask
@@ -415,7 +474,47 @@ __device__ __forceinline__ void dq_body(const CUtensorMap& map_q, const CUtensor
   __syncthreads();
 
   if (warp == 8) {
-    if (lane == 0 && n_tiles > 0) {
+    if constexpr (SKIP) {
+      if (n_tiles > 0) {
+        // ================= TMA producer over the key tiles the column mask does not hide: lane l classifies tile jb + l =================
+        const int* tiles = p.tiles + ((int64_t)batch * p.mask_heads + (p.mask_heads > 1 ? head : 0)) * p.n_ktiles * 8;
+        if (lane == 0) {
+          mbar_expect_tx(qdo_full, 2 * kBigBytes<D>);
+          tma_load_4d(sQ, &map_q, qdo_full, 0, m0, head, batch);
+          if constexpr (kHalves == 2) tma_load_4d(sQ + BIG_HALF, &map_q, qdo_full, 64, m0, head, batch);
+          tma_load_4d(sDO, &map_do, qdo_full, 0, m0, head, batch);
+          if constexpr (kHalves == 2) tma_load_4d(sDO + BIG_HALF, &map_do, qdo_full, 64, m0, head, batch);
+        }
+        int cnt = 0;
+        for (int jb = 0; jb < n_tiles; jb += 32) {
+          const int cls = jb + lane < n_tiles ? mask_skip::tile_class(tiles + ((jb + lane) * BK / mask_skip::kTileKeys) * 8, m0, m0 + BM)
+                                              : mask_skip::kHidden;
+          uint32_t vis = __ballot_sync(0xffffffffu, cls != mask_skip::kHidden);
+          const uint32_t open = __ballot_sync(0xffffffffu, cls == mask_skip::kOpen);
+          while (vis) {
+            const int bit = __ffs(vis) - 1;
+            vis &= vis - 1;
+            if (lane == 0) {
+              const int j = jb + bit, s = cnt & 1, n0 = j * BK;
+              mbar_wait(kv_empty(s), ((cnt >> 1) & 1) ^ 1);
+              mask_skip::st_slot(slot(s), 2 * j + ((open >> bit) & 1));
+              mbar_expect_tx(kv_full(s), 2 * kSmallBytes<D>);
+              tma_load_4d(sK(s), &map_k, kv_full(s), 0, n0, kv_head, batch);
+              if constexpr (kHalves == 2) tma_load_4d(sK(s) + SMALL_HALF, &map_k, kv_full(s), 64, n0, kv_head, batch);
+              tma_load_4d(sV(s), &map_v, kv_full(s), 0, n0, kv_head, batch);
+              if constexpr (kHalves == 2) tma_load_4d(sV(s) + SMALL_HALF, &map_v, kv_full(s), 64, n0, kv_head, batch);
+            }
+            ++cnt;
+          }
+        }
+        if (lane == 0 && cnt < n_tiles) {   // the consumers' loop would go on: end it
+          const int s = cnt & 1;
+          mbar_wait(kv_empty(s), ((cnt >> 1) & 1) ^ 1);
+          mask_skip::st_slot(slot(s), -1);
+          mbar_arrive(kv_full(s));
+        }
+      }
+    } else if (lane == 0 && n_tiles > 0) {
       // ================= TMA producer: one box per 64-wide d chunk =================
       mbar_expect_tx(qdo_full, 2 * kBigBytes<D>);
       tma_load_4d(sQ, &map_q, qdo_full, 0, m0, head, batch);
@@ -473,13 +572,22 @@ __device__ __forceinline__ void dq_body(const CUtensorMap& map_q, const CUtensor
     };
     uint32_t keep = 0;
     if constexpr (DROPOUT) {
-      if (n_tiles > 0) keep = draw(0);
+      if (!SKIP && n_tiles > 0) keep = draw(0);
     }
     (void)draw;
     if (n_tiles > 0) mbar_wait(qdo_full, 0);
-    for (int j = 0; j < n_tiles; ++j) {
-      const int s = j & 1, n0 = j * BK;
+    for (int j = 0; j < n_tiles; ++j) {   // SKIP: j counts the tiles processed, jt is the one published for stage s
+      const int s = j & 1;
       mbar_wait(kv_full(s), (j >> 1) & 1);
+      int jt = j;
+      bool open = false;   // SKIP: no key of the tile hides a row of the CTA
+      if constexpr (SKIP) {
+        const int w = mask_skip::ld_slot(slot(s));
+        if (w < 0) break;
+        jt = w >> 1; open = w & 1;
+        if constexpr (DROPOUT) keep = draw(jt);   // before the MMAs: the next tile is not known yet
+      }
+      const int n0 = jt * BK;
       float sv[BK / 2], dpv[BK / 2];
       wgmma_fence_regs(sv);
       wgmma_fence_regs(dpv);
@@ -505,7 +613,7 @@ __device__ __forceinline__ void dq_body(const CUtensorMap& map_q, const CUtensor
         for (int e = 0; e < 2; ++e) {
           const int key = n0 + jn * 8 + 2 * q + e;
           int4 m = make_int4(0, 0, 0, 0);
-          if constexpr (MASKED) { if (key < p.sk) m = __ldg(cmp + key); }
+          if constexpr (MASKED) { if (!open && key < p.sk) m = __ldg(cmp + key); }
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const int row = m0 + rl + h * 8;
@@ -531,7 +639,7 @@ __device__ __forceinline__ void dq_body(const CUtensorMap& map_q, const CUtensor
         else wgmma_rs_n64<BF16, 1>(dq_acc, dsa[ks], desc, 1);
       }
       wgmma_commit();
-      if constexpr (DROPOUT) {
+      if constexpr (DROPOUT && !SKIP) {
         if (j + 1 < n_tiles) keep = draw(j + 1);
       }
       wgmma_wait<0>();

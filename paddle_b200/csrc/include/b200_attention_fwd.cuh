@@ -6,15 +6,34 @@
 // rows are never loaded and their block-table entries never read, so blocks wholly below the window may hold anything.
 #pragma once
 #include <cuda.h>
+#include <cmath>
 #include <type_traits>
 
 #include "b200_common.cuh"
 #include "b200_kv8.cuh"
+#include "b200_mask_tiles.cuh"
 #include "b200_ops.h"
 #include "b200_philox.cuh"
 #include "b200_ptx.cuh"
 
 namespace b200 {
+namespace dropout {
+
+// A dropout kernel's parameters: the dropout-free ones plus the rate and generator state of AttnDropoutArgs.
+template <typename P>
+DropoutParams<P> with_dropout(const P& base, const AttnDropoutArgs& d) {
+  DropoutParams<P> p{};
+  static_cast<P&>(p) = base;
+  p.keep = (uint32_t)std::lrint((1.0 - d.p) * 65536.0);
+  p.rscale = (float)(1.0 / (1.0 - d.p));
+  p.seed_offset = d.seed_offset;
+  p.seed_ptr = d.seed_ptr; p.offset_ptr = d.offset_ptr; p.offset_add = d.offset_add;
+  p.seed = d.seed; p.offset = d.offset;
+  return p;
+}
+
+}  // namespace dropout
+
 namespace attn {
 using namespace ptx;
 
@@ -63,7 +82,8 @@ __device__ __forceinline__ void st_shared_zero16(uint32_t addr) {
 // MASKED, PAGED, KV, D: see fwd_kernel in attention_sm100.cu.
 // WINDOW (PAGED only, P = WindowParams<...>): sliding window p.window, see fwd_body's key range below
 // DROPOUT (dense only, P = dropout::DropoutParams<Params>): attention dropout, see attention_dropout_sm100.cu
-template <typename T, bool MASKED, bool PAGED, typename KV, int D, bool WINDOW, bool DROPOUT = false, typename P>
+// SKIP (MASKED dense only, P = mask_skip::SkipParams<...>): walk only the key tiles the column mask does not hide, see b200_mask_tiles.cuh
+template <typename T, bool MASKED, bool PAGED, typename KV, int D, bool WINDOW, bool DROPOUT = false, bool SKIP = false, typename P>
 __device__ __forceinline__ void fwd_body(const CUtensorMap& map_q, const CUtensorMap& map_k, const CUtensorMap& map_v, const P p) {
   constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
   constexpr bool Q8 = !std::is_same<KV, T>::value;
@@ -71,6 +91,7 @@ __device__ __forceinline__ void fwd_body(const CUtensorMap& map_q, const CUtenso
   static_assert(D == HD || (D == 64 && !Q8), "head_dim 64 reads 16-bit K / V only");
   static_assert(!WINDOW || (PAGED && !MASKED), "sliding windows are paged only");
   static_assert(!DROPOUT || !PAGED, "dropout is dense (training) only");
+  static_assert(!SKIP || (MASKED && !PAGED), "tile skipping is for the dense column-masked kernels");
   constexpr int kHalves = D / 64;                            // 64-wide d chunks (128-byte swizzle spans) of a row
   constexpr uint32_t kTile = BM * D * 2;                     // one Q, K or V tile
   constexpr uint32_t kVBlock = kHalves * 8192;               // one 64-key block of a V tile (its d chunks 8192 B apart)
@@ -85,6 +106,11 @@ __device__ __forceinline__ void fwd_body(const CUtensorMap& map_q, const CUtenso
   auto v_full = [&](int s) { return bars + 8u * (3 + s); };
   auto k_empty = [&](int s) { return bars + 8u * (5 + s); };    // 8 warp arrivals
   auto v_empty = [&](int s) { return bars + 8u * (7 + s); };
+  // SKIP: stage s's key tile, 2 j + open (-1: end of the list), published before k_full(s); the next tile (-1: none), published before
+  // v_full(s), so it stays valid until the consumers release v_empty(s); the first tile (-1: none), published before q_full
+  auto k_slot = [&](int s) { return bars + 80u + 4u * s; };
+  auto v_slot = [&](int s) { return bars + 88u + 4u * s; };
+  const uint32_t first_slot = bars + 96u;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   int m_tile, head, batch, sk, causal_off, nrows, q0 = 0;
@@ -223,6 +249,62 @@ __device__ __forceinline__ void fwd_body(const CUtensorMap& map_q, const CUtenso
             tma_load_4d(sV(s) + (c * R / 64) * kVBlock + half * 8192 + (c * R % 64) * 128, &map_v, v_full(s), half * 64, row, kv_head, blk);
         }
       }
+    } else if constexpr (SKIP) {
+      if (n_tiles > 0) {
+        // ================= TMA producer over the key tiles the column mask does not hide (b200_mask_tiles.cuh) =================
+        // lane l classifies key tile jb + l; lane 0 loads a visible tile once the next one is known, which goes to v_slot for the
+        // dropout kernels' bits, and loads Q once the first one is known, which goes to first_slot
+        const int* tiles = p.tiles + ((int64_t)batch * p.mask_heads + (p.mask_heads > 1 ? head : 0)) * p.n_ktiles * 8;
+        int cnt = 0, pend = -1;   // pend: 2 j + open of the visible tile waiting for its successor
+        auto issue = [&](int next) {
+          if (lane == 0) {
+            if (cnt == 0) {
+              mask_skip::st_slot(first_slot, pend >> 1);
+              mbar_expect_tx(q_full, kTile);
+              tma_load_4d(sQ, &map_q, q_full, 0, m0, head, batch);
+              if constexpr (kHalves == 2) tma_load_4d(sQ + HALF_BYTES, &map_q, q_full, 64, m0, head, batch);
+            }
+            const int s = cnt & 1, n0 = (pend >> 1) * BN;
+            const uint32_t ph = ((cnt >> 1) & 1) ^ 1;
+            mbar_wait(k_empty(s), ph);
+            mask_skip::st_slot(k_slot(s), pend);
+            mbar_expect_tx(k_full(s), kTile);
+            tma_load_4d(sK(s), &map_k, k_full(s), 0, n0, kv_head, batch);
+            if constexpr (kHalves == 2) tma_load_4d(sK(s) + HALF_BYTES, &map_k, k_full(s), 64, n0, kv_head, batch);
+            mbar_wait(v_empty(s), ph);
+            mask_skip::st_slot(v_slot(s), next);
+            mbar_expect_tx(v_full(s), kTile);
+#pragma unroll
+            for (int kb = 0; kb < 2; ++kb)
+#pragma unroll
+              for (int i = 0; i < kHalves; ++i)
+                tma_load_4d(sV(s) + kb * kVBlock + i * 8192, &map_v, v_full(s), i * 64, n0 + kb * 64, kv_head, batch);
+          }
+          ++cnt;
+        };
+        for (int jb = 0; jb < n_tiles; jb += 32) {
+          const int cls = jb + lane < n_tiles ? mask_skip::tile_class(tiles + (jb + lane) * 8, m0, m0 + BM) : mask_skip::kHidden;
+          uint32_t vis = __ballot_sync(0xffffffffu, cls != mask_skip::kHidden);
+          const uint32_t open = __ballot_sync(0xffffffffu, cls == mask_skip::kOpen);
+          while (vis) {
+            const int bit = __ffs(vis) - 1;
+            vis &= vis - 1;
+            if (pend >= 0) issue(jb + bit);
+            pend = 2 * (jb + bit) + ((open >> bit) & 1);
+          }
+        }
+        if (pend >= 0) issue(-1);
+        if (lane == 0 && cnt == 0) {   // nothing visible: the consumers still wait for Q
+          mask_skip::st_slot(first_slot, -1);
+          mbar_arrive(q_full);
+        }
+        if (lane == 0 && cnt < n_tiles) {   // the consumers' loop would go on: end it
+          const int s = cnt & 1;
+          mbar_wait(k_empty(s), ((cnt >> 1) & 1) ^ 1);
+          mask_skip::st_slot(k_slot(s), -1);
+          mbar_arrive(k_full(s));
+        }
+      }
     } else if (lane == 0 && n_tiles > 0) {
       // ================= TMA producer =================
       // one box per 64-wide d chunk: two per Q / K tile and four per V tile at D = 128, one and two at D = 64
@@ -282,19 +364,33 @@ __device__ __forceinline__ void fwd_body(const CUtensorMap& map_q, const CUtenso
     // the bits wait in shared memory past the barriers (kDropoutSmemBytes more), not in registers, while S and O fill the register file
     uint64_t* const keep_slot = reinterpret_cast<uint64_t*>(smem_raw + (bars + 128 - smem_u32(smem_raw))) + threadIdx.x;
     (void)keep_slot;
+    (void)k_slot; (void)v_slot; (void)first_slot;
     if constexpr (DROPOUT) {
       if ((blockIdx.x | blockIdx.y | blockIdx.z | threadIdx.x) == 0) {   // the pair this launch used, for the backward
         p.seed_offset[0] = p.seed_ptr ? __ldg(p.seed_ptr) : (int64_t)p.seed;
         p.seed_offset[1] = p.seed_ptr ? __ldg(p.offset_ptr) + p.offset_add : (int64_t)p.offset;
       }
-      if (j0 < n_tiles) *keep_slot = draw(j0);
+      if (!SKIP && j0 < n_tiles) *keep_slot = draw(j0);
     }
     (void)draw;
     if (n_tiles > 0) mbar_wait(q_full, 0);
-    for (int j = j0; j < n_tiles; ++j) {
+    if constexpr (SKIP && DROPOUT) {
+      const int first = n_tiles > 0 ? mask_skip::ld_slot(first_slot) : -1;
+      if (first >= 0) *keep_slot = draw(first);
+    }
+    for (int j = j0; j < n_tiles; ++j) {   // SKIP: j counts the tiles processed, jt is the one published for stage s
       const int s = (j - j0) & 1, ph = ((j - j0) >> 1) & 1;
       float sv[BN / 2];
       mbar_wait(k_full(s), ph);
+      if constexpr (SKIP) {
+        if (mask_skip::ld_slot(k_slot(s)) < 0) break;
+      }
+      // SKIP: the tile's index and class are read from k_slot(s) where they are used, not held in registers; the slot stays valid until
+      // k_empty(s) is released, after the masks
+      auto tile = [&] {
+        if constexpr (SKIP) return mask_skip::ld_slot(k_slot(s)) >> 1;
+        else return j;
+      };
       wgmma_fence_regs(sv);
       wgmma_fence();
 #pragma unroll
@@ -307,15 +403,16 @@ __device__ __forceinline__ void fwd_body(const CUtensorMap& map_q, const CUtenso
       wgmma_wait<0>();
       wgmma_fence_regs(sv);
       __syncwarp();
-      if (lane == 0) mbar_arrive(k_empty(s));
+      if (!SKIP && lane == 0) mbar_arrive(k_empty(s));
       // ---- masks (raw logits; the softmax scale is folded into the exp2 FFMA) ----
-      const bool edge = PAGED ? (j * BN + BN > sk) || (j * BN + BN - 1 > m0 + causal_off)
-                              : (j * BN + BN > p.sk) || (p.causal && j * BN + BN - 1 > m0 + p.causal_off);
+      const int jt = tile();
+      const bool edge = PAGED ? (jt * BN + BN > sk) || (jt * BN + BN - 1 > m0 + causal_off)
+                              : (jt * BN + BN > p.sk) || (p.causal && jt * BN + BN - 1 > m0 + p.causal_off);
       if (edge) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int row = m0 + rl + h * 8;
-          const int lim = (p.causal ? min(sk - 1, row + causal_off) : sk - 1) - j * BN;   // last visible key, tile-relative
+          const int lim = (p.causal ? min(sk - 1, row + causal_off) : sk - 1) - jt * BN;   // last visible key, tile-relative
 #pragma unroll
           for (int jn = 0; jn < BN / 8; ++jn)
 #pragma unroll
@@ -324,10 +421,10 @@ __device__ __forceinline__ void fwd_body(const CUtensorMap& map_q, const CUtenso
         }
       }
       if constexpr (WINDOW) {     // the window's left edge: only the tiles below the last row's first visible key
-        if (j * BN < m0 + BM + causal_off - p.window) {
+        if (jt * BN < m0 + BM + causal_off - p.window) {
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            const int first = m0 + rl + h * 8 + causal_off - p.window + 1 - j * BN;   // this row's first visible key, tile-relative
+            const int first = m0 + rl + h * 8 + causal_off - p.window + 1 - jt * BN;   // this row's first visible key, tile-relative
 #pragma unroll
             for (int jn = 0; jn < BN / 8; ++jn)
 #pragma unroll
@@ -336,13 +433,15 @@ __device__ __forceinline__ void fwd_body(const CUtensorMap& map_q, const CUtenso
           }
         }
       }
-      if constexpr (MASKED) {     // flashmask / varlen: key column j hides the query rows [lt_start, lt_end) and [ut_start, ut_end)
+      // flashmask / varlen: key column j hides the query rows [lt_start, lt_end) and [ut_start, ut_end) (SKIP: tested unless the tile is open)
+      if (MASKED && !(SKIP && (mask_skip::ld_slot(k_slot(s)) & 1))) {
         const int4* cm = p.colmask + ((int64_t)batch * p.mask_heads + (p.mask_heads > 1 ? head : 0)) * p.sk;
+        const int k0 = tile() * BN;
 #pragma unroll
         for (int jn = 0; jn < BN / 8; ++jn)
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
-            const int key = j * BN + jn * 8 + 2 * q + e;
+            const int key = k0 + jn * 8 + 2 * q + e;
             if (key < p.sk) {
               const int4 m = __ldg(cm + key);
 #pragma unroll
@@ -352,6 +451,10 @@ __device__ __forceinline__ void fwd_body(const CUtensorMap& map_q, const CUtenso
               }
             }
           }
+      }
+      if constexpr (SKIP) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(k_empty(s));
       }
       // ---- online softmax: a row lives in the four lanes of a quad ----
 #pragma unroll
@@ -430,7 +533,10 @@ __device__ __forceinline__ void fwd_body(const CUtensorMap& map_q, const CUtenso
         else wgmma_rs_n64<BF16, 1>(o_acc, pa[ks], vdesc, 1);
       }
       wgmma_commit();
-      if constexpr (DROPOUT) {
+      if constexpr (DROPOUT && SKIP) {
+        const int jn = mask_skip::ld_slot(v_slot(s));
+        if (jn >= 0) *keep_slot = draw(jn);
+      } else if constexpr (DROPOUT) {
         if (j + 1 < n_tiles) *keep_slot = draw(j + 1);
       }
       wgmma_wait<0>();

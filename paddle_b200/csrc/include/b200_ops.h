@@ -332,6 +332,9 @@ struct AttnArgs {
   // colmask == nullptr: no mask.  mask_heads is 1 (shared by all heads) or h.
   const int* colmask = nullptr;
   int mask_heads = 1;
+  // With a column mask: scratch int32 [attention_mask_tiles_ints(b, mask_heads, sq, sk)] for the tile summary of the tile-skipping
+  // kernels (attention_flashmask_sm100.cu), which every masked call then takes; nullptr: the masked kernels test every element.
+  int* mask_tiles = nullptr;
 };
 int attention_fwd_supported(const AttnArgs& a);
 int attention_fwd(const AttnArgs& a, cudaStream_t s);
@@ -393,6 +396,11 @@ struct AttnDropoutArgs {
 };
 int attention_fwd_dropout(const AttnArgs& a, const AttnDropoutArgs& d, cudaStream_t s);
 int attention_bwd_dropout(const AttnBwdArgs& a, const AttnDropoutArgs& d, cudaStream_t s);
+// Column-masked attention that skips the tiles the mask hides (attention_flashmask_sm100.cu), called by the four entry points above
+// when colmask and mask_tiles are set; d == nullptr: no dropout.
+int attention_mask_tiles_ints(int b, int mask_heads, int sq, int sk);
+int attention_fwd_flashmask(const AttnArgs& a, const AttnDropoutArgs* d, cudaStream_t s);
+int attention_bwd_flashmask(const AttnBwdArgs& a, const AttnDropoutArgs* d, cudaStream_t s);
 
 // Token sampling (sampling.cu): one CTA per row of x [rows, vocab] (row stride `stride` elements, unit column stride).  Per-row device
 // arrays: temperature (<= 0: greedy), top_k (int32, 0: off), top_p (1: off), threshold (optional), seed / offset (int64).  Writes ids and

@@ -6,7 +6,10 @@ Dispatch: the sm_90a wgmma flash kernels for fp16/bf16, head_dim 128 (csrc/atten
 projection, and a column-wise row-range mask (attention_colmask) runs on the same kernels.  Attention dropout (0 < p < 1) runs on
 their dropout instantiations (csrc/attention_dropout_sm100.cu): the mask is a pure function of (seed, offset, batch, head, query,
 key) (dropout_keep_mask is its torch twin), drawn from torch's CUDA generator or a given `seed_offset` (int64 [2]), and the backward
-regenerates it from the pair the forward used.  Other head sizes, dense masks and dropout >= 1 take the PyTorch SDPA (library) path.  Backward: csrc/attention_bwd_sm100.cu (B200_ATTN_BWD=own, default) or, for comparison, a library backward
+regenerates it from the pair the forward used.  Column-masked calls run kernels that skip the tiles the mask hides and leave out the
+per-element mask test where it hides nothing (csrc/attention_flashmask_sm100.cu; colmask_tile_classes is the torch twin of their tile
+classes); B200_ATTN_MASK_SKIP=0 sends them to the kernels that test every element instead, for comparison.  Other head sizes, dense
+masks and dropout >= 1 take the PyTorch SDPA (library) path.  Backward: csrc/attention_bwd_sm100.cu (B200_ATTN_BWD=own, default) or, for comparison, a library backward
 fed with our forward's (out, logsumexp) (B200_ATTN_BWD=cudnn|flash).  The own backward is a single pass that bulk-reduces dQ in
 arrival order (reproducible to rounding); FLAGS_cudnn_deterministic switches it to a bitwise-reproducible dK/dV + dQ kernel pair.
 """
@@ -37,6 +40,8 @@ def attention_ref(q, k, v, mask=None, dropout_p=0.0, causal=False, scale=None):
 
 
 _bwd_backend = [__import__("os").environ.get("B200_ATTN_BWD", "own")]   # own | cudnn | flash
+# column-masked calls: True: the tile-skipping kernels; False (B200_ATTN_MASK_SKIP=0): the kernels that test every element
+_mask_skip = [__import__("os").environ.get("B200_ATTN_MASK_SKIP", "1") != "0"]
 
 
 _U32 = 0xFFFFFFFF
@@ -133,11 +138,12 @@ class _FlashAttnColMask(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, q, k, v, colmask, scale, causal, dropout_p=0.0, seed_offset=None):
-        res = ext().attention_fwd(q, k, v, scale, causal, False, colmask, dropout_p, seed_offset)
+        skip = _mask_skip[0]
+        res = ext().attention_fwd(q, k, v, scale, causal, False, colmask, dropout_p, seed_offset, skip)
         out, lse = res[0], res[1]
         so = res[2] if dropout_p > 0.0 else None
         ctx.save_for_backward(q, k, v, out, lse, colmask, so)
-        ctx.scale, ctx.causal, ctx.dropout_p = scale, causal, dropout_p
+        ctx.scale, ctx.causal, ctx.dropout_p, ctx.skip = scale, causal, dropout_p, skip
         if so is not None:
             ctx.mark_non_differentiable(so)
         return out, so
@@ -145,10 +151,7 @@ class _FlashAttnColMask(torch.autograd.Function):
     @staticmethod
     def backward(ctx, do, _dso=None):
         q, k, v, out, lse, colmask, so = ctx.saved_tensors
-        if ctx.dropout_p > 0.0:
-            dq, dk, dv = ext().attention_bwd(q, k, v, out, lse, do.contiguous(), ctx.scale, ctx.causal, colmask, ctx.dropout_p, so)
-        else:
-            dq, dk, dv = ext().attention_bwd(q, k, v, out, lse, do.contiguous(), ctx.scale, ctx.causal, colmask)
+        dq, dk, dv = ext().attention_bwd(q, k, v, out, lse, do.contiguous(), ctx.scale, ctx.causal, colmask, ctx.dropout_p, so, ctx.skip)
         return dq, dk, dv, None, None, None, None, None
 
 
@@ -173,8 +176,11 @@ def colmask_from_startend(startend_row_indices, causal, sq):
     return torch.stack([lts, lte, uts, ute], -1).contiguous()
 
 
-def colmask_from_cu_seqlens(cu_q, cu_k, total_k):
-    """Packed variable-length batch -> document mask: key j of sequence s is visible to the query rows [cu_q[s], cu_q[s+1]) only."""
+def colmask_from_cu_seqlens(cu_q, cu_k, total_k, causal=False):
+    """Packed variable-length batch -> document mask: key j of sequence s is visible to the query rows [cu_q[s], cu_q[s+1]) only.
+    causal: also the causal mask within each sequence, bottom-right aligned like the kernels' causal flag (local query i of a sequence
+    of len_q queries and len_k keys sees local key kj iff kj <= i + len_k - len_q), for q and k packed differently; run it with
+    causal=False."""
     cu_q, cu_k = raw(cu_q).to(torch.int64), raw(cu_k).to(torch.int64)
     keys = torch.arange(total_k, device=cu_k.device)
     seq = torch.bucketize(keys, cu_k[1:], right=True).clamp(max=cu_q.numel() - 2)
@@ -183,6 +189,10 @@ def colmask_from_cu_seqlens(cu_q, cu_k, total_k):
     zero = torch.zeros_like(qs)
     lts = torch.where(valid, qe, zero)                          # rows >= qe hidden; keys beyond the last sequence hide every row
     lte = torch.full_like(qs, _INT_MAX)
+    if causal:                                                  # rows < qs + max(0, kj - (len_k - len_q)) hidden
+        kj = keys - cu_k[seq]
+        shift = (cu_k[seq + 1] - cu_k[seq]) - (cu_q[seq + 1] - cu_q[seq])
+        qs = qs + (kj - shift).clamp(min=0).to(torch.int32)
     ute = torch.where(valid, qs, zero)                          # rows < qs hidden
     return torch.stack([lts, lte, zero, ute], -1).reshape(1, 1, total_k, 4).contiguous()
 
@@ -211,6 +221,33 @@ def attention_colmask(q, k, v, colmask, causal=False, scale=None, dropout_p=0.0,
     return (wrap(out), so) if return_seed_offset else wrap(out)
 
 
+def colmask_tile_classes(colmask, sq, sk, bm, bn, causal):
+    """The tile classes of the tile-skipping kernels, int8 [B, Hm, ceil(sq / bm), ceil(sk / bn)], for query tiles of bm rows against
+    key tiles of bn keys: 0 hidden (every key of the tile hides every row of the query tile, or the tile is past the causal limit of the
+    query tile's last row: not computed), 1 partial (the per-element mask test runs), 2 open (no key hides a row: no mask test).
+    From the min / max of each bound over the tile's keys below sk (csrc/include/b200_mask_tiles.cuh); the kernels use bn = 128 (bm = 128
+    in the forward and the deterministic dQ, 64 in dK / dV).  Shapes only: valid without a GPU."""
+    m = raw(colmask).long()[..., :sk, :]
+    b, hm = m.shape[0], m.shape[1]
+    nm, nn = -(-sq // bm), -(-sk // bn)
+    pad = nn * bn - sk
+    big = torch.iinfo(torch.int64).max
+
+    def ext_(fill, red):
+        x = torch.nn.functional.pad(m, (0, 0, 0, pad), value=fill).reshape(b, hm, nn, bn, 4)
+        return (x.amax(3) if red == "max" else x.amin(3)).unsqueeze(2)         # [b, hm, 1, nn, 4]
+    mx, mn = ext_(-big, "max"), ext_(big, "min")
+    r0 = (torch.arange(nm, device=m.device) * bm).reshape(1, 1, nm, 1)
+    r1 = r0 + bm
+    hidden = ((mx[..., 0] <= r0) & (mn[..., 1] >= r1)) | ((mx[..., 2] <= r0) & (mn[..., 3] >= r1))
+    open_ = ((mn[..., 0] >= r1) | (mx[..., 1] <= r0)) & ((mn[..., 2] >= r1) | (mx[..., 3] <= r0))
+    cls = torch.where(hidden, 0, torch.where(open_, 2, 1))
+    if causal:
+        n0 = (torch.arange(nn, device=m.device) * bn).reshape(1, 1, 1, nn)
+        cls = torch.where(n0 <= r0 + bm - 1 + (sk - sq), cls, 0)
+    return cls.to(torch.int8)
+
+
 def colmask_to_dense(colmask, sq):
     """Boolean visibility [B, Hm, Sq, Sk] of an int4 column mask (reference path / tests)."""
     m = raw(colmask).long()
@@ -226,42 +263,48 @@ class _FlashAttnPacked(torch.autograd.Function):
     autograd never builds zero-filled slice gradients and the sequence-parallel layout needs no transpose copies."""
 
     @staticmethod
-    def forward(ctx, qkv, nh, nkv, scale, causal, seq_major, dropout_p=0.0, seed_offset=None):
+    def forward(ctx, qkv, nh, nkv, scale, causal, seq_major, dropout_p=0.0, seed_offset=None, colmask=None):
         x = qkv.transpose(0, 1) if seq_major else qkv
         q, k, v = x[:, :, :nh], x[:, :, nh:nh + nkv], x[:, :, nh + nkv:]
-        res = ext().attention_fwd(q, k, v, scale, causal, seq_major, None, dropout_p, seed_offset)    # out: same memory order as qkv
+        skip = _mask_skip[0]
+        res = ext().attention_fwd(q, k, v, scale, causal, seq_major, colmask, dropout_p, seed_offset, skip)    # out: same memory order as qkv
         out, lse = res[0], res[1]
         so = res[2] if dropout_p > 0.0 else None
-        ctx.save_for_backward(qkv, out, lse, so)
-        ctx.cfg = (nh, nkv, scale, causal, seq_major, dropout_p)
+        ctx.save_for_backward(qkv, out, lse, so, colmask)
+        ctx.cfg = (nh, nkv, scale, causal, seq_major, dropout_p, skip)
         if so is not None:
             ctx.mark_non_differentiable(so)
         return out, so
 
     @staticmethod
     def backward(ctx, do, _dso=None):
-        qkv, out, lse, so = ctx.saved_tensors
-        nh, nkv, scale, causal, seq_major, dropout_p = ctx.cfg
-        if dropout_p > 0.0:
-            dqkv = ext().attention_bwd_packed(qkv, nh, nkv, out, lse, do.contiguous(), scale, causal, seq_major, dropout_p, so)
+        qkv, out, lse, so, colmask = ctx.saved_tensors
+        nh, nkv, scale, causal, seq_major, dropout_p, skip = ctx.cfg
+        if dropout_p > 0.0 or colmask is not None:
+            dqkv = ext().attention_bwd_packed(qkv, nh, nkv, out, lse, do.contiguous(), scale, causal, seq_major, dropout_p, so, colmask, skip)
         else:
             dqkv = ext().attention_bwd_packed(qkv, nh, nkv, out, lse, do.contiguous(), scale, causal, seq_major)
-        return dqkv, None, None, None, None, None, None, None
+        return dqkv, None, None, None, None, None, None, None, None
 
 
-def attention_packed(qkv, nh, nkv, causal=True, scale=None, seq_major=False, dropout_p=0.0, seed_offset=None, return_seed_offset=False):
+def attention_packed(qkv, nh, nkv, causal=True, scale=None, seq_major=False, dropout_p=0.0, seed_offset=None, return_seed_offset=False,
+                     colmask=None):
     """qkv: [B,S,nh+2*nkv,D] contiguous (q heads | k heads | v heads), or [S,B,...] with seq_major=True (the layout of
-    sequence-parallel layers). Returns [B,S,nh,D] (resp. [S,B,nh,D]).  dropout_p, seed_offset, return_seed_offset: as `attention`."""
+    sequence-parallel layers). Returns [B,S,nh,D] (resp. [S,B,nh,D]).  dropout_p, seed_offset, return_seed_offset: as `attention`.
+    colmask: int32 [B, 1|nh, S, 4] column mask over the [B,S] view, as attention_colmask; the backward still writes d(qkv) in place.
+    Where the kernels do not apply, the reference attention runs with colmask_to_dense."""
     x = raw(qkv)
     xb = x.transpose(0, 1) if seq_major else x
     q, k, v = xb[:, :, :nh], xb[:, :, nh:nh + nkv], xb[:, :, nh + nkv:]
+    cm = raw(colmask).to(torch.int32).contiguous() if colmask is not None else None
     if _bwd_backend[0] == "own" and x.is_contiguous() and fused_ok(q, k, v, None, dropout_p, causal):
         sc = float(scale) if scale is not None else 1.0 / math.sqrt(x.shape[-1])
-        out, so = _FlashAttnPacked.apply(x, int(nh), int(nkv), sc, bool(causal), bool(seq_major), float(dropout_p), _seed_offset_arg(seed_offset))
+        out, so = _FlashAttnPacked.apply(x, int(nh), int(nkv), sc, bool(causal), bool(seq_major), float(dropout_p), _seed_offset_arg(seed_offset),
+                                         cm)
         return (wrap(out), so) if return_seed_offset else wrap(out)
     if return_seed_offset:
         raise ValueError("attention_packed: return_seed_offset needs the own kernels (fp16/bf16, head_dim 64 or 128, 0 <= dropout_p < 1)")
-    out = attention(q, k, v, None, dropout_p, causal, scale)
+    out = attention(q, k, v, colmask_to_dense(cm, q.shape[1]) if cm is not None else None, dropout_p, causal, scale)
     return wrap(raw(out).transpose(0, 1).contiguous()) if seq_major else out
 
 

@@ -132,27 +132,35 @@ class LlamaAttention(nn.Layer):
             self.qkv_proj = nn.Linear(h, h + 2 * kv, weight_attr=wattr, bias_attr=False)
             self.o_proj = nn.Linear(h, h, weight_attr=oattr, bias_attr=False)
 
-    def forward(self, x, cos, sin, position_ids=None):
-        return self.attend(self.qkv_proj(x), cos, sin, position_ids)
+    def forward(self, x, cos, sin, position_ids=None, colmask=None):
+        return self.attend(self.qkv_proj(x), cos, sin, position_ids, colmask)
 
-    def attend(self, qkv, cos, sin, position_ids=None):
-        """Everything after the QKV projection: rotary, attention, output projection."""
+    def attend(self, qkv, cos, sin, position_ids=None, colmask=None):
+        """Everything after the QKV projection: rotary, attention, output projection.  colmask: int32 [B, 1, S, 4] column mask of packed
+        documents (and the sliding window, if any), built once per forward by LlamaModel."""
         cfg = self.config
         nh, nkv, hd = self.num_heads, self.num_kv_heads, self.head_dim
         total = nh + 2 * nkv
-        if cfg.sequence_parallel and self.mp > 1 and position_ids is None and _raw(qkv).is_cuda and cfg.sliding_window is None:
-            # sequence-parallel layout [S, B, *] is kept end to end: rotary gets explicit positions (token t = s*B + b -> s) and the
-            # attention kernels address [B, S, h, d] views of the [S, B, ...] memory through their TMA strides - no transpose copies
+        seq_major = cfg.sequence_parallel and self.mp > 1 and _raw(qkv).is_cuda
+        if seq_major and (colmask is not None or (position_ids is None and cfg.sliding_window is None)):
+            # sequence-parallel layout [S, B, *] is kept end to end: rotary gets explicit positions (token t = s*B + b -> s, or the
+            # documents' positions in that order) and the attention kernels address [B, S, h, d] views of the [S, B, ...] memory through
+            # their TMA strides - no transpose copies
             s, b = qkv.shape[0], qkv.shape[1]
-            pid = _seq_major_positions(s, b, _raw(qkv).device)
+            if position_ids is None:
+                pid = _seq_major_positions(s, b, _raw(qkv).device)
+            else:
+                pid = _raw(position_ids).to(torch.int64).expand(b, s).transpose(0, 1).reshape(1, s * b)
             qkv = KR.apply_rope_packed(qkv, cos, sin, nh + nkv, total, hd, pid, neox=True)   # in place on the GEMM output (explicit positions)
-            out = KAT.attention_packed(_raw(qkv).view(s, b, total, hd), nh, nkv, True, None, seq_major=True)   # [S, B, nh, hd]
+            out = KAT.attention_packed(_raw(qkv).view(s, b, total, hd), nh, nkv, True, None, seq_major=True, colmask=colmask)   # [S, B, nh, hd]
             return self.o_proj(_w(_raw(out).reshape(s, b, nh * hd)))
         if cfg.sequence_parallel and self.mp > 1:   # [S, B, *] -> [B, S, *]
             qkv = qkv.transpose([1, 0, 2]).contiguous()
         b, s = qkv.shape[0], qkv.shape[1]
         qkv = KR.apply_rope_packed(qkv, cos, sin, nh + nkv, total, hd, position_ids, neox=True)
-        if cfg.sliding_window is None:
+        if colmask is not None:   # packed documents (the window, if any, is in the mask): in place as below
+            out = KAT.attention_packed(_raw(qkv).view(b, s, total, hd), nh, nkv, True, None, colmask=colmask)
+        elif cfg.sliding_window is None:
             out = KAT.attention_packed(_raw(qkv).view(b, s, total, hd), nh, nkv, True, None)   # [B, S, nh, hd]; q/k/v read in place
         else:
             out = _window_attention(_raw(qkv).view(b, s, total, hd), nh, nkv, cfg.sliding_window)
@@ -168,6 +176,19 @@ def window_mask(sq, sk, window, device):
     qpos = torch.arange(sk - sq, sk, device=device)[:, None]
     kpos = torch.arange(sk, device=device)[None, :]
     return (kpos <= qpos) & (kpos > qpos - window)
+
+
+def document_colmask(attn_mask_startend_row_indices, seq_len, sliding_window=None):
+    """The column mask [B, 1, S, 4] of packed causal documents, from PaddleNLP's attn_mask_startend_row_indices (int [B, 1, S, 1]: key j
+    hides the rows >= its value, the end of its document).  With a sliding window, each key's lt_start is the smaller of the document's
+    and the window's: both hide the rows from a start row to the end, so the minimum is their intersection."""
+    idx = _raw(attn_mask_startend_row_indices)
+    cm = KAT.colmask_from_startend(idx.reshape(idx.shape[0], 1, seq_len, 1), True, seq_len)
+    if sliding_window is not None:
+        win = KAT.colmask_from_window(seq_len, seq_len, sliding_window - 1, 0, True, cm.device)
+        cm = cm.clone()
+        cm[..., 0] = torch.minimum(cm[..., 0], win[..., 0])
+    return cm.contiguous()
 
 
 def _window_attention(x, nh, nkv, window):
@@ -213,11 +234,11 @@ class LlamaDecoderLayer(nn.Layer):
         self.post_attention_layernorm = LlamaRMSNorm(config)
         self.mlp = LlamaMLP(config)
 
-    def _forward(self, h, cos, sin, position_ids=None):
+    def _forward(self, h, cos, sin, position_ids=None, colmask=None):
         if self._lean():
-            return self._forward_lean(h, cos, sin, position_ids)
+            return self._forward_lean(h, cos, sin, position_ids, colmask)
         x = self.input_layernorm(h)
-        a = self.self_attn(x, cos, sin, position_ids)
+        a = self.self_attn(x, cos, sin, position_ids, colmask)
         x, h = self.post_attention_layernorm(a, residual=h)     # fused: h = h + a ; x = rmsnorm(h)
         return h + self.mlp(x)
 
@@ -225,21 +246,21 @@ class LlamaDecoderLayer(nn.Layer):
         # single-GPU (no tensor parallel) CUDA training: norm->linear and swiglu->linear run as memory-lean fused autograd nodes
         return self.self_attn.mp == 1 and self.training and self.input_layernorm.weight.is_cuda and self.config.lean_activations
 
-    def _forward_lean(self, h, cos, sin, position_ids=None):
+    def _forward_lean(self, h, cos, sin, position_ids=None, colmask=None):
         from ..kernels import fused_blocks as FB
 
         at, mlp = self.self_attn, self.mlp
         qkv = FB.norm_linear(h, self.input_layernorm.weight, at.qkv_proj.weight, self.input_layernorm.eps)
-        a = at.attend(qkv, cos, sin, position_ids)
+        a = at.attend(qkv, cos, sin, position_ids, colmask)
         gu, h = FB.norm_linear(a, self.post_attention_layernorm.weight, mlp.gate_up_proj.weight, self.post_attention_layernorm.eps, residual=h)
         return h + FB.swiglu_linear(gu, mlp.down_proj.weight)
 
-    def forward(self, h, cos=None, sin=None, position_ids=None):
+    def forward(self, h, cos=None, sin=None, position_ids=None, colmask=None):
         if cos is None:
             cos, sin = rope_cache(self.config, h.device)
         if self.config.recompute and self.training and torch.is_grad_enabled() and not getattr(self, "_skip_recompute", False):
-            return recompute(self._forward, h, cos, sin, position_ids)
-        return self._forward(h, cos, sin, position_ids)
+            return recompute(self._forward, h, cos, sin, position_ids, colmask)
+        return self._forward(h, cos, sin, position_ids, colmask)
 
 
 _pid_cache = {}
@@ -340,11 +361,16 @@ class LlamaModel(nn.Layer):
         for l in list(self.layers)[len(self.layers) - config.recompute_skip_layers:] if config.recompute_skip_layers else []:
             l._skip_recompute = True
 
-    def forward(self, input_ids, position_ids=None):
+    def forward(self, input_ids, position_ids=None, attn_mask_startend_row_indices=None):
+        """attn_mask_startend_row_indices: int [B, 1, S, 1], causal packed documents as in PaddleNLP (key j hides the rows >= the value);
+        pass document-local position_ids with it."""
         h = self.embedding(input_ids)
         cos, sin = rope_cache(self.config, h.device)
+        colmask = None
+        if attn_mask_startend_row_indices is not None:
+            colmask = document_colmask(attn_mask_startend_row_indices, input_ids.shape[1], self.config.sliding_window)
         for layer in self.layers:
-            h = layer(h, cos, sin, position_ids)
+            h = layer(h, cos, sin, position_ids, colmask) if colmask is not None else layer(h, cos, sin, position_ids)
         return h
 
 
@@ -356,8 +382,8 @@ class LlamaForCausalLM(nn.Layer):
         self.lm_head = LlamaLMHead(config)
         self.criterion = LlamaPretrainingCriterion(config)
 
-    def forward(self, input_ids, labels=None, position_ids=None):
-        h = self.llama(input_ids, position_ids)
+    def forward(self, input_ids, labels=None, position_ids=None, attn_mask_startend_row_indices=None):
+        h = self.llama(input_ids, position_ids, attn_mask_startend_row_indices)
         logits = self.lm_head(h)
         if labels is None:
             return logits

@@ -46,13 +46,13 @@ def flash_attn_unpadded(query, key, value, cu_seqlens_q, cu_seqlens_k, max_seqle
     p = dropout if training else 0.0
     if q.is_cuda and q.dim() == 3:
         # packed batch as ONE sequence under a document mask: no host read of cu_seqlens, no per-sequence launches.
-        # (causal: the diagonal of every sequence is the global diagonal when q and k are packed alike - self attention)
+        # (causal: the diagonal of every sequence is the global diagonal when q and k are packed alike - self attention; otherwise the
+        # mask carries each sequence's own bottom-right aligned causal limit and the kernels run without theirs)
         same = cu_seqlens_q is cu_seqlens_k or (raw(cu_seqlens_q).shape == raw(cu_seqlens_k).shape and q.size(0) == k.size(0))
-        if same or not causal:
-            cm = K.colmask_from_cu_seqlens(cu_seqlens_q, cu_seqlens_k, k.size(0))
-            out = K.attention_colmask(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), cm, causal and same, scale, p, fixed_seed_offset)
-            if out is not None:
-                return out.squeeze(0), None
+        cm = K.colmask_from_cu_seqlens(cu_seqlens_q, cu_seqlens_k, k.size(0), causal=causal and not same)
+        out = K.attention_colmask(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), cm, causal and same, scale, p, fixed_seed_offset)
+        if out is not None:
+            return out.squeeze(0), None
     cq, ck = raw(cu_seqlens_q).tolist(), raw(cu_seqlens_k).tolist()
     outs = []
     for i in range(len(cq) - 1):
